@@ -16,7 +16,7 @@ cost evaluations, parameter update) on the synthetic 2M-voxel / 200-frame hashed
             measured HBM peak.
 `cpu_baseline`: the CPU oracle (float64 restatement of the reference + Ceres semantics) timed on this box's cores on the
             FULL workload (one GN iteration), next to `parity_check`: engine vs oracle on a z-slab of the same scene.
-`--impl reference`: the same oracle with all host threads on the full workload (steps clipped, see the line's `steps`).
+`--impl reference`: the same oracle with all host threads on the full workload (`--ref-max-steps` clips the steps).
 Under torchrun (N > 1) voxels are sharded across ranks (one process per GPU); `mg_selfcheck` compares the sharded engine
 with an unsharded one on the same GPU after 3 iterations.
 `--workload c5`: BASELINE config 5, the coarse-to-fine schedule of Intrinsic3D::refine (0.5M -> 2M -> 8M voxels, 500 frames);
@@ -61,7 +61,36 @@ def lambda_schedule(p, it):
 def base_config(workload, n, F):
     """Identical in both arms (the driver compares the dicts): what the workload IS, nothing about how it is run."""
     return {"workload": f"{workload}: {WORKLOADS[workload]}", "voxels": int(n), "frames": int(F), "iterations_schedule": ITERATIONS, "lm_steps": 50,
-            "inputs_vs_l2": "E_g Jacobian streamed per PCG iteration is ~0.8 GB >> 126 MB L2 (no flush needed)"}
+            "inputs_vs_l2": "E_g Jacobian streamed per PCG iteration is ~0.8 GB >> 50 MB L2 of an H100 (no flush needed)"}
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def write_outputs(out_dir, arrays):
+    """--dump-outputs: <out_dir>/<name>.npy in float32/float64; above DUMP_LIMIT_BYTES the per-voxel arrays keep one seeded row sample
+    (indices in sample_rows.npy), so two builds are compared on the same voxels."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrs = {k: np.ascontiguousarray(v, np.float32 if np.asarray(v).dtype == np.float32 else np.float64) for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrs.values())
+    if total > DUMP_LIMIT_BYTES:
+        n = max(a.shape[0] for a in arrs.values() if a.ndim)
+        long_ = [k for k, a in arrs.items() if a.ndim and a.shape[0] == n]
+        per_row = sum(arrs[k].nbytes // n for k in long_) + 8
+        m = min(n, (DUMP_LIMIT_BYTES - (total - sum(arrs[k].nbytes for k in long_)) - 4096) // per_row)
+        rows = np.sort(np.random.default_rng(0).choice(n, m, replace=False))
+        for k in long_:
+            arrs[k] = np.ascontiguousarray(arrs[k][rows])
+        arrs["sample_rows"] = rows.astype(np.float64)
+    for k, a in arrs.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), a)
+
+
+def iteration_outputs(info):
+    """what i3d_gn_iteration returns besides the state"""
+    nlm = int(info.lm_iterations)
+    return {"cost": [info.cost_initial, info.cost_final], "type_residuals": list(info.type_residuals), "type_costs": list(info.type_costs),
+            "step_accepted": [info.step_accepted], "cg_iterations": list(info.cg_iterations)[:nlm]}
 
 
 class ClockSampler:
@@ -230,14 +259,13 @@ def reference_arm(args, ncores):
     wl = "c3" if args.workload == "c5" else args.workload
     scene = config_scene(wl, device=dev)
     n, F = scene["xyz"].shape[0], scene["lum"].shape[0]
-    # The restated path stops scaling well before 128 threads (round-1 probe on this pool: 32 threads fastest); steps are clipped so that the
-    # FULL-grid run fits the driver's window: 25 full-C3 iterations would take > 5 minutes per N.
+    # The restated path stops scaling well before 128 threads (32 threads were fastest on a 128-core host)
     threads = min(ncores, 32)
-    steps = max(1, min(args.steps, args.ref_max_steps))
+    steps = max(1, args.steps if args.ref_max_steps is None else min(args.steps, args.ref_max_steps))
     warmup = min(args.warmup, 1)
     r = run_cpu(scene, steps, warmup, threads, parallel_cg=True)
-    sample = (f"FULL workload ({n} voxels, {F} frames), one GN iteration per step; steps clipped to {steps} timed + {warmup} warm-up "
-              f"(requested {args.steps} + {args.warmup}): a full-C3 CPU iteration takes ~13 s")
+    sample = (f"FULL workload ({n} voxels, {F} frames), one GN iteration per step; {steps} timed + {warmup} warm-up "
+              f"(requested {args.steps} + {args.warmup})")
     line = {"impl": "reference", "metric": "gauss_newton_iterations_per_sec", "value": r["value"], "unit": "GN iter/s", "n_gpus": args.gpus,
             "steps": steps, "warmup": warmup, "steps_requested": args.steps, "warmup_requested": args.warmup,
             "ms_per_step": 1e3 * r["s_per_step"], "higher_is_better": True, "scaling": "strong",
@@ -258,13 +286,15 @@ def main():
     ap.add_argument("--workload", default=os.environ.get("I3D_WORKLOAD", "c3"), choices=sorted(WORKLOADS))
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--parity-fraction", type=float, default=1.0 / 16.0)
-    ap.add_argument("--ref-max-steps", type=int, default=3)
+    ap.add_argument("--ref-max-steps", type=int, default=None, help="--impl reference: clip the timed steps (a full-C3 CPU iteration takes ~15 s)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity-check", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--e2e-steps", type=int, default=3)
     ap.add_argument("--no-lighting", action="store_true")
     ap.add_argument("--no-selfcheck", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (refined state + iteration info) as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -294,7 +324,9 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     if args.workload == "c5":
         import bench_c5
-        bench_c5.run(args, rank, world, local_rank, dist, ClockSampler)
+        outputs = bench_c5.run(args, rank, world, local_rank, dist, ClockSampler)
+        if args.dump_outputs and outputs is not None:
+            write_outputs(args.dump_outputs, outputs)
         return
     from intrinsic3d_b200.engine import Engine, shard_range
 
@@ -359,6 +391,8 @@ def main():
     elapsed = max_over_ranks(time.perf_counter() - t0)
     clocks = sampler.stop() if rank == 0 else None
     value = args.steps / elapsed
+    if args.dump_outputs and rank == 0 and infos:
+        write_outputs(args.dump_outputs, {**eng.download_state(), **iteration_outputs(infos[-1])})
     # per-kernel table: ONE extra, untimed step with an event pair around every kernel (in the timed region only the phases, the
     # two roofline kernels k_eg_rows / k_eg_apply and k_select_obs carry events: an event between two kernels suppresses their
     # programmatic-dependent-launch overlap)
@@ -374,8 +408,8 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak_gbs = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "data sheet 3350 GB/s (H100 SXM HBM3, not measured)"
     U = 2 * n + 6 * F + 9
     K = p.num_observations
     # rows / active voxels this rank owns (I3DIterInfo carries the GLOBAL sums when sharded)

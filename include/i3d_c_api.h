@@ -1,5 +1,5 @@
 /*
- * i3d_c_api.h — C-ABI of the B200-native joint-refinement engine (libi3d_b200.so).
+ * i3d_c_api.h — C-ABI of the H100-native joint-refinement engine (libi3d_b200.so).
  *
  * This is the drop-in boundary for the ONE hot path of NVlabs/intrinsic3d that this
  * repository replaces: Optimizer::optimize's outer Gauss-Newton iteration
@@ -13,7 +13,7 @@
  * copied during the call (pinned memory makes the copies asynchronous-capable but is not
  * required); one handle is not thread-safe; every function returns 0 on success, non-zero
  * on error with a message available from i3d_last_error().  There is NO CPU fallback:
- * i3d_engine_create fails if no sm_100 device is present.
+ * i3d_engine_create fails if no sm_90 (H100) device is present.
  *
  * Each entry point cites the reference interface it replaces (paths relative to
  * libintrinsic3d/).

@@ -1,5 +1,5 @@
 /*
- * i3d_types.h — plain-C parameter / result structs shared by the B200 engine
+ * i3d_types.h — plain-C parameter / result structs shared by the H100 engine
  * C-ABI (include/i3d_c_api.h) and by the CPU oracle (oracle/oracle_api.h).
  *
  * Field meanings follow the reference (paths relative to the NVlabs/intrinsic3d

@@ -1,6 +1,6 @@
 // nv/lighting/lighting_svsh.h — spatially-varying SH lighting with the reference's call surface (constructor arguments, estimate(),
 // computeVoxelShCoeffs(), interpolate(), shCoeffs(), subvolumes(); libintrinsic3d/include/nv/lighting/lighting_svsh.h:47-70), computed by
-// the B200 engine (i3d_estimate_lighting, include/i3d_c_api.h) instead of Ceres.
+// the H100 engine (i3d_estimate_lighting, include/i3d_c_api.h) instead of Ceres.
 //
 //   LightingSVSH lighting(grid, subvolume_size, lambda_reg, thres_shell, weighted);
 //   if (!lighting.estimate()) ...                          // src/refinement/intrinsic3d.cpp:255-262

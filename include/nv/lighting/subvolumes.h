@@ -1,5 +1,5 @@
 // nv/lighting/subvolumes.h — Subvolumes with the reference's query API (libintrinsic3d/include/nv/lighting/subvolumes.h:47-90),
-// filled from the B200 engine's subvolume table (i3d_download_lighting) instead of a host pass over the hash.
+// filled from the H100 engine's subvolume table (i3d_download_lighting) instead of a host pass over the hash.
 //
 // Numbering: ascending (z, y, x) of the integer cube index (the reference numbers in std::unordered_map iteration order, which
 // is unspecified; nothing downstream depends on it).  bounds()/color() exist for API completeness (debug visualisation only).

@@ -1,6 +1,6 @@
 // nv/refinement/intrinsic3d.h — the refinement orchestrator with the reference's control flow
 // (libintrinsic3d/include/nv/refinement/intrinsic3d.h:60-176, src/refinement/intrinsic3d.cpp:206-409), driving ONE resident
-// B200 engine through the C-ABI for the whole coarse-to-fine schedule:
+// H100 engine through the C-ABI for the whole coarse-to-fine schedule:
 //
 //   refine(grid):  convert -> init (initial recolouring) ->
 //     for grid level (coarse -> fine):   prepareGridLevel   thin-shell threshold + i3d_clear_voxels_outside_thin_shell

@@ -1,5 +1,5 @@
 // nv/refinement/optimizer.h — Optimizer with the reference's API surface (include/nv/refinement/optimizer.h:59-141), driving the
-// B200 engine through the C-ABI (include/i3d_c_api.h) instead of Ceres.
+// H100 engine through the C-ABI (include/i3d_c_api.h) instead of Ceres.
 //
 // optimize() mutates, in place and like the reference: grid voxels' sdf_refined / albedo, image_formation.poses /
 // intrinsics / distortion_coeffs.  Returns false only if the grid is null or iterations < 1 (optimizer.cpp:113-114) or if the

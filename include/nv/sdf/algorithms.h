@@ -1,6 +1,6 @@
 // nv/sdf/algorithms.h — the two SDFAlgorithms entry points of the refinement loop's grid-level transitions, with the
 // reference's signatures (libintrinsic3d/include/nv/sdf/algorithms.h; src/sdf/algorithms.cpp:200-235, 368-458), computed by
-// the B200 engine (i3d_clear_voxels_outside_thin_shell / i3d_upsample_grid) instead of host hash-map passes:
+// the H100 engine (i3d_clear_voxels_outside_thin_shell / i3d_upsample_grid) instead of host hash-map passes:
 //
 //   SDFAlgorithms::clearVoxelsOutsideThinShell(grid, thres_shell);     // Intrinsic3D::prepareGridLevel  (intrinsic3d.cpp:307-313)
 //   SparseVoxelGrid<VoxelSBR>* up = SDFAlgorithms::upsample(grid);      // Intrinsic3D::finishGridLevel   (intrinsic3d.cpp:320-331)

@@ -1,10 +1,10 @@
 #!/bin/bash
-# Builds libi3d_b200.so (sm_100a only) in-tree: intrinsic3d_b200/libi3d_b200.so
+# Builds libi3d_b200.so (sm_90a only, H100) in-tree: intrinsic3d_b200/libi3d_b200.so
 set -e
 HERE="$(cd "$(dirname "$0")" && pwd)"
 OUT="$HERE/../libi3d_b200.so"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-"$NVCC" -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 \
+"$NVCC" -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 \
     -Xcompiler -fPIC,-O3 -ccbin /usr/bin/g++ -shared $EXTRA_NVCC_FLAGS \
     -o "$OUT" "$HERE/i3d_engine.cu"
 echo "built $OUT"

@@ -1,5 +1,5 @@
 /*
- * i3d_engine.cu — host side of the B200 joint-refinement engine + the C-ABI of include/i3d_c_api.h.
+ * i3d_engine.cu — host side of the H100 joint-refinement engine + the C-ABI of include/i3d_c_api.h.
  *
  * One I3DEngine = one GPU.  i3d_gn_iteration() is one outer iteration of Optimizer::optimize
  * (libintrinsic3d/src/refinement/optimizer.cpp:119-171): observation selection (k_select_obs),
@@ -150,6 +150,7 @@ struct I3DEngine
     Dev<int> fail_flag;
     // vectors
     Dev<float> v_bg, v_cg, v_s, v_jtj, v_b, v_x, v_r, v_z, v_p, v_ps, v_qg, v_tr, v_delta;
+    Dev<double> v_bgd, v_cgd, v_qgd, cam_accd;     // double accumulators of k_eg_accum / k_eg_apply
     Dev<CgCtl> ctl;
     // reductions
     Dev<double> red_partials, red_out;
@@ -316,6 +317,9 @@ void ensure_vectors(I3DEngine* e)
     const size_t U = static_cast<size_t>(e->U());
     Dev<float>* vs[] = {&e->v_bg, &e->v_cg, &e->v_s, &e->v_jtj, &e->v_b, &e->v_x, &e->v_r, &e->v_z, &e->v_p, &e->v_ps, &e->v_qg, &e->v_delta};
     for (auto* v : vs) v->ensure(U);
+    Dev<double>* vd[] = {&e->v_bgd, &e->v_cgd, &e->v_qgd};
+    for (auto* v : vd) v->ensure(U);
+    e->cam_accd.ensure(CamAccLayout{e->F}.size());
     e->v_tr.ensure(static_cast<size_t>(e->n));
     e->ctl.ensure(1);
     e->minv.ensure(36 * static_cast<size_t>(e->F) + 41);
@@ -330,7 +334,7 @@ SolveVecs solve_vecs(I3DEngine* e)
     SolveVecs sv;
     sv.n = e->n; sv.F = e->F; sv.U = e->U();
     sv.bg = e->v_bg.p; sv.cg = e->v_cg.p; sv.s = e->v_s.p; sv.jtj = e->v_jtj.p; sv.b = e->v_b.p;
-    sv.x = e->v_x.p; sv.r = e->v_r.p; sv.z = e->v_z.p; sv.p = e->v_p.p; sv.ps = e->v_ps.p; sv.qg = e->v_qg.p; sv.tr = e->v_tr.p;
+    sv.x = e->v_x.p; sv.r = e->v_r.p; sv.z = e->v_z.p; sv.p = e->v_p.p; sv.ps = e->v_ps.p; sv.qg = e->v_qg.p; sv.qgd = e->v_qgd.p; sv.tr = e->v_tr.p;
     return sv;
 }
 
@@ -476,7 +480,7 @@ void exchange(I3DEngine* e, float* v0, float* v1, float* extra_f, int n_extra_f,
 
 size_t apply_smem_bytes(int F, int K)
 {
-    return (static_cast<size_t>((6 * F + 9 + 31) & ~31) + static_cast<size_t>(K) * 6 * kThreads) * sizeof(float);
+    return static_cast<size_t>((6 * F + 9 + 15) & ~15) * sizeof(double) + static_cast<size_t>(K) * 6 * kThreads * sizeof(float);
 }
 
 // applies the CGNR operator to the vector whose Jacobi-scaled copy is in sv.ps: afterwards qg holds the (globally summed)
@@ -556,6 +560,10 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     CK(cudaMemsetAsync(e->v_delta.p, 0, U * sizeof(float), st));
     CK(cudaMemsetAsync(e->v_tr.p, 0, static_cast<size_t>(n) * sizeof(float), st));      // E_r row values: only active ring voxels are written (k_eg_apply)
     CK(cudaMemsetAsync(e->cam_acc.p, 0, lay.size() * sizeof(float), st));
+    CK(cudaMemsetAsync(e->v_bgd.p, 0, U * sizeof(double), st));
+    CK(cudaMemsetAsync(e->v_cgd.p, 0, U * sizeof(double), st));
+    CK(cudaMemsetAsync(e->v_qgd.p, 0, U * sizeof(double), st));
+    CK(cudaMemsetAsync(e->cam_accd.p, 0, lay.size() * sizeof(double), st));
     CK(cudaMemsetAsync(e->red_out.p, 0, 2 * kSiteVals * sizeof(double), st));   // SITE_BUILD, SITE_REG (a rank without rows skips the kernels)
     e->Rt.ensure(12 * static_cast<size_t>(F));
     e->pose_ctx.ensure(F); e->pose_ctx_c.ensure(F);
@@ -625,11 +633,15 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
             KernelTimer kt(e, "k_eg_build", 0);
             launch_eg_rows<ROWS_BUILD>(e, g, cv, rows, e->obs_frame.p, e->obs_w.p);
         }
-        const size_t smem = (static_cast<size_t>((lay.size() + 31) & ~31) + static_cast<size_t>(K) * 8 * kThreads) * sizeof(float);
+        const size_t smem = static_cast<size_t>((lay.size() + 15) & ~15) * sizeof(double) + static_cast<size_t>(K) * 8 * kThreads * sizeof(float);
         if (smem > 48 * 1024) CK(cudaFuncSetAttribute(k_eg_accum, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-        KernelTimer kt(e, "k_eg_accum");
-        pdl_launch(e, k_eg_accum, blocks_for(static_cast<size_t>(n_active)), kThreads, smem, g, rows, F, e->v_bg.p, e->v_cg.p, e->cam_acc.p, e->site(SITE_BUILD));
-        e->launches += 2;
+        {
+            KernelTimer kt(e, "k_eg_accum");
+            pdl_launch(e, k_eg_accum, blocks_for(static_cast<size_t>(n_active)), kThreads, smem, g, rows, F, e->v_bgd.p, e->v_cgd.p, e->cam_accd.p, e->site(SITE_BUILD));
+        }
+        pdl_launch(e, k_acc_to_float, blocks_for(std::max(U, static_cast<size_t>(lay.size()))), kThreads, 0, static_cast<int64_t>(U), lay.size(),
+                   e->v_bgd.p, e->v_cgd.p, e->cam_accd.p, e->v_bg.p, e->v_cg.p, e->cam_acc.p);
+        e->launches += 3;
     }
     RegView rv;
     rv.flags = e->flags.p; rv.ea_w = e->ea_w.p; rv.lap = e->lap.p;
@@ -876,7 +888,8 @@ int i3d_engine_create(int device, I3DEngine** out)
     if (device < 0 || device >= count) return fail(nullptr, "i3d_engine_create: device %d out of range (%d devices)", device, count);
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, "i3d_engine_create: cannot query device %d", device);
-    if (prop.major < 10) return fail(nullptr, "i3d_engine_create: device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+    // arch-specific sm_90a code runs on compute capability 9.0 only
+    if (prop.major != 9 || prop.minor != 0) return fail(nullptr, "i3d_engine_create: device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
     I3DEngine* e = new I3DEngine();
     e->device = device;
     const int rc = guarded(e, [&]() {

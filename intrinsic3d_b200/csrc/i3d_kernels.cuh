@@ -1,5 +1,5 @@
 /*
- * i3d_kernels.cuh — sm_100a kernels of the joint-refinement engine.
+ * i3d_kernels.cuh — sm_90a kernels of the joint-refinement engine.
  *
  * Data layout in HBM (all SoA, voxel index = position in the host's iteration order):
  *   grid      x,y,z int32[n]; sdf0, sdf, albedo double[n]; weight float[n]; rgb uchar4[n];
@@ -1078,15 +1078,16 @@ k_eg_rows(GridView g, FrameView fr, CamView cv, EgRows rows, const int32_t* __re
 // memory, then the warp walks over the DISTINCT frames among its 32 x K rows and reduces the 33 products of each with a
 // 32-wide butterfly reduce-scatter + one scalar all-reduce.
 __global__ void __launch_bounds__(kThreads)
-k_eg_accum(GridView g, EgRows rows, int F, float* __restrict__ bg, float* __restrict__ cg, float* __restrict__ cam_acc /* CamAccLayout.size() */,
+k_eg_accum(GridView g, EgRows rows, int F, double* __restrict__ bg, double* __restrict__ cg, double* __restrict__ cam_acc /* CamAccLayout.size() */,
            ReduceSite site /* out: [0] sum raw weights, [1] sum raw w*r^2, [2] valid rows */)
 {
+    // summed in double like k_eg_apply; k_acc_to_float rounds the totals once
     pdl_prologue();
-    extern __shared__ float s_dyn[];
+    extern __shared__ double s_dyn_d[];
     const CamAccLayout lay{F};
-    float* s_cam = s_dyn;
-    float* s_park = s_dyn + ((lay.size() + 31) & ~31);        // [K][8][kThreads]
-    for (int i = threadIdx.x; i < lay.size(); i += blockDim.x) s_cam[i] = 0.0f;
+    double* s_cam = s_dyn_d;
+    float* s_park = reinterpret_cast<float*>(s_dyn_d + ((lay.size() + 15) & ~15));   // [K][8][kThreads]
+    for (int i = threadIdx.x; i < lay.size(); i += blockDim.x) s_cam[i] = 0.0;
     __syncthreads();
     const int tid = threadIdx.x, lane = tid & 31;
     const int a = blockIdx.x * blockDim.x + tid;
@@ -1143,7 +1144,7 @@ k_eg_accum(GridView g, EgRows rows, int F, float* __restrict__ bg, float* __rest
         for (int i = 0; i < 2; ++i)
         {
             const int id = rs_index<64>(i, lane);
-            if (id < 43 && tl[i] != 0.0f) atomicAdd(s_cam + lay.tail() + id, tl[i]);
+            if (id < 43 && tl[i] != 0.0f) atomicAdd(s_cam + lay.tail() + id, static_cast<double>(tl[i]));
         }
     }
     // ---- pose blocks: walk over the distinct frames of the warp's rows
@@ -1190,9 +1191,9 @@ k_eg_accum(GridView g, EgRows rows, int F, float* __restrict__ bg, float* __rest
         warp_reduce_scatter<32>(v, lane);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) last += __shfl_xor_sync(0xffffffffu, last, o);
-        float* dst = s_cam + lay.pose_stride() * f0;
-        if (v[0] != 0.0f) atomicAdd(dst + lane, v[0]);              // rs_index<32>(0, lane) == lane
-        if (lane == 0 && last != 0.0f) atomicAdd(dst + 32, last);
+        double* dst = s_cam + lay.pose_stride() * f0;
+        if (v[0] != 0.0f) atomicAdd(dst + lane, static_cast<double>(v[0]));              // rs_index<32>(0, lane) == lane
+        if (lane == 0 && last != 0.0f) atomicAdd(dst + 32, static_cast<double>(last));
     }
     if (in_range && acc[2] > 0.0)
     {
@@ -1205,11 +1206,21 @@ k_eg_accum(GridView g, EgRows rows, int F, float* __restrict__ bg, float* __rest
         idx[10] = n + v; idx[11] = n + xp; idx[12] = n + yp; idx[13] = n + zp;
 #pragma unroll
         for (int m = 0; m < 14; ++m)
-            if (csum[m] != 0.0f) { atomicAdd(bg + idx[m], gsum[m]); atomicAdd(cg + idx[m], csum[m]); }
+            if (csum[m] != 0.0f) { atomicAdd(bg + idx[m], static_cast<double>(gsum[m])); atomicAdd(cg + idx[m], static_cast<double>(csum[m])); }
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < lay.size(); i += blockDim.x) { const float vv = s_cam[i]; if (vv != 0.0f) atomicAdd(cam_acc + i, vv); }
+    for (int i = threadIdx.x; i < lay.size(); i += blockDim.x) { const float vv = static_cast<float>(s_cam[i]); if (vv != 0.0f) atomicAdd(cam_acc + i, static_cast<double>(vv)); }
     grid_reduce<3>(acc, site);
+}
+
+// k_eg_accum's double totals -> the float vectors the iteration reads
+__global__ void k_acc_to_float(int64_t U, int ncam, const double* __restrict__ bgd, const double* __restrict__ cgd, const double* __restrict__ camd,
+                               float* __restrict__ bg, float* __restrict__ cg, float* __restrict__ cam_acc)
+{
+    pdl_prologue();
+    const int64_t j = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    if (j < U) { bg[j] = static_cast<float>(bgd[j]); cg[j] = static_cast<float>(cgd[j]); }
+    if (j < ncam) cam_acc[j] = static_cast<float>(camd[j]);
 }
 
 // final per-row weights once the type weight is known (NLSSolver::normalizeCostTermWeights, nls_solver.cpp:379-394)
@@ -1332,6 +1343,7 @@ struct SolveVecs
     float* b;       // J'^T f
     // PCG
     float* x; float* r; float* z; float* p; float* ps; float* qg;
+    double* qgd;    // [U] E_g part of qg in double (k_eg_apply), consumed and cleared by k_op_partial
     float* tr;      // [n] E_r row values of the current input vector (unweighted)
 };
 
@@ -1541,20 +1553,21 @@ enum { APPLY_CG = 0, APPLY_MODEL = 1 };
 //                                (A first version reduced per row slot: ~20 passes per warp, 49 % of the kernel's
 //                                instructions were shuffle/select traffic; profiles/r01_summary.md.)
 //   APPLY_MODEL: partial model_cost_change += -w_k u_k (r_k + u_k/2)          (TrustRegionMinimizer::ComputeTrustRegionStep)
+// Contributions are added in double (exact for a few float terms): the result does not depend on the atomics' order.
 // (A bulk-async / mbarrier staged variant was measured slower: the kernel is issue-bound, not latency-bound.)
 template <int MODE>
 __global__ void __launch_bounds__(kThreads)
 k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __restrict__ ps, const CgCtl* __restrict__ ctl, int respect_done, ReduceSite site)
 {
     pdl_prologue();
-    extern __shared__ float s_dyn[];     // [6F + 9] camera accumulators | [K][6][kThreads] parked pose contributions
+    extern __shared__ double s_dyn_d[];  // [6F + 9] camera accumulators (double) | [K][6][kThreads] parked pose contributions (float)
     if (respect_done && ctl->done) return;
     const int ncam = 6 * sv.F + 9;
-    float* s_cam = s_dyn;
-    float* s_jp = s_dyn + ((ncam + 31) & ~31);
+    double* s_cam = s_dyn_d;
+    float* s_jp = reinterpret_cast<float*>(s_dyn_d + ((ncam + 15) & ~15));
     if (MODE == APPLY_CG)
     {
-        for (int i = threadIdx.x; i < ncam; i += blockDim.x) s_cam[i] = 0.0f;
+        for (int i = threadIdx.x; i < ncam; i += blockDim.x) s_cam[i] = 0.0;
         __syncthreads();
     }
     const int tid = threadIdx.x, lane = tid & 31;
@@ -1681,12 +1694,12 @@ k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __res
             val += __shfl_xor_sync(0xffffffffu, val, 2);
             val += __shfl_xor_sync(0xffffffffu, val, 1);
             const int id = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
-            if ((lane & 3) == 0 && id < 6 && val != 0.0f) atomicAdd(s_cam + 6 * f0 + id, val);
+            if ((lane & 3) == 0 && id < 6 && val != 0.0f) atomicAdd(s_cam + 6 * f0 + id, static_cast<double>(val));
         }
         if (any)
         {
 #pragma unroll
-            for (int m = 0; m < 14; ++m) atomicAdd(sv.qg + idx[m], out[m]);
+            for (int m = 0; m < 14; ++m) atomicAdd(sv.qgd + idx[m], static_cast<double>(out[m]));
         }
         {
             float vv[32];
@@ -1695,10 +1708,11 @@ k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __res
 #pragma unroll
             for (int m = 9; m < 32; ++m) vv[m] = 0.0f;
             warp_reduce_scatter<32>(vv, lane);
-            if (lane < 9 && vv[0] != 0.0f) atomicAdd(s_cam + 6 * sv.F + lane, vv[0]);
+            if (lane < 9 && vv[0] != 0.0f) atomicAdd(s_cam + 6 * sv.F + lane, static_cast<double>(vv[0]));
         }
         __syncthreads();
-        for (int i = tid; i < ncam; i += blockDim.x) { const float vv = s_cam[i]; if (vv != 0.0f) atomicAdd(sv.qg + 2 * sv.n + i, vv); }
+        // block partial rounded to float: the sum over blocks stays exact in double
+        for (int i = tid; i < ncam; i += blockDim.x) { const float vv = static_cast<float>(s_cam[i]); if (vv != 0.0f) atomicAdd(sv.qgd + 2 * sv.n + i, static_cast<double>(vv)); }
     }
     grid_reduce<1>(acc, site);
 }
@@ -1767,7 +1781,8 @@ __global__ void k_epilogue(CgCtl* __restrict__ ctl, const double* __restrict__ s
 }
 
 // Per-unknown part of the operator: adds the regulariser rows OWNED by this rank (gather form) into qg, in place:
-//     qg[j] += sum over owned E_r / E_s / E_a rows touching j          (raw, Jacobi scale applied by the consumer)
+//     qg[j] += qgd[j] (k_eg_apply's E_g part, rounded once; qgd is cleared) + sum over owned E_r / E_s / E_a rows touching j
+//     (raw, Jacobi scale applied by the consumer)
 // The operator output  q_j = s_j * qg_j(total) + D_j^2 p_j  is never materialised: k_cg_update forms it on the fly.
 // MODE APPLY_CG   : partial p.q += (owned regulariser rows)^2 + D^2 p^2 (owned unknowns); last block: alpha = rho / pq.
 // MODE APPLY_MODEL: partial model_cost_change of the owned regulariser rows (qg untouched).
@@ -1861,7 +1876,14 @@ k_op_partial(GridView g, RegView rv, SolveVecs sv, Shard sh, int64_t count, cons
     if (MODE == APPLY_CG)
     {
 #pragma unroll
-        for (int e = 0; e < VEC; ++e) if (regs[e] != 0.0f) sv.qg[js[e]] += regs[e];
+        for (int e = 0; e < VEC; ++e)
+        {
+            if (tbase + e >= count) break;
+            const double eg = sv.qgd[js[e]];
+            if (eg != 0.0) sv.qgd[js[e]] = 0.0;
+            const float add = static_cast<float>(eg) + regs[e];
+            if (add != 0.0f) sv.qg[js[e]] += add;
+        }
     }
     if (grid_reduce<1>(acc, site) && threadIdx.x == 0)
     {

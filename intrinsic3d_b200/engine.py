@@ -2,7 +2,7 @@
 
 This is plumbing for tests and bench.py: it passes HOST numpy buffers through the same
 extern "C" entry points a C++ caller (include/nv/refinement/ shims) uses.  There is no CPU
-fallback: if the CUDA library is missing or no sm_100 device is present, construction raises.
+fallback: if the CUDA library is missing or no sm_90 (H100) device is present, construction raises.
 """
 from __future__ import annotations
 

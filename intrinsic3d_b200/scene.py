@@ -4,7 +4,7 @@ A bumpy sphere (radius rho0*(1+bump*sin(6*theta)*sin(5*phi))) lit by a 9-term
 un-normalised SH environment (basis order of the reference,
 libintrinsic3d/include/nv/shading.h:57-65), with a 3-D checker albedo, observed
 by F pinhole cameras on a helix looking at the centre.  The function emits the
-flat arrays that both the B200 engine (i3d_upload_*) and the CPU oracle consume:
+flat arrays that both the H100 engine (i3d_upload_*) and the CPU oracle consume:
 
     xyz[n,3] int32, sdf0/sdf_refined/albedo[n] f64, weight[n] f32, rgb[n,3] u8,
     lum/depth[F,H,W] f32 (already at the pyramid level used), poses[F,6] f64

@@ -42,7 +42,7 @@ def main():
                 hist[cur][m.group(1)] += 1
     out = os.path.join(HERE, f"{tag}_sass.txt")
     with open(out, "w") as f:
-        f.write("# static SASS opcode counts (cuobjdump -sass intrinsic3d_b200/libi3d_b200.so, sm_100a), top 24 per kernel\n")
+        f.write("# static SASS opcode counts (cuobjdump -sass intrinsic3d_b200/libi3d_b200.so, sm_90a), top 24 per kernel\n")
         tot_special = collections.Counter()
         for fn, h in hist.items():
             for op in ("ACQBULK", "PREEXIT", "UBLKCP", "UTMALDG", "UTCMMA", "HMMA", "TLD4", "SYNCS"):
