@@ -78,7 +78,11 @@ int         i3d_set_sh(I3DEngine* e, const double* sh9n);
 /* ONE outer iteration of Optimizer::optimize (optimizer.cpp:119-171): observation selection,
  * residual collection, weight normalisation, parameter fixing, LM solve that stops at the
  * first successful step.  State (sdf_refined, albedo, poses, intrinsics, distortion) is
- * updated on the device.  info mirrors NLSSolver::ProblemInfo/SolverInfo. */
+ * updated on the device.  info mirrors NLSSolver::ProblemInfo/SolverInfo.
+ * Frame-count limit: k_eg_accum holds the camera sums of all F frames plus K x 8 KB of parked rows in one block's shared memory,
+ * (33F + 43) * 8 + K * 8 KB bytes next to its static buffers, against the device's opt-in limit per block (227 KB on H100): about
+ * 629 frames at K = 8 (measured on H100) or about 720 at K = 5.  Beyond it the call fails before launching anything, with a message that names F, K and the
+ * largest F allowed; the engine stays usable (fewer frames or a smaller K). */
 int         i3d_gn_iteration(I3DEngine* e, const I3DParams* params, I3DIterInfo* info);
 
 /* Reads the refined parameters back (the in-place mutation the reference performs through
@@ -186,6 +190,15 @@ int         i3d_debug_get_observations(I3DEngine* e, int32_t K, int32_t* frames,
 /* last evaluated LM trial step in unknown space [sdf n | albedo n | poses 6F | intr 4 | dist 5]
  * (unscaled delta), the free mask and the Jacobi column scale. */
 int         i3d_debug_get_step(I3DEngine* e, double* step, uint8_t* free_mask, double* col_scale);
+/* normal-equation pieces of the last iteration (build_only = 1 is enough), unknown space [U = 2n + 6F + 9]: b[U] = J'^T f (Jacobi
+ * scaled gradient), s[U] (Jacobi column scale, 0 for fixed unknowns), jtj[U] = s^2 * column norm^2, and the raw (unweighted by the
+ * type weight, unscaled) E_g camera sums cam_acc[33F + 43]: per frame 6 gradient (sum w_raw r J), 6 column norms, the upper 6x6
+ * triangle row by row (21); then 9 gradient, 9 column norms of intrinsics | distortion, the upper 4x4 (10) and 5x5 (15) triangles.
+ * Any pointer may be NULL. */
+int         i3d_debug_get_normal_equations(I3DEngine* e, float* b, float* s, float* jtj, float* cam_acc);
+/* q[U] = S (J^T W J) S v for the rows of the last iteration (all four terms, no D^2 term): the raw operator output of the production
+ * k_eg_apply + k_op_partial pair times s, in float.  Leaves nothing behind that a following i3d_gn_iteration reads.  Single GPU only. */
+int         i3d_debug_apply_operator(I3DEngine* e, const float* v, float* q);
 
 #ifdef __cplusplus
 }

@@ -158,6 +158,7 @@ struct I3DEngine
     size_t max_blocks = 0;
     // debug
     bool keep_raw = false;
+    Dev<float> dbg_v;            // input vector of i3d_debug_apply_operator
     I3DParams last_params{};
     bool have_iter = false;
     std::map<std::string, Phase> phases;
@@ -483,6 +484,29 @@ size_t apply_smem_bytes(int F, int K)
     return static_cast<size_t>((6 * F + 9 + 15) & ~15) * sizeof(double) + static_cast<size_t>(K) * 6 * kThreads * sizeof(float);
 }
 
+size_t accum_smem_bytes(int F, int K)
+{
+    return static_cast<size_t>((CamAccLayout{F}.size() + 15) & ~15) * sizeof(double) + static_cast<size_t>(K) * 8 * kThreads * sizeof(float);
+}
+
+// The per-frame camera accumulators of k_eg_accum and k_eg_apply live in one block's shared memory: refuse, before anything is
+// launched, a frame count whose dynamic plus static shared memory exceeds the device's opt-in limit per block.
+int check_frame_limit(I3DEngine* e, int F, int K)
+{
+    int optin = 0;
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->device));
+    cudaFuncAttributes fa_acc{}, fa_app{};
+    CK(cudaFuncGetAttributes(&fa_acc, k_eg_accum));
+    CK(cudaFuncGetAttributes(&fa_app, k_eg_apply<APPLY_CG>));
+    const size_t lim = static_cast<size_t>(optin);
+    auto fits = [&](int f) { return fa_acc.sharedSizeBytes + accum_smem_bytes(f, K) <= lim && fa_app.sharedSizeBytes + apply_smem_bytes(f, K) <= lim; };
+    if (fits(F)) return 0;
+    int fmax = 0;
+    while (fits(fmax + 1)) ++fmax;
+    return fail(e, "i3d_gn_iteration: %d frames at K = %d observations need %zu bytes of shared memory per block in k_eg_accum (device limit %d): "
+                   "at most %d frames at K = %d", F, K, fa_acc.sharedSizeBytes + accum_smem_bytes(F, K), optin, fmax, K);
+}
+
 // applies the CGNR operator to the vector whose Jacobi-scaled copy is in sv.ps: afterwards qg holds the (globally summed)
 // raw J'^T J' part; k_cg_update forms q = s*qg + D^2 v on the fly and resets qg.
 void launch_operator(I3DEngine* e, const GridView& g, const RegView& rv, const EgRows& rows, const SolveVecs& sv, const Shard& sh, const float* vin,
@@ -524,6 +548,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     if (K > I3D_MAX_OBS) return fail(e, "i3d_gn_iteration: num_observations (%d) exceeds I3D_MAX_OBS (%d)", K, I3D_MAX_OBS);
     if (P.lm_steps < 1) return fail(e, "i3d_gn_iteration: lm_steps < 1");
     if (P.residual_reset_period < 1) return fail(e, "i3d_gn_iteration: residual_reset_period < 1");
+    if (check_frame_limit(e, e->F, K) != 0) return 1;
     e->K = K;
     e->last_params = P;
     e->phases.clear(); e->timed.clear(); e->ev_used = 0; e->launches = 0; e->host_syncs = 0;
@@ -633,7 +658,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
             KernelTimer kt(e, "k_eg_build", 0);
             launch_eg_rows<ROWS_BUILD>(e, g, cv, rows, e->obs_frame.p, e->obs_w.p);
         }
-        const size_t smem = static_cast<size_t>((lay.size() + 15) & ~15) * sizeof(double) + static_cast<size_t>(K) * 8 * kThreads * sizeof(float);
+        const size_t smem = accum_smem_bytes(F, K);
         if (smem > 48 * 1024) CK(cudaFuncSetAttribute(k_eg_accum, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
         {
             KernelTimer kt(e, "k_eg_accum");
@@ -962,7 +987,7 @@ int i3d_upload_frames(I3DEngine* e, int32_t F, int32_t W, int32_t H, const float
     if (F <= 0 || W <= 0 || H <= 0) return fail(e, "i3d_upload_frames: bad dimensions");
     return guarded(e, [&]() {
         const size_t cnt = static_cast<size_t>(F) * W * H;
-        if (F != e->F) e->have_cam = false;
+        if (F != e->F) { e->have_cam = false; e->have_iter = false; }     // the unknown space of the last iteration no longer matches
         if (F != e->F || W != e->W || H != e->H) e->have_color = false;
         e->F = F; e->W = W; e->H = H; e->pyr_scale = pyr_scale;
         e->lum.ensure(cnt); e->depth.ensure(cnt);
@@ -1573,6 +1598,69 @@ int i3d_debug_get_step(I3DEngine* e, double* step, uint8_t* free_mask, double* c
             if (free_mask) free_mask[j] = s[j] != 0.0f;
             if (col_scale) col_scale[j] = s[j];
         }
+        return 0;
+    });
+}
+
+int i3d_debug_get_normal_equations(I3DEngine* e, float* b, float* s, float* jtj, float* cam_acc)
+{
+    if (!e || !e->have_iter) return fail(e, "i3d_debug_get_normal_equations: no iteration yet");
+    return guarded(e, [&]() {
+        const size_t U = static_cast<size_t>(e->U());
+        cudaStream_t st = e->stream;
+        if (b) CK(cudaMemcpyAsync(b, e->v_b.p, U * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (s) CK(cudaMemcpyAsync(s, e->v_s.p, U * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (jtj) CK(cudaMemcpyAsync(jtj, e->v_jtj.p, U * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (cam_acc) CK(cudaMemcpyAsync(cam_acc, e->cam_acc.p, CamAccLayout{e->F}.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    });
+}
+
+int i3d_debug_apply_operator(I3DEngine* e, const float* v, float* q)
+{
+    if (!e || !e->have_iter) return fail(e, "i3d_debug_apply_operator: no iteration yet");
+    if (!v || !q) return fail(e, "i3d_debug_apply_operator: NULL vector");
+    if (e->world > 1) return fail(e, "i3d_debug_apply_operator: single GPU only");
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t U = static_cast<size_t>(e->U());
+        const I3DParams& P = e->last_params;
+        e->dbg_v.ensure(U);
+        // the operator kernels are no-ops once the PCG has stopped: run them under a running copy of the control block and
+        // put the original back afterwards (with is_cg_iteration = 0 they do not write it)
+        CgCtl saved{}, running{};
+        CK(cudaMemcpyAsync(&saved, e->ctl.p, sizeof(CgCtl), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        running = saved; running.done = 0; running.inv_radius = 0.0;
+        CK(cudaMemcpyAsync(e->ctl.p, &running, sizeof(CgCtl), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(e->dbg_v.p, v, U * sizeof(float), cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(e->v_qg.p, 0, U * sizeof(float), st));
+        const int timer_level = e->timer_level;
+        const int64_t launches = e->launches;
+        e->timer_level = -1;                       // keep the last iteration's kernel table
+        GridView g = e->grid_view(e->sdf, e->alb);
+        RegView rv;
+        rv.flags = e->flags.p; rv.ea_w = e->ea_w.p; rv.lap = e->lap.p;
+        rv.use_er = P.use_er; rv.use_es = P.use_es; rv.use_ea = P.use_ea;
+        EgRows rows;
+        rows.n_active = e->n_active; rows.K = e->K; rows.stride = e->stride; rows.act = e->act.p; rows.J = e->J.p; rows.row_frame = e->row_frame.p;
+        rows.row_res = e->row_res.p; rows.row_wraw = e->row_wraw.p; rows.row_w = e->row_w.p;
+        const SolveVecs sv = solve_vecs(e);
+        const Shard sh = e->shard();
+        const int64_t hc = e->held_count();
+        pdl_launch(e, k_scale_vec, blocks_for(static_cast<size_t>(hc)), kThreads, 0, sv, sh, hc, e->dbg_v.p, 1.0f, sv.ps, e->ctl.p, 0);
+        launch_operator(e, g, rv, rows, sv, sh, e->dbg_v.p, 0.0f, 0.0f, 0);
+        e->timer_level = timer_level;
+        e->launches = launches;
+        std::vector<float> qg(U), s(U);
+        CK(cudaMemcpyAsync(qg.data(), e->v_qg.p, U * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(s.data(), e->v_s.p, U * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemsetAsync(e->v_qg.p, 0, U * sizeof(float), st));      // k_op_partial cleared qgd
+        CK(cudaMemcpyAsync(e->ctl.p, &saved, sizeof(CgCtl), cudaMemcpyHostToDevice, st));
+        CK(cudaStreamSynchronize(st));
+        CK(cudaGetLastError());
+        for (size_t j = 0; j < U; ++j) q[j] = s[j] * qg[j];       // k_cg_update's q_j = s_j qg_j, without D^2
         return 0;
     });
 }

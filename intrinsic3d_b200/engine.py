@@ -28,7 +28,8 @@ EXPORTED_SYMBOLS = [
     "i3d_num_voxels", "i3d_clear_voxels_outside_thin_shell", "i3d_upsample_grid", "i3d_download_grid",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
-    "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step",
+    "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_normal_equations",
+    "i3d_debug_apply_operator",
 ]
 
 
@@ -267,6 +268,23 @@ class Engine:
         cs = np.zeros(U, np.float64)
         self._check(self.L.i3d_debug_get_step(self.h, _p(st, C.c_double), _p(fm, C.c_uint8), _p(cs, C.c_double)))
         return st, fm, cs
+
+    def debug_normal_equations(self):
+        """b = J'^T f, Jacobi scale s, jtj = s^2 colnorm^2 (float32 [U]) and the raw E_g camera sums cam_acc (float32 [33F + 43])."""
+        U = 2 * self.n + 6 * self.F + 9
+        b, s, jtj = np.empty(U, np.float32), np.empty(U, np.float32), np.empty(U, np.float32)
+        cam = np.empty(33 * self.F + 43, np.float32)
+        self._check(self.L.i3d_debug_get_normal_equations(self.h, _p(b, C.c_float), _p(s, C.c_float), _p(jtj, C.c_float), _p(cam, C.c_float)))
+        return dict(b=b, s=s, jtj=jtj, cam_acc=cam)
+
+    def debug_apply_operator(self, v):
+        """q = S (J^T W J) S v for the rows of the last iteration (float32 [U]), through the production operator kernels."""
+        U = 2 * self.n + 6 * self.F + 9
+        v = np.ascontiguousarray(v, np.float32)
+        assert v.shape == (U,)
+        q = np.empty(U, np.float32)
+        self._check(self.L.i3d_debug_apply_operator(self.h, _p(v, C.c_float), _p(q, C.c_float)))
+        return q
 
 
 def shard_range(n: int, rank: int, world: int, align: int = 512):

@@ -1,5 +1,5 @@
 """Round-2 GPU tests: parity on the configurations the numbers are quoted on (C2 whole, a C3 z-slab with all 200 frames),
-camera state across frame re-uploads (pyramid-level switches of Intrinsic3D::refine), run-to-run reproducibility."""
+camera state across frame re-uploads (pyramid-level switches of Intrinsic3D::refine), run-to-run bit-identity (small and full C3)."""
 import json
 import os
 
@@ -51,9 +51,20 @@ def test_camera_state_survives_frame_reupload(small_scene):
     assert accepted >= 2          # odd and even numbers of buffer swaps were both exercised
 
 
+def _lambda_ramp(p, it):
+    """computeVaryingLambda (cost.h:130-143) over 10 iterations, yml defaults"""
+    p.lambda_[1] = 80.0 - 70.0 / 9.0 * it
+    p.lambda_[2] = 120.0 - 110.0 / 9.0 * it
+
+
+def _info_bytes(info):
+    """the bytes of every I3DIterInfo field before the wall-clock timers (time_add, time_build, time_solve come last)"""
+    return bytes(info)[:type(info).time_add.offset]
+
+
 def test_run_to_run_reproducibility(small_scene):
-    """Two engines on identical inputs: float atomics make the accumulation order differ between runs; quantify the
-    difference after 3 iterations relative to the size of the accumulated update."""
+    """Two engines on identical inputs give bit-identical results: every float contribution of the iteration is summed in double,
+    where the totals are exact and so independent of the order of the atomics, and rounded to float once."""
     from intrinsic3d_b200.engine import Engine
     s = small_scene
     outs, infos = [], []
@@ -63,22 +74,53 @@ def test_run_to_run_reproducibility(small_scene):
         p = _params(s)
         ii = []
         for it in range(3):
-            p.lambda_[1] = 80.0 - 70.0 / 9.0 * it
-            p.lambda_[2] = 120.0 - 110.0 / 9.0 * it
+            _lambda_ramp(p, it)
             ii.append(e.gn_iteration(p))
         outs.append(e.download_state())
         infos.append(ii)
         e.close()
     moved = np.abs(outs[0]["sdf_refined"] - s["sdf_refined"]).max()
-    d_sdf = np.abs(outs[0]["sdf_refined"] - outs[1]["sdf_refined"]).max()
-    d_alb = np.abs(outs[0]["albedo"] - outs[1]["albedo"]).max()
-    d_pose = np.abs(outs[0]["poses"] - outs[1]["poses"]).max()
     cg = [[list(i.cg_iterations)[:i.lm_iterations] for i in ii] for ii in infos]
-    _note("reproducibility", dict(scene="small", iterations=3, max_abs_sdf_update=float(moved), run_to_run_max_abs_sdf=float(d_sdf),
-                                  run_to_run_rel_of_update=float(d_sdf / moved), run_to_run_max_abs_albedo=float(d_alb), run_to_run_max_abs_pose=float(d_pose),
-                                  cg_iterations=cg))
-    assert cg[0] == cg[1]
-    assert moved > 0 and d_sdf <= 1e-3 * moved
+    _note("reproducibility", dict(scene="small", iterations=3, max_abs_sdf_update=float(moved), cg_iterations=cg))
+    assert moved > 0
+    for k in ("sdf_refined", "albedo", "poses", "intr", "dist"):
+        assert outs[0][k].tobytes() == outs[1][k].tobytes(), k
+    for a, b in zip(*infos):
+        assert _info_bytes(a) == _info_bytes(b)
+
+
+def test_c3_run_to_run_bit_identical():
+    """The full C3 scene (2 M voxels, 200 frames; thousands of blocks add camera partials into the same double entries): two
+    engines in turn, three GN iterations of the lambda ramp, byte-equal state and iteration info, then byte-equal b, s, jtj,
+    cam_acc and one operator application."""
+    import torch
+    from intrinsic3d_b200.engine import Engine
+    from intrinsic3d_b200.scene import config_scene
+    s = config_scene("c3", device="cuda" if torch.cuda.is_available() else "cpu")
+    engines = [Engine(0), Engine(0)]
+    for e in engines:
+        e.load_scene(s)
+    p = _params(s)
+    infos = [[], []]
+    for it in range(3):
+        _lambda_ramp(p, it)
+        for i, e in enumerate(engines):
+            infos[i].append(e.gn_iteration(p))
+    for a, b in zip(*infos):
+        assert _info_bytes(a) == _info_bytes(b)
+    st = [e.download_state() for e in engines]
+    for k in st[0]:
+        assert st[0][k].tobytes() == st[1][k].tobytes(), k
+    ne = [e.debug_normal_equations() for e in engines]
+    for k in ne[0]:
+        assert ne[0][k].tobytes() == ne[1][k].tobytes(), k
+    U = 2 * engines[0].n + 6 * engines[0].F + 9
+    v = np.random.default_rng(3).standard_normal(U).astype(np.float32)
+    q = [e.debug_apply_operator(v) for e in engines]
+    assert q[0].tobytes() == q[1].tobytes()
+    n_active = int(infos[0][-1].num_active)
+    _note("c3_reproducibility", dict(iterations=3, num_active=n_active, blocks_of_256=-(-n_active // 256),
+                                     cg_iterations=[list(i.cg_iterations)[:i.lm_iterations] for i in infos[0]]))
 
 
 def test_parity_c2_whole():

@@ -2,7 +2,7 @@
   (1) against the float64 ORACLE driven through the same two-level schedule (src/refinement/intrinsic3d.cpp:206-295: convert -> initial
       recolouring -> per grid level {thin-shell pruning -> per pyramid level {lighting, GN iterations, recolouring} -> upsample}),
   (2) against the same schedule driven from Python through the C-ABI (same engine: isolates the C++ host code).
-A voxel on the pruning threshold can flip between two runs (float atomics in the engine, f32 Jacobian vs the oracle's f64), so the
+A voxel on the pruning threshold can fall on either side of it in the engine and the oracle (f32 Jacobian vs the oracle's f64), so the
 comparison is on counts (within 0.5 %) and, for the voxels both runs hold, on the distribution of the differences."""
 import ctypes as C
 import json
@@ -186,7 +186,6 @@ def test_cpp_refine_matches_oracle_schedule():
     r = _compare(ref, ref_state, out, out_state, s)
     print("test_refine_vs_oracle:", json.dumps(r))
     assert abs(r["voxels_out"] - r["voxels_ref"]) <= 0.005 * r["voxels_ref"] and r["common"] >= 0.995 * r["voxels_out"]
-    # the bounds leave a margin for float-atomic run-to-run differences
     assert r["sdf_update_max"] > 0 and r["sdf_err_rel_median"] <= 1e-4 and r["sdf_frac_within_1e3"] > 0.99 and r["sdf_frac_within_1e2"] > 0.999
     assert r["albedo_frac_within_1e3"] > 0.99 and r["color_frac_within_1"] > 0.99
     assert r["pose_update_max"] > 1e-4 and r["pose_err_max"] <= 1e-3 * r["pose_update_max"]
