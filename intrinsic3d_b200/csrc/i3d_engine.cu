@@ -141,7 +141,9 @@ struct I3DEngine
     Dev<float> Rt;
     Dev<FramePose> pose_ctx, pose_ctx_c;
     Dev<int32_t> obs_frame, row_frame;
-    Dev<float> obs_w, J, row_w;
+    Dev<float> obs_w;
+    Dev<float4> Jt;                  // E_g rows, layout in EgRows
+    Dev<float2> Jtail;
     Dev<double> row_res, row_wraw;
     Dev<float> ea_w;
     Dev<double> lap;
@@ -339,6 +341,14 @@ SolveVecs solve_vecs(I3DEngine* e)
     return sv;
 }
 
+EgRows eg_rows(I3DEngine* e)
+{
+    EgRows rows;
+    rows.n_active = e->n_active; rows.K = e->K; rows.stride = e->stride; rows.act = e->act.p; rows.Jt = e->Jt.p; rows.Jtail = e->Jtail.p;
+    rows.row_frame = e->row_frame.p; rows.row_res = e->row_res.p; rows.row_wraw = e->row_wraw.p;
+    return rows;
+}
+
 // brackets one kernel launch with two events from the pool; resolved by collect_kernel_times()
 // (an event record between two kernels makes the second one wait for the first one's completion the ordinary way: no programmatic
 // overlap across it.  `level` 0 = always timed: the two roofline kernels (k_eg_rows, k_eg_apply) and k_select_obs; level 1 = only when i3d_debug_set_kernel_timers(e, 1) asked for the per-kernel table.)
@@ -481,7 +491,7 @@ void exchange(I3DEngine* e, float* v0, float* v1, float* extra_f, int n_extra_f,
 
 size_t apply_smem_bytes(int F, int K)
 {
-    return static_cast<size_t>((6 * F + 9 + 15) & ~15) * sizeof(double) + static_cast<size_t>(K) * 6 * kThreads * sizeof(float);
+    return static_cast<size_t>((6 * F + 9 + 15) & ~15) * sizeof(double) + static_cast<size_t>(14 + 6 * K) * kThreads * sizeof(float);
 }
 
 size_t accum_smem_bytes(int F, int K)
@@ -640,17 +650,13 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
 
     // ------------------------------------------------------------------ k2 build
     Timer t_build(e, "build", 2);
-    e->J.ensure(static_cast<size_t>(I3D_EG_COLS) * S + 1);
-    e->row_frame.ensure(S + 1); e->row_res.ensure(S + 1); e->row_wraw.ensure(S + 1); e->row_w.ensure(S + 1);
+    e->Jt.ensure(EgRows::kTiles * S + 1); e->Jtail.ensure(S + 1);
+    e->row_frame.ensure(S + 1); e->row_res.ensure(S + 1); e->row_wraw.ensure(S + 1);
     e->ea_w.ensure(3 * static_cast<size_t>(n)); e->lap.ensure(n);
-    if (apply_smem_bytes(F, K) > 48 * 1024)
-    {
-        CK(cudaFuncSetAttribute(k_eg_apply<APPLY_CG>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(apply_smem_bytes(F, K))));
-        CK(cudaFuncSetAttribute(k_eg_apply<APPLY_MODEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(apply_smem_bytes(F, K))));
-    }
-    EgRows rows;
-    rows.n_active = n_active; rows.K = K; rows.stride = stride; rows.act = e->act.p; rows.J = e->J.p; rows.row_frame = e->row_frame.p;
-    rows.row_res = e->row_res.p; rows.row_wraw = e->row_wraw.p; rows.row_w = e->row_w.p;
+    // set unconditionally: the default limit is 48 KB minus the kernel's static shared memory, not 48 KB
+    CK(cudaFuncSetAttribute(k_eg_apply<APPLY_CG>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(apply_smem_bytes(F, K))));
+    CK(cudaFuncSetAttribute(k_eg_apply<APPLY_MODEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(apply_smem_bytes(F, K))));
+    const EgRows rows = eg_rows(e);
     CamView cv{e->cam, e->pose_ctx.p, F};
     if (n_active > 0)
     {
@@ -680,7 +686,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     if (multi) exchange(e, e->v_bg.p, e->v_cg.p, e->cam_acc.p, lay.size(), e->red_out.p, 2 * kSiteVals, 0);   // SITE_BUILD + SITE_REG are adjacent
     // NLSSolver::normalizeCostTermWeights (nls_solver.cpp:379-394) on the device
     pdl_launch(e, k_type_weights, 1, 32, 0, e->iter_dev.p, e->site(SITE_BUILD).out, e->site(SITE_REG).out, P, n, e->type_w.p);
-    if (S > 0) pdl_launch(e, k_row_weights, blocks_for(S), kThreads, 0, S, e->row_wraw.p, e->type_w.p, e->row_w.p);
+    if (S > 0) pdl_launch(e, k_row_weights, blocks_for(S), kThreads, 0, rows, e->type_w.p);
     SolveVecs sv = solve_vecs(e);
     pdl_launch(e, k_finish_problem, blocks_for(static_cast<size_t>((hc + 3) / 4)), kThreads, 0, g, rv, sv, sh, hc, e->type_w.p, e->cam_acc.p, P.fix_poses, P.fix_intrinsics,
                                                                               P.fix_distortion, e->site(SITE_FINISH), e->cam);
@@ -1528,8 +1534,25 @@ int i3d_debug_get_rows(I3DEngine* e, int32_t* voxel, int32_t* frame, double* res
         if (frame) CK(cudaMemcpyAsync(frame, e->row_frame.p, S * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         if (residual) CK(cudaMemcpyAsync(residual, e->row_res.p, S * sizeof(double), cudaMemcpyDeviceToHost, st));
         if (raw_weight) CK(cudaMemcpyAsync(raw_weight, e->row_wraw.p, S * sizeof(double), cudaMemcpyDeviceToHost, st));
-        if (jac_colmajor) CK(cudaMemcpyAsync(jac_colmajor, e->J.p, I3D_EG_COLS * S * sizeof(float), cudaMemcpyDeviceToHost, st));
+        std::vector<float4> jt(jac_colmajor ? EgRows::kTiles * S : 0);
+        std::vector<float2> jtail(jac_colmajor ? S : 0);
+        if (jac_colmajor)
+        {
+            CK(cudaMemcpyAsync(jt.data(), e->Jt.p, jt.size() * sizeof(float4), cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(jtail.data(), e->Jtail.p, jtail.size() * sizeof(float2), cudaMemcpyDeviceToHost, st));
+        }
         CK(cudaStreamSynchronize(st));
+        if (jac_colmajor)
+            for (size_t i = 0; i < S; ++i)
+            {
+                for (int c = 0; c < EgRows::kTiles; ++c)
+                {
+                    const float4 t = jt[c * S + i];
+                    jac_colmajor[(4 * c) * S + i] = t.x; jac_colmajor[(4 * c + 1) * S + i] = t.y;
+                    jac_colmajor[(4 * c + 2) * S + i] = t.z; jac_colmajor[(4 * c + 3) * S + i] = t.w;
+                }
+                jac_colmajor[28 * S + i] = jtail[i].x;
+            }
         // the padding slots [n_active, stride) of every k are never written by the kernels: report them as "no row"
         for (int k = 0; k < e->K; ++k)
             for (int a = e->n_active; a < e->stride; ++a)
@@ -1643,9 +1666,7 @@ int i3d_debug_apply_operator(I3DEngine* e, const float* v, float* q)
         RegView rv;
         rv.flags = e->flags.p; rv.ea_w = e->ea_w.p; rv.lap = e->lap.p;
         rv.use_er = P.use_er; rv.use_es = P.use_es; rv.use_ea = P.use_ea;
-        EgRows rows;
-        rows.n_active = e->n_active; rows.K = e->K; rows.stride = e->stride; rows.act = e->act.p; rows.J = e->J.p; rows.row_frame = e->row_frame.p;
-        rows.row_res = e->row_res.p; rows.row_wraw = e->row_wraw.p; rows.row_w = e->row_w.p;
+        const EgRows rows = eg_rows(e);
         const SolveVecs sv = solve_vecs(e);
         const Shard sh = e->shard();
         const int64_t hc = e->held_count();

@@ -8,9 +8,10 @@
  *   frames    lum, depth float[F][H][W]; camera double[6F+9] (poses | intrinsics | distortion)
  *   per GN iteration
  *             flags uint8[n]; act int32[n_a] (compacted active voxels, ascending)
- *             E_g row slots, k-major: slot = k*n_a + a
- *                 J float[29][K*n_a] raw rows (column-major => coalesced for thread-per-voxel access)
- *                 row_frame int32, row_res double (unweighted), row_wraw double, row_w float (final weight)
+ *             E_g row slots, k-major: slot = k*stride + a (stride = n_a rounded up to 64)
+ *                 Jt float4[7][K*stride] raw rows in 4-column tiles, Jtail float2[K*stride] (column 28, final weight)
+ *                 (one 16 B tile per thread and load => a warp's access is 512 contiguous bytes; see EgRows)
+ *                 row_frame int32, row_res double (unweighted), row_wraw double
  *   unknown-space vectors float[U], U = 2n + 6F + 9 : [sdf | albedo | poses | intrinsics | distortion]
  *
  * Reference functions replaced (libintrinsic3d/): see each kernel.
@@ -851,16 +852,45 @@ struct CamView
     int F;
 };
 
+// The raw J row of a slot is 7 tiles of 4 columns plus a tail that carries column 28 and the row's final weight, each array
+// indexed by slot: a warp's access to one tile is 32 x 16 B contiguous (one LDG.128 / STG.128 per tile and thread instead of
+// four scalar accesses), and a row is still 120 B.  The kernels go through load_row / store_row only.
 struct EgRows
 {
     int n_active, K;
-    int stride;            // slots per k (n_active rounded up to 64): slot = k*stride + a; keeps every column segment 256 B aligned for bulk copies
+    int stride;            // slots per k (n_active rounded up to 64): slot = k*stride + a; keeps every tile segment 1 KB aligned
     const int32_t* act;
-    float* J;              // [29][K*n_a]
-    int32_t* row_frame;    // [K*n_a] valid rows: frame, else -1
+    float4* Jt;            // [7][K*stride]: tile c = columns 4c .. 4c+3
+    float2* Jtail;         // [K*stride]: (column 28, final weight = raw weight * type weight)
+    int32_t* row_frame;    // [K*stride] valid rows: frame, else -1
     double* row_res;       // unweighted residual
     double* row_wraw;      // raw weight = obs.weight * sdfToWeight
-    float* row_w;          // final weight (raw * type weight)
+    static constexpr int kTiles = 7;
+    __host__ __device__ size_t slots() const { return static_cast<size_t>(K) * stride; }
+    // columns 0..28 of the row; the final weight is not written here (k_row_weights sets it once the type weight is known)
+    __device__ __forceinline__ void store_row(size_t slot, const float row[29]) const
+    {
+        const size_t S = slots();
+#pragma unroll
+        for (int c = 0; c < kTiles; ++c) Jt[c * S + slot] = make_float4(row[4 * c], row[4 * c + 1], row[4 * c + 2], row[4 * c + 3]);
+        Jtail[slot].x = row[28];
+    }
+    // columns 0..28 into jr, returns the final weight.  STREAM: evict-first loads (the row is read once per operator application
+    // and J is far larger than L2)
+    template <bool STREAM>
+    __device__ __forceinline__ float load_row(size_t slot, float jr[29]) const
+    {
+        const size_t S = slots();
+#pragma unroll
+        for (int c = 0; c < kTiles; ++c)
+        {
+            const float4 t = STREAM ? __ldcs(Jt + c * S + slot) : Jt[c * S + slot];
+            jr[4 * c] = t.x; jr[4 * c + 1] = t.y; jr[4 * c + 2] = t.z; jr[4 * c + 3] = t.w;
+        }
+        const float2 t = STREAM ? __ldcs(Jtail + slot) : Jtail[slot];
+        jr[28] = t.x;
+        return t.y;
+    }
 };
 
 __device__ __forceinline__ void make_cam_params(const CamView& cv, double pyr_scale, int W, int H, CamParams<double>* c)
@@ -916,8 +946,8 @@ struct CamAccLayout
 // profiles/r01c_final_k_eg_build.csv).  Per voxel, once: stencil gather, the four normals / shading values / iso-points
 // (voxel_geom_make, float64).  Per selected frame: rigid transform, projection with distortion, bicubic luminance
 // (float64 value, float32 gradient), then
-//   ROWS_BUILD: the 29-column row by the closed-form chain rule (float32) -> raw J row (column-major: every store of a
-//               warp is one full 128 B line), unweighted residual, raw weight
+//   ROWS_BUILD: the 29-column row by the closed-form chain rule (float32) -> raw J row (EgRows::store_row: 7 16 B tile stores
+//               + column 28), unweighted residual, raw weight
 //   ROWS_COST : sum of raw_weight * r^2 at an arbitrary state (rows fixed at creation; invalid -> 0 like the functor)
 // Neighbouring threads are neighbouring voxels of the compacted active list: their stencil gathers hit the same lines, they
 // mostly select the same frame in the same slot (k_select_obs orders slots by frame id), so the per-frame constants are
@@ -987,7 +1017,6 @@ k_eg_rows(GridView g, FrameView fr, CamView cv, EgRows rows, const int32_t* __re
         __syncthreads();          // the barrier object is initialised before anyone polls it
     }
     const int a = blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t S = static_cast<size_t>(rows.K) * rows.stride;
     double acc[1] = {0.0};
     // per-voxel state of the frame loop parked in shared memory (15 doubles + 40 floats per thread)
     const VoxelGeomView vg{s_vg + threadIdx.x, THREADS};
@@ -1055,9 +1084,7 @@ k_eg_rows(GridView g, FrameView fr, CamView cv, EgRows rows, const int32_t* __re
                         eg_frame_deriv(vd, fp, cf, sv, e, row);
                         rf = f;
                         wraw = static_cast<double>(obs_w[slot]) * wsdf;
-                        float* __restrict__ jc = rows.J + slot;
-#pragma unroll
-                        for (int m = 0; m < 29; ++m) jc[static_cast<size_t>(m) * S] = row[m];
+                        rows.store_row(slot, row);
                     }
                 }
                 else acc[0] += rows.row_wraw[slot] * res * res;
@@ -1093,7 +1120,6 @@ k_eg_accum(GridView g, EgRows rows, int F, double* __restrict__ bg, double* __re
     const int tid = threadIdx.x, lane = tid & 31;
     const int a = blockIdx.x * blockDim.x + tid;
     const bool in_range = a < rows.n_active;
-    const size_t S = static_cast<size_t>(rows.K) * rows.stride;
     double acc[3] = {0.0, 0.0, 0.0};
     float gsum[14], csum[14];
 #pragma unroll
@@ -1113,8 +1139,7 @@ k_eg_accum(GridView g, EgRows rows, int F, double* __restrict__ bg, double* __re
         if (f >= 0)
         {
             float row[29];
-#pragma unroll
-            for (int m = 0; m < 29; ++m) row[m] = rows.J[static_cast<size_t>(m) * S + slot];
+            rows.load_row<false>(slot, row);
             const double wraw = rows.row_wraw[slot], res = rows.row_res[slot];
             const float wf = static_cast<float>(wraw), wr = static_cast<float>(wraw * res);
             acc[0] += wraw; acc[1] += wraw * res * res; acc[2] += 1.0;
@@ -1225,12 +1250,12 @@ __global__ void k_acc_to_float(int64_t U, int ncam, const double* __restrict__ b
 }
 
 // final per-row weights once the type weight is known (NLSSolver::normalizeCostTermWeights, nls_solver.cpp:379-394)
-__global__ void k_row_weights(size_t S, const double* __restrict__ row_wraw, const double* __restrict__ type_w, float* __restrict__ row_w)
+__global__ void k_row_weights(EgRows rows, const double* __restrict__ type_w)
 {
     pdl_prologue();
     const size_t s = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
-    if (s >= S) return;
-    row_w[s] = static_cast<float>(row_wraw[s] * type_w[0]);
+    if (s >= rows.slots()) return;
+    rows.Jtail[s].y = static_cast<float>(rows.row_wraw[s] * type_w[0]);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -1541,9 +1566,25 @@ __global__ void k_cam_precond(SolveVecs sv, const float* __restrict__ cam_acc, c
 // ----------------------------------------------------------------------------------------------
 enum { APPLY_CG = 0, APPLY_MODEL = 1 };
 
+// unknown-space indices of the 14 voxel columns of voxel v's E_g rows: the sdf stencil in the reference's parameter order
+// (as gather_stencil), then the 4 albedo entries
+__device__ __forceinline__ void eg_voxel_unknowns(const GridView& g, int64_t v, uint32_t idx[14])
+{
+    const int64_t n = g.n;
+    const uint32_t xp = g.nbr[NB_XP * n + v], yp = g.nbr[NB_YP * n + v], zp = g.nbr[NB_ZP * n + v];
+    const uint32_t un = static_cast<uint32_t>(n);
+    idx[0] = static_cast<uint32_t>(v); idx[1] = yp; idx[2] = g.nbr[NB_Y2 * n + v]; idx[3] = g.nbr[NB_YZ * n + v]; idx[4] = zp; idx[5] = g.nbr[NB_Z2 * n + v];
+    idx[6] = xp; idx[7] = g.nbr[NB_XY * n + v]; idx[8] = g.nbr[NB_XZ * n + v]; idx[9] = g.nbr[NB_X2 * n + v];
+    idx[10] = un + idx[0]; idx[11] = un + xp; idx[12] = un + yp; idx[13] = un + zp;
+}
 
-// k5: the E_g part of the CGNR operator.  One thread per active voxel; streams the K raw J rows of the voxel once
-// (column-major J: every load of a warp is one full 128 B line).
+// k5: the E_g part of the CGNR operator.  One thread per active voxel; streams the K raw J rows of the voxel once, each as
+// 7 evict-first 16 B tile loads + one 8 B tail load (EgRows).
+// Occupancy: 80 registers, 3 blocks (24 warps) per SM, no spills.  The ps entries of the 14 voxel columns sit in shared memory
+// and the camera tail of ps is staged once per block, so neither is held in registers across the row loop; the unknown
+// indices are read again for the scatter.  Measured at C3 on an H100 SXM (400 W), 20-step runs: 0.381 ms per launch vs 0.394 ms for the
+// same tiles at 124 registers and 2 blocks per SM (the index re-read alone, at 2 blocks, cost 0.412); parking the indices in
+// shared memory as well (0.408), 128-thread blocks x 6 (0.427) and an L2 prefetch of the next row (0.380) did not help.
 //   u_k = J_k . ps          (ps = s o p, the Jacobi-scaled input)
 //   APPLY_CG   : qg[cols] += sum_k w_k u_k J_k ; partial p.q += w_k u_k^2
 //       voxel columns          : per-thread sums over the K rows, one global atomic per column per voxel
@@ -1560,25 +1601,27 @@ enum { APPLY_CG = 0, APPLY_MODEL = 1 };
 // run to run over three GN iterations (tests/test_gpu_round2.py::test_c3_run_to_run_bit_identical).
 // (A bulk-async / mbarrier staged variant was measured slower: the kernel is issue-bound, not latency-bound.)
 template <int MODE>
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kThreads, 3)
 k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __restrict__ ps, const CgCtl* __restrict__ ctl, int respect_done, ReduceSite site)
 {
     pdl_prologue();
-    extern __shared__ double s_dyn_d[];  // [6F + 9] camera accumulators (double) | [K][6][kThreads] parked pose contributions (float)
+    // [6F + 9] camera accumulators (double) | [14][kThreads] ps of the voxel columns | [K][6][kThreads] parked pose contributions
+    extern __shared__ double s_dyn_d[];
     if (respect_done && ctl->done) return;
     const int ncam = 6 * sv.F + 9;
     double* s_cam = s_dyn_d;
-    float* s_jp = reinterpret_cast<float*>(s_dyn_d + ((ncam + 15) & ~15));
+    float* s_pv = reinterpret_cast<float*>(s_dyn_d + ((ncam + 15) & ~15));
+    float* s_jp = s_pv + 14 * kThreads;
+    const int64_t n = g.n;
+    // the intrinsics / distortion entries of ps, the same for every row
+    __shared__ float s_pt[9];
+    if (threadIdx.x < 9) s_pt[threadIdx.x] = ps[2 * n + 6 * static_cast<int64_t>(sv.F) + threadIdx.x];
     if (MODE == APPLY_CG)
-    {
         for (int i = threadIdx.x; i < ncam; i += blockDim.x) s_cam[i] = 0.0;
-        __syncthreads();
-    }
+    __syncthreads();
     const int tid = threadIdx.x, lane = tid & 31;
     const int a = blockIdx.x * blockDim.x + tid;
     const bool in_range = a < rows.n_active;
-    const int64_t n = g.n;
-    const size_t S = static_cast<size_t>(rows.K) * rows.stride;
     double acc[1] = {0.0};
     int fk[I3D_MAX_OBS];
     bool any = false;
@@ -1588,12 +1631,11 @@ k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __res
         fk[k] = (in_range && k < rows.K) ? rows.row_frame[static_cast<size_t>(k) * rows.stride + a] : -1;
         any = any || (fk[k] >= 0);
     }
-    float pv[14], out[14], pt[9], tail[9];
+    float out[14], tail[9];
 #pragma unroll
-    for (int m = 0; m < 14; ++m) { pv[m] = 0.0f; out[m] = 0.0f; }
+    for (int m = 0; m < 14; ++m) out[m] = 0.0f;
 #pragma unroll
-    for (int m = 0; m < 9; ++m) { pt[m] = ps[2 * n + 6 * static_cast<int64_t>(sv.F) + m]; tail[m] = 0.0f; }
-    uint32_t idx[14];
+    for (int m = 0; m < 9; ++m) tail[m] = 0.0f;
     // E_r row of this voxel (rows exist exactly on the active voxels with a valid 6-ring, i.e. a subset of this kernel's voxels): its
     // value for the input vector, consumed by k_op_partial in gather form.  tr is zeroed once per GN iteration, so only these voxels
     // ever write it.  (Round 1 ran a separate kernel over all owned voxels for this: one launch per operator application.)
@@ -1610,14 +1652,10 @@ k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __res
     }
     if (any)
     {
-        const int64_t v = rows.act[a];
-        const uint32_t xp = g.nbr[NB_XP * n + v], yp = g.nbr[NB_YP * n + v], zp = g.nbr[NB_ZP * n + v];
-        const uint32_t un = static_cast<uint32_t>(n);
-        idx[0] = static_cast<uint32_t>(v); idx[1] = yp; idx[2] = g.nbr[NB_Y2 * n + v]; idx[3] = g.nbr[NB_YZ * n + v]; idx[4] = zp; idx[5] = g.nbr[NB_Z2 * n + v];
-        idx[6] = xp; idx[7] = g.nbr[NB_XY * n + v]; idx[8] = g.nbr[NB_XZ * n + v]; idx[9] = g.nbr[NB_X2 * n + v];
-        idx[10] = un + idx[0]; idx[11] = un + xp; idx[12] = un + yp; idx[13] = un + zp;
+        uint32_t idx[14];
+        eg_voxel_unknowns(g, rows.act[a], idx);
 #pragma unroll
-        for (int m = 0; m < 14; ++m) pv[m] = ps[idx[m]];
+        for (int m = 0; m < 14; ++m) s_pv[m * kThreads + tid] = ps[idx[m]];
     }
 #pragma unroll
     for (int k = 0; k < I3D_MAX_OBS; ++k)
@@ -1627,22 +1665,25 @@ k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __res
         if (f >= 0)
         {
             const size_t slot = static_cast<size_t>(k) * rows.stride + a;
-            const float* __restrict__ jc = rows.J + slot;
             float jr[29];
-#pragma unroll
-            for (int m = 0; m < 29; ++m) jr[m] = __ldcs(jc + static_cast<size_t>(m) * S);
-            const float w = rows.row_w[slot];
+            const float w = rows.load_row<true>(slot, jr);
             const float* pp = ps + 2 * n + 6 * static_cast<int64_t>(f);
             // four independent partial sums instead of one 29-long dependent FMA chain
             float u0 = 0.0f, u1 = 0.0f, u2 = 0.0f, u3 = 0.0f;
 #pragma unroll
-            for (int m = 0; m < 12; m += 4) { u0 += jr[m] * pv[m]; u1 += jr[m + 1] * pv[m + 1]; u2 += jr[m + 2] * pv[m + 2]; u3 += jr[m + 3] * pv[m + 3]; }
-            u0 += jr[12] * pv[12]; u1 += jr[13] * pv[13];
+            const float* pv = s_pv + tid;
+#pragma unroll
+            for (int m = 0; m < 12; m += 4)
+            {
+                u0 += jr[m] * pv[m * kThreads]; u1 += jr[m + 1] * pv[(m + 1) * kThreads];
+                u2 += jr[m + 2] * pv[(m + 2) * kThreads]; u3 += jr[m + 3] * pv[(m + 3) * kThreads];
+            }
+            u0 += jr[12] * pv[12 * kThreads]; u1 += jr[13] * pv[13 * kThreads];
 #pragma unroll
             for (int c = 0; c < 6; c += 2) { u2 += jr[14 + c] * pp[c]; u3 += jr[15 + c] * pp[c + 1]; }
 #pragma unroll
-            for (int m = 0; m < 8; m += 4) { u0 += jr[20 + m] * pt[m]; u1 += jr[21 + m] * pt[m + 1]; u2 += jr[22 + m] * pt[m + 2]; u3 += jr[23 + m] * pt[m + 3]; }
-            u0 += jr[28] * pt[8];
+            for (int m = 0; m < 8; m += 4) { u0 += jr[20 + m] * s_pt[m]; u1 += jr[21 + m] * s_pt[m + 1]; u2 += jr[22 + m] * s_pt[m + 2]; u3 += jr[23 + m] * s_pt[m + 3]; }
+            u0 += jr[28] * s_pt[8];
             const float u = (u0 + u1) + (u2 + u3);
             if (MODE == APPLY_CG)
             {
@@ -1702,6 +1743,8 @@ k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __res
         }
         if (any)
         {
+            uint32_t idx[14];      // read again (L1 hits) rather than held in 14 registers across the row loop
+            eg_voxel_unknowns(g, rows.act[a], idx);
 #pragma unroll
             for (int m = 0; m < 14; ++m) atomicAdd(sv.qgd + idx[m], static_cast<double>(out[m]));
         }
