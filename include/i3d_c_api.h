@@ -152,6 +152,33 @@ int         i3d_upsample_grid(I3DEngine* e, int64_t* num_voxels_out);
 int         i3d_download_grid(I3DEngine* e, int32_t* xyz, double* sdf0, double* sdf_refined, double* albedo,
                               float* weight, uint8_t* rgb, float* voxel_size);
 
+/* ---- RGB-D fusion: the producer of the grid (DESIGN.md §6h) ---- */
+uint64_t    i3d_sizeof_fusion_params(void);
+/* voxel_size 0.004, depth range [0.1, 4.0], integration_weight_sample 10, no clipping, discont_window_size 2,
+ * correct_sdf_iterations 10, default capacity. */
+void        i3d_default_fusion_params(I3DFusionParams* p);
+/* Starts an empty fusion volume (SparseVoxelGrid<Voxel>::create + setClipBounds, app_fusion.cpp:123-139).  The grid the engine
+ * currently holds is left alone until i3d_fusion_finish.  Fails for voxel_size <= 1e-5 (as create() returns nullptr) and on an
+ * engine with world > 1 (fusion runs on one GPU). */
+int         i3d_fusion_begin(I3DEngine* e, const I3DFusionParams* params);
+/* Fuses F frames in order, each as the loop body of AppFusion::fuseSDF (app_fusion.cpp:146-165): erodeDiscontinuities,
+ * computeNormals (only when integration_weight_sample > 0, the only case that reads them), then SparseVoxelGrid::integrate
+ * (computeFrustumBounds, alloc, per-voxel update; src/sparse_voxel_grid.cpp:300-395, 572-602).
+ *   depth    float metres [F][depth_cam.height][depth_cam.width], already range-thresholded as the sensor classes do
+ *   bgr      uint8 [F][color_cam.height][color_cam.width][3], interleaved B,G,R like i3d_upload_color_frames
+ *   pose_cam_to_world, pose_world_to_cam   float [F][12]: rotation row-major (9), translation (3)
+ * Divergence: integrate() inverts the camera-to-world Mat4f itself with Eigen's 4x4 float inverse (sparse_voxel_grid.cpp:305),
+ * which is not restated bit for bit; the caller supplies both directions instead (as i3d_recompute_colors takes pose_world_to_cam).
+ * Fails with a message when a voxel to allocate lies outside the +-2^20 coordinate range of the device hash. */
+int         i3d_fusion_integrate(I3DEngine* e, int32_t F, const I3DFusionCamera* depth_cam, const float* depth,
+                                 const I3DFusionCamera* color_cam, const uint8_t* bgr,
+                                 const float* pose_cam_to_world, const float* pose_world_to_cam);
+/* After the last frame (app_fusion.cpp:167-173): SDFAlgorithms::correctSDF (src/sdf/algorithms.cpp:260-337, run as Jacobi sweeps:
+ * DESIGN.md §6h), clearInvalidVoxels (:342-363), SDFAlgorithms::convert (sdf0 = sdf_refined = sdf, albedo 0.6), then the result
+ * becomes the engine's grid exactly as i3d_upload_grid of it would: voxel size, truncation, hash and neighbour tables.  Voxels are
+ * in canonical 8^3-brick-major order (sorted by floor(c/8) z,y,x then c mod 8 z,y,x).  Per-voxel SH, the shard and the last
+ * iteration are invalidated.  Ends the fusion.  An empty result leaves an empty grid (num_voxels_out = 0). */
+int         i3d_fusion_finish(I3DEngine* e, int64_t* num_voxels_out);
 /* ---- multi-GPU (one process per GPU; voxel ranges sharded, see DESIGN.md §multi-GPU) ---- */
 /* 128-byte NCCL unique id created on rank 0 and distributed by the host (e.g. torch.distributed). */
 int         i3d_comm_unique_id(uint8_t id128[128]);
@@ -199,6 +226,12 @@ int         i3d_debug_get_normal_equations(I3DEngine* e, float* b, float* s, flo
 /* q[U] = S (J^T W J) S v for the rows of the last iteration (all four terms, no D^2 term): the raw operator output of the production
  * k_eg_apply + k_op_partial pair times s, in float.  Leaves nothing behind that a following i3d_gn_iteration reads.  Single GPU only. */
 int         i3d_debug_apply_operator(I3DEngine* e, const float* v, float* q);
+/* Voxels of the fusion volume in progress (allocated ones included, integrated or not); 0 outside a fusion. */
+int64_t     i3d_debug_fusion_num_voxels(const I3DEngine* e);
+/* The fusion volume in progress in canonical order (see i3d_fusion_finish): xyz[3n], sdf[n] (Voxel::sdf, float), weight[n],
+ * rgb[3n] (r,g,b).  Any pointer may be NULL.  Fusion stage timings: i3d_phase_ms("fusion_prep" | "fusion_alloc" |
+ * "fusion_integrate" | "fusion_correct" | "fusion_finish"); i3d_phase_count("fusion_growths" | "fusion_sweeps"). */
+int         i3d_debug_get_fusion_volume(I3DEngine* e, int32_t* xyz, float* sdf, float* weight, uint8_t* rgb);
 
 #ifdef __cplusplus
 }

@@ -146,6 +146,27 @@ typedef struct I3DLightingInfo
     double  time_accumulate, time_solve, time_interpolate;   /* seconds (device time) */
 } I3DLightingInfo;
 
+/* ---- RGB-D fusion (AppFusion::fuseSDF, apps/src/app_fusion.cpp:107-200) ---- */
+/* SparseVoxelGrid<Voxel>::create(voxel_size, depth_min, depth_max) (src/sparse_voxel_grid.cpp:42-64) plus the fusion config
+ * (data/fusion.yml).  Truncation is 5 * voxel_size, as the reference's constructor sets it. */
+typedef struct I3DFusionParams
+{
+    float   voxel_size;                   /* metres (fusion.yml: 0.004); must be > 1e-5 */
+    float   depth_min, depth_max;         /* Sensor::depthMin / depthMax: frustum bounds and the depth weight */
+    float   integration_weight_sample;    /* 10, the constant of SparseVoxelGrid's constructor; 0 = unit weights */
+    float   clip_bounds[6];               /* x0,x1,y0,y1,z0,z1 in metres; all zero = off (the reference's norm() > 0 test) */
+    int32_t discont_window_size;          /* erodeDiscontinuities window (fusion.yml: 2); 0 = no erosion */
+    int32_t correct_sdf_iterations;       /* correctSDF sweeps at most (10) */
+    int64_t initial_capacity;             /* hash slots to start with, 0 = default.  Only useful to force table growth in tests */
+} I3DFusionParams;
+
+/* A pinhole camera as Camera::project2 / unproject2 use it (src/camera.cpp:157-199): no distortion. */
+typedef struct I3DFusionCamera
+{
+    int32_t width, height;
+    float   fx, fy, cx, cy;
+} I3DFusionCamera;
+
 #ifdef __cplusplus
 }
 #endif

@@ -64,7 +64,7 @@ public:
     T& voxel(const Vec3i& p) { return nodes_[index_.find(p)->second].second; }
     const T& voxel(const Vec3i& p) const { return nodes_[index_.find(p)->second].second; }
     T& voxel(int x, int y, int z) { return voxel(Vec3i{x, y, z}); }
-    // insertion (the reference fills the grid by TSDF fusion / file load, both out of scope here)
+    // insertion (the reference fills the grid by TSDF fusion / file load; fusion runs on the device, i3d_fusion_* in i3d_c_api.h)
     T& insert(const Vec3i& p, const T& v = T())
     {
         auto it = index_.find(p);

@@ -30,6 +30,9 @@
 #include "i3d_lighting.cuh"
 #include "i3d_recolor.cuh"
 #include "i3d_gridops.cuh"
+#include "i3d_fusion.cuh"
+
+#include <cub/device/device_radix_sort.cuh>
 
 using namespace i3d;
 
@@ -187,6 +190,16 @@ struct I3DEngine
     Dev<uint8_t> sh_has;
     int sv_S = 0;
     double* sv_x = nullptr;            // [S][9] subvolume SH of the last estimate (inside sv_work)
+    // RGB-D fusion in progress (i3d_fusion.cuh): own hash table and Voxel arrays, one entry per hash slot
+    bool fu_active = false;
+    I3DFusionParams fu_p{};
+    uint64_t fu_cap = 0;
+    int64_t fu_n = 0;
+    Dev<unsigned long long> fu_keys; Dev<unsigned> fu_vals;
+    Dev<int32_t> fu_x, fu_y, fu_z; Dev<float> fu_sdf, fu_w, fu_sdf2, fu_w2; Dev<uchar4> fu_rgb;
+    Dev<int> fu_ctl;                   // [0] allocated voxels, [1] alloc status, [2] correctSDF "changed", [3] valid voxels
+    Dev<float> fu_depth_in, fu_depth, fu_nrm; Dev<uint8_t> fu_bgr;
+    Dev<unsigned long long> fu_sk, fu_sk2; Dev<int32_t> fu_si, fu_si2; Dev<uint8_t> fu_cub;
     // shard (multi-GPU)
     int64_t shard_begin = 0, shard_end = -1;
     int rank = 0, world = 1;
@@ -298,6 +311,128 @@ int install_grid(I3DEngine* e, int64_t m, Dev<int32_t>& x, Dev<int32_t>& y, Dev<
     e->have_sh = false; e->have_iter = false; e->shard_ready = false; e->sv_S = 0; e->sv_x = nullptr;
     if (e->world > 1) { e->shard_begin = 0; e->shard_end = -1; }
     return rebuild_topology(e);
+}
+
+// ---- RGB-D fusion helpers ---------------------------------------------------------------------
+FuseTable fuse_table(I3DEngine* e)
+{
+    FuseTable t;
+    t.keys = e->fu_keys.p; t.vals = e->fu_vals.p; t.mask = e->fu_cap - 1; t.count = e->fu_ctl.p; t.status = e->fu_ctl.p + 1;
+    t.limit = static_cast<int>(e->fu_cap / 2);           // load factor 0.5
+    return t;
+}
+FuseVolume fuse_volume(I3DEngine* e) { return FuseVolume{e->fu_x.p, e->fu_y.p, e->fu_z.p, e->fu_sdf.p, e->fu_w.p, e->fu_rgb.p}; }
+
+FuseConst fuse_const(const I3DFusionParams& P)
+{
+    FuseConst c;
+    c.voxel_size = P.voxel_size; c.inv_voxel_size = 1.0f / P.voxel_size;
+    c.truncation = P.voxel_size * 5.0f; c.ray_step = P.voxel_size * 0.25f;      // sparse_voxel_grid.cpp:48, :403
+    c.depth_min = P.depth_min; c.depth_max = P.depth_max; c.weight_sample = P.integration_weight_sample;
+    float sq = 0.0f;
+    for (int k = 0; k < 6; ++k) { c.clip[k] = P.clip_bounds[k]; sq += P.clip_bounds[k] * P.clip_bounds[k]; }
+    c.use_clip = sq > 0.0f ? 1 : 0;                      // clip_bounds.norm() > 0 (app_fusion.cpp:138)
+    return c;
+}
+
+// (int) cast of a float, saturating where the C++ cast is undefined (same values as __float2int_rz on the device)
+int fuse_f2i_host(float v)
+{
+    if (!(v == v)) return 0;
+    if (v >= 2147483648.0f) return INT_MAX;
+    if (v < -2147483648.0f) return INT_MIN;
+    return static_cast<int>(v);
+}
+
+// SparseVoxelGrid::computeFrustumBounds (sparse_voxel_grid.cpp:572-602) with math::computeFrustumPoints (src/math.cpp:131-148).
+// floor / ceil act on the WORLD point in metres before worldToVoxel, so the bounds are whole-metre aligned.
+void fuse_frustum_bounds(const I3DFusionCamera& cam, float dmin, float dmax, float vs, const float R[9], const float t[3], int b[6])
+{
+    const float inv = 1.0f / vs;
+    const int px[4] = {0, cam.width - 1, cam.width - 1, 0}, py[4] = {0, 0, cam.height - 1, cam.height - 1};
+    b[0] = b[2] = b[4] = INT_MAX; b[1] = b[3] = b[5] = INT_MIN;
+    for (int i = 0; i < 8; ++i)
+    {
+        const float d = i < 4 ? dmin : dmax;
+        float c[3] = {0.0f, 0.0f, 0.0f};
+        if (d != 0.0f)                                   // Camera::unproject2 returns zero for depth 0
+        {
+            const float x = (static_cast<float>(px[i & 3]) - cam.cx) / cam.fx, y = (static_cast<float>(py[i & 3]) - cam.cy) / cam.fy;
+            c[0] = d * x; c[1] = d * y; c[2] = d;
+        }
+        for (int k = 0; k < 3; ++k)
+        {
+            float p = R[3 * k] * c[0];
+            p = p + R[3 * k + 1] * c[1];
+            p = p + R[3 * k + 2] * c[2];
+            p = p + t[k];
+            const int pl = fuse_f2i_host(static_cast<float>(fuse_f2i_host(std::floor(p))) * inv + 0.5f);
+            const int pu = fuse_f2i_host(static_cast<float>(fuse_f2i_host(std::ceil(p))) * inv + 0.5f);
+            b[2 * k] = std::min(b[2 * k], std::min(pl, pu));
+            b[2 * k + 1] = std::max(b[2 * k + 1], std::max(pl, pu));
+        }
+    }
+}
+
+void fuse_reset_table(I3DEngine* e, uint64_t cap)
+{
+    cudaStream_t st = e->stream;
+    e->fu_keys.ensure(cap); e->fu_vals.ensure(cap); e->fu_ctl.ensure(4);
+    e->fu_x.ensure(cap); e->fu_y.ensure(cap); e->fu_z.ensure(cap); e->fu_sdf.ensure(cap); e->fu_w.ensure(cap); e->fu_rgb.ensure(cap);
+    e->fu_cap = cap;
+    CK(cudaMemsetAsync(e->fu_keys.p, 0xFF, cap * sizeof(unsigned long long), st));
+    CK(cudaMemsetAsync(e->fu_vals.p, 0, cap * sizeof(unsigned), st));
+    CK(cudaMemsetAsync(e->fu_ctl.p, 0, 4 * sizeof(int), st));
+    CK(cudaStreamSynchronize(st));
+}
+
+template <class T>
+void fuse_grow_copy(I3DEngine* e, Dev<T>& a, size_t cap, size_t keep)
+{
+    Dev<T> b;
+    b.ensure(cap);
+    if (keep) CK(cudaMemcpyAsync(b.p, a.p, keep * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    a.swap(b);
+}
+
+// new table of `cap` slots: every claimed slot (key, voxel index, block bit) is re-inserted; the volume keeps its indices
+void fuse_grow_table(I3DEngine* e, uint64_t cap)
+{
+    cudaStream_t st = e->stream;
+    const size_t keep = static_cast<size_t>(e->fu_n);
+    Dev<unsigned long long> nk; Dev<unsigned> nv;
+    nk.ensure(cap); nv.ensure(cap);
+    CK(cudaMemsetAsync(nk.p, 0xFF, cap * sizeof(unsigned long long), st));
+    CK(cudaMemsetAsync(nv.p, 0, cap * sizeof(unsigned), st));
+    k_fuse_rehash<<<blocks_for(e->fu_cap), kThreads, 0, st>>>(e->fu_cap, e->fu_keys.p, e->fu_vals.p, nk.p, nv.p, cap - 1);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
+    e->fu_keys.swap(nk); e->fu_vals.swap(nv);
+    fuse_grow_copy(e, e->fu_x, cap, keep); fuse_grow_copy(e, e->fu_y, cap, keep); fuse_grow_copy(e, e->fu_z, cap, keep);
+    fuse_grow_copy(e, e->fu_sdf, cap, keep); fuse_grow_copy(e, e->fu_w, cap, keep); fuse_grow_copy(e, e->fu_rgb, cap, keep);
+    e->fu_cap = cap;
+}
+
+// sorts the fusion volume into canonical order: e->fu_si[0..) = volume indices.  valid_only: voxels with weight <= 0 sort last and
+// are not counted.  Returns the number of voxels in the order (valid ones only when valid_only).
+int fuse_sort(I3DEngine* e, bool valid_only)
+{
+    cudaStream_t st = e->stream;
+    const int n = static_cast<int>(e->fu_n);
+    e->fu_sk.ensure(n); e->fu_sk2.ensure(n); e->fu_si.ensure(n); e->fu_si2.ensure(n);
+    CK(cudaMemsetAsync(e->fu_ctl.p + 3, 0, sizeof(int), st));
+    k_fuse_sort_keys<<<blocks_for(n), kThreads, 0, st>>>(n, e->fu_x.p, e->fu_y.p, e->fu_z.p, e->fu_w.p, valid_only ? 1 : 0, e->fu_sk.p, e->fu_si.p, e->fu_ctl.p + 3);
+    size_t bytes = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, e->fu_sk.p, e->fu_sk2.p, e->fu_si.p, e->fu_si2.p, n, 0, 64, st));
+    e->fu_cub.ensure(bytes);
+    CK(cub::DeviceRadixSort::SortPairs(e->fu_cub.p, bytes, e->fu_sk.p, e->fu_sk2.p, e->fu_si.p, e->fu_si2.p, n, 0, 64, st));
+    e->fu_si.swap(e->fu_si2);                            // sorted indices now in fu_si
+    int m = n;
+    if (valid_only) CK(cudaMemcpyAsync(&m, e->fu_ctl.p + 3, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
+    return m;
 }
 
 void ensure_reduction_scratch(I3DEngine* e)
@@ -1412,6 +1547,166 @@ int i3d_download_grid(I3DEngine* e, int32_t* xyz, double* sdf0, double* sdf_refi
     });
 }
 
+// ---- RGB-D fusion (i3d_fusion.cuh) ------------------------------------------------------------
+uint64_t i3d_sizeof_fusion_params(void) { return sizeof(I3DFusionParams); }
+
+void i3d_default_fusion_params(I3DFusionParams* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    p->voxel_size = 0.004f; p->depth_min = 0.1f; p->depth_max = 4.0f;
+    p->integration_weight_sample = 10.0f;
+    p->discont_window_size = 2; p->correct_sdf_iterations = 10;
+}
+
+int i3d_fusion_begin(I3DEngine* e, const I3DFusionParams* params)
+{
+    if (!e || !params) return 1;
+    e->fu_active = false;
+    if (e->world > 1) return fail(e, "i3d_fusion_begin: fusion runs on one GPU (world = %d)", e->world);
+    if (!(params->voxel_size > 0.00001f)) return fail(e, "i3d_fusion_begin: voxel_size %g must be > 1e-5 (SparseVoxelGrid::create)", params->voxel_size);
+    if (params->correct_sdf_iterations < 0 || params->discont_window_size < 0 || params->initial_capacity < 0)
+        return fail(e, "i3d_fusion_begin: negative correct_sdf_iterations, discont_window_size or initial_capacity");
+    return guarded(e, [&]() {
+        e->fu_p = *params;
+        uint64_t cap = params->initial_capacity > 0 ? 64 : (1ull << 22);
+        while (cap < static_cast<uint64_t>(params->initial_capacity)) cap <<= 1;
+        fuse_reset_table(e, cap);
+        e->fu_n = 0;
+        for (const char* nm : {"fusion_prep", "fusion_alloc", "fusion_integrate", "fusion_correct", "fusion_finish", "fusion_growths", "fusion_sweeps"})
+            e->phases.erase(nm);
+        e->fu_active = true;
+        return 0;
+    });
+}
+
+int i3d_fusion_integrate(I3DEngine* e, int32_t F, const I3DFusionCamera* depth_cam, const float* depth, const I3DFusionCamera* color_cam,
+                         const uint8_t* bgr, const float* pose_cam_to_world, const float* pose_world_to_cam)
+{
+    if (!e) return 1;
+    if (!e->fu_active) return fail(e, "i3d_fusion_integrate: no fusion in progress (call i3d_fusion_begin first)");
+    if (F < 0 || !depth_cam || !color_cam || (F > 0 && (!depth || !bgr || !pose_cam_to_world || !pose_world_to_cam)))
+        return fail(e, "i3d_fusion_integrate: bad arguments");
+    if (depth_cam->width <= 0 || depth_cam->height <= 0 || color_cam->width <= 0 || color_cam->height <= 0)
+        return fail(e, "i3d_fusion_integrate: bad camera dimensions");
+    const int rc = guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const I3DFusionParams& P = e->fu_p;
+        const size_t dimg = static_cast<size_t>(depth_cam->width) * depth_cam->height;
+        const size_t cimg = static_cast<size_t>(color_cam->width) * color_cam->height * 3;
+        e->fu_depth_in.ensure(dimg * F); e->fu_depth.ensure(dimg); e->fu_bgr.ensure(cimg * F);
+        const bool want_normals = P.integration_weight_sample > 0.0f;
+        if (want_normals) e->fu_nrm.ensure(3 * dimg);
+        CK(cudaMemcpyAsync(e->fu_depth_in.p, depth, dimg * F * sizeof(float), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(e->fu_bgr.p, bgr, cimg * F, cudaMemcpyHostToDevice, st));
+        const FuseCam dc{depth_cam->width, depth_cam->height, depth_cam->fx, depth_cam->fy, depth_cam->cx, depth_cam->cy};
+        const FuseCam cc{color_cam->width, color_cam->height, color_cam->fx, color_cam->fy, color_cam->cx, color_cam->cy};
+        const FuseConst c = fuse_const(P);
+        for (int f = 0; f < F; ++f)
+        {
+            FuseFrame fr;
+            std::memcpy(fr.R_cw, pose_cam_to_world + 12 * f, 9 * sizeof(float)); std::memcpy(fr.t_cw, pose_cam_to_world + 12 * f + 9, 3 * sizeof(float));
+            std::memcpy(fr.R_wc, pose_world_to_cam + 12 * f, 9 * sizeof(float)); std::memcpy(fr.t_wc, pose_world_to_cam + 12 * f + 9, 3 * sizeof(float));
+            fuse_frustum_bounds(*depth_cam, P.depth_min, P.depth_max, P.voxel_size, fr.R_cw, fr.t_cw, fr.bounds);
+            {
+                Timer t(e, "fusion_prep", 0);
+                k_fuse_erode<<<blocks_for(dimg), kThreads, 0, st>>>(dc.W, dc.H, P.discont_window_size, e->fu_depth_in.p + dimg * f, e->fu_depth.p);
+                if (want_normals) k_fuse_normals<<<blocks_for(dimg), kThreads, 0, st>>>(dc, e->fu_depth.p, e->fu_nrm.p);
+            }
+            int ctl[2] = {0, 0};
+            for (int attempt = 0;; ++attempt)
+            {
+                {
+                    Timer t(e, "fusion_alloc", 0);
+                    CK(cudaMemsetAsync(e->fu_ctl.p + 1, 0, sizeof(int), st));
+                    k_fuse_alloc<<<blocks_for(dimg), kThreads, 0, st>>>(dc, fr, c, e->fu_depth.p, fuse_table(e), fuse_volume(e), attempt == 0 ? 1 : 0);
+                    CK(cudaMemcpyAsync(ctl, e->fu_ctl.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+                }
+                collect_kernel_times(e);         // synchronises: ctl is on the host
+                CK(cudaGetLastError());
+                e->fu_n = ctl[0];
+                if (ctl[1] & 2)
+                    return fail(e, "i3d_fusion_integrate: frame %d allocates voxels outside the +-2^20 coordinate range of the device hash "
+                                "(voxel size %g); the fusion is ended", f, static_cast<double>(P.voxel_size));
+                if (!(ctl[1] & 1)) break;
+                // the table is too full: grow it, then run this frame's allocation again (the voxel set is a union: re-inserting is harmless)
+                uint64_t cap = e->fu_cap * 2;
+                while (static_cast<uint64_t>(e->fu_n) * 4 > cap) cap <<= 1;
+                if (cap > (1ull << 31)) return fail(e, "i3d_fusion_integrate: more than 2^30 allocated voxels; the fusion is ended");
+                fuse_grow_table(e, cap);
+                e->phases["fusion_growths"].count += 1;
+            }
+            {
+                Timer t(e, "fusion_integrate", 0);
+                if (e->fu_n > 0)
+                    k_fuse_integrate<<<blocks_for(static_cast<size_t>(e->fu_n)), kThreads, 0, st>>>(e->fu_n, dc, cc, fr, c, e->fu_depth.p,
+                                                                                                    want_normals ? e->fu_nrm.p : nullptr,
+                                                                                                    e->fu_bgr.p + cimg * f, fuse_volume(e));
+            }
+        }
+        collect_kernel_times(e);
+        CK(cudaGetLastError());
+        return 0;
+    });
+    if (rc != 0) e->fu_active = false;
+    return rc;
+}
+
+int i3d_fusion_finish(I3DEngine* e, int64_t* num_voxels_out)
+{
+    if (!e) return 1;
+    if (!e->fu_active) return fail(e, "i3d_fusion_finish: no fusion in progress (call i3d_fusion_begin first)");
+    e->fu_active = false;
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const int64_t n = e->fu_n;
+        if (n > 0)
+        {
+            Timer t(e, "fusion_correct", 0);
+            e->fu_sdf2.ensure(e->fu_sdf.cap); e->fu_w2.ensure(e->fu_w.cap);
+            for (int it = 0; it < e->fu_p.correct_sdf_iterations; ++it)
+            {
+                int changed = 0;
+                CK(cudaMemsetAsync(e->fu_ctl.p + 2, 0, sizeof(int), st));
+                k_fuse_correct<<<blocks_for(static_cast<size_t>(n)), kThreads, 0, st>>>(n, e->fu_p.voxel_size, e->fu_keys.p, e->fu_vals.p, e->fu_cap - 1,
+                                                                                      e->fu_x.p, e->fu_y.p, e->fu_z.p, e->fu_sdf.p, e->fu_w.p,
+                                                                                      e->fu_sdf2.p, e->fu_w2.p, e->fu_ctl.p + 2);
+                e->fu_sdf.swap(e->fu_sdf2); e->fu_w.swap(e->fu_w2);
+                CK(cudaMemcpyAsync(&changed, e->fu_ctl.p + 2, sizeof(int), cudaMemcpyDeviceToHost, st));
+                CK(cudaStreamSynchronize(st));
+                e->phases["fusion_sweeps"].count += 1;
+                if (!changed) break;
+            }
+        }
+        int m = 0;
+        {
+            Timer t(e, "fusion_finish", 0);
+            if (n > 0) m = fuse_sort(e, true);
+            if (m > 0)
+            {
+                Dev<int32_t>&nx = e->sp_x, &ny = e->sp_y, &nz = e->sp_z; Dev<double>&nsdf0 = e->sp_sdf0, &nsdf = e->sp_sdf, &nalb = e->sp_alb; Dev<float>& nw = e->sp_w; Dev<uchar4>& nrgb = e->sp_rgb;
+                nx.ensure(std::max<size_t>(m, e->x.cap)); ny.ensure(std::max<size_t>(m, e->y.cap)); nz.ensure(std::max<size_t>(m, e->z.cap));
+                nsdf0.ensure(std::max<size_t>(m, e->sdf0.cap)); nsdf.ensure(std::max<size_t>(m, e->sdfA.cap)); nalb.ensure(std::max<size_t>(m, e->albA.cap));
+                nw.ensure(std::max<size_t>(m, e->weight.cap)); nrgb.ensure(std::max<size_t>(m, e->rgb.cap));
+                VoxelArrays out{nx.p, ny.p, nz.p, nsdf0.p, nsdf.p, nalb.p, nw.p, nrgb.p};
+                k_fuse_convert<<<blocks_for(static_cast<size_t>(m)), kThreads, 0, st>>>(m, e->fu_si.p, fuse_volume(e), out);
+                CK(cudaStreamSynchronize(st));
+                CK(cudaGetLastError());
+                e->voxel_size = e->fu_p.voxel_size; e->truncation = e->fu_p.voxel_size * 5.0f;
+                if (install_grid(e, m, nx, ny, nz, nsdf0, nsdf, nalb, nw, nrgb)) return fail(e, "i3d_fusion_finish: internal error (duplicate voxels)");
+            }
+            else
+            {
+                // clearInvalidVoxels left nothing: an empty grid, as after a pruning that removes everything
+                e->n = 0; e->have_sh = false; e->have_iter = false; e->shard_ready = false; e->sv_S = 0; e->sv_x = nullptr;
+            }
+        }
+        collect_kernel_times(e);
+        e->fu_n = 0;
+        if (num_voxels_out) *num_voxels_out = m;
+        return 0;
+    });
+}
+
 int i3d_comm_unique_id(uint8_t id128[128])
 {
     std::string err;
@@ -1682,6 +1977,30 @@ int i3d_debug_apply_operator(I3DEngine* e, const float* v, float* q)
         CK(cudaStreamSynchronize(st));
         CK(cudaGetLastError());
         for (size_t j = 0; j < U; ++j) q[j] = s[j] * qg[j];       // k_cg_update's q_j = s_j qg_j, without D^2
+        return 0;
+    });
+}
+
+int64_t i3d_debug_fusion_num_voxels(const I3DEngine* e) { return (e && e->fu_active) ? e->fu_n : 0; }
+
+int i3d_debug_get_fusion_volume(I3DEngine* e, int32_t* xyz, float* sdf, float* weight, uint8_t* rgb)
+{
+    if (!e || !e->fu_active) return fail(e, "i3d_debug_get_fusion_volume: no fusion in progress");
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const int64_t n = e->fu_n;
+        if (n <= 0) return 0;
+        fuse_sort(e, false);
+        const size_t un = static_cast<size_t>(n);
+        Dev<int32_t> dxyz; Dev<float> dsdf, dw; Dev<uint8_t> drgb;
+        dxyz.ensure(3 * un); dsdf.ensure(un); dw.ensure(un); drgb.ensure(3 * un);
+        k_fuse_gather<<<blocks_for(un), kThreads, 0, st>>>(n, e->fu_si.p, fuse_volume(e), dxyz.p, dsdf.p, dw.p, drgb.p);
+        if (xyz) CK(cudaMemcpyAsync(xyz, dxyz.p, 3 * un * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        if (sdf) CK(cudaMemcpyAsync(sdf, dsdf.p, un * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (weight) CK(cudaMemcpyAsync(weight, dw.p, un * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (rgb) CK(cudaMemcpyAsync(rgb, drgb.p, 3 * un, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        CK(cudaGetLastError());
         return 0;
     });
 }

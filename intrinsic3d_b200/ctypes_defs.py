@@ -160,3 +160,27 @@ class I3DLightingInfo(C.Structure, _Dictable):
         ("time_solve", C.c_double),
         ("time_interpolate", C.c_double),
     ]
+
+
+class I3DFusionParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("voxel_size", C.c_float),
+        ("depth_min", C.c_float),
+        ("depth_max", C.c_float),
+        ("integration_weight_sample", C.c_float),
+        ("clip_bounds", C.c_float * 6),
+        ("discont_window_size", C.c_int32),
+        ("correct_sdf_iterations", C.c_int32),
+        ("initial_capacity", C.c_int64),
+    ]
+
+
+class I3DFusionCamera(C.Structure, _Dictable):
+    _fields_ = [
+        ("width", C.c_int32),
+        ("height", C.c_int32),
+        ("fx", C.c_float),
+        ("fy", C.c_float),
+        ("cx", C.c_float),
+        ("cy", C.c_float),
+    ]

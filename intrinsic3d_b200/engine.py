@@ -11,7 +11,7 @@ import os
 
 import numpy as np
 
-from .ctypes_defs import I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DParams
+from .ctypes_defs import I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DParams
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("I3D_LIB", os.path.join(_HERE, "libi3d_b200.so"))   # I3D_LIB: A/B builds of the same library
@@ -26,10 +26,11 @@ EXPORTED_SYMBOLS = [
     "i3d_lighting_num_subvolumes", "i3d_download_lighting", "i3d_download_voxel_sh",
     "i3d_upload_color_frames", "i3d_recompute_colors", "i3d_download_colors",
     "i3d_num_voxels", "i3d_clear_voxels_outside_thin_shell", "i3d_upsample_grid", "i3d_download_grid",
+    "i3d_sizeof_fusion_params", "i3d_default_fusion_params", "i3d_fusion_begin", "i3d_fusion_integrate", "i3d_fusion_finish",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
     "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_normal_equations",
-    "i3d_debug_apply_operator",
+    "i3d_debug_apply_operator", "i3d_debug_fusion_num_voxels", "i3d_debug_get_fusion_volume",
 ]
 
 
@@ -59,10 +60,15 @@ def load_library():
     L.i3d_lighting_num_subvolumes.argtypes = [C.c_void_p]
     L.i3d_num_voxels.restype = C.c_int64
     L.i3d_num_voxels.argtypes = [C.c_void_p]
+    L.i3d_sizeof_fusion_params.restype = C.c_uint64
+    L.i3d_debug_fusion_num_voxels.restype = C.c_int64
+    L.i3d_debug_fusion_num_voxels.argtypes = [C.c_void_p]
     if L.i3d_sizeof_params() != C.sizeof(I3DParams) or L.i3d_sizeof_iter_info() != C.sizeof(I3DIterInfo):
         raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so")
     if L.i3d_sizeof_lighting_params() != C.sizeof(I3DLightingParams) or L.i3d_sizeof_lighting_info() != C.sizeof(I3DLightingInfo):
         raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (lighting structs)")
+    if L.i3d_sizeof_fusion_params() != C.sizeof(I3DFusionParams):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (fusion params)")
     _LIB = L
     return L
 
@@ -81,6 +87,18 @@ def default_lighting_params() -> I3DLightingParams:
     p = I3DLightingParams()
     load_library().i3d_default_lighting_params(C.byref(p))
     return p
+
+
+def default_fusion_params() -> I3DFusionParams:
+    p = I3DFusionParams()
+    load_library().i3d_default_fusion_params(C.byref(p))
+    return p
+
+
+def fusion_camera(cam) -> I3DFusionCamera:
+    """(W, H, fx, fy, cx, cy) -> I3DFusionCamera."""
+    W, H, fx, fy, cx, cy = cam
+    return I3DFusionCamera(int(W), int(H), float(fx), float(fy), float(cx), float(cy))
 
 
 class Engine:
@@ -220,6 +238,38 @@ class Engine:
         self._check(self.L.i3d_download_grid(self.h, _p(out["xyz"], C.c_int32), _p(out["sdf0"], C.c_double), _p(out["sdf_refined"], C.c_double),
                                              _p(out["albedo"], C.c_double), _p(out["weight"], C.c_float), _p(out["rgb"], C.c_uint8), C.byref(vs)))
         out["voxel_size"] = np.float32(vs.value)
+        return out
+
+    # ---- RGB-D fusion (AppFusion::fuseSDF) -------------------------------------------------------
+    def fusion_begin(self, params: I3DFusionParams):
+        self._check(self.L.i3d_fusion_begin(self.h, C.byref(params)))
+
+    def fusion_integrate(self, depth_cam, depth, color_cam, bgr, pose_cam_to_world, pose_world_to_cam):
+        """depth float32 [F, Hd, Wd] metres; bgr uint8 [F, Hc, Wc, 3]; cameras (W, H, fx, fy, cx, cy); poses float32 [F, 12] (R row-major | t)."""
+        depth = np.ascontiguousarray(depth, np.float32)
+        bgr = np.ascontiguousarray(bgr, np.uint8)
+        c2w = np.ascontiguousarray(pose_cam_to_world, np.float32)
+        w2c = np.ascontiguousarray(pose_world_to_cam, np.float32)
+        F = int(depth.shape[0])
+        dc, cc = fusion_camera(depth_cam), fusion_camera(color_cam)
+        assert depth.shape == (F, dc.height, dc.width) and bgr.shape == (F, cc.height, cc.width, 3)
+        assert c2w.shape == (F, 12) and w2c.shape == (F, 12)
+        self._check(self.L.i3d_fusion_integrate(self.h, C.c_int32(F), C.byref(dc), _p(depth, C.c_float), C.byref(cc), _p(bgr, C.c_uint8),
+                                                _p(c2w, C.c_float), _p(w2c, C.c_float)))
+
+    def fusion_finish(self) -> int:
+        """correctSDF, clearInvalidVoxels, convert; the result becomes the engine's grid.  Returns its voxel count."""
+        m = C.c_int64(0)
+        self._check(self.L.i3d_fusion_finish(self.h, C.byref(m)))
+        self.n = int(m.value)
+        return self.n
+
+    def fusion_volume(self):
+        """The fusion volume in progress in canonical order: xyz, sdf (float32), weight, rgb."""
+        n = int(self.L.i3d_debug_fusion_num_voxels(self.h))
+        out = dict(xyz=np.empty((n, 3), np.int32), sdf=np.empty(n, np.float32), weight=np.empty(n, np.float32), rgb=np.empty((n, 3), np.uint8))
+        self._check(self.L.i3d_debug_get_fusion_volume(self.h, _p(out["xyz"], C.c_int32), _p(out["sdf"], C.c_float), _p(out["weight"], C.c_float),
+                                                       _p(out["rgb"], C.c_uint8)))
         return out
 
     def download_state(self):
