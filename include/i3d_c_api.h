@@ -179,6 +179,25 @@ int         i3d_fusion_integrate(I3DEngine* e, int32_t F, const I3DFusionCamera*
  * in canonical 8^3-brick-major order (sorted by floor(c/8) z,y,x then c mod 8 z,y,x).  Per-voxel SH, the shard and the last
  * iteration are invalidated.  Ends the fusion.  An empty result leaves an empty grid (num_voxels_out = 0). */
 int         i3d_fusion_finish(I3DEngine* e, int64_t* num_voxels_out);
+
+/* ---- keyframe selection and the RGB-D image pyramid: the inputs of fusion and refinement (DESIGN.md §6i) ---- */
+/* Frames scored per device pass by i3d_keyframe_scores: bounds its scratch memory (I3D_KEYFRAME_CHUNK * W * H * 3 bytes). */
+#define I3D_KEYFRAME_CHUNK 32
+/* KeyframeSelection::add / estimateBlur (src/keyframe_selection.cpp:64-70, 219-310) for F frames: bgr uint8 [F][H][W][3] interleaved
+ * B,G,R; scores[F] = the Crete-2007 no-reference blur score (1 = sharp), NaN for a frame without vertical variation as in the reference.
+ * A frame's score depends only on its own pixels (not on F or on the other frames).  Fails for F <= 0 or frames under 5 px on an axis.
+ * Device time of the last call: i3d_phase_ms("keyframe_scores"); passes: i3d_phase_count("keyframe_chunks"). */
+int         i3d_keyframe_scores(I3DEngine* e, int32_t F, int32_t W, int32_t H, const uint8_t* bgr, double* scores);
+/* The level-0 keyframes (Pyramid::create's inputs, src/rgbd/pyramid.cpp:59-79) into a device-resident frame store: bgr uint8 [F][H][W][3],
+ * depth float metres [F][H][W], lum float [F][H][W] = Pyramid::intensity(0), or NULL to compute it from bgr (float B,G,R / 255, then
+ * (B 0.114 + G 0.587) + R 0.299).  The store replaces any previous one; the frames the engine is using are left alone. */
+int         i3d_upload_rgbd_frames(I3DEngine* e, int32_t F, int32_t W, int32_t H, const uint8_t* bgr, const float* depth, const float* lum);
+/* Builds Pyramid::intensity(lvl) (cv::pyrDown chain) and Pyramid::depth(lvl) (downsampleDepth chain) of every stored frame on the device and
+ * installs them exactly as i3d_upload_frames(F, W_lvl, H_lvl, lum, depth, 2^-lvl) would (same camera, iteration and colour invalidation);
+ * at lvl 0 the stored colours also become resident as i3d_upload_color_frames would make them.  *W_out / *H_out (may be NULL) get the
+ * level's size.  Fails without a store, for lvl < 0, and when a level on the way is under 3 px on an axis.
+ * Device time of the last call: i3d_phase_ms("frames_level"). */
+int         i3d_use_rgbd_level(I3DEngine* e, int32_t lvl, int32_t* W_out, int32_t* H_out);
 /* ---- multi-GPU (one process per GPU; voxel ranges sharded, see DESIGN.md §multi-GPU) ---- */
 /* 128-byte NCCL unique id created on rank 0 and distributed by the host (e.g. torch.distributed). */
 int         i3d_comm_unique_id(uint8_t id128[128]);
@@ -232,6 +251,9 @@ int64_t     i3d_debug_fusion_num_voxels(const I3DEngine* e);
  * rgb[3n] (r,g,b).  Any pointer may be NULL.  Fusion stage timings: i3d_phase_ms("fusion_prep" | "fusion_alloc" |
  * "fusion_integrate" | "fusion_correct" | "fusion_finish"); i3d_phase_count("fusion_growths" | "fusion_sweeps"). */
 int         i3d_debug_get_fusion_volume(I3DEngine* e, int32_t* xyz, float* sdf, float* weight, uint8_t* rgb);
+/* The frames of the current level as the device holds them: lum[F][H][W], depth[F][H][W], bgr[F][H][W][3] (fails when asked for colours
+ * that are not resident at this size).  Any pointer may be NULL. */
+int         i3d_debug_get_frames(I3DEngine* e, float* lum, float* depth, uint8_t* bgr);
 
 #ifdef __cplusplus
 }

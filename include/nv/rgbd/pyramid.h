@@ -1,6 +1,7 @@
 // nv/rgbd/pyramid.h — per-keyframe image pyramid as the optimiser sees it (reference: include/nv/rgbd/pyramid.h:47-69).
-// Building pyramids (cv::pyrDown etc.) is image preparation and out of scope; the caller attaches float luminance and depth
-// images per level.
+// The caller attaches float luminance and depth images per level.  A pyramid that carries only level 0 and its colour image is
+// enough for Intrinsic3D::refine: the engine then builds the coarser levels on the device (Pyramid::create's pyrDown and
+// downsampleDepth chains, i3d_use_rgbd_level; DESIGN.md §6i).
 #pragma once
 #include <vector>
 

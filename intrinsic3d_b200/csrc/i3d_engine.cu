@@ -31,6 +31,7 @@
 #include "i3d_recolor.cuh"
 #include "i3d_gridops.cuh"
 #include "i3d_fusion.cuh"
+#include "i3d_frames.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 
@@ -200,6 +201,11 @@ struct I3DEngine
     Dev<int> fu_ctl;                   // [0] allocated voxels, [1] alloc status, [2] correctSDF "changed", [3] valid voxels
     Dev<float> fu_depth_in, fu_depth, fu_nrm; Dev<uint8_t> fu_bgr;
     Dev<unsigned long long> fu_sk, fu_sk2; Dev<int32_t> fu_si, fu_si2; Dev<uint8_t> fu_cub;
+    // keyframe scores (i3d_frames.cuh): one chunk of host frames and its per-tile partial sums
+    Dev<uint8_t> kf_bgr; Dev<double> kf_partials, kf_scores;
+    // RGB-D frame store (i3d_upload_rgbd_frames): level-0 keyframes; i3d_use_rgbd_level builds level l from it
+    int st_F = 0, st_W = 0, st_H = 0;
+    Dev<float> st_lum, st_depth, st_tmp[4]; Dev<uint8_t> st_bgr;      // st_tmp: intermediate levels, luminance [0..1], depth [2..3]
     // shard (multi-GPU)
     int64_t shard_begin = 0, shard_end = -1;
     int rank = 0, world = 1;
@@ -311,6 +317,34 @@ int install_grid(I3DEngine* e, int64_t m, Dev<int32_t>& x, Dev<int32_t>& y, Dev<
     e->have_sh = false; e->have_iter = false; e->shard_ready = false; e->sv_S = 0; e->sv_x = nullptr;
     if (e->world > 1) { e->shard_begin = 0; e->shard_end = -1; }
     return rebuild_topology(e);
+}
+
+// Installs F frames of W x H as the engine's luminance / depth planes at scale pyr_scale: `fill` writes e->lum / e->depth (sized here) on
+// e->stream.  The one place that knows what a frame change invalidates: a new frame count drops the camera and the last iteration, a new
+// size drops the colour planes, and the depth tiles of the frame culling are rebuilt.
+template <class Fill>
+void install_frames(I3DEngine* e, int32_t F, int32_t W, int32_t H, double pyr_scale, Fill&& fill)
+{
+    const size_t cnt = static_cast<size_t>(F) * W * H;
+    if (F != e->F) { e->have_cam = false; e->have_iter = false; }     // the unknown space of the last iteration no longer matches
+    if (F != e->F || W != e->W || H != e->H) e->have_color = false;
+    e->F = F; e->W = W; e->H = H; e->pyr_scale = pyr_scale;
+    e->lum.ensure(cnt); e->depth.ensure(cnt);
+    // The live camera state may sit in camB (every accepted LM step swaps cam / c_cam): a re-upload of the frames of another
+    // pyramid level with the SAME frame count must not touch it.  Only a new frame count (camera invalidated above) or a first
+    // allocation resets the pair.
+    if (!e->have_cam || e->cam == nullptr)
+    {
+        e->camA.ensure(6 * static_cast<size_t>(F) + 9); e->camB.ensure(6 * static_cast<size_t>(F) + 9);
+        e->cam = e->camA.p; e->c_cam = e->camB.p;
+    }
+    fill();
+    {
+        const int TW = (W + kCullTile - 1) / kCullTile, TH = (H + kCullTile - 1) / kCullTile;
+        const size_t nt = static_cast<size_t>(F) * TW * TH;
+        e->tile_min.ensure(nt); e->tile_max.ensure(nt);
+        k_depth_tiles<<<static_cast<unsigned>(nt), 256, 0, e->stream>>>(F, W, H, e->depth.p, e->tile_min.p, e->tile_max.p);
+    }
 }
 
 // ---- RGB-D fusion helpers ---------------------------------------------------------------------
@@ -1128,26 +1162,10 @@ int i3d_upload_frames(I3DEngine* e, int32_t F, int32_t W, int32_t H, const float
     if (F <= 0 || W <= 0 || H <= 0) return fail(e, "i3d_upload_frames: bad dimensions");
     return guarded(e, [&]() {
         const size_t cnt = static_cast<size_t>(F) * W * H;
-        if (F != e->F) { e->have_cam = false; e->have_iter = false; }     // the unknown space of the last iteration no longer matches
-        if (F != e->F || W != e->W || H != e->H) e->have_color = false;
-        e->F = F; e->W = W; e->H = H; e->pyr_scale = pyr_scale;
-        e->lum.ensure(cnt); e->depth.ensure(cnt);
-        // The live camera state may sit in camB (every accepted LM step swaps cam / c_cam): a re-upload of the frames of another
-        // pyramid level with the SAME frame count must not touch it.  Only a new frame count (camera invalidated above) or a first
-        // allocation resets the pair.
-        if (!e->have_cam || e->cam == nullptr)
-        {
-            e->camA.ensure(6 * static_cast<size_t>(F) + 9); e->camB.ensure(6 * static_cast<size_t>(F) + 9);
-            e->cam = e->camA.p; e->c_cam = e->camB.p;
-        }
-        CK(cudaMemcpyAsync(e->lum.p, lum, cnt * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-        CK(cudaMemcpyAsync(e->depth.p, depth, cnt * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-        {
-            const int TW = (W + kCullTile - 1) / kCullTile, TH = (H + kCullTile - 1) / kCullTile;
-            const size_t nt = static_cast<size_t>(F) * TW * TH;
-            e->tile_min.ensure(nt); e->tile_max.ensure(nt);
-            k_depth_tiles<<<static_cast<unsigned>(nt), 256, 0, e->stream>>>(F, W, H, e->depth.p, e->tile_min.p, e->tile_max.p);
-        }
+        install_frames(e, F, W, H, pyr_scale, [&]() {
+            CK(cudaMemcpyAsync(e->lum.p, lum, cnt * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+            CK(cudaMemcpyAsync(e->depth.p, depth, cnt * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+        });
         CK(cudaStreamSynchronize(e->stream));
         CK(cudaGetLastError());
         return 0;
@@ -1703,6 +1721,131 @@ int i3d_fusion_finish(I3DEngine* e, int64_t* num_voxels_out)
         collect_kernel_times(e);
         e->fu_n = 0;
         if (num_voxels_out) *num_voxels_out = m;
+        return 0;
+    });
+}
+
+// ---- keyframe selection and the RGB-D pyramid (i3d_frames.cuh, DESIGN.md §6i) --------------------
+int i3d_keyframe_scores(I3DEngine* e, int32_t F, int32_t W, int32_t H, const uint8_t* bgr, double* scores)
+{
+    if (!e) return 1;
+    if (F <= 0 || !bgr || !scores) return fail(e, "i3d_keyframe_scores: need F > 0 frames and non-NULL buffers (F = %d)", F);
+    if (W < 5 || H < 5) return fail(e, "i3d_keyframe_scores: frames of %d x %d px; the 9-tap blur filter needs at least 5 px on each axis", W, H);
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t img = static_cast<size_t>(W) * H * 3;
+        const int tx = (W + kBlurTileW - 1) / kBlurTileW, ty = (H + kBlurTileH - 1) / kBlurTileH;
+        const int chunk = std::min<int>(F, I3D_KEYFRAME_CHUNK);
+        e->kf_bgr.ensure(img * chunk); e->kf_partials.ensure(static_cast<size_t>(chunk) * tx * ty * 4); e->kf_scores.ensure(chunk);
+        e->phases.erase("keyframe_scores"); e->phases.erase("keyframe_chunks");
+        for (int f0 = 0; f0 < F; f0 += chunk)
+        {
+            const int n = std::min(chunk, F - f0);
+            CK(cudaMemcpyAsync(e->kf_bgr.p, bgr + img * f0, img * n, cudaMemcpyHostToDevice, st));
+            {
+                Timer t(e, "keyframe_scores", 0);
+                k_blur_partials<<<dim3(tx, ty, n), dim3(32, 8), 0, st>>>(n, W, H, e->kf_bgr.p, e->kf_partials.p);
+                k_blur_finish<<<(n + 3) / 4, 128, 0, st>>>(n, tx * ty, e->kf_partials.p, e->kf_scores.p);
+            }
+            CK(cudaMemcpyAsync(scores + f0, e->kf_scores.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+            collect_kernel_times(e);          // synchronises: the chunk buffer is free again
+            CK(cudaGetLastError());
+            e->phases["keyframe_chunks"].count += 1;
+        }
+        return 0;
+    });
+}
+
+int i3d_upload_rgbd_frames(I3DEngine* e, int32_t F, int32_t W, int32_t H, const uint8_t* bgr, const float* depth, const float* lum)
+{
+    if (!e) return 1;
+    if (F <= 0 || W <= 0 || H <= 0) return fail(e, "i3d_upload_rgbd_frames: bad dimensions (F = %d, %d x %d)", F, W, H);
+    if (!bgr || !depth) return fail(e, "i3d_upload_rgbd_frames: bgr and depth must not be NULL");
+    e->st_F = 0;
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t cnt = static_cast<size_t>(F) * W * H;
+        e->st_lum.ensure(cnt); e->st_depth.ensure(cnt); e->st_bgr.ensure(3 * cnt);
+        CK(cudaMemcpyAsync(e->st_bgr.p, bgr, 3 * cnt, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(e->st_depth.p, depth, cnt * sizeof(float), cudaMemcpyHostToDevice, st));
+        if (lum) CK(cudaMemcpyAsync(e->st_lum.p, lum, cnt * sizeof(float), cudaMemcpyHostToDevice, st));
+        else k_frames_lum0<<<blocks_for(cnt), kThreads, 0, st>>>(cnt, e->st_bgr.p, e->st_lum.p);
+        CK(cudaStreamSynchronize(st));
+        CK(cudaGetLastError());
+        e->st_F = F; e->st_W = W; e->st_H = H;
+        return 0;
+    });
+}
+
+int i3d_use_rgbd_level(I3DEngine* e, int32_t lvl, int32_t* W_out, int32_t* H_out)
+{
+    if (!e) return 1;
+    if (e->st_F <= 0) return fail(e, "i3d_use_rgbd_level: no frame store (call i3d_upload_rgbd_frames first)");
+    if (lvl < 0) return fail(e, "i3d_use_rgbd_level: negative level %d", lvl);
+    int W = e->st_W, H = e->st_H;
+    for (int k = 1; k <= lvl; ++k)
+    {
+        if (W < 3 || H < 3)
+            return fail(e, "i3d_use_rgbd_level: level %d would be built from a %d x %d level; downsampling needs at least 3 px on each axis", lvl, W, H);
+        W /= 2; H /= 2;
+    }
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const int F = e->st_F;
+        const size_t cnt = static_cast<size_t>(F) * W * H;
+        e->phases.erase("frames_level");
+        install_frames(e, F, W, H, std::ldexp(1.0, -lvl), [&]() {
+            Timer t(e, "frames_level", 0);
+            if (lvl == 0)
+            {
+                CK(cudaMemcpyAsync(e->lum.p, e->st_lum.p, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st));
+                CK(cudaMemcpyAsync(e->depth.p, e->st_depth.p, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st));
+                return;
+            }
+            // the chain level 0 -> 1 -> ... -> lvl, intermediate levels in two ping-pong pairs, the last one straight into lum / depth
+            const float* sl = e->st_lum.p; const float* sd = e->st_depth.p;
+            int w = e->st_W, h = e->st_H;
+            for (int k = 1; k <= lvl; ++k)
+            {
+                const int wd = w / 2, hd = h / 2;
+                float* dl = e->lum.p; float* dd = e->depth.p;
+                if (k < lvl)
+                {
+                    const size_t c = static_cast<size_t>(F) * wd * hd;
+                    e->st_tmp[k & 1].ensure(c); e->st_tmp[2 + (k & 1)].ensure(c);
+                    dl = e->st_tmp[k & 1].p; dd = e->st_tmp[2 + (k & 1)].p;
+                }
+                const dim3 grid((wd + 31) / 32, (hd + 7) / 8, std::min(F, 65535));
+                k_frames_pyrdown<<<grid, dim3(32, 8), 0, st>>>(F, w, h, sl, dl);
+                k_frames_depthdown<<<grid, dim3(32, 8), 0, st>>>(F, w, h, sd, dd);
+                sl = dl; sd = dd; w = wd; h = hd;
+            }
+        });
+        if (lvl == 0)
+        {
+            e->color.ensure(3 * cnt);
+            CK(cudaMemcpyAsync(e->color.p, e->st_bgr.p, 3 * cnt, cudaMemcpyDeviceToDevice, st));
+            e->have_color = true;
+        }
+        collect_kernel_times(e);
+        CK(cudaGetLastError());
+        if (W_out) *W_out = W;
+        if (H_out) *H_out = H;
+        return 0;
+    });
+}
+
+int i3d_debug_get_frames(I3DEngine* e, float* lum, float* depth, uint8_t* bgr)
+{
+    if (!e) return 1;
+    if (e->F <= 0) return fail(e, "i3d_debug_get_frames: no frames on the device");
+    if (bgr && !e->have_color) return fail(e, "i3d_debug_get_frames: no colour frames at the current size");
+    return guarded(e, [&]() {
+        const size_t cnt = static_cast<size_t>(e->F) * e->W * e->H;
+        if (lum) CK(cudaMemcpyAsync(lum, e->lum.p, cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+        if (depth) CK(cudaMemcpyAsync(depth, e->depth.p, cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+        if (bgr) CK(cudaMemcpyAsync(bgr, e->color.p, 3 * cnt, cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaStreamSynchronize(e->stream));
         return 0;
     });
 }

@@ -27,11 +27,13 @@ EXPORTED_SYMBOLS = [
     "i3d_upload_color_frames", "i3d_recompute_colors", "i3d_download_colors",
     "i3d_num_voxels", "i3d_clear_voxels_outside_thin_shell", "i3d_upsample_grid", "i3d_download_grid",
     "i3d_sizeof_fusion_params", "i3d_default_fusion_params", "i3d_fusion_begin", "i3d_fusion_integrate", "i3d_fusion_finish",
+    "i3d_keyframe_scores", "i3d_upload_rgbd_frames", "i3d_use_rgbd_level",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
     "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_normal_equations",
-    "i3d_debug_apply_operator", "i3d_debug_fusion_num_voxels", "i3d_debug_get_fusion_volume",
+    "i3d_debug_apply_operator", "i3d_debug_fusion_num_voxels", "i3d_debug_get_fusion_volume", "i3d_debug_get_frames",
 ]
+KEYFRAME_CHUNK = 32       # I3D_KEYFRAME_CHUNK of include/i3d_c_api.h: frames scored per device pass
 
 
 def load_library():
@@ -152,6 +154,7 @@ class Engine:
         self._check(self.L.i3d_upload_frames(self.h, C.c_int32(F), C.c_int32(W), C.c_int32(H), _p(lum, C.c_float), _p(depth, C.c_float),
                                              C.c_double(float(pyr_scale))))
         self.F = F
+        self.frame_size = (W, H)
 
     def set_camera(self, poses, intr, dist):
         poses = np.ascontiguousarray(poses, np.float64)
@@ -271,6 +274,48 @@ class Engine:
         self._check(self.L.i3d_debug_get_fusion_volume(self.h, _p(out["xyz"], C.c_int32), _p(out["sdf"], C.c_float), _p(out["weight"], C.c_float),
                                                        _p(out["rgb"], C.c_uint8)))
         return out
+
+    # ---- keyframe selection and the RGB-D pyramid (KeyframeSelection::estimateBlur, Pyramid::create) ----------------------
+    def keyframe_scores(self, bgr):
+        """Blur score (Crete 2007, 1 = sharp) of every frame: bgr uint8 [F, H, W, 3] (B, G, R) -> float64 [F]; NaN for a frame without
+        vertical variation.  Pick the keyframes with keyframes.select_keyframes."""
+        bgr = np.ascontiguousarray(bgr, np.uint8)
+        assert bgr.ndim == 4 and bgr.shape[3] == 3
+        F, H, W = bgr.shape[:3]
+        out = np.empty(F, np.float64)
+        self._check(self.L.i3d_keyframe_scores(self.h, C.c_int32(F), C.c_int32(W), C.c_int32(H), _p(bgr, C.c_uint8), _p(out, C.c_double)))
+        return out
+
+    def upload_rgbd_frames(self, bgr, depth, lum=None):
+        """Level-0 keyframes into the device frame store: bgr uint8 [F, H, W, 3], depth float32 [F, H, W] metres, lum float32 [F, H, W] or
+        None (computed from bgr).  use_rgbd_level(l) then installs pyramid level l."""
+        bgr = np.ascontiguousarray(bgr, np.uint8)
+        depth = np.ascontiguousarray(depth, np.float32)
+        F, H, W = depth.shape
+        assert bgr.shape == (F, H, W, 3)
+        if lum is not None:
+            lum = np.ascontiguousarray(lum, np.float32)
+            assert lum.shape == (F, H, W)
+        self._check(self.L.i3d_upload_rgbd_frames(self.h, C.c_int32(F), C.c_int32(W), C.c_int32(H), _p(bgr, C.c_uint8), _p(depth, C.c_float),
+                                                  _p(lum, C.c_float)))
+        self._store_F = F
+
+    def use_rgbd_level(self, lvl: int):
+        """Builds pyramid level `lvl` of the stored keyframes on the device and makes it the engine's frames (as upload_frames would, at scale
+        2^-lvl; at level 0 the colours too).  Returns (W, H) of the level."""
+        w, h = C.c_int32(0), C.c_int32(0)
+        self._check(self.L.i3d_use_rgbd_level(self.h, C.c_int32(int(lvl)), C.byref(w), C.byref(h)))
+        self.F = self._store_F
+        self.frame_size = (int(w.value), int(h.value))
+        return self.frame_size
+
+    def debug_frames(self, with_color=False):
+        """(lum, depth, bgr or None) of the current level as the device holds them."""
+        W, H = self.frame_size
+        lum, depth = np.empty((self.F, H, W), np.float32), np.empty((self.F, H, W), np.float32)
+        bgr = np.empty((self.F, H, W, 3), np.uint8) if with_color else None
+        self._check(self.L.i3d_debug_get_frames(self.h, _p(lum, C.c_float), _p(depth, C.c_float), _p(bgr, C.c_uint8)))
+        return lum, depth, bgr
 
     def download_state(self):
         sdf = np.empty(self.n, np.float64)

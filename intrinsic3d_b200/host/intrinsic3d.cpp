@@ -86,8 +86,13 @@ bool Intrinsic3D::refine(SparseVoxelGrid<Voxel>* grid_in)
     }
     Optimizer::ImageFormationModel& im = *image_model_;
     const size_t F = im.poses.size();
+    // Keyframes that carry only level 0 and its colour image: the engine builds the coarser levels itself from a device frame store
+    // (i3d_upload_rgbd_frames / i3d_use_rgbd_level).  Pyramids that carry every level are uploaded level by level from the host.
+    bool device_pyramid = cfg_.num_rgbd_levels > 1;
     for (size_t f = 0; f < F; ++f)
-        if (im.rgbd_pyr[f].levels() < cfg_.num_rgbd_levels || im.rgbd_pyr[f].color(0).empty())
+        device_pyramid = device_pyramid && im.rgbd_pyr[f].levels() == 1 && !im.rgbd_pyr[f].color(0).empty();
+    for (size_t f = 0; f < F; ++f)
+        if ((!device_pyramid && im.rgbd_pyr[f].levels() < cfg_.num_rgbd_levels) || im.rgbd_pyr[f].color(0).empty())
         {
             std::cerr << "Intrinsic3D::refine: frame " << f << " lacks pyramid levels or its colour image" << std::endl;
             return false;
@@ -124,7 +129,36 @@ bool Intrinsic3D::refine(SparseVoxelGrid<Voxel>* grid_in)
     std::vector<uint8_t> color;
     int cur_level = -1;
     bool color_resident = false;
+    if (device_pyramid)
+    {
+        const ImageF l0 = im.rgbd_pyr[0].intensity(0);
+        const int W = l0.cols, H = l0.rows;
+        const size_t px = static_cast<size_t>(W) * H;
+        lum.resize(F * px); depth.resize(F * px); color.resize(F * px * 3);
+        for (size_t f = 0; f < F; ++f)
+        {
+            const ImageF l = im.rgbd_pyr[f].intensity(0), d = im.rgbd_pyr[f].depth(0);
+            const ImageBGR c = im.rgbd_pyr[f].color(0);
+            if (l.rows != H || l.cols != W || d.rows != H || d.cols != W || c.rows != H || c.cols != W) return fail("keyframes of different sizes");
+            std::memcpy(&lum[f * px], l.data, px * sizeof(float));
+            std::memcpy(&depth[f * px], d.data, px * sizeof(float));
+            std::memcpy(&color[f * px * 3], c.data, px * 3);
+        }
+        if (i3d_upload_rgbd_frames(eng, static_cast<int32_t>(F), W, H, color.data(), depth.data(), lum.data()) != 0) return fail("upload keyframes");
+        std::vector<float>().swap(lum); std::vector<float>().swap(depth); std::vector<uint8_t>().swap(color);
+    }
     auto upload_level = [&](int lvl, bool with_color) -> bool {
+        if (device_pyramid)
+        {
+            // a level switch builds the level on the device; level 0 brings the colour planes along
+            if (lvl != cur_level || (with_color && !color_resident))
+            {
+                if (i3d_use_rgbd_level(eng, lvl, nullptr, nullptr) != 0) return false;
+                cur_level = lvl;
+                color_resident = lvl == 0;
+            }
+            return !with_color || color_resident;
+        }
         const ImageF l0 = im.rgbd_pyr[0].intensity(lvl);
         const int W = l0.cols, H = l0.rows;
         const size_t px = static_cast<size_t>(W) * H;
