@@ -180,6 +180,20 @@ int         i3d_fusion_integrate(I3DEngine* e, int32_t F, const I3DFusionCamera*
  * iteration are invalidated.  Ends the fusion.  An empty result leaves an empty grid (num_voxels_out = 0). */
 int         i3d_fusion_finish(I3DEngine* e, int64_t* num_voxels_out);
 
+/* ---- surface extraction: the grid as a coloured triangle mesh (DESIGN.md §6j) ---- */
+uint64_t    i3d_sizeof_mesh_info(void);
+/* MarchingCubes<VoxelSBR>::extractMesh + MeshUtil::removeDegenerateFaces (src/mesh/marching_cubes.cpp:64-317, src/mesh/util.cpp:168-198)
+ * and, with largest_component_only, removeLooseComponents + removeUnusedVertices (util.cpp:47-165), over the resident grid.  The mesh
+ * stays on the device until i3d_download_mesh; *info (may be NULL) gets the counts of every stage and its device time.
+ * Faces are in (voxel index, triangle slot) order; vertex ids in order of first appearance over the face corners; two corners are one
+ * vertex iff their float positions compare equal; without the component filter, vertices that only degenerate faces used are kept.
+ * Reads the grid only: state, camera, lighting, frames and the last iteration are unchanged.  A change of the voxel set (upload,
+ * prune, upsample, fusion) drops the resident mesh.  Fails without a grid and for an sdf_source other than 0 or 1. */
+int         i3d_extract_mesh(I3DEngine* e, const I3DMeshParams* params, I3DMeshInfo* info);
+/* The resident mesh: xyz float [V][3] metres, rgb uint8 [V][3], faces int32 [F][3] (V, F: info->num_vertices / num_faces).  Any
+ * pointer may be NULL.  Fails when no mesh of the current grid has been extracted. */
+int         i3d_download_mesh(I3DEngine* e, float* xyz, uint8_t* rgb, int32_t* faces);
+
 /* ---- keyframe selection and the RGB-D image pyramid: the inputs of fusion and refinement (DESIGN.md §6i) ---- */
 /* Frames scored per device pass by i3d_keyframe_scores: bounds its scratch memory (I3D_KEYFRAME_CHUNK * W * H * 3 bytes). */
 #define I3D_KEYFRAME_CHUNK 32

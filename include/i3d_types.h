@@ -167,6 +167,25 @@ typedef struct I3DFusionCamera
     float   fx, fy, cx, cy;
 } I3DFusionCamera;
 
+/* ---- surface extraction (MarchingCubes::extractSurface + MeshUtil, src/mesh/marching_cubes.cpp, src/mesh/util.cpp) ---- */
+typedef struct I3DMeshParams
+{
+    int32_t sdf_source;                   /* 0 = sdf0 (what AppFusion meshes), 1 = sdf_refined (what onSDFRefined meshes) */
+    int32_t largest_component_only;       /* 1 = MeshUtil::removeLooseComponents + removeUnusedVertices (output_mesh_largest_comp_only) */
+} I3DMeshParams;
+
+typedef struct I3DMeshInfo
+{
+    int64_t num_cubes;                    /* cubes whose 8 corners exist with weight != 0 */
+    int64_t num_faces_raw;                /* triangles emitted by marching cubes */
+    int64_t num_vertices_welded;          /* distinct float positions among their corners */
+    int64_t num_faces_clean;              /* faces left by removeDegenerateFaces */
+    int64_t num_faces, num_vertices;      /* the resident mesh: after the component filter when asked for, else the cleaned faces and
+                                             every welded vertex */
+    double  ms_classify, ms_emit, ms_weld, ms_clean, ms_components;   /* device time per stage: CUDA events around its device-only
+                                                                           segments, the host read-backs of counts excluded */
+} I3DMeshInfo;
+
 #ifdef __cplusplus
 }
 #endif

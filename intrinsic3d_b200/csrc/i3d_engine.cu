@@ -32,6 +32,7 @@
 #include "i3d_gridops.cuh"
 #include "i3d_fusion.cuh"
 #include "i3d_frames.cuh"
+#include "i3d_mesh.h"
 
 #include <cub/device/device_radix_sort.cuh>
 
@@ -206,6 +207,17 @@ struct I3DEngine
     // RGB-D frame store (i3d_upload_rgbd_frames): level-0 keyframes; i3d_use_rgbd_level builds level l from it
     int st_F = 0, st_W = 0, st_H = 0;
     Dev<float> st_lum, st_depth, st_tmp[4]; Dev<uint8_t> st_bgr;      // st_tmp: intermediate levels, luminance [0..1], depth [2..3]
+    // surface extraction (i3d_mesh.cuh): scratch that only grows, and the resident mesh of the last i3d_extract_mesh
+    bool have_mesh = false;
+    int64_t mesh_V = 0, mesh_F = 0;
+    float* mesh_vpos = nullptr; uint8_t* mesh_vcol = nullptr; int3* mesh_faces = nullptr;
+    Dev<uint8_t> ms_case, ms_keep, ms_cub; Dev<int32_t> ms_cnt, ms_sel; Dev<int64_t> ms_off; Dev<unsigned long long> ms_cubes, ms_best;
+    Dev<float> ms_cpos, ms_vpos, ms_vpos2; Dev<uint8_t> ms_ccol, ms_vcol, ms_vcol2;
+    Dev<uint32_t> ms_klo, ms_klo2; Dev<unsigned long long> ms_khi, ms_khi2;
+    Dev<int32_t> ms_perm, ms_perm2, ms_first, ms_fid, ms_head, ms_seg, ms_cvid, ms_parent, ms_used, ms_newid;
+    Dev<int3> ms_faces, ms_faces2; Dev<unsigned> ms_ccount, ms_cminf;
+    cudaEvent_t ms_ev[16] = {};        // begin / end of up to 8 device-only segments of one extraction (MeshSegments)
+    bool ms_ev_ready = false;
     // shard (multi-GPU)
     int64_t shard_begin = 0, shard_end = -1;
     int rank = 0, world = 1;
@@ -290,6 +302,7 @@ int rebuild_topology(I3DEngine* e)
 {
     cudaStream_t st = e->stream;
     const int64_t n = e->n;
+    e->have_mesh = false;      // a new voxel set: the resident mesh no longer belongs to the grid
     e->nbr.ensure(static_cast<size_t>(NB_COUNT) * n);
     uint64_t cap = 1; while (cap < static_cast<uint64_t>(2 * n)) cap <<= 1;
     e->up_keys.ensure(cap); e->up_vals.ensure(cap); e->up_dup.ensure(1);
@@ -1055,6 +1068,159 @@ int setup_shard(I3DEngine* e)
     return 0;
 }
 
+// ---- surface extraction (i3d_mesh.cuh, DESIGN.md §6j) ----------------------------------------------
+// runs one CUB-style device call twice: temp-size query, then the call on e->ms_cub (grown, never shrunk)
+template <class Fn>
+void cub_call(I3DEngine* e, Fn&& fn)
+{
+    size_t bytes = 0;
+    CK(fn(static_cast<void*>(nullptr), bytes));
+    e->ms_cub.ensure(bytes);
+    CK(fn(static_cast<void*>(e->ms_cub.p), bytes));
+}
+
+// Device time per stage of one extraction: event pairs around device-only segments, each credited to a stage.  The host round trips
+// that read counts back fall between segments, so they are not counted.
+struct MeshSegments
+{
+    I3DEngine* e; int used = 0; int stage[8];
+    void begin(int s) { CK(cudaEventRecord(e->ms_ev[2 * used], e->stream)); stage[used] = s; }
+    void end() { CK(cudaEventRecord(e->ms_ev[2 * used + 1], e->stream)); ++used; }
+};
+
+template <class T>
+T read_back(I3DEngine* e, const T* d)
+{
+    T h{};
+    CK(cudaMemcpyAsync(&h, d, sizeof(T), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    return h;
+}
+
+// Marching cubes over the resident grid, welding, degenerate-face removal and (optionally) the largest component.  Every count is
+// read back before the buffers of the next stage are sized.  Reads the grid; writes only the ms_* scratch and the resident mesh.
+int extract_mesh(I3DEngine* e, const I3DMeshParams& prm, I3DMeshInfo* info)
+{
+    cudaStream_t st = e->stream;
+    const int64_t n = e->n;
+    e->have_mesh = false;
+    if (!e->ms_ev_ready) { for (auto& ev : e->ms_ev) CK(cudaEventCreate(&ev)); e->ms_ev_ready = true; }
+    I3DMeshInfo inf{};
+    MeshGrid g;
+    g.n = n; g.x = e->x.p; g.y = e->y.p; g.z = e->z.p; g.sdf = prm.sdf_source == 0 ? e->sdf0.p : e->sdf; g.weight = e->weight.p; g.rgb = e->rgb.p;
+    g.nbr = e->nbr.p; g.keys = e->up_keys.p; g.vals = e->up_vals.p; g.mask = e->hash_cap - 1; g.voxel_size = e->voxel_size;
+
+    enum { CLASSIFY, EMIT, WELD, CLEAN, COMPONENTS };
+    MeshSegments seg{e};
+
+    // 1. cube cases and per-voxel triangle counts -> face offsets
+    e->ms_case.ensure(n); e->ms_cnt.ensure(n); e->ms_off.ensure(n); e->ms_cubes.ensure(1); e->ms_sel.ensure(1); e->ms_best.ensure(1);
+    seg.begin(CLASSIFY);
+    CK(cudaMemsetAsync(e->ms_cubes.p, 0, sizeof(unsigned long long), st));
+    mesh::classify(g, e->ms_case.p, e->ms_cnt.p, e->ms_cubes.p, st);
+    cub_call(e, [&](void* t, size_t& b) { return mesh::face_offsets(t, b, e->ms_cnt.p, e->ms_off.p, static_cast<int>(n), st); });
+    seg.end();
+    inf.num_cubes = static_cast<int64_t>(read_back(e, e->ms_cubes.p));
+    const int64_t F0 = read_back(e, e->ms_off.p + (n - 1)) + read_back(e, e->ms_cnt.p + (n - 1));
+    inf.num_faces_raw = F0;
+    // corner and vertex ids are int32 (as the PLY's indices); element offsets into the interleaved arrays are computed in int64
+    if (3 * F0 > INT_MAX) return fail(e, "i3d_extract_mesh: %lld triangles exceed the int32 corner indices of the mesh", static_cast<long long>(F0));
+    const int32_t M = static_cast<int32_t>(3 * F0);
+    float* vpos = nullptr; uint8_t* vcol = nullptr; int3* faces = nullptr;
+    int64_t V = 0, F = 0;
+    if (M > 0)
+    {
+        // 2. the triangle soup, corner by corner
+        e->ms_cpos.ensure(3 * static_cast<size_t>(M)); e->ms_ccol.ensure(3 * static_cast<size_t>(M));
+        e->ms_klo.ensure(M); e->ms_klo2.ensure(M); e->ms_khi.ensure(M); e->ms_khi2.ensure(M); e->ms_perm.ensure(M); e->ms_perm2.ensure(M);
+        seg.begin(EMIT);
+        mesh::emit(g, e->ms_case.p, e->ms_cnt.p, e->ms_off.p, MeshCorners{e->ms_cpos.p, e->ms_ccol.p, e->ms_klo.p, e->ms_khi.p}, st);
+        seg.end();
+
+        // 3. welding: stable sort of the corner indices by position (z bits, then x|y bits), segment heads, ids by first appearance
+        e->ms_first.ensure(M); e->ms_fid.ensure(M); e->ms_head.ensure(M); e->ms_seg.ensure(M); e->ms_cvid.ensure(M);
+        seg.begin(WELD);
+        mesh::iota(M, e->ms_perm2.p, st);
+        cub_call(e, [&](void* t, size_t& b) { return mesh::sort_z(t, b, e->ms_klo.p, e->ms_klo2.p, e->ms_perm2.p, e->ms_perm.p, M, st); });
+        mesh::gather_key_hi(M, e->ms_perm.p, e->ms_khi.p, e->ms_khi2.p, st);
+        cub_call(e, [&](void* t, size_t& b) { return mesh::sort_xy(t, b, e->ms_khi2.p, e->ms_khi.p, e->ms_perm.p, e->ms_perm2.p, M, st); });
+        mesh::weld_heads(M, e->ms_perm2.p, e->ms_khi.p, e->ms_klo.p, e->ms_first.p, e->ms_head.p, st);
+        cub_call(e, [&](void* t, size_t& b) { return mesh::exclusive_sum(t, b, e->ms_first.p, e->ms_fid.p, M, st); });
+        cub_call(e, [&](void* t, size_t& b) { return mesh::inclusive_max(t, b, e->ms_head.p, e->ms_seg.p, M, st); });
+        seg.end();
+        const int64_t Vw = read_back(e, e->ms_fid.p + (M - 1)) + read_back(e, e->ms_first.p + (M - 1));
+        e->ms_vpos.ensure(3 * static_cast<size_t>(Vw)); e->ms_vcol.ensure(3 * static_cast<size_t>(Vw));
+        seg.begin(WELD);
+        mesh::weld_assign(M, e->ms_perm2.p, e->ms_seg.p, e->ms_fid.p, e->ms_cpos.p, e->ms_ccol.p, e->ms_cvid.p, e->ms_vpos.p, e->ms_vcol.p, st);
+        seg.end();
+        inf.num_vertices_welded = Vw;
+
+        // 4. degenerate faces, survivors kept in order; the vertices stay
+        const int32_t F0i = static_cast<int32_t>(F0);
+        const int3* faces0 = reinterpret_cast<const int3*>(e->ms_cvid.p);
+        e->ms_keep.ensure(F0); e->ms_faces.ensure(F0);
+        seg.begin(CLEAN);
+        mesh::face_clean(F0i, faces0, e->ms_vpos.p, e->ms_keep.p, st);
+        cub_call(e, [&](void* t, size_t& b) { return mesh::select_faces(t, b, faces0, e->ms_keep.p, e->ms_faces.p, e->ms_sel.p, F0i, st); });
+        seg.end();
+        const int32_t F1 = read_back(e, e->ms_sel.p);
+        inf.num_faces_clean = F1;
+        vpos = e->ms_vpos.p; vcol = e->ms_vcol.p; faces = e->ms_faces.p; V = Vw; F = F1;
+
+        // 5. the largest face-connected component, then only the vertices it uses
+        if (prm.largest_component_only)
+        {
+            const int32_t Vi = static_cast<int32_t>(Vw);
+            e->ms_parent.ensure(Vw); e->ms_ccount.ensure(Vw); e->ms_cminf.ensure(Vw); e->ms_used.ensure(Vw); e->ms_newid.ensure(Vw);
+            e->ms_faces2.ensure(std::max<int32_t>(F1, 1));
+            int32_t F2 = 0, V2 = 0;
+            if (F1 > 0)
+            {
+                seg.begin(COMPONENTS);
+                mesh::iota(Vi, e->ms_parent.p, st);
+                mesh::cc_union(F1, e->ms_faces.p, e->ms_parent.p, st);
+                mesh::cc_flatten(Vi, e->ms_parent.p, st);
+                CK(cudaMemsetAsync(e->ms_ccount.p, 0, Vw * sizeof(unsigned), st));
+                CK(cudaMemsetAsync(e->ms_cminf.p, 0xFF, Vw * sizeof(unsigned), st));
+                CK(cudaMemsetAsync(e->ms_best.p, 0, sizeof(unsigned long long), st));
+                mesh::cc_count(F1, e->ms_faces.p, e->ms_parent.p, e->ms_ccount.p, e->ms_cminf.p, st);
+                mesh::cc_best(Vi, e->ms_ccount.p, e->ms_cminf.p, e->ms_best.p, st);
+                mesh::cc_keep(F1, e->ms_faces.p, e->ms_parent.p, e->ms_best.p, e->ms_keep.p, st);
+                cub_call(e, [&](void* t, size_t& b) { return mesh::select_faces(t, b, e->ms_faces.p, e->ms_keep.p, e->ms_faces2.p, e->ms_sel.p, F1, st); });
+                seg.end();
+                F2 = read_back(e, e->ms_sel.p);
+                seg.begin(COMPONENTS);
+                CK(cudaMemsetAsync(e->ms_used.p, 0, Vw * sizeof(int32_t), st));
+                if (F2 > 0) mesh::mark_used(F2, e->ms_faces2.p, e->ms_used.p, st);
+                cub_call(e, [&](void* t, size_t& b) { return mesh::exclusive_sum(t, b, e->ms_used.p, e->ms_newid.p, Vi, st); });
+                seg.end();
+                V2 = read_back(e, e->ms_newid.p + (Vi - 1)) + read_back(e, e->ms_used.p + (Vi - 1));
+                e->ms_vpos2.ensure(3 * static_cast<size_t>(V2)); e->ms_vcol2.ensure(3 * static_cast<size_t>(V2));
+                seg.begin(COMPONENTS);
+                mesh::compact_vertices(Vi, e->ms_used.p, e->ms_newid.p, e->ms_vpos.p, e->ms_vcol.p, e->ms_vpos2.p, e->ms_vcol2.p, st);
+                if (F2 > 0) mesh::remap_faces(F2, e->ms_newid.p, e->ms_faces2.p, st);
+                seg.end();
+            }
+            vpos = e->ms_vpos2.p; vcol = e->ms_vcol2.p; faces = e->ms_faces2.p; V = V2; F = F2;
+        }
+    }
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
+    double ms[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int k = 0; k < seg.used; ++k)
+    {
+        float t = 0.f;
+        CK(cudaEventElapsedTime(&t, e->ms_ev[2 * k], e->ms_ev[2 * k + 1]));
+        ms[seg.stage[k]] += t;
+    }
+    inf.ms_classify = ms[CLASSIFY]; inf.ms_emit = ms[EMIT]; inf.ms_weld = ms[WELD]; inf.ms_clean = ms[CLEAN]; inf.ms_components = ms[COMPONENTS];
+    inf.num_faces = F; inf.num_vertices = V;
+    e->mesh_vpos = vpos; e->mesh_vcol = vcol; e->mesh_faces = faces; e->mesh_V = V; e->mesh_F = F;
+    e->have_mesh = true;
+    if (info) *info = inf;
+    return 0;
+}
+
 } // namespace
 
 // =================================================================================================
@@ -1114,6 +1280,7 @@ void i3d_engine_destroy(I3DEngine* e)
     if (e->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
     for (auto& ev : e->ev) cudaEventDestroy(ev);
     for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
+    if (e->ms_ev_ready) for (auto& ev : e->ms_ev) cudaEventDestroy(ev);
     cudaStreamDestroy(e->stream);
     delete e;
 }
@@ -1487,7 +1654,7 @@ int i3d_clear_voxels_outside_thin_shell(I3DEngine* e, double thres_shell, int64_
             {
                 // the reference leaves an EMPTY grid here (clearVoxelsOutsideThinShell erases everything; the following lighting estimate
                 // then fails and Intrinsic3D::refine skips the level): same state, not an error
-                e->n = 0; e->have_sh = false; e->have_iter = false; e->shard_ready = false; e->sv_S = 0; e->sv_x = nullptr;
+                e->n = 0; e->have_sh = false; e->have_iter = false; e->shard_ready = false; e->sv_S = 0; e->sv_x = nullptr; e->have_mesh = false;
                 collect_kernel_times(e);
                 if (num_voxels_out) *num_voxels_out = 0;
                 return 0;
@@ -1715,12 +1882,39 @@ int i3d_fusion_finish(I3DEngine* e, int64_t* num_voxels_out)
             else
             {
                 // clearInvalidVoxels left nothing: an empty grid, as after a pruning that removes everything
-                e->n = 0; e->have_sh = false; e->have_iter = false; e->shard_ready = false; e->sv_S = 0; e->sv_x = nullptr;
+                e->n = 0; e->have_sh = false; e->have_iter = false; e->shard_ready = false; e->sv_S = 0; e->sv_x = nullptr; e->have_mesh = false;
             }
         }
         collect_kernel_times(e);
         e->fu_n = 0;
         if (num_voxels_out) *num_voxels_out = m;
+        return 0;
+    });
+}
+
+// ---- surface extraction (i3d_mesh.cuh, DESIGN.md §6j) ----------------------------------------------
+uint64_t i3d_sizeof_mesh_info(void) { return sizeof(I3DMeshInfo); }
+
+int i3d_extract_mesh(I3DEngine* e, const I3DMeshParams* params, I3DMeshInfo* info)
+{
+    if (!e) return 1;
+    if (!params) return fail(e, "i3d_extract_mesh: params is NULL");
+    if (e->n <= 0) return fail(e, "i3d_extract_mesh: no grid");
+    if (params->sdf_source != 0 && params->sdf_source != 1) return fail(e, "i3d_extract_mesh: sdf_source must be 0 (sdf0) or 1 (sdf_refined), got %d", params->sdf_source);
+    return guarded(e, [&]() { return extract_mesh(e, *params, info); });
+}
+
+int i3d_download_mesh(I3DEngine* e, float* xyz, uint8_t* rgb, int32_t* faces)
+{
+    if (!e) return 1;
+    if (!e->have_mesh) return fail(e, "i3d_download_mesh: no mesh (call i3d_extract_mesh after the last change of the voxel set)");
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t V = static_cast<size_t>(e->mesh_V), F = static_cast<size_t>(e->mesh_F);
+        if (xyz && V) CK(cudaMemcpyAsync(xyz, e->mesh_vpos, 3 * V * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (rgb && V) CK(cudaMemcpyAsync(rgb, e->mesh_vcol, 3 * V, cudaMemcpyDeviceToHost, st));
+        if (faces && F) CK(cudaMemcpyAsync(faces, e->mesh_faces, F * sizeof(int3), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
         return 0;
     });
 }

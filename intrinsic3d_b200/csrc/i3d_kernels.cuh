@@ -21,13 +21,11 @@
 #include <stdint.h>
 #include <limits.h>
 #include "i3d_math.cuh"
+#include "i3d_grid.cuh"
 #include "../../include/i3d_types.h"
 
 namespace i3d
 {
-
-// neighbour-table slots
-enum { NB_XP = 0, NB_XM, NB_YP, NB_YM, NB_ZP, NB_ZM, NB_X2, NB_Y2, NB_Z2, NB_XY, NB_XZ, NB_YZ, NB_COUNT };
 
 // voxel flags
 enum : uint8_t { FL_VALID = 1, FL_ACTIVE = 2, FL_RING = 4, FL_FREE_SDF = 8, FL_FREE_ALB = 16, FL_ES_JAC = 32, FL_ROW = 64 /* active and owned by this rank */ };
@@ -71,8 +69,6 @@ struct Shard
         return (j & 3) == 0;
     }
 };
-
-constexpr int kThreads = 256;
 
 // Programmatic dependent launch (sm_90+): the host launches every kernel of the Gauss-Newton iteration with
 // cudaLaunchAttributeProgrammaticStreamSerialization (pdl_launch, i3d_engine.cu).  griddepcontrol.wait blocks until the preceding
@@ -228,17 +224,6 @@ __device__ __forceinline__ int fk_select(const int (&fk)[I3D_MAX_OBS], int k)
 // ----------------------------------------------------------------------------------------------
 // grid upload: hash table + neighbour table (replaces unordered_map::find, sparse_voxel_grid.cpp:166-259)
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t pack_key(int x, int y, int z)
-{
-    return ((static_cast<uint64_t>(x + (1 << 20)) & 0x1FFFFFull) << 42) | ((static_cast<uint64_t>(y + (1 << 20)) & 0x1FFFFFull) << 21) |
-           (static_cast<uint64_t>(z + (1 << 20)) & 0x1FFFFFull);
-}
-__device__ __forceinline__ uint64_t mix64(uint64_t k)
-{
-    k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
-    return k;
-}
-constexpr unsigned long long kEmptyKey = 0xFFFFFFFFFFFFFFFFull;
 
 __global__ void k_deinterleave_xyz(int64_t n, const int32_t* __restrict__ xyz, int32_t* __restrict__ x, int32_t* __restrict__ y, int32_t* __restrict__ z,
                                    const uint8_t* __restrict__ rgb3, uchar4* __restrict__ rgb4)
@@ -265,20 +250,6 @@ __global__ void k_hash_insert(int64_t n, const int32_t* __restrict__ x, const in
     }
 }
 
-// (noinline: runs once per grid upload; keeps the 12 probe loops out of the caller)
-__device__ __noinline__ int32_t hash_find(const unsigned long long* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask, int x, int y, int z)
-{
-    const unsigned long long key = pack_key(x, y, z);
-    uint64_t slot = mix64(key) & mask;
-    while (true)
-    {
-        const unsigned long long k = keys[slot];
-        if (k == key) return vals[slot];
-        if (k == kEmptyKey) return -1;
-        slot = (slot + 1) & mask;
-    }
-}
-
 __global__ void k_build_nbr(int64_t n, const int32_t* __restrict__ x, const int32_t* __restrict__ y, const int32_t* __restrict__ z,
                             const unsigned long long* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask, int32_t* __restrict__ nbr)
 {
@@ -297,14 +268,6 @@ __global__ void k_transpose_sh(int64_t n, const double* __restrict__ sh_aos, dou
     const int64_t v = i / 9; const int k = static_cast<int>(i - 9 * v);
     sh_soa[static_cast<int64_t>(k) * n + v] = sh_aos[i];
 }
-
-// ----------------------------------------------------------------------------------------------
-// exact float arithmetic (no FMA contraction): must round like oracle.cpp / the reference's float code
-// ----------------------------------------------------------------------------------------------
-#define FM(a, b) __fmul_rn((a), (b))
-#define FA(a, b) __fadd_rn((a), (b))
-#define FS(a, b) __fsub_rn((a), (b))
-#define FD(a, b) __fdiv_rn((a), (b))
 
 // SDFOperators::computeSurfaceNormal (src/sdf/operators.cpp:58-77): float forward differences.
 __device__ __forceinline__ bool surface_normal_f(const GridView& g, int64_t v, float nrm[3])

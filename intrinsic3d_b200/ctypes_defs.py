@@ -184,3 +184,26 @@ class I3DFusionCamera(C.Structure, _Dictable):
         ("cx", C.c_float),
         ("cy", C.c_float),
     ]
+
+
+class I3DMeshParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("sdf_source", C.c_int32),
+        ("largest_component_only", C.c_int32),
+    ]
+
+
+class I3DMeshInfo(C.Structure, _Dictable):
+    _fields_ = [
+        ("num_cubes", C.c_int64),
+        ("num_faces_raw", C.c_int64),
+        ("num_vertices_welded", C.c_int64),
+        ("num_faces_clean", C.c_int64),
+        ("num_faces", C.c_int64),
+        ("num_vertices", C.c_int64),
+        ("ms_classify", C.c_double),
+        ("ms_emit", C.c_double),
+        ("ms_weld", C.c_double),
+        ("ms_clean", C.c_double),
+        ("ms_components", C.c_double),
+    ]

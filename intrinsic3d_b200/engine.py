@@ -11,7 +11,8 @@ import os
 
 import numpy as np
 
-from .ctypes_defs import I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DParams
+from .ctypes_defs import (I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo, I3DMeshParams,
+                          I3DParams)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("I3D_LIB", os.path.join(_HERE, "libi3d_b200.so"))   # I3D_LIB: A/B builds of the same library
@@ -28,6 +29,7 @@ EXPORTED_SYMBOLS = [
     "i3d_num_voxels", "i3d_clear_voxels_outside_thin_shell", "i3d_upsample_grid", "i3d_download_grid",
     "i3d_sizeof_fusion_params", "i3d_default_fusion_params", "i3d_fusion_begin", "i3d_fusion_integrate", "i3d_fusion_finish",
     "i3d_keyframe_scores", "i3d_upload_rgbd_frames", "i3d_use_rgbd_level",
+    "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
     "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_normal_equations",
@@ -71,6 +73,9 @@ def load_library():
         raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (lighting structs)")
     if L.i3d_sizeof_fusion_params() != C.sizeof(I3DFusionParams):
         raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (fusion params)")
+    L.i3d_sizeof_mesh_info.restype = C.c_uint64
+    if L.i3d_sizeof_mesh_info() != C.sizeof(I3DMeshInfo):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (mesh info)")
     _LIB = L
     return L
 
@@ -273,6 +278,25 @@ class Engine:
         out = dict(xyz=np.empty((n, 3), np.int32), sdf=np.empty(n, np.float32), weight=np.empty(n, np.float32), rgb=np.empty((n, 3), np.uint8))
         self._check(self.L.i3d_debug_get_fusion_volume(self.h, _p(out["xyz"], C.c_int32), _p(out["sdf"], C.c_float), _p(out["weight"], C.c_float),
                                                        _p(out["rgb"], C.c_uint8)))
+        return out
+
+    # ---- surface extraction (MarchingCubes::extractSurface + MeshUtil) ------------------------------------------------------
+    MESH_SOURCES = {"fused": 0, "refined": 1}
+
+    def extract_mesh(self, source: str = "refined", largest_component_only: bool = False):
+        """The grid's zero level set as a coloured triangle mesh, extracted on the device: source "fused" meshes sdf0 (as AppFusion does),
+        "refined" the refined sdf (as AppIntrinsic3D::onSDFRefined does); colours are the voxel colours.  largest_component_only keeps
+        the face-connected component with the most faces (output_mesh_largest_comp_only).  Returns a dict with vertices float32 [V, 3]
+        (metres), colors uint8 [V, 3], faces int32 [F, 3] and info (I3DMeshInfo: counts per stage, device ms per stage).  Write it
+        with mesh.save_ply."""
+        if source not in self.MESH_SOURCES:
+            raise ValueError(f"extract_mesh: source must be one of {sorted(self.MESH_SOURCES)}, got {source!r}")
+        prm = I3DMeshParams(self.MESH_SOURCES[source], 1 if largest_component_only else 0)
+        info = I3DMeshInfo()
+        self._check(self.L.i3d_extract_mesh(self.h, C.byref(prm), C.byref(info)))
+        V, F = int(info.num_vertices), int(info.num_faces)
+        out = dict(vertices=np.empty((V, 3), np.float32), colors=np.empty((V, 3), np.uint8), faces=np.empty((F, 3), np.int32), info=info)
+        self._check(self.L.i3d_download_mesh(self.h, _p(out["vertices"], C.c_float), _p(out["colors"], C.c_uint8), _p(out["faces"], C.c_int32)))
         return out
 
     # ---- keyframe selection and the RGB-D pyramid (KeyframeSelection::estimateBlur, Pyramid::create) ----------------------
