@@ -5,6 +5,8 @@
 
 Runs, each the median of --reps calls after one warm-up call: both sdf sources with and without the component filter on the workload's
 grid (C3: 2 M voxels), then the refined source with and without the filter on the grid after one i3d_upsample_grid (C3: 16 M voxels).
+On both grids, after a lighting estimate, the refined mesh coloured by the "albedo" and "shading_sv" modes, with the device time of the
+colour pass (phase "mesh_colorize") beside the stage times, its share of the extraction's device time and its byte model.
 Reported per run: the counts of every stage, device ms per stage (CUDA events inside the library), wall ms of Engine.extract_mesh
 (extraction + download into numpy), and the byte models of the two per-voxel kernels over their device time as a share of the HBM peak
 (MEASURED_PEAKS.json hbm_gbs if present, else the H100 SXM data sheet's 3350 GB/s):
@@ -26,6 +28,10 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 STAGES = ("ms_classify", "ms_emit", "ms_weld", "ms_clean", "ms_components")
+# bytes per voxel of the colour pass: albedo reads the albedo (8 B) and writes a colour (4 B); shading_sv reads the weights of the voxel
+# and its +x/+y/+z neighbours (16 B), the 3 neighbour slots (12 B), 4 sdf values (32 B), the albedo (8 B) and the coordinates (12 B) and
+# writes 4 B (the subvolume SH, a few kB, stay in cache)
+COLORIZE_BYTES = {"albedo": 12, "shading_sv": 84}
 COUNTS = ("num_cubes", "num_faces_raw", "num_vertices_welded", "num_faces_clean", "num_faces", "num_vertices")
 
 
@@ -37,14 +43,15 @@ def gpu_info():
         return None
 
 
-def run(e, source, lc, reps, peak_gbs):
-    e.extract_mesh(source, lc)
-    walls, infos, digest = [], [], None
+def run(e, source, lc, reps, peak_gbs, mode=""):
+    e.extract_mesh(source, lc, mode)
+    walls, infos, colorize, digest = [], [], [], None
     for _ in range(reps):
         t0 = time.perf_counter()
-        m = e.extract_mesh(source, lc)
+        m = e.extract_mesh(source, lc, mode)
         walls.append(1e3 * (time.perf_counter() - t0))
         infos.append(m["info"])
+        colorize.append(e.phase_ms("mesh_colorize") if mode else 0.0)
         d = hash(m["vertices"].tobytes() + m["colors"].tobytes() + m["faces"].tobytes())
         assert digest is None or d == digest, "extraction not run-to-run identical"
         digest = d
@@ -54,10 +61,26 @@ def run(e, source, lc, reps, peak_gbs):
     cls_bytes, emit_bytes = n * (28 + 12 + 4 + 8 + 1 + 4 + 16), n * 4 + M * 27
     cls_gbs = cls_bytes / (dev["ms_classify"] * 1e-3) / 1e9
     emit_gbs = emit_bytes / (dev["ms_emit"] * 1e-3) / 1e9 if dev["ms_emit"] > 0 else 0.0
-    return {"source": source, "largest_component_only": bool(lc), "voxels": int(n), **{k: int(getattr(info, k)) for k in COUNTS},
-            "device_ms": {**dev, "total": float(sum(dev.values()))}, "wall_ms": float(np.median(walls)),
+    out = {"source": source, "largest_component_only": bool(lc), "color_mode": mode, "voxels": int(n), **{k: int(getattr(info, k)) for k in COUNTS},
+           "device_ms": {**dev, "total": float(sum(dev.values()))}, "wall_ms": float(np.median(walls)),
             "classify": {"bytes_model": cls_bytes, "gbs": cls_gbs, "share_of_peak": cls_gbs / peak_gbs},
             "emit": {"bytes_model": emit_bytes, "gbs": emit_gbs, "share_of_peak": emit_gbs / peak_gbs}}
+    if mode:
+        col_ms = float(np.median(colorize))
+        col_bytes = n * COLORIZE_BYTES[mode]
+        col_gbs = col_bytes / (col_ms * 1e-3) / 1e9
+        out["colorize"] = {"device_ms": col_ms, "share_of_extraction": col_ms / out["device_ms"]["total"], "bytes_model": col_bytes,
+                           "gbs": col_gbs, "share_of_peak": col_gbs / peak_gbs}
+    return out
+
+
+def light(e, scene):
+    """a lighting estimate of the current grid (0.2 m subvolumes, as data/intrinsic3d.yml), which the shading modes blend"""
+    from intrinsic3d_b200 import engine
+    lp = engine.default_lighting_params()
+    lp.thres_shell = scene["thres_shell"]
+    lp.subvolume_size = 0.2
+    e.estimate_lighting(lp)
 
 
 def main():
@@ -82,8 +105,12 @@ def main():
     e.load_scene(scene)
     reps = max(1, args.reps)
     runs = [run(e, src, lc, reps, peak_gbs) for src in ("fused", "refined") for lc in (False, True)]
+    light(e, scene)
+    runs += [run(e, "refined", False, reps, peak_gbs, mode) for mode in ("albedo", "shading_sv")]
     e.upsample_grid()
     runs += [run(e, "refined", lc, reps, peak_gbs) for lc in (False, True)]
+    light(e, scene)
+    runs += [run(e, "refined", False, reps, peak_gbs, mode) for mode in ("albedo", "shading_sv")]
     line = {"metric": "mesh_refined_wall_ms", "value": runs[2]["wall_ms"], "unit": "ms", "higher_is_better": False, "workload": args.workload,
             "gpu": gpu, "reps": reps, "runs": runs, "peak_gbs": peak_gbs, "peak_source": peak_src}
     print(json.dumps(line))

@@ -190,6 +190,17 @@ uint64_t    i3d_sizeof_mesh_info(void);
  * Reads the grid only: state, camera, lighting, frames and the last iteration are unchanged.  A change of the voxel set (upload,
  * prune, upsample, fusion) drops the resident mesh.  Fails without a grid and for an sdf_source other than 0 or 1. */
 int         i3d_extract_mesh(I3DEngine* e, const I3DMeshParams* params, I3DMeshInfo* info);
+/* i3d_extract_mesh with the mesh coloured by a colour mode of SDFVisualization::colorize (src/sdf/visualization.cpp:101-164; color_mode:
+ * I3D_MESH_COLOR_*).  I3D_MESH_COLOR_VOXEL is i3d_extract_mesh itself; any other mode first computes every voxel's colour in that mode on
+ * the device (the geometric modes from the sdf the mesh is cut from) and extracts with those colours.  The shading modes blend the
+ * subvolume SH of the last i3d_estimate_lighting.  The mesh replaces the resident mesh that i3d_download_mesh reads; the device time
+ * of the colour pass is i3d_phase_ms("mesh_colorize").  The voxel colours and every other engine state are left alone.  Fails, as
+ * i3d_extract_mesh does, without a grid or for a bad sdf_source, and for a bad color_mode or a shading mode without a lighting estimate
+ * of the current voxel set (the per-voxel SH of i3d_set_sh is not one). */
+int         i3d_extract_mesh_colored(I3DEngine* e, const I3DMeshParams* params, int32_t color_mode, I3DMeshInfo* info);
+/* The colours of every voxel in a colour mode: rgb uint8 [n][3], in the grid's order; sdf_source as in I3DMeshParams.  Mode
+ * I3D_MESH_COLOR_VOXEL gives the voxel colours.  Writes no engine state; fails as i3d_extract_mesh_colored does. */
+int         i3d_mode_colors(I3DEngine* e, int32_t sdf_source, int32_t color_mode, uint8_t* rgb);
 /* The resident mesh: xyz float [V][3] metres, rgb uint8 [V][3], faces int32 [F][3] (V, F: info->num_vertices / num_faces).  Any
  * pointer may be NULL.  Fails when no mesh of the current grid has been extracted. */
 int         i3d_download_mesh(I3DEngine* e, float* xyz, uint8_t* rgb, int32_t* faces);

@@ -186,6 +186,23 @@ typedef struct I3DMeshInfo
                                                                            segments, the host read-backs of counts excluded */
 } I3DMeshInfo;
 
+/* Colour modes of a mesh (SDFVisualization::colorize, src/sdf/visualization.cpp:101-416; mode strings "", "normals", "lap", "lum",
+ * "lum_grad", "albedo", "shading_sv", "shading_sv_const", "chroma").  VOXEL is the voxel colours; the others are computed per voxel from
+ * the voxel and its ±1 ring (DESIGN.md §6k).  The reference's subvolume modes ("subvol", "subvol_interp") have no number. */
+enum
+{
+    I3D_MESH_COLOR_VOXEL = 0,
+    I3D_MESH_COLOR_NORMALS,
+    I3D_MESH_COLOR_LAPLACIAN,
+    I3D_MESH_COLOR_INTENSITY,
+    I3D_MESH_COLOR_INTENSITY_GRAD,
+    I3D_MESH_COLOR_ALBEDO,
+    I3D_MESH_COLOR_SHADING_SV,
+    I3D_MESH_COLOR_SHADING_SV_CONST,
+    I3D_MESH_COLOR_CHROMACITY,
+    I3D_MESH_COLOR_COUNT
+};
+
 #ifdef __cplusplus
 }
 #endif

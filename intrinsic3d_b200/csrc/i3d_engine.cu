@@ -192,6 +192,7 @@ struct I3DEngine
     Dev<uint8_t> sh_has;
     int sv_S = 0;
     double* sv_x = nullptr;            // [S][9] subvolume SH of the last estimate (inside sv_work)
+    SubvolGrid sv_grid{};              // the subvolume table of the last estimate (sv_table), valid while sv_S > 0
     // RGB-D fusion in progress (i3d_fusion.cuh): own hash table and Voxel arrays, one entry per hash slot
     bool fu_active = false;
     I3DFusionParams fu_p{};
@@ -218,6 +219,7 @@ struct I3DEngine
     Dev<int3> ms_faces, ms_faces2; Dev<unsigned> ms_ccount, ms_cminf;
     cudaEvent_t ms_ev[16] = {};        // begin / end of up to 8 device-only segments of one extraction (MeshSegments)
     bool ms_ev_ready = false;
+    Dev<uchar4> vis_rgb;               // per-voxel colours of the last colour pass (i3d_vis.cuh): scratch that only grows
     // shard (multi-GPU)
     int64_t shard_begin = 0, shard_end = -1;
     int rank = 0, world = 1;
@@ -1097,17 +1099,45 @@ T read_back(I3DEngine* e, const T* d)
     return h;
 }
 
+// The checks shared by the calls that take a colour mode (the grid, the sdf source and the mode are checked by the caller): a shading
+// mode needs the subvolume SH of a lighting estimate of the current voxel set.
+int check_color_mode(I3DEngine* e, const char* who, int32_t mode)
+{
+    if (mode < I3D_MESH_COLOR_VOXEL || mode >= I3D_MESH_COLOR_COUNT)
+        return fail(e, "%s: color_mode must be in [0, %d], got %d", who, I3D_MESH_COLOR_COUNT - 1, mode);
+    if ((mode == I3D_MESH_COLOR_SHADING_SV || mode == I3D_MESH_COLOR_SHADING_SV_CONST) && (e->sv_S <= 0 || !e->sv_x))
+        return fail(e, "%s: the shading modes need a lighting estimate of the current grid (i3d_estimate_lighting)", who);
+    return 0;
+}
+
+// The colour pass (i3d_vis.cuh) of a mode other than I3D_MESH_COLOR_VOXEL into e->vis_rgb, timed as phase "mesh_colorize".  The
+// geometric modes read the sdf the mesh is cut from.  Writes nothing but e->vis_rgb.
+void colorize(I3DEngine* e, int32_t sdf_source, int32_t mode)
+{
+    e->timed.clear(); e->ev_used = 0; e->phases.erase("mesh_colorize");
+    e->vis_rgb.ensure(static_cast<size_t>(e->n));
+    {
+        Timer t(e, "mesh_colorize", 0);
+        mesh::colorize(e->grid_view(sdf_source == 0 ? e->sdf0.p : e->sdf, e->alb), e->sv_grid, e->sv_x, e->sv_S, mode, e->vis_rgb.p, e->stream);
+    }
+    collect_kernel_times(e);
+    CK(cudaGetLastError());
+}
+
 // Marching cubes over the resident grid, welding, degenerate-face removal and (optionally) the largest component.  Every count is
-// read back before the buffers of the next stage are sized.  Reads the grid; writes only the ms_* scratch and the resident mesh.
-int extract_mesh(I3DEngine* e, const I3DMeshParams& prm, I3DMeshInfo* info)
+// read back before the buffers of the next stage are sized.  Reads the grid; writes only the ms_* scratch and the resident mesh (and,
+// for a colour mode other than the voxel colours, e->vis_rgb, which then colours the mesh).
+int extract_mesh(I3DEngine* e, const I3DMeshParams& prm, int32_t color_mode, I3DMeshInfo* info)
 {
     cudaStream_t st = e->stream;
     const int64_t n = e->n;
     e->have_mesh = false;
     if (!e->ms_ev_ready) { for (auto& ev : e->ms_ev) CK(cudaEventCreate(&ev)); e->ms_ev_ready = true; }
+    if (color_mode != I3D_MESH_COLOR_VOXEL) colorize(e, prm.sdf_source, color_mode);
     I3DMeshInfo inf{};
     MeshGrid g;
-    g.n = n; g.x = e->x.p; g.y = e->y.p; g.z = e->z.p; g.sdf = prm.sdf_source == 0 ? e->sdf0.p : e->sdf; g.weight = e->weight.p; g.rgb = e->rgb.p;
+    g.n = n; g.x = e->x.p; g.y = e->y.p; g.z = e->z.p; g.sdf = prm.sdf_source == 0 ? e->sdf0.p : e->sdf; g.weight = e->weight.p;
+    g.rgb = color_mode == I3D_MESH_COLOR_VOXEL ? e->rgb.p : e->vis_rgb.p;
     g.nbr = e->nbr.p; g.keys = e->up_keys.p; g.vals = e->up_vals.p; g.mask = e->hash_cap - 1; g.voxel_size = e->voxel_size;
 
     enum { CLASSIFY, EMIT, WELD, CLEAN, COMPONENTS };
@@ -1467,6 +1497,7 @@ int i3d_estimate_lighting(I3DEngine* e, const I3DLightingParams* params, I3DLigh
             CK(cudaGetLastError());
             if (S <= 0) return fail(e, "i3d_estimate_lighting: no subvolumes");
             e->sv_S = S;
+            e->sv_grid = sg;
             e->sv_index.ensure(3 * static_cast<size_t>(S)); e->sv_nbr.ensure(6 * static_cast<size_t>(S)); e->sv_deg.ensure(static_cast<size_t>(S));
             k_svsh_indices<<<blocks_for(static_cast<size_t>(cells)), kThreads, 0, st>>>(sg, e->sv_index.p, e->sv_nbr.p, S);
         }
@@ -1901,7 +1932,37 @@ int i3d_extract_mesh(I3DEngine* e, const I3DMeshParams* params, I3DMeshInfo* inf
     if (!params) return fail(e, "i3d_extract_mesh: params is NULL");
     if (e->n <= 0) return fail(e, "i3d_extract_mesh: no grid");
     if (params->sdf_source != 0 && params->sdf_source != 1) return fail(e, "i3d_extract_mesh: sdf_source must be 0 (sdf0) or 1 (sdf_refined), got %d", params->sdf_source);
-    return guarded(e, [&]() { return extract_mesh(e, *params, info); });
+    return guarded(e, [&]() { return extract_mesh(e, *params, I3D_MESH_COLOR_VOXEL, info); });
+}
+
+int i3d_extract_mesh_colored(I3DEngine* e, const I3DMeshParams* params, int32_t color_mode, I3DMeshInfo* info)
+{
+    if (!e) return 1;
+    if (!params) return fail(e, "i3d_extract_mesh_colored: params is NULL");
+    if (e->n <= 0) return fail(e, "i3d_extract_mesh_colored: no grid");
+    if (params->sdf_source != 0 && params->sdf_source != 1)
+        return fail(e, "i3d_extract_mesh_colored: sdf_source must be 0 (sdf0) or 1 (sdf_refined), got %d", params->sdf_source);
+    if (check_color_mode(e, "i3d_extract_mesh_colored", color_mode)) return 1;
+    return guarded(e, [&]() { return extract_mesh(e, *params, color_mode, info); });
+}
+
+int i3d_mode_colors(I3DEngine* e, int32_t sdf_source, int32_t color_mode, uint8_t* rgb)
+{
+    if (!e) return 1;
+    if (e->n <= 0) return fail(e, "i3d_mode_colors: no grid");
+    if (!rgb) return fail(e, "i3d_mode_colors: rgb is NULL");
+    if (sdf_source != 0 && sdf_source != 1) return fail(e, "i3d_mode_colors: sdf_source must be 0 (sdf0) or 1 (sdf_refined), got %d", sdf_source);
+    if (check_color_mode(e, "i3d_mode_colors", color_mode)) return 1;
+    return guarded(e, [&]() {
+        const uchar4* src = e->rgb.p;
+        if (color_mode != I3D_MESH_COLOR_VOXEL) { colorize(e, sdf_source, color_mode); src = e->vis_rgb.p; }
+        e->up_rgb.ensure(3 * static_cast<size_t>(e->n));
+        k_interleave_rgb<<<blocks_for(e->n), kThreads, 0, e->stream>>>(e->n, src, e->up_rgb.p);
+        CK(cudaMemcpyAsync(rgb, e->up_rgb.p, 3 * static_cast<size_t>(e->n), cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaStreamSynchronize(e->stream));
+        CK(cudaGetLastError());
+        return 0;
+    });
 }
 
 int i3d_download_mesh(I3DEngine* e, float* xyz, uint8_t* rgb, int32_t* faces)

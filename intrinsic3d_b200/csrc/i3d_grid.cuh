@@ -1,7 +1,8 @@
 /*
  * i3d_grid.cuh — what every device module of the engine shares about the grid: the neighbour-table slots, the block size, the device
- * hash (coordinates -> voxel index) and the explicitly rounded float operations.  No kernels: i3d_kernels.cuh (the engine's module)
- * and i3d_mesh.cuh (the surface extraction's module) both include it.
+ * hash (coordinates -> voxel index), the explicitly rounded float operations, the grid view with the per-voxel operators both modules
+ * evaluate (surface normal, intensity) and the subvolume table of the lighting.  No kernels: i3d_kernels.cuh (the engine's module) and
+ * i3d_mesh.cuh / i3d_vis.cuh (the surface extraction's module) both include it.
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -51,5 +52,59 @@ inline __device__ __noinline__ int32_t hash_find(const unsigned long long* __res
         slot = (slot + 1) & mask;
     }
 }
+
+// ----------------------------------------------------------------------------------------------
+// the engine's grid as the per-voxel operators read it
+// ----------------------------------------------------------------------------------------------
+struct GridView
+{
+    int64_t n;
+    const int32_t* x; const int32_t* y; const int32_t* z;
+    const double* sdf0; const double* sdf; const double* albedo;
+    const float* weight;
+    const uchar4* rgb;
+    const int32_t* nbr;    // [12][n]
+    const double* sh;      // [9][n]
+    float voxel_size, truncation;
+};
+
+// SDFOperators::computeSurfaceNormal (src/sdf/operators.cpp:58-77): float forward differences.
+__device__ __forceinline__ bool surface_normal_f(const GridView& g, int64_t v, float nrm[3])
+{
+    nrm[0] = nrm[1] = nrm[2] = 0.0f;
+    const int32_t ix = g.nbr[NB_XP * g.n + v], iy = g.nbr[NB_YP * g.n + v], iz = g.nbr[NB_ZP * g.n + v];
+    if (!(g.weight[v] > 0.0f) || ix < 0 || iy < 0 || iz < 0) return false;
+    if (!(g.weight[ix] > 0.0f) || !(g.weight[iy] > 0.0f) || !(g.weight[iz] > 0.0f)) return false;
+    const float s0 = static_cast<float>(g.sdf[v]);
+    float g0 = FS(static_cast<float>(g.sdf[ix]), s0);
+    float g1 = FS(static_cast<float>(g.sdf[iy]), s0);
+    float g2 = FS(static_cast<float>(g.sdf[iz]), s0);
+    const float sq = FA(FA(FM(g0, g0), FM(g1, g1)), FM(g2, g2));
+    const float len = __fsqrt_rn(sq);
+    if (len != 0.0f) { g0 = FD(g0, len); g1 = FD(g1, len); g2 = FD(g2, len); }
+    nrm[0] = g0; nrm[1] = g1; nrm[2] = g2;
+    return !(g0 == 0.0f && g1 == 0.0f && g2 == 0.0f);
+}
+
+// nv::intensity(unsigned char r, g, b) (src/color_util.cpp:41-46)
+__device__ __forceinline__ float intensity_u8(uchar4 c) { return FA(FA(FM(0.299f, static_cast<float>(c.x)), FM(0.587f, static_cast<float>(c.y))), FM(0.114f, static_cast<float>(c.z))); }
+
+// ----------------------------------------------------------------------------------------------
+// subvolumes of the SVSH lighting (Subvolumes, src/lighting/subvolumes.cpp)
+// ----------------------------------------------------------------------------------------------
+struct SubvolGrid
+{
+    int lo[3];
+    int dim[3];
+    const int32_t* table;    // [dim z][dim y][dim x] -> subvolume id or -1
+    float inv_size;          // 1.0f / size_ (Subvolumes::pointToIndexFloat, src/lighting/subvolumes.cpp:262-265)
+    __host__ __device__ int64_t cells() const { return static_cast<int64_t>(dim[0]) * dim[1] * dim[2]; }
+    __device__ __forceinline__ int find(int x, int y, int z) const
+    {
+        x -= lo[0]; y -= lo[1]; z -= lo[2];
+        if (x < 0 || y < 0 || z < 0 || x >= dim[0] || y >= dim[1] || z >= dim[2]) return -1;
+        return table[(static_cast<int64_t>(z) * dim[1] + y) * dim[0] + x];
+    }
+};
 
 } // namespace i3d

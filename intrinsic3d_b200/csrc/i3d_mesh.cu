@@ -1,8 +1,10 @@
 /*
- * i3d_mesh.cu — the surface-extraction kernels (i3d_mesh.cuh) and their CUB passes, compiled as a translation unit of their own, and
- * the host wrappers of i3d_mesh.h that launch them.  Keeping them out of i3d_engine.cu leaves the engine's device module as it is.
+ * i3d_mesh.cu — the surface-extraction kernels (i3d_mesh.cuh), the colour modes they can take their colours from (i3d_vis.cuh) and
+ * their CUB passes, compiled as a translation unit of their own, and the host wrappers of i3d_mesh.h that launch them.  Keeping them
+ * out of i3d_engine.cu leaves the engine's device module as it is.
  */
 #include "i3d_mesh.cuh"
+#include "i3d_vis.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -18,6 +20,22 @@ struct AddI64 { __device__ __forceinline__ int64_t operator()(int64_t a, int64_t
 struct MaxI32 { __device__ __forceinline__ int32_t operator()(int32_t a, int32_t b) const { return a > b ? a : b; } };
 inline unsigned blocks(int64_t n) { return static_cast<unsigned>((n + kThreads - 1) / kThreads); }
 } // namespace
+
+void colorize(const GridView& g, const SubvolGrid& sg, const double* sub_sh, int S, int mode, uchar4* out, cudaStream_t st)
+{
+    switch (mode)
+    {
+    case I3D_MESH_COLOR_NORMALS: k_vis_colors<I3D_MESH_COLOR_NORMALS><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+    case I3D_MESH_COLOR_LAPLACIAN: k_vis_colors<I3D_MESH_COLOR_LAPLACIAN><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+    case I3D_MESH_COLOR_INTENSITY: k_vis_colors<I3D_MESH_COLOR_INTENSITY><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+    case I3D_MESH_COLOR_INTENSITY_GRAD: k_vis_colors<I3D_MESH_COLOR_INTENSITY_GRAD><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+    case I3D_MESH_COLOR_ALBEDO: k_vis_colors<I3D_MESH_COLOR_ALBEDO><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+    case I3D_MESH_COLOR_SHADING_SV: k_vis_colors<I3D_MESH_COLOR_SHADING_SV><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+    case I3D_MESH_COLOR_SHADING_SV_CONST: k_vis_colors<I3D_MESH_COLOR_SHADING_SV_CONST><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+    case I3D_MESH_COLOR_CHROMACITY: k_vis_colors<I3D_MESH_COLOR_CHROMACITY><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+    default: break;     // the engine validates the mode before it calls
+    }
+}
 
 void classify(const MeshGrid& g, uint8_t* cube_case, int32_t* tri_count, unsigned long long* num_cubes, cudaStream_t st)
 {

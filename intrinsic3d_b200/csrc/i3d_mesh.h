@@ -9,6 +9,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "i3d_grid.cuh"
+
 namespace i3d
 {
 
@@ -36,6 +38,9 @@ struct MeshCorners
 
 namespace mesh
 {
+// 0. the per-voxel colours of a colour mode (i3d_vis.cuh; mode 1 .. I3D_MESH_COLOR_COUNT - 1) into out [n]; g.sdf is the sdf the mesh is
+// cut from, sg / sub_sh [S][9] the subvolumes and subvolume SH of the last lighting estimate (read by the shading modes only)
+void colorize(const GridView& g, const SubvolGrid& sg, const double* sub_sh, int S, int mode, uchar4* out, cudaStream_t st);
 // 1. cube cases, triangle counts, used-cube count; face offsets (int64 exclusive scan of the counts)
 void classify(const MeshGrid& g, uint8_t* cube_case, int32_t* tri_count, unsigned long long* num_cubes, cudaStream_t st);
 cudaError_t face_offsets(void* tmp, size_t& bytes, const int32_t* tri_count, int64_t* face_off, int n, cudaStream_t st);

@@ -29,13 +29,15 @@ EXPORTED_SYMBOLS = [
     "i3d_num_voxels", "i3d_clear_voxels_outside_thin_shell", "i3d_upsample_grid", "i3d_download_grid",
     "i3d_sizeof_fusion_params", "i3d_default_fusion_params", "i3d_fusion_begin", "i3d_fusion_integrate", "i3d_fusion_finish",
     "i3d_keyframe_scores", "i3d_upload_rgbd_frames", "i3d_use_rgbd_level",
-    "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh",
+    "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh", "i3d_extract_mesh_colored", "i3d_mode_colors",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
     "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_normal_equations",
     "i3d_debug_apply_operator", "i3d_debug_fusion_num_voxels", "i3d_debug_get_fusion_volume", "i3d_debug_get_frames",
 ]
 KEYFRAME_CHUNK = 32       # I3D_KEYFRAME_CHUNK of include/i3d_c_api.h: frames scored per device pass
+# SDFVisualization's colour mode strings -> I3D_MESH_COLOR_* of include/i3d_types.h
+COLOR_MODES = {"": 0, "normals": 1, "lap": 2, "lum": 3, "lum_grad": 4, "albedo": 5, "shading_sv": 6, "shading_sv_const": 7, "chroma": 8}
 
 
 def load_library():
@@ -76,6 +78,10 @@ def load_library():
     L.i3d_sizeof_mesh_info.restype = C.c_uint64
     if L.i3d_sizeof_mesh_info() != C.sizeof(I3DMeshInfo):
         raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (mesh info)")
+    L.i3d_extract_mesh_colored.restype = C.c_int
+    L.i3d_extract_mesh_colored.argtypes = [C.c_void_p, C.POINTER(I3DMeshParams), C.c_int32, C.POINTER(I3DMeshInfo)]
+    L.i3d_mode_colors.restype = C.c_int
+    L.i3d_mode_colors.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_uint8)]
     _LIB = L
     return L
 
@@ -283,21 +289,47 @@ class Engine:
     # ---- surface extraction (MarchingCubes::extractSurface + MeshUtil) ------------------------------------------------------
     MESH_SOURCES = {"fused": 0, "refined": 1}
 
-    def extract_mesh(self, source: str = "refined", largest_component_only: bool = False):
-        """The grid's zero level set as a coloured triangle mesh, extracted on the device: source "fused" meshes sdf0 (as AppFusion does),
-        "refined" the refined sdf (as AppIntrinsic3D::onSDFRefined does); colours are the voxel colours.  largest_component_only keeps
-        the face-connected component with the most faces (output_mesh_largest_comp_only).  Returns a dict with vertices float32 [V, 3]
-        (metres), colors uint8 [V, 3], faces int32 [F, 3] and info (I3DMeshInfo: counts per stage, device ms per stage).  Write it
-        with mesh.save_ply."""
+    def _mesh_source(self, source):
         if source not in self.MESH_SOURCES:
-            raise ValueError(f"extract_mesh: source must be one of {sorted(self.MESH_SOURCES)}, got {source!r}")
-        prm = I3DMeshParams(self.MESH_SOURCES[source], 1 if largest_component_only else 0)
+            raise ValueError(f"source must be one of {sorted(self.MESH_SOURCES)}, got {source!r}")
+        return self.MESH_SOURCES[source]
+
+    @staticmethod
+    def _color_mode(mode):
+        if mode not in COLOR_MODES:
+            raise ValueError(f"colour mode must be one of {sorted(COLOR_MODES)} (the subvolume modes are not supported), got {mode!r}")
+        return COLOR_MODES[mode]
+
+    def extract_mesh(self, source: str = "refined", largest_component_only: bool = False, color_mode: str = ""):
+        """The grid's zero level set as a coloured triangle mesh, extracted on the device: source "fused" meshes sdf0 (as AppFusion does),
+        "refined" the refined sdf (as AppIntrinsic3D::onSDFRefined does).  color_mode is a mode string of SDFVisualization::colorize:
+        "" (the voxel colours), "normals", "lap", "lum", "lum_grad", "albedo", "shading_sv", "shading_sv_const" or "chroma"; the shading
+        modes need a lighting estimate of the current grid (estimate_lighting).  largest_component_only keeps the face-connected
+        component with the most faces (output_mesh_largest_comp_only).  Returns a dict with vertices float32 [V, 3] (metres), colors
+        uint8 [V, 3], faces int32 [F, 3] and info (I3DMeshInfo: counts per stage, device ms per stage; the colour pass is
+        phase_ms("mesh_colorize")).  Write it with mesh.save_ply."""
+        src = self._mesh_source(source)
+        mode = self._color_mode(color_mode)
+        prm = I3DMeshParams(src, 1 if largest_component_only else 0)
         info = I3DMeshInfo()
-        self._check(self.L.i3d_extract_mesh(self.h, C.byref(prm), C.byref(info)))
+        if mode == 0:
+            self._check(self.L.i3d_extract_mesh(self.h, C.byref(prm), C.byref(info)))
+        else:
+            self._check(self.L.i3d_extract_mesh_colored(self.h, C.byref(prm), mode, C.byref(info)))
         V, F = int(info.num_vertices), int(info.num_faces)
         out = dict(vertices=np.empty((V, 3), np.float32), colors=np.empty((V, 3), np.uint8), faces=np.empty((F, 3), np.int32), info=info)
         self._check(self.L.i3d_download_mesh(self.h, _p(out["vertices"], C.c_float), _p(out["colors"], C.c_uint8), _p(out["faces"], C.c_int32)))
         return out
+
+    def mode_colors(self, mode: str, source: str = "refined"):
+        """Every voxel's colour in colour mode `mode` (a mode string of extract_mesh), uint8 [n, 3] in the grid's order: the colours a
+        mesh of that mode interpolates.  The geometric modes read the sdf of `source`."""
+        src = self._mesh_source(source)
+        m = self._color_mode(mode)
+        n = int(self.L.i3d_num_voxels(self.h))
+        rgb = np.empty((n, 3), np.uint8)
+        self._check(self.L.i3d_mode_colors(self.h, src, m, _p(rgb, C.c_uint8)))
+        return rgb
 
     # ---- keyframe selection and the RGB-D pyramid (KeyframeSelection::estimateBlur, Pyramid::create) ----------------------
     def keyframe_scores(self, bgr):

@@ -36,3 +36,58 @@ def save_ply(path, mesh) -> None:
     data = ply_bytes(mesh)
     with open(path, "wb") as fh:
         fh.write(data)
+
+
+# SDFVisualization::getOutputModes (src/sdf/visualization.cpp:72-89): settings key -> colour mode, in this order
+OUTPUT_MODE_KEYS = (
+    ("output_mesh_normals", "normals"),
+    ("output_mesh_laplacian", "lap"),
+    ("output_mesh_intensity", "lum"),
+    ("output_mesh_intensity_grad", "lum_grad"),
+    ("output_mesh_albedo", "albedo"),
+    ("output_mesh_shading_sv", "shading_sv"),
+    ("output_mesh_shading_sv_const", "shading_sv_const"),
+    ("output_mesh_chromacity", "chroma"),
+    ("output_mesh_subvolumes", "subvol"),
+    ("output_mesh_subvolumes_interpolated", "subvol_interp"),
+)
+
+
+def _setting_true(v) -> bool:
+    """Settings::get<bool>: the yml stores "0" / "1", read with operator>>; only 1 is true."""
+    if isinstance(v, bool):
+        return v
+    try:
+        return int(str(v).strip()) == 1
+    except ValueError:
+        return False
+
+
+def output_modes(settings, add_voxel_colors: bool = True):
+    """The colour modes of the meshes to write, as SDFVisualization::getOutputModes lists them: "" (the voxel colours) first when
+    add_voxel_colors, then each mode whose key is present in `settings` (a mapping such as the loaded data/intrinsic3d.yml) and true.
+    May include the subvolume modes "subvol" / "subvol_interp", which export_meshes refuses."""
+    modes = [""] if add_voxel_colors else []
+    modes += [mode for key, mode in OUTPUT_MODE_KEYS if key in settings and _setting_true(settings[key])]
+    return modes
+
+
+def mesh_file(prefix: str, mode: str) -> str:
+    """SDFVisualization::exportMesh's file name: prefix, "_" + mode unless the mode is "", ".ply"."""
+    return prefix + ("_" + mode if mode else "") + ".ply"
+
+
+def export_meshes(engine, prefix: str, modes, largest_component_only: bool = False, source: str = "refined"):
+    """SDFVisualization::colorize + exportMesh for every mode in `modes`: extracts the mesh of the engine's grid coloured in that mode on
+    the device and writes it to mesh_file(prefix, mode).  Returns the paths written.  Every mode is checked before anything is extracted:
+    the subvolume modes are refused (the reference colours subvolumes with random colours, so there is nothing reproducible to write)."""
+    from .engine import COLOR_MODES
+    bad = [m for m in modes if m not in COLOR_MODES]
+    if bad:
+        raise ValueError(f"export_meshes: unsupported colour modes {bad} (supported: {sorted(COLOR_MODES)})")
+    paths = []
+    for mode in modes:
+        path = mesh_file(prefix, mode)
+        save_ply(path, engine.extract_mesh(source, largest_component_only, mode))
+        paths.append(path)
+    return paths
