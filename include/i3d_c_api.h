@@ -223,6 +223,33 @@ int         i3d_upload_rgbd_frames(I3DEngine* e, int32_t F, int32_t W, int32_t H
  * level's size.  Fails without a store, for lvl < 0, and when a level on the way is under 3 px on an axis.
  * Device time of the last call: i3d_phase_ms("frames_level"). */
 int         i3d_use_rgbd_level(I3DEngine* e, int32_t lvl, int32_t* W_out, int32_t* H_out);
+
+/* ---- the sensor store: the raw RGB-D sequence on the device, uploaded once (DESIGN.md §6l) ---- */
+/* Starts an empty store of `capacity` frames (Sensor::depth(i) / Sensor::color(i)) and allocates its device memory for all of them:
+ * depth float metres [depth_cam.height][depth_cam.width], already range-thresholded as i3d_fusion_integrate takes it, and colour uint8
+ * [color_cam.height][color_cam.width][3] interleaved B,G,R.  Replaces any previous store; the frame store of i3d_upload_rgbd_frames is a
+ * separate one and is left alone.  Fails for a camera without a positive size, finite intrinsics and fx, fy > 0, and for capacity <= 0. */
+int         i3d_sensor_frames_begin(I3DEngine* e, const I3DFusionCamera* depth_cam, const I3DFusionCamera* color_cam, int32_t capacity);
+/* Appends F frames (ids i3d_sensor_num_frames(), +1, ...): depth [F][...] and bgr [F][...] in the layouts above.  Fails without a store,
+ * for F <= 0 and beyond the capacity. */
+int         i3d_sensor_frames_add(I3DEngine* e, int32_t F, const float* depth, const uint8_t* bgr);
+/* Frames in the store (0 without one). */
+int32_t     i3d_sensor_num_frames(const I3DEngine* e);
+/* i3d_keyframe_scores of every stored frame, read from the store: scores[i3d_sensor_num_frames()], byte-equal to i3d_keyframe_scores of
+ * the same frames.  Fails without stored frames and for colour frames under 5 px on an axis.  Device time: i3d_phase_ms("keyframe_scores"). */
+int         i3d_sensor_keyframe_scores(I3DEngine* e, double* scores);
+/* i3d_fusion_integrate of the stored frames ids[0..n), in list order, with the store's two cameras; pose_cam_to_world and
+ * pose_world_to_cam are [n][12] as there.  The store is only read.  Fails, leaving the fusion in progress, without a fusion in progress,
+ * without stored frames, for n <= 0 and for an id out of range; a failure while fusing ends the fusion as i3d_fusion_integrate does. */
+int         i3d_fusion_integrate_sensor(I3DEngine* e, int32_t n, const int32_t* ids, const float* pose_cam_to_world,
+                                        const float* pose_world_to_cam);
+/* The per-keyframe part of Intrinsic3D::init (src/refinement/intrinsic3d.cpp:176-190) for the stored frames ids[0..n) (any order, repeats
+ * allowed): the colour, resizeDepth of the depth to the colour camera (src/rgbd/processing.cpp:129-183; a copy when the sizes agree) and
+ * the level-0 intensity fill the frame store exactly as i3d_upload_rgbd_frames(n, color W, color H, bgr[ids], resizeDepth(depth[ids]), NULL)
+ * would; i3d_use_rgbd_level then works as after that call.  Fails without stored frames, for n <= 0 and for an id out of range, leaving
+ * both stores as they were.  Device time: i3d_phase_ms("sensor_select"), of which k_resize_depth is i3d_phase_ms("resize_depth"). */
+int         i3d_select_rgbd_frames(I3DEngine* e, int32_t n, const int32_t* ids);
+
 /* ---- multi-GPU (one process per GPU; voxel ranges sharded, see DESIGN.md §multi-GPU) ---- */
 /* 128-byte NCCL unique id created on rank 0 and distributed by the host (e.g. torch.distributed). */
 int         i3d_comm_unique_id(uint8_t id128[128]);

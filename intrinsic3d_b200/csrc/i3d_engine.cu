@@ -208,6 +208,11 @@ struct I3DEngine
     // RGB-D frame store (i3d_upload_rgbd_frames): level-0 keyframes; i3d_use_rgbd_level builds level l from it
     int st_F = 0, st_W = 0, st_H = 0;
     Dev<float> st_lum, st_depth, st_tmp[4]; Dev<uint8_t> st_bgr;      // st_tmp: intermediate levels, luminance [0..1], depth [2..3]
+    // sensor store (i3d_sensor_frames_begin / add): the raw sequence, depth [sn_cap][depth cam] in thresholded metres, colour
+    // [sn_cap][colour cam][3] B,G,R.  Keyframe scores, fusion and i3d_select_rgbd_frames read it; only add writes it.
+    int sn_cap = 0, sn_F = 0;
+    I3DFusionCamera sn_dcam{}, sn_ccam{};
+    Dev<float> sn_depth; Dev<uint8_t> sn_bgr; Dev<int32_t> sn_ids;
     // surface extraction (i3d_mesh.cuh): scratch that only grows, and the resident mesh of the last i3d_extract_mesh
     bool have_mesh = false;
     int64_t mesh_V = 0, mesh_F = 0;
@@ -421,6 +426,13 @@ void fuse_frustum_bounds(const I3DFusionCamera& cam, float dmin, float dmax, flo
             b[2 * k + 1] = std::max(b[2 * k + 1], std::max(pl, pu));
         }
     }
+}
+
+// A camera the fusion and resizeDepth can use: a positive size and finite intrinsics with fx, fy > 0
+bool pinhole_ok(const I3DFusionCamera* c)
+{
+    return c && c->width > 0 && c->height > 0 && c->fx > 0.0f && c->fy > 0.0f && std::isfinite(c->fx) && std::isfinite(c->fy) &&
+           std::isfinite(c->cx) && std::isfinite(c->cy);
 }
 
 void fuse_reset_table(I3DEngine* e, uint64_t cap)
@@ -1795,6 +1807,70 @@ int i3d_fusion_begin(I3DEngine* e, const I3DFusionParams* params)
     });
 }
 
+// The loop body of AppFusion::fuseSDF for n frames already on the device: frame f is depth[ids[f]] / bgr[ids[f]] (frame f when ids is
+// NULL), with pose row f.  Erosion writes into fu_depth, so the source planes are only read.  Runs inside guarded(); `who` names the entry
+// point in messages.
+static int fuse_frames(I3DEngine* e, const char* who, int32_t n, const I3DFusionCamera& depth_cam, const float* depth, const I3DFusionCamera& color_cam,
+                       const uint8_t* bgr, const int32_t* ids, const float* pose_cam_to_world, const float* pose_world_to_cam)
+{
+    cudaStream_t st = e->stream;
+    const I3DFusionParams& P = e->fu_p;
+    const size_t dimg = static_cast<size_t>(depth_cam.width) * depth_cam.height;
+    const size_t cimg = static_cast<size_t>(color_cam.width) * color_cam.height * 3;
+    e->fu_depth.ensure(dimg);
+    const bool want_normals = P.integration_weight_sample > 0.0f;
+    if (want_normals) e->fu_nrm.ensure(3 * dimg);
+    const FuseCam dc{depth_cam.width, depth_cam.height, depth_cam.fx, depth_cam.fy, depth_cam.cx, depth_cam.cy};
+    const FuseCam cc{color_cam.width, color_cam.height, color_cam.fx, color_cam.fy, color_cam.cx, color_cam.cy};
+    const FuseConst c = fuse_const(P);
+    for (int f = 0; f < n; ++f)
+    {
+        const size_t src = static_cast<size_t>(ids ? ids[f] : f);
+        FuseFrame fr;
+        std::memcpy(fr.R_cw, pose_cam_to_world + 12 * f, 9 * sizeof(float)); std::memcpy(fr.t_cw, pose_cam_to_world + 12 * f + 9, 3 * sizeof(float));
+        std::memcpy(fr.R_wc, pose_world_to_cam + 12 * f, 9 * sizeof(float)); std::memcpy(fr.t_wc, pose_world_to_cam + 12 * f + 9, 3 * sizeof(float));
+        fuse_frustum_bounds(depth_cam, P.depth_min, P.depth_max, P.voxel_size, fr.R_cw, fr.t_cw, fr.bounds);
+        {
+            Timer t(e, "fusion_prep", 0);
+            k_fuse_erode<<<blocks_for(dimg), kThreads, 0, st>>>(dc.W, dc.H, P.discont_window_size, depth + dimg * src, e->fu_depth.p);
+            if (want_normals) k_fuse_normals<<<blocks_for(dimg), kThreads, 0, st>>>(dc, e->fu_depth.p, e->fu_nrm.p);
+        }
+        int ctl[2] = {0, 0};
+        for (int attempt = 0;; ++attempt)
+        {
+            {
+                Timer t(e, "fusion_alloc", 0);
+                CK(cudaMemsetAsync(e->fu_ctl.p + 1, 0, sizeof(int), st));
+                k_fuse_alloc<<<blocks_for(dimg), kThreads, 0, st>>>(dc, fr, c, e->fu_depth.p, fuse_table(e), fuse_volume(e), attempt == 0 ? 1 : 0);
+                CK(cudaMemcpyAsync(ctl, e->fu_ctl.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+            }
+            collect_kernel_times(e);         // synchronises: ctl is on the host
+            CK(cudaGetLastError());
+            e->fu_n = ctl[0];
+            if (ctl[1] & 2)
+                return fail(e, "%s: frame %d allocates voxels outside the +-2^20 coordinate range of the device hash "
+                            "(voxel size %g); the fusion is ended", who, f, static_cast<double>(P.voxel_size));
+            if (!(ctl[1] & 1)) break;
+            // the table is too full: grow it, then run this frame's allocation again (the voxel set is a union: re-inserting is harmless)
+            uint64_t cap = e->fu_cap * 2;
+            while (static_cast<uint64_t>(e->fu_n) * 4 > cap) cap <<= 1;
+            if (cap > (1ull << 31)) return fail(e, "%s: more than 2^30 allocated voxels; the fusion is ended", who);
+            fuse_grow_table(e, cap);
+            e->phases["fusion_growths"].count += 1;
+        }
+        {
+            Timer t(e, "fusion_integrate", 0);
+            if (e->fu_n > 0)
+                k_fuse_integrate<<<blocks_for(static_cast<size_t>(e->fu_n)), kThreads, 0, st>>>(e->fu_n, dc, cc, fr, c, e->fu_depth.p,
+                                                                                                want_normals ? e->fu_nrm.p : nullptr,
+                                                                                                bgr + cimg * src, fuse_volume(e));
+        }
+    }
+    collect_kernel_times(e);
+    CK(cudaGetLastError());
+    return 0;
+}
+
 int i3d_fusion_integrate(I3DEngine* e, int32_t F, const I3DFusionCamera* depth_cam, const float* depth, const I3DFusionCamera* color_cam,
                          const uint8_t* bgr, const float* pose_cam_to_world, const float* pose_world_to_cam)
 {
@@ -1806,65 +1882,150 @@ int i3d_fusion_integrate(I3DEngine* e, int32_t F, const I3DFusionCamera* depth_c
         return fail(e, "i3d_fusion_integrate: bad camera dimensions");
     const int rc = guarded(e, [&]() {
         cudaStream_t st = e->stream;
-        const I3DFusionParams& P = e->fu_p;
         const size_t dimg = static_cast<size_t>(depth_cam->width) * depth_cam->height;
         const size_t cimg = static_cast<size_t>(color_cam->width) * color_cam->height * 3;
-        e->fu_depth_in.ensure(dimg * F); e->fu_depth.ensure(dimg); e->fu_bgr.ensure(cimg * F);
-        const bool want_normals = P.integration_weight_sample > 0.0f;
-        if (want_normals) e->fu_nrm.ensure(3 * dimg);
+        e->fu_depth_in.ensure(dimg * F); e->fu_bgr.ensure(cimg * F);
         CK(cudaMemcpyAsync(e->fu_depth_in.p, depth, dimg * F * sizeof(float), cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(e->fu_bgr.p, bgr, cimg * F, cudaMemcpyHostToDevice, st));
-        const FuseCam dc{depth_cam->width, depth_cam->height, depth_cam->fx, depth_cam->fy, depth_cam->cx, depth_cam->cy};
-        const FuseCam cc{color_cam->width, color_cam->height, color_cam->fx, color_cam->fy, color_cam->cx, color_cam->cy};
-        const FuseConst c = fuse_const(P);
-        for (int f = 0; f < F; ++f)
+        return fuse_frames(e, "i3d_fusion_integrate", F, *depth_cam, e->fu_depth_in.p, *color_cam, e->fu_bgr.p, nullptr, pose_cam_to_world,
+                           pose_world_to_cam);
+    });
+    if (rc != 0) e->fu_active = false;
+    return rc;
+}
+
+// ---- the sensor store: the raw sequence on the device (DESIGN.md §6l) -------------------------------
+int i3d_sensor_frames_begin(I3DEngine* e, const I3DFusionCamera* depth_cam, const I3DFusionCamera* color_cam, int32_t capacity)
+{
+    if (!e) return 1;
+    if (!pinhole_ok(depth_cam) || !pinhole_ok(color_cam))
+        return fail(e, "i3d_sensor_frames_begin: bad camera (a positive size, finite intrinsics and fx, fy > 0 are needed)");
+    if (capacity <= 0) return fail(e, "i3d_sensor_frames_begin: capacity must be > 0 (got %d)", capacity);
+    e->sn_F = 0; e->sn_cap = 0;
+    return guarded(e, [&]() {
+        const size_t dimg = static_cast<size_t>(depth_cam->width) * depth_cam->height;
+        const size_t cimg = static_cast<size_t>(color_cam->width) * color_cam->height * 3;
+        e->sn_depth.ensure(dimg * capacity); e->sn_bgr.ensure(cimg * capacity);
+        e->sn_dcam = *depth_cam; e->sn_ccam = *color_cam; e->sn_cap = capacity;
+        return 0;
+    });
+}
+
+int i3d_sensor_frames_add(I3DEngine* e, int32_t F, const float* depth, const uint8_t* bgr)
+{
+    if (!e) return 1;
+    if (e->sn_cap <= 0) return fail(e, "i3d_sensor_frames_add: no sensor store (call i3d_sensor_frames_begin first)");
+    if (F <= 0 || !depth || !bgr) return fail(e, "i3d_sensor_frames_add: need F > 0 frames and non-NULL buffers (F = %d)", F);
+    if (F > e->sn_cap - e->sn_F)
+        return fail(e, "i3d_sensor_frames_add: %d more frames exceed the capacity of %d (%d stored)", F, e->sn_cap, e->sn_F);
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t dimg = static_cast<size_t>(e->sn_dcam.width) * e->sn_dcam.height;
+        const size_t cimg = static_cast<size_t>(e->sn_ccam.width) * e->sn_ccam.height * 3;
+        CK(cudaMemcpyAsync(e->sn_depth.p + dimg * e->sn_F, depth, dimg * F * sizeof(float), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(e->sn_bgr.p + cimg * e->sn_F, bgr, cimg * F, cudaMemcpyHostToDevice, st));
+        CK(cudaStreamSynchronize(st));
+        e->sn_F += F;
+        return 0;
+    });
+}
+
+int32_t i3d_sensor_num_frames(const I3DEngine* e) { return e ? e->sn_F : 0; }
+
+int i3d_sensor_keyframe_scores(I3DEngine* e, double* scores)
+{
+    if (!e) return 1;
+    if (e->sn_F <= 0) return fail(e, "i3d_sensor_keyframe_scores: no frames in the sensor store");
+    if (!scores) return fail(e, "i3d_sensor_keyframe_scores: scores is NULL");
+    const int W = e->sn_ccam.width, H = e->sn_ccam.height, F = e->sn_F;
+    if (W < 5 || H < 5) return fail(e, "i3d_sensor_keyframe_scores: frames of %d x %d px; the 9-tap blur filter needs at least 5 px on each axis", W, H);
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t img = static_cast<size_t>(W) * H * 3;
+        const int tx = (W + kBlurTileW - 1) / kBlurTileW, ty = (H + kBlurTileH - 1) / kBlurTileH;
+        const int chunk = std::min<int>(F, I3D_KEYFRAME_CHUNK);
+        e->kf_partials.ensure(static_cast<size_t>(chunk) * tx * ty * 4); e->kf_scores.ensure(F);
+        e->phases.erase("keyframe_scores"); e->phases.erase("keyframe_chunks");
         {
-            FuseFrame fr;
-            std::memcpy(fr.R_cw, pose_cam_to_world + 12 * f, 9 * sizeof(float)); std::memcpy(fr.t_cw, pose_cam_to_world + 12 * f + 9, 3 * sizeof(float));
-            std::memcpy(fr.R_wc, pose_world_to_cam + 12 * f, 9 * sizeof(float)); std::memcpy(fr.t_wc, pose_world_to_cam + 12 * f + 9, 3 * sizeof(float));
-            fuse_frustum_bounds(*depth_cam, P.depth_min, P.depth_max, P.voxel_size, fr.R_cw, fr.t_cw, fr.bounds);
+            // the chunks share the partials buffer in stream order: no host synchronisation between them
+            Timer t(e, "keyframe_scores", 0);
+            for (int f0 = 0; f0 < F; f0 += chunk)
             {
-                Timer t(e, "fusion_prep", 0);
-                k_fuse_erode<<<blocks_for(dimg), kThreads, 0, st>>>(dc.W, dc.H, P.discont_window_size, e->fu_depth_in.p + dimg * f, e->fu_depth.p);
-                if (want_normals) k_fuse_normals<<<blocks_for(dimg), kThreads, 0, st>>>(dc, e->fu_depth.p, e->fu_nrm.p);
-            }
-            int ctl[2] = {0, 0};
-            for (int attempt = 0;; ++attempt)
-            {
-                {
-                    Timer t(e, "fusion_alloc", 0);
-                    CK(cudaMemsetAsync(e->fu_ctl.p + 1, 0, sizeof(int), st));
-                    k_fuse_alloc<<<blocks_for(dimg), kThreads, 0, st>>>(dc, fr, c, e->fu_depth.p, fuse_table(e), fuse_volume(e), attempt == 0 ? 1 : 0);
-                    CK(cudaMemcpyAsync(ctl, e->fu_ctl.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
-                }
-                collect_kernel_times(e);         // synchronises: ctl is on the host
-                CK(cudaGetLastError());
-                e->fu_n = ctl[0];
-                if (ctl[1] & 2)
-                    return fail(e, "i3d_fusion_integrate: frame %d allocates voxels outside the +-2^20 coordinate range of the device hash "
-                                "(voxel size %g); the fusion is ended", f, static_cast<double>(P.voxel_size));
-                if (!(ctl[1] & 1)) break;
-                // the table is too full: grow it, then run this frame's allocation again (the voxel set is a union: re-inserting is harmless)
-                uint64_t cap = e->fu_cap * 2;
-                while (static_cast<uint64_t>(e->fu_n) * 4 > cap) cap <<= 1;
-                if (cap > (1ull << 31)) return fail(e, "i3d_fusion_integrate: more than 2^30 allocated voxels; the fusion is ended");
-                fuse_grow_table(e, cap);
-                e->phases["fusion_growths"].count += 1;
-            }
-            {
-                Timer t(e, "fusion_integrate", 0);
-                if (e->fu_n > 0)
-                    k_fuse_integrate<<<blocks_for(static_cast<size_t>(e->fu_n)), kThreads, 0, st>>>(e->fu_n, dc, cc, fr, c, e->fu_depth.p,
-                                                                                                    want_normals ? e->fu_nrm.p : nullptr,
-                                                                                                    e->fu_bgr.p + cimg * f, fuse_volume(e));
+                const int n = std::min(chunk, F - f0);
+                k_blur_partials<<<dim3(tx, ty, n), dim3(32, 8), 0, st>>>(n, W, H, e->sn_bgr.p + img * f0, e->kf_partials.p);
+                k_blur_finish<<<(n + 3) / 4, 128, 0, st>>>(n, tx * ty, e->kf_partials.p, e->kf_scores.p + f0);
+                e->phases["keyframe_chunks"].count += 1;
             }
         }
+        CK(cudaMemcpyAsync(scores, e->kf_scores.p, F * sizeof(double), cudaMemcpyDeviceToHost, st));
         collect_kernel_times(e);
         CK(cudaGetLastError());
         return 0;
     });
+}
+
+// Checks n > 0 and every id against the store; the message names `who`
+static int check_sensor_ids(I3DEngine* e, const char* who, int32_t n, const int32_t* ids)
+{
+    if (e->sn_F <= 0) return fail(e, "%s: no frames in the sensor store", who);
+    if (n <= 0 || !ids) return fail(e, "%s: need n > 0 frame ids (n = %d)", who, n);
+    for (int32_t k = 0; k < n; ++k)
+        if (ids[k] < 0 || ids[k] >= e->sn_F) return fail(e, "%s: frame id %d (entry %d) is out of range [0, %d)", who, ids[k], k, e->sn_F);
+    return 0;
+}
+
+int i3d_fusion_integrate_sensor(I3DEngine* e, int32_t n, const int32_t* ids, const float* pose_cam_to_world, const float* pose_world_to_cam)
+{
+    if (!e) return 1;
+    if (!e->fu_active) return fail(e, "i3d_fusion_integrate_sensor: no fusion in progress (call i3d_fusion_begin first)");
+    if (check_sensor_ids(e, "i3d_fusion_integrate_sensor", n, ids)) return 1;
+    if (!pose_cam_to_world || !pose_world_to_cam) return fail(e, "i3d_fusion_integrate_sensor: poses must not be NULL");
+    const int rc = guarded(e, [&]() {
+        return fuse_frames(e, "i3d_fusion_integrate_sensor", n, e->sn_dcam, e->sn_depth.p, e->sn_ccam, e->sn_bgr.p, ids, pose_cam_to_world,
+                           pose_world_to_cam);
+    });
     if (rc != 0) e->fu_active = false;
     return rc;
+}
+
+int i3d_select_rgbd_frames(I3DEngine* e, int32_t n, const int32_t* ids)
+{
+    if (!e) return 1;
+    if (check_sensor_ids(e, "i3d_select_rgbd_frames", n, ids)) return 1;
+    e->st_F = 0;
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const I3DFusionCamera &dc = e->sn_dcam, &cc = e->sn_ccam;
+        const int W = cc.width, H = cc.height;
+        const size_t cnt = static_cast<size_t>(n) * W * H, dimg = static_cast<size_t>(dc.width) * dc.height, cimg = static_cast<size_t>(W) * H * 3;
+        e->st_lum.ensure(cnt); e->st_depth.ensure(cnt); e->st_bgr.ensure(3 * cnt);
+        e->phases.erase("sensor_select"); e->phases.erase("resize_depth");
+        {
+            Timer t(e, "sensor_select", 0);
+            for (int32_t k = 0; k < n; ++k)
+                CK(cudaMemcpyAsync(e->st_bgr.p + cimg * k, e->sn_bgr.p + cimg * ids[k], cimg, cudaMemcpyDeviceToDevice, st));
+            if (dc.width == W && dc.height == H)
+            {
+                // resizeDepth returns the plane unchanged when the sizes agree, whatever the intrinsics (Q51)
+                for (int32_t k = 0; k < n; ++k)
+                    CK(cudaMemcpyAsync(e->st_depth.p + dimg * k, e->sn_depth.p + dimg * ids[k], dimg * sizeof(float), cudaMemcpyDeviceToDevice, st));
+            }
+            else
+            {
+                e->sn_ids.ensure(n);
+                CK(cudaMemcpyAsync(e->sn_ids.p, ids, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+                const ResizeCams rc{dc.width, dc.height, dc.fx, dc.fy, dc.cx, dc.cy, W, H, cc.fx, cc.fy, cc.cx, cc.cy};
+                Timer tr(e, "resize_depth", 0);
+                k_resize_depth<<<dim3((W + 31) / 32, (H + 7) / 8, std::min(n, 65535)), dim3(32, 8), 0, st>>>(n, e->sn_ids.p, rc, e->sn_depth.p,
+                                                                                                           e->st_depth.p);
+            }
+            k_frames_lum0<<<blocks_for(cnt), kThreads, 0, st>>>(cnt, e->st_bgr.p, e->st_lum.p);
+        }
+        collect_kernel_times(e);
+        CK(cudaGetLastError());
+        e->st_F = n; e->st_W = W; e->st_H = H;
+        return 0;
+    });
 }
 
 int i3d_fusion_finish(I3DEngine* e, int64_t* num_voxels_out)

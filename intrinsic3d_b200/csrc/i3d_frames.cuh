@@ -6,6 +6,7 @@
  *   k_frames_lum0                     Pyramid::create's BGR -> float intensity (level 0)     src/rgbd/pyramid.cpp:68-71
  *   k_frames_pyrdown                  Pyramid::downsample (cv::pyrDown, REFLECT_101)         :108-113
  *   k_frames_depthdown                Pyramid::downsampleDepth (masked 2x2 mean)             :116-141
+ *   k_resize_depth                    resizeDepth + interpolate<float> (DESIGN.md §6l)        src/rgbd/processing.cpp:129-183, 236-291
  *
  * Every float operation is written with FM/FA/FS/FD (no contraction), in the order tests/frames_ref.py restates, so that a numpy float32
  * restatement reproduces every plane bit for bit.  Equality with a particular OpenCV build is not claimed (it may use FMA or IPP).
@@ -198,6 +199,55 @@ __global__ void __launch_bounds__(256) k_frames_depthdown(int F, int W, int H, c
             if (d[k] > 0.0f) { sum = FA(sum, d[k]); ++cnt; }
         dst[static_cast<size_t>(f) * Wd * Hd + static_cast<size_t>(y) * Wd + x] = cnt > 0 ? FD(sum, static_cast<float>(cnt)) : 0.0f;
     }
+}
+
+// The two pinhole cameras of resizeDepth: the depth plane's (in) and the colour camera's (out)
+struct ResizeCams
+{
+    int in_w, in_h;
+    float in_fx, in_fy, in_cx, in_cy;
+    int out_w, out_h;
+    float out_fx, out_fy, out_cx, out_cy;
+};
+
+// processing.cpp's resizeDepth + interpolate<float> of one output pixel (DESIGN.md §6l).  The tap (int)(u + 0.5) lies in [0, in_w) exactly
+// when u + 0.5 is in (-1, in_w): tested on the float, so an out-of-range or NaN coordinate gives 0 without an undefined cast.  A zero-depth
+// tap counts with its weight (Q50); a result of 0 is stored as +0, as the reference leaves the pixel of its zero-initialised output.
+__device__ __forceinline__ float resize_depth_px(const ResizeCams& c, const float* __restrict__ src, int x, int y)
+{
+    const float ifx = FD(1.0f, c.out_fx), ify = FD(1.0f, c.out_fy);
+    const float u = FA(FM(c.in_fx, FM(FS(static_cast<float>(x), c.out_cx), ifx)), c.in_cx);
+    const float v = FA(FM(c.in_fy, FM(FS(static_cast<float>(y), c.out_cy), ify)), c.in_cy);
+    const float tu = FA(u, 0.5f), tv = FA(v, 0.5f);
+    if (!(tu > -1.0f && tu < static_cast<float>(c.in_w) && tv > -1.0f && tv < static_cast<float>(c.in_h))) return 0.0f;
+    const int x0 = static_cast<int>(floorf(u)), y0 = static_cast<int>(floorf(v)), x1 = x0 + 1, y1 = y0 + 1;
+    float wx1 = FS(u, static_cast<float>(x0)), wy1 = FS(v, static_cast<float>(y0));
+    float wx0 = FS(1.0f, wx1), wy0 = FS(1.0f, wy1);
+    if (x0 < 0 || x0 >= c.in_w) wx0 = 0.0f;
+    if (x1 < 0 || x1 >= c.in_w) wx1 = 0.0f;
+    if (y0 < 0 || y0 >= c.in_h) wy0 = 0.0f;
+    if (y1 < 0 || y1 >= c.in_h) wy1 = 0.0f;
+    const float w00 = FM(wx0, wy0), w10 = FM(wx1, wy0), w01 = FM(wx0, wy1), w11 = FM(wx1, wy1);
+    const float sw = FA(FA(FA(w00, w10), w01), w11);
+    float sum = 0.0f;
+    if (w00 > 0.0f) sum = FA(sum, FM(__ldg(src + static_cast<size_t>(y0) * c.in_w + x0), w00));
+    if (w01 > 0.0f) sum = FA(sum, FM(__ldg(src + static_cast<size_t>(y1) * c.in_w + x0), w01));
+    if (w10 > 0.0f) sum = FA(sum, FM(__ldg(src + static_cast<size_t>(y0) * c.in_w + x1), w10));
+    if (w11 > 0.0f) sum = FA(sum, FM(__ldg(src + static_cast<size_t>(y1) * c.in_w + x1), w11));
+    if (!(sw > 0.0f)) return 0.0f;
+    const float d = FD(sum, sw);
+    return d == 0.0f ? 0.0f : d;
+}
+
+// resizeDepth of the stored depth planes ids[0..n) into dst [n][out_h][out_w] (output frames: blockIdx.z + k * gridDim.z)
+__global__ void __launch_bounds__(256) k_resize_depth(int n, const int32_t* __restrict__ ids, ResizeCams c, const float* __restrict__ src,
+                                                      float* __restrict__ dst)
+{
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= c.out_w || y >= c.out_h) return;
+    const size_t in_px = static_cast<size_t>(c.in_w) * c.in_h, out_px = static_cast<size_t>(c.out_w) * c.out_h;
+    for (int f = blockIdx.z; f < n; f += gridDim.z)
+        dst[static_cast<size_t>(f) * out_px + static_cast<size_t>(y) * c.out_w + x] = resize_depth_px(c, src + static_cast<size_t>(ids[f]) * in_px, x, y);
 }
 
 } // namespace i3d

@@ -29,6 +29,8 @@ EXPORTED_SYMBOLS = [
     "i3d_num_voxels", "i3d_clear_voxels_outside_thin_shell", "i3d_upsample_grid", "i3d_download_grid",
     "i3d_sizeof_fusion_params", "i3d_default_fusion_params", "i3d_fusion_begin", "i3d_fusion_integrate", "i3d_fusion_finish",
     "i3d_keyframe_scores", "i3d_upload_rgbd_frames", "i3d_use_rgbd_level",
+    "i3d_sensor_frames_begin", "i3d_sensor_frames_add", "i3d_sensor_num_frames", "i3d_sensor_keyframe_scores", "i3d_fusion_integrate_sensor",
+    "i3d_select_rgbd_frames",
     "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh", "i3d_extract_mesh_colored", "i3d_mode_colors",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
@@ -82,6 +84,8 @@ def load_library():
     L.i3d_extract_mesh_colored.argtypes = [C.c_void_p, C.POINTER(I3DMeshParams), C.c_int32, C.POINTER(I3DMeshInfo)]
     L.i3d_mode_colors.restype = C.c_int
     L.i3d_mode_colors.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_uint8)]
+    L.i3d_sensor_num_frames.restype = C.c_int32
+    L.i3d_sensor_num_frames.argtypes = [C.c_void_p]
     _LIB = L
     return L
 
@@ -364,6 +368,52 @@ class Engine:
         self.F = self._store_F
         self.frame_size = (int(w.value), int(h.value))
         return self.frame_size
+
+    # ---- the sensor store: the raw sequence on the device (Sensor::depth / Sensor::color) ------------------------------------
+    def sensor_frames_begin(self, depth_cam, color_cam, capacity: int):
+        """Starts an empty device store of `capacity` frames for a depth camera and a colour camera, each (W, H, fx, fy, cx, cy); its
+        device memory is allocated here, so a long sequence can be added in chunks."""
+        dc, cc = fusion_camera(depth_cam), fusion_camera(color_cam)
+        self._check(self.L.i3d_sensor_frames_begin(self.h, C.byref(dc), C.byref(cc), C.c_int32(int(capacity))))
+        self._sensor_cams = (dc, cc)
+
+    def sensor_frames_add(self, depth, bgr):
+        """Appends frames: depth float32 [F, Hd, Wd] metres (range-thresholded), bgr uint8 [F, Hc, Wc, 3] (B, G, R)."""
+        dc, cc = self._sensor_cams
+        depth = np.ascontiguousarray(depth, np.float32)
+        bgr = np.ascontiguousarray(bgr, np.uint8)
+        F = int(depth.shape[0])
+        assert depth.shape == (F, dc.height, dc.width) and bgr.shape == (F, cc.height, cc.width, 3)
+        self._check(self.L.i3d_sensor_frames_add(self.h, C.c_int32(F), _p(depth, C.c_float), _p(bgr, C.c_uint8)))
+
+    def sensor_num_frames(self) -> int:
+        return int(self.L.i3d_sensor_num_frames(self.h))
+
+    def sensor_keyframe_scores(self):
+        """keyframe_scores of every stored frame, read from the store: float64 [sensor_num_frames()]."""
+        out = np.empty(self.sensor_num_frames(), np.float64)
+        self._check(self.L.i3d_sensor_keyframe_scores(self.h, _p(out, C.c_double)))
+        return out
+
+    @staticmethod
+    def _ids(ids):
+        ids = np.ascontiguousarray(ids, np.int32).ravel()
+        return ids, int(ids.shape[0])
+
+    def fusion_integrate_sensor(self, ids, pose_cam_to_world, pose_world_to_cam):
+        """fusion_integrate of the stored frames `ids`, in list order; poses float32 [len(ids), 12] (R row-major | t)."""
+        ids, n = self._ids(ids)
+        c2w = np.ascontiguousarray(pose_cam_to_world, np.float32)
+        w2c = np.ascontiguousarray(pose_world_to_cam, np.float32)
+        assert c2w.shape == (n, 12) and w2c.shape == (n, 12)
+        self._check(self.L.i3d_fusion_integrate_sensor(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(c2w, C.c_float), _p(w2c, C.c_float)))
+
+    def select_rgbd_frames(self, ids):
+        """The stored frames `ids` (any order, repeats allowed) become the level-0 keyframes of the frame store, their depth resized to the
+        colour camera (resizeDepth), as upload_rgbd_frames would make them; use_rgbd_level(l) then installs level l."""
+        ids, n = self._ids(ids)
+        self._check(self.L.i3d_select_rgbd_frames(self.h, C.c_int32(n), _p(ids, C.c_int32)))
+        self._store_F = n
 
     def debug_frames(self, with_color=False):
         """(lum, depth, bgr or None) of the current level as the device holds them."""
