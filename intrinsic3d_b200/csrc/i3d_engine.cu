@@ -885,7 +885,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     if (S > 0) pdl_launch(e, k_row_weights, blocks_for(S), kThreads, 0, rows, e->type_w.p);
     SolveVecs sv = solve_vecs(e);
     pdl_launch(e, k_finish_problem, blocks_for(static_cast<size_t>((hc + 3) / 4)), kThreads, 0, g, rv, sv, sh, hc, e->type_w.p, e->cam_acc.p, P.fix_poses, P.fix_intrinsics,
-                                                                              P.fix_distortion, e->site(SITE_FINISH), e->cam);
+                                                                              P.fix_distortion, P.gradient_tolerance, e->site(SITE_FINISH), e->cam);
     allreduce_scalars(e, e->site(SITE_FINISH).out, 3, -1, 0);
     pdl_launch(e, k_iter_finish, 1, 32, 0, e->iter_dev.p, e->site(SITE_FINISH).out, P);
     e->launches += 5;

@@ -460,6 +460,8 @@ struct FramePose
     int small;
     int pad;
 };
+// k_eg_rows<ROWS_COST> stages F of these into shared memory; tests/test_gpu_lm_trial.py derives the staging boundary from this size
+static_assert(sizeof(FramePose) == 176, "FramePose size changed: update the pose-table staging boundary and its test");
 
 I3D_HD void frame_pose_make(const double* __restrict__ pose, FramePose* fp)
 {
