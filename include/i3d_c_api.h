@@ -288,6 +288,9 @@ int         i3d_debug_get_observations(I3DEngine* e, int32_t K, int32_t* frames,
 /* last evaluated LM trial step in unknown space [sdf n | albedo n | poses 6F | intr 4 | dist 5]
  * (unscaled delta), the free mask and the Jacobi column scale. */
 int         i3d_debug_get_step(I3DEngine* e, double* step, uint8_t* free_mask, double* col_scale);
+/* PCG iterate x[U] and search direction p[U] (Jacobi-scaled unknown space) as the last LM trial's solve left them.  Any pointer may be
+ * NULL. */
+int         i3d_debug_get_pcg_vectors(I3DEngine* e, float* x, float* p);
 /* normal-equation pieces of the last iteration (build_only = 1 is enough), unknown space [U = 2n + 6F + 9]: b[U] = J'^T f (Jacobi
  * scaled gradient), s[U] (Jacobi column scale, 0 for fixed unknowns), jtj[U] = s^2 * column norm^2, and the raw (unweighted by the
  * type weight, unscaled) E_g camera sums cam_acc[33F + 43]: per frame 6 gradient (sum w_raw r J), 6 column norms, the upper 6x6

@@ -180,6 +180,9 @@ struct I3DEngine
     int timer_level = 0;         // 0: phases + the roofline kernels (sampled); 1: every kernel of the iteration (i3d_debug_set_kernel_timers)
     Dev<IterDev> iter_dev;       // device-resident result / LM state of the current iteration
     int last_cg_iterations = 4, prev_cg_iterations = 4;  // PCG iteration counts of the previous two solves: their maximum sizes the first launch batch
+    bool pcg_fused = true;       // k_cg_step where it applies (I3D_PCG_FUSED=0 at engine creation: the four-kernel chain)
+    int64_t step_n = -1;         // grid size k_cg_step's launch shape was planned for (step_grid = 0: does not fit)
+    unsigned step_grid = 0; int step_K = 0; size_t step_smem = 0;
     // colour frames for the recolouring pass (i3d_recolor.cuh)
     Dev<uint8_t> color;
     bool have_color = false;
@@ -715,15 +718,21 @@ int check_frame_limit(I3DEngine* e, int F, int K)
 
 // applies the CGNR operator to the vector whose Jacobi-scaled copy is in sv.ps: afterwards qg holds the (globally summed)
 // raw J'^T J' part; k_cg_update forms q = s*qg + D^2 v on the fly and resets qg.
-void launch_operator(I3DEngine* e, const GridView& g, const RegView& rv, const EgRows& rows, const SolveVecs& sv, const Shard& sh, const float* vin,
-                     float dmin, float dmax, int is_cg_iteration, bool sample_timing = false)
+void launch_eg_apply(I3DEngine* e, const GridView& g, const RegView& rv, const EgRows& rows, const SolveVecs& sv)
 {
     if (rows.n_active > 0)
     {
         KernelTimer kt(e, "k_eg_apply", 0);     // the dominant kernel: every launch is timed (roofline = true average)
         pdl_launch(e, k_eg_apply<APPLY_CG>, blocks_for(rows.n_active), kThreads, apply_smem_bytes(e->F, rows.K), g, rows, rv, sv, sv.ps, e->ctl.p, 1, e->site(SITE_EG_APPLY));
     }
-    e->launches += 2;
+    e->launches += 1;
+}
+
+void launch_operator(I3DEngine* e, const GridView& g, const RegView& rv, const EgRows& rows, const SolveVecs& sv, const Shard& sh, const float* vin,
+                     float dmin, float dmax, int is_cg_iteration, bool sample_timing = false)
+{
+    launch_eg_apply(e, g, rv, rows, sv);
+    e->launches += 1;
     {
         KernelTimer kt(e, "k_op_partial");
         pdl_launch(e, (k_op_partial<APPLY_CG, 4>), blocks_for(static_cast<size_t>((e->held_count() + 3) / 4)), kThreads, 0, 
@@ -734,6 +743,59 @@ void launch_operator(I3DEngine* e, const GridView& g, const RegView& rv, const E
         KernelTimer kt(e, "exchange");
         exchange(e, sv.qg, nullptr, sv.qg + 2 * e->n, 6 * e->F + 9, e->site(SITE_OP_POST).out, 1, 1, is_cg_iteration ? EPI_OPERATOR_CG : -1);
     }
+}
+
+// Launch shape of k_cg_step for the current grid: the most blocks per SM at which every block is resident together with its
+// K = ceil(items / threads) shared-memory slots.  Returns false (the four-kernel chain runs) when no shape fits.
+bool plan_cg_step(I3DEngine* e)
+{
+    if (e->step_n == e->n) return e->step_grid > 0;
+    e->step_n = e->n; e->step_grid = 0;
+    int sms = 0, optin = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->device));
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->device));
+    cudaFuncAttributes fa0{}, fa1{};
+    CK(cudaFuncGetAttributes(&fa0, k_cg_step<false>));
+    CK(cudaFuncGetAttributes(&fa1, k_cg_step<true>));
+    const size_t dyn_max = static_cast<size_t>(optin) - std::max(fa0.sharedSizeBytes, fa1.sharedSizeBytes);
+    CK(cudaFuncSetAttribute(k_cg_step<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn_max)));
+    CK(cudaFuncSetAttribute(k_cg_step<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn_max)));
+    const int64_t items = (e->n + 3) / 4;
+    for (int bps = 2048 / kStepThreads; bps >= 1; --bps)
+    {
+        const int64_t threads = static_cast<int64_t>(bps) * sms * kStepThreads;
+        const int64_t K = (items + threads - 1) / threads;
+        const size_t smem = static_cast<size_t>(K) * kStepSlots * kStepThreads * sizeof(float);
+        if (smem > dyn_max) break;
+        int occ0 = 0, occ1 = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ0, k_cg_step<false>, kStepThreads, smem));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ1, k_cg_step<true>, kStepThreads, smem));
+        if (std::min(occ0, occ1) < bps) continue;
+        if (static_cast<size_t>(bps) * sms + 8 > e->max_blocks) break;     // block partials live in the reduction scratch
+        e->step_grid = static_cast<unsigned>(bps * sms); e->step_K = static_cast<int>(K); e->step_smem = smem;
+        return true;
+    }
+    return false;
+}
+
+// k_cg_step is a cooperative launch (grid barriers between its phases); it keeps programmatic stream serialization like every other
+// kernel of the iteration (pdl_launch): its blocks wait in griddepcontrol.wait until k_eg_apply has finished.
+template <bool INIT>
+void launch_cg_step(I3DEngine* e, const GridView& g, const RegView& rv, const SolveVecs& sv, float dmin, float dmax)
+{
+    static const bool pdl = [] { const char* v = std::getenv("I3D_PDL"); return !(v && v[0] == '0'); }();
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(e->step_grid); cfg.blockDim = dim3(kStepThreads); cfg.dynamicSmemBytes = e->step_smem; cfg.stream = e->stream;
+    cudaLaunchAttribute at[2];
+    at[0].id = cudaLaunchAttributeCooperative;
+    at[0].val.cooperative = 1;
+    at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = pdl ? 2 : 1;
+    const int64_t items = (e->n + 3) / 4;
+    CK(cudaLaunchKernelEx(&cfg, k_cg_step<INIT>, g, rv, sv, items, e->step_K, static_cast<const double*>(e->type_w.p), static_cast<const double*>(e->minv.p),
+                          dmin, dmax, e->ctl.p, e->site(SITE_OP_POST), static_cast<const double*>(e->site(SITE_EG_APPLY).out), e->site(SITE_UPDATE)));
+    e->launches += 1;
 }
 
 // One outer Gauss-Newton iteration.  Host synchronisations: ONE after the activity scan (row count -> launch sizes) and ONE
@@ -915,16 +977,29 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     };
     const unsigned vec_blocks = blocks_for(static_cast<size_t>(hc));
     const int max_it = P.forced_cg_iterations > 0 ? P.forced_cg_iterations : P.max_linear_solver_iterations;
+    // single GPU: the per-unknown half of a PCG iteration is one cooperative k_cg_step (operator finish, update, next direction)
+    const bool fused = e->pcg_fused && !multi && plan_cg_step(e);
     int enq = 0;                 // PCG iterations enqueued in the current trial
+    bool dir_ready = false;      // p and ps of the next iteration were formed by the k_cg_step before it
     auto enqueue_pcg = [&](int count) {
         for (int bidx = 0; bidx < count && enq < max_it; ++bidx)
         {
             ++enq;
             const bool refresh = (enq % P.residual_reset_period == 0);
+            if (!dir_ready)
             {
                 KernelTimer kt(e, "k_cg_dir");
                 pdl_launch(e, k_cg_dir4, blocks_for(static_cast<size_t>((hc + 3) / 4)), kThreads, 0, sv, sh, hc, e->ctl.p);
                 e->launches += 1;
+            }
+            dir_ready = false;
+            if (fused && !refresh)
+            {
+                launch_eg_apply(e, g, rv, rows, sv);
+                KernelTimer kt(e, "k_cg_update");        // k_cg_step is timed in k_cg_update's place
+                launch_cg_step<false>(e, g, rv, sv, dmin, dmax);
+                dir_ready = true;
+                continue;
             }
             launch_operator(e, g, rv, rows, sv, sh, sv.p, dmin, dmax, 1, enq == 1);
             if (refresh)
@@ -974,7 +1049,9 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
         pdl_launch(e, k_lm_begin, 1, 32, 0, e->iter_dev.p, e->ctl.p, e->fail_flag.p, P);
         pdl_launch(e, k_cam_precond, blocks_for(static_cast<size_t>(F) + 2, 64), 64, 0, sv, e->cam_acc.p, e->type_w.p, e->ctl.p, dmin, dmax, e->minv.p, e->fail_flag.p);
         e->launches += 2;
-        launch_update(true, 0);
+        if (fused) launch_cg_step<true>(e, g, rv, sv, dmin, dmax);
+        else launch_update(true, 0);
+        dir_ready = fused;
         if (multi) allreduce_scalars(e, e->site(SITE_UPDATE).out, 3, EPI_UPDATE_INIT, 0);
         enq = 0;
         // Kernels of iterations enqueued past convergence are no-ops but still cost a grid launch each, and every extra round
@@ -1300,6 +1377,7 @@ int i3d_engine_create(int device, I3DEngine** out)
     if (prop.major != 9 || prop.minor != 0) return fail(nullptr, "i3d_engine_create: device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
     I3DEngine* e = new I3DEngine();
     e->device = device;
+    { const char* v = std::getenv("I3D_PCG_FUSED"); e->pcg_fused = !(v && v[0] == '0'); }
     const int rc = guarded(e, [&]() {
         CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
         for (auto& ev : e->ev) CK(cudaEventCreate(&ev));
@@ -2475,6 +2553,18 @@ int i3d_debug_get_step(I3DEngine* e, double* step, uint8_t* free_mask, double* c
             if (free_mask) free_mask[j] = s[j] != 0.0f;
             if (col_scale) col_scale[j] = s[j];
         }
+        return 0;
+    });
+}
+
+int i3d_debug_get_pcg_vectors(I3DEngine* e, float* x, float* p)
+{
+    if (!e || !e->have_iter) return fail(e, "i3d_debug_get_pcg_vectors: no iteration yet");
+    return guarded(e, [&]() {
+        const size_t U = static_cast<size_t>(e->U());
+        if (x) CK(cudaMemcpyAsync(x, e->v_x.p, U * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+        if (p) CK(cudaMemcpyAsync(p, e->v_p.p, U * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaStreamSynchronize(e->stream));
         return 0;
     });
 }

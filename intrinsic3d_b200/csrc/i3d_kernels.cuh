@@ -18,6 +18,7 @@
  */
 #pragma once
 #include <cuda_runtime.h>
+#include <cooperative_groups.h>
 #include <stdint.h>
 #include <limits.h>
 #include "i3d_math.cuh"
@@ -2064,6 +2065,362 @@ k_cg_dir4(SolveVecs sv, Shard sh, int64_t count, const CgCtl* __restrict__ ctl)
             const float p = (beta == 0.0f) ? sv.z[j] : sv.z[j] + beta * sv.p[j];
             sv.p[j] = p; sv.ps[j] = sv.s[j] * p;
         }
+}
+
+// ---- the per-unknown half of a PCG iteration as ONE cooperative grid (single GPU) ------------------------------------------
+// k_cg_step<false> = k_op_partial<APPLY_CG> + k_cg_update<false, 4> + the next k_cg_dir4;  k_cg_step<true> = k_cg_update<true, 4> +
+// the first k_cg_dir4.  Those kernels exist only because alpha and beta need grid-wide sums; here each sum is a grid barrier:
+//   A  operator finish: q_j = s_j (float(qgd_j) + reg_j) + D_j^2 p_j (qgd cleared, qg never written), partial p.q   | barrier, alpha
+//   B  update: x, r, z (z kept on chip), partials rho, 2Q, x.D^2 x; camera blocks z = M^-1 r                        | barrier, beta
+//   C  direction: p = z + beta p, ps = s o p
+// A work item is 4 consecutive voxels with their sdf AND albedo unknowns, so the 6 neighbour ids are read once for both regulariser
+// gathers.  Item i of thread t (grid-stride) keeps its 8 values of q, then z, in shared memory slot [k][8][blockDim] (k = i / T): the
+// grid is sized to full residency, T = blocks * 256 threads, and the launcher refuses the fused path when K = ceil(items / T) slots do
+// not fit (the whole unknown vector is on chip: 4 B per unknown, ~121 KB per SM at C3).  The camera blocks are taken by the last F + 2
+// threads of the grid, which park their <= 6 values of q, then z, in their own entries of z (a scratch vector on this path).
+// Every float operation per unknown is the one of the kernels it replaces, rounded as their compiled code rounds it: the operations
+// are written with explicit-rounding intrinsics, because the compiler fuses multiply-adds differently in different kernels (the chain's
+// k_op_partial fuses -6 t0 + tr[nb_0] in two of its four unrolled elements, k_cg_update's q differs between its 16 B path and its
+// scalar/camera path).  The double partial sums are decomposed differently
+// (block partials, then every block sums all partials in one fixed order, so the scalar epilogues run on identical inputs in every
+// block on a shared-memory copy of the control block; block 0 stores it).  ctl->done is read once, before the first barrier: the grid
+// leaves together.
+// sm_90a, -Xptxas -v: <false> 80 registers and 8 B of spill (predicates saved around the slow-path division calls, once per thread),
+// <true> 74 registers, no spill; 3 blocks of 256 threads per SM (396 blocks on 132 SMs).  At C3: 0.20 ms per iteration against
+// 0.27 ms for the three kernels it replaces (H100 80GB HBM3, 700 W limit).
+constexpr int kStepThreads = 256;
+constexpr int kStepSlots = 8;       // unknowns of one work item: sdf and albedo of 4 voxels
+
+__device__ __forceinline__ void ld4n(const float* __restrict__ p, int64_t j, int cnt, bool vec, float (&v)[4])
+{
+    if (vec) { ld4(p, j, v); return; }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[i] = i < cnt ? p[j + i] : 0.0f;
+}
+__device__ __forceinline__ void st4n(float* __restrict__ p, int64_t j, int cnt, bool vec, const float (&v)[4])
+{
+    if (vec) { st4(p, j, v); return; }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) if (i < cnt) p[j + i] = v[i];
+}
+
+// block partials of NV per-thread values -> partials[blockIdx][NV]
+template <int NV>
+__device__ __forceinline__ void step_partials(const double (&vals)[NV], double* __restrict__ partials, double* red_smem)
+{
+#pragma unroll
+    for (int i = 0; i < NV; ++i)
+    {
+        const double s = block_sum<double>(vals[i], red_smem);
+        if (threadIdx.x == 0) partials[static_cast<size_t>(blockIdx.x) * NV + i] = s;
+    }
+}
+// after the grid barrier: the grid totals in thread 0, summed in the same fixed order by every block (warp 0 only)
+template <int NV>
+__device__ __forceinline__ void step_totals(const double* __restrict__ partials, double (&tot)[NV])
+{
+#pragma unroll
+    for (int i = 0; i < NV; ++i)
+    {
+        double s = 0.0;
+        for (unsigned int b = threadIdx.x; b < gridDim.x; b += 32) s += __ldcg(&partials[static_cast<size_t>(b) * NV + i]);
+        tot[i] = warp_sum(s);
+    }
+}
+
+template <bool INIT>
+__global__ void __launch_bounds__(kStepThreads, 3)
+k_cg_step(GridView g, RegView rv, SolveVecs sv, int64_t items, int K, const double* __restrict__ type_w, const double* __restrict__ minv,
+          float dmin, float dmax, CgCtl* __restrict__ ctl, ReduceSite op_site, const double* __restrict__ eg_partial, ReduceSite upd_site)
+{
+    extern __shared__ float s_slot[];       // [K][8][blockDim]: q (A -> B), then z (B -> C)
+    __shared__ CgCtl s_ctl;
+    __shared__ double red_smem[32];
+    pdl_prologue();
+    cooperative_groups::grid_group grid = cooperative_groups::this_grid();
+    const int tid = threadIdx.x;
+    if (tid == 0) s_ctl = *ctl;
+    __syncthreads();
+    if (!INIT && s_ctl.done) return;
+    const int64_t n = sv.n;
+    const int64_t T = static_cast<int64_t>(gridDim.x) * blockDim.x;
+    const int64_t gt = blockIdx.x * static_cast<int64_t>(blockDim.x) + tid;
+    const float inv_radius = static_cast<float>(s_ctl.inv_radius);
+    const int64_t tail0 = (2 * n) & ~int64_t(3);     // first unknown k_cg_update takes on its scalar path
+    auto slot = [&](int k, int u) -> float& { return s_slot[(k * kStepSlots + u) * blockDim.x + tid]; };
+
+    // camera block of this thread (poses f < F: 6, intrinsics: 4, distortion: 5 unknowns)
+    const int64_t cblk = T - 1 - gt;
+    int m = 0; int64_t cbase = 0; const double* Mi = nullptr;
+    if (cblk < sv.F + 2)
+    {
+        const int blk = static_cast<int>(cblk);
+        const int64_t n2 = 2 * n;
+        if (blk < sv.F) { m = 6; cbase = n2 + 6 * static_cast<int64_t>(blk); Mi = minv + 36 * static_cast<size_t>(blk); }
+        else if (blk == sv.F) { m = 4; cbase = n2 + 6 * static_cast<int64_t>(sv.F); Mi = minv + 36 * static_cast<size_t>(sv.F); }
+        else { m = 5; cbase = n2 + 6 * static_cast<int64_t>(sv.F) + 4; Mi = minv + 36 * static_cast<size_t>(sv.F) + 16; }
+    }
+
+    // ------------------------------------------------------------------ A: operator finish (k_op_partial<APPLY_CG>)
+    if (!INIT)
+    {
+        double acc[1] = {0.0};
+        const float wr = static_cast<float>(type_w[1]), ws = static_cast<float>(type_w[2]), wa = static_cast<float>(type_w[3]);
+        const float* __restrict__ ps = sv.ps;
+        for (int k = 0; k < K; ++k)
+        {
+            const int64_t item = gt + k * T;
+            if (item >= items) break;
+            const int64_t v0 = 4 * item;
+            const int cnt = n - v0 < 4 ? static_cast<int>(n - v0) : 4;
+            float regs[2][4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+            {
+                regs[0][i] = 0.0f; regs[1][i] = 0.0f;
+                if (i >= cnt) continue;
+                const int64_t v = v0 + i;
+                int32_t nb[6];
+#pragma unroll
+                for (int o = 0; o < 6; ++o) nb[o] = (rv.use_er || rv.use_ea) ? g.nbr[static_cast<int64_t>(o) * n + v] : -1;
+                // sdf unknown v
+                float reg = 0.0f;
+                if (rv.use_er)
+                {
+                    const float t0 = sv.tr[v];
+                    // the chain's k_op_partial fuses -6 t0 + tr[nb_0] into one FMA for the voxels v % 4 < 2 (the first two of
+                    // its four unrolled elements) and rounds the product for the other two
+                    float tt;
+                    if (i < 2 && nb[0] >= 0) tt = __fmaf_rn(t0, -6.0f, sv.tr[nb[0]]);
+                    else { tt = __fmul_rn(t0, -6.0f); if (nb[0] >= 0) tt = __fadd_rn(tt, sv.tr[nb[0]]); }
+#pragma unroll
+                    for (int o = 1; o < 6; ++o) if (nb[o] >= 0) tt = __fadd_rn(tt, sv.tr[nb[o]]);
+                    reg = __fmaf_rn(wr, tt, reg);
+                    acc[0] += static_cast<double>(wr) * t0 * t0;
+                }
+                const uint8_t fl = rv.flags[v];
+                if (rv.use_es && (fl & FL_ACTIVE) && (fl & FL_ES_JAC))
+                {
+                    const float u = ps[v];
+                    reg = __fmaf_rn(ws, u, reg);
+                    acc[0] += static_cast<double>(ws) * u * u;
+                }
+                regs[0][i] = reg;
+                // albedo unknown n + v
+                reg = 0.0f;
+                if (rv.use_ea)
+                {
+                    const float pa = ps[n + v];
+#pragma unroll
+                    for (int d = 0; d < 3; ++d)
+                    {
+                        const float wp = rv.ea_w[static_cast<int64_t>(d) * n + v];
+                        if (wp != 0.0f)
+                        {
+                            const float du = __fsub_rn(pa, ps[n + nb[2 * d]]);
+                            reg = __fmaf_rn(__fmul_rn(wa, wp), du, reg);
+                            acc[0] += static_cast<double>(wa) * wp * du * du;
+                        }
+                        const int32_t mm = nb[2 * d + 1];
+                        if (mm >= 0)
+                        {
+                            const float wm = rv.ea_w[static_cast<int64_t>(d) * n + mm];
+                            if (wm != 0.0f) reg = __fmaf_rn(__fmul_rn(wa, wm), __fsub_rn(pa, ps[n + mm]), reg);
+                        }
+                    }
+                }
+                regs[1][i] = reg;
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+            {
+                const int64_t j0 = h * n + v0;
+                const bool vec = cnt == 4 && (h == 0 || (n & 3) == 0);      // albedo unknowns n + 4i: 16 B aligned when n is
+                float pj[4], jt[4], sj[4];
+                double eg[4];
+                ld4n(sv.p, j0, cnt, vec, pj); ld4n(sv.jtj, j0, cnt, vec, jt); ld4n(sv.s, j0, cnt, vec, sj);
+                if (vec)
+                {
+                    const double2 e01 = *reinterpret_cast<const double2*>(sv.qgd + j0), e23 = *reinterpret_cast<const double2*>(sv.qgd + j0 + 2);
+                    eg[0] = e01.x; eg[1] = e01.y; eg[2] = e23.x; eg[3] = e23.y;
+                }
+                else
+                {
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) eg[i] = i < cnt ? sv.qgd[j0 + i] : 0.0;
+                }
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                {
+                    if (i >= cnt) continue;
+                    if (eg[i] != 0.0) sv.qgd[j0 + i] = 0.0;
+                    // qg_j as k_op_partial leaves it (qg is zero on entry): its update is skipped when the sum is zero
+                    const float add = __fadd_rn(static_cast<float>(eg[i]), regs[h][i]);
+                    const float qg = (add != 0.0f) ? add : 0.0f;
+                    const float d2 = __fmul_rn(lm_diag(jt[i], dmin, dmax), inv_radius);
+                    acc[0] += static_cast<double>(d2) * pj[i] * pj[i];
+                    // k_cg_update's q: fma(s, qg, D^2 p) on its 16 B path, fma(D^2, p, s qg) on its scalar tail (the last 2n % 4
+                    // unknowns) and for the camera blocks
+                    slot(k, 4 * h + i) = (j0 + i < tail0) ? __fmaf_rn(sj[i], qg, __fmul_rn(d2, pj[i])) : __fmaf_rn(d2, pj[i], __fmul_rn(sj[i], qg));
+                }
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 6; ++k)
+        {
+            if (k >= m) break;
+            const int64_t j = cbase + k;
+            const double eg = sv.qgd[j];
+            if (eg != 0.0) sv.qgd[j] = 0.0;
+            const float add = __fadd_rn(static_cast<float>(eg), 0.0f);
+            const float qg = (add != 0.0f) ? add : 0.0f;
+            const float pj = sv.p[j];
+            const float d2 = __fmul_rn(lm_diag(sv.jtj[j], dmin, dmax), inv_radius);
+            acc[0] += static_cast<double>(d2) * pj * pj;
+            sv.z[j] = __fmaf_rn(d2, pj, __fmul_rn(sv.s[j], qg));
+        }
+        step_partials<1>(acc, op_site.partials, red_smem);
+        grid.sync();
+        if (tid < 32)
+        {
+            double tot[1];
+            step_totals<1>(op_site.partials, tot);
+            if (tid == 0)
+            {
+                const double total = tot[0] + eg_partial[0];
+                epilogue_operator(&s_ctl, total, APPLY_CG, 1);
+                if (blockIdx.x == 0) { op_site.out[0] = total; if (s_ctl.done) *ctl = s_ctl; }
+            }
+        }
+        __syncthreads();
+        if (s_ctl.done) return;
+    }
+
+    // ------------------------------------------------------------------ B: update (k_cg_update)
+    {
+        double acc[3] = {0.0, 0.0, 0.0};      // rho = r.z, 2Q = -x.(b + r), x.D^2 x
+        const float alpha = INIT ? 0.0f : static_cast<float>(s_ctl.alpha);
+        for (int k = 0; k < K; ++k)
+        {
+            const int64_t item = gt + k * T;
+            if (item >= items) break;
+            const int64_t v0 = 4 * item;
+            const int cnt = n - v0 < 4 ? static_cast<int>(n - v0) : 4;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+            {
+                const int64_t j0 = h * n + v0;
+                const bool vec = cnt == 4 && (h == 0 || (n & 3) == 0);      // albedo unknowns n + 4i: 16 B aligned when n is
+                float bj[4], jt[4], vj[4], xo[4], ro[4], xn[4], rn[4];
+                ld4n(sv.b, j0, cnt, vec, bj); ld4n(sv.jtj, j0, cnt, vec, jt);
+                if (!INIT) { ld4n(sv.p, j0, cnt, vec, vj); ld4n(sv.x, j0, cnt, vec, xo); ld4n(sv.r, j0, cnt, vec, ro); }
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                {
+                    const float d2 = __fmul_rn(lm_diag(jt[i], dmin, dmax), inv_radius);
+                    if (INIT) { xn[i] = 0.0f; rn[i] = bj[i]; }
+                    else
+                    {
+                        const float qj = (i < cnt) ? slot(k, 4 * h + i) : 0.0f;
+                        xn[i] = __fmaf_rn(alpha, vj[i], xo[i]);
+                        rn[i] = __fmaf_rn(-alpha, qj, ro[i]);
+                    }
+                    if (i >= cnt) continue;
+                    const float zn = __fdiv_rn(rn[i], __fadd_rn(jt[i], d2));
+                    slot(k, 4 * h + i) = zn;
+                    acc[0] += static_cast<double>(rn[i]) * zn;
+                    acc[1] -= static_cast<double>(xn[i]) * (static_cast<double>(bj[i]) + rn[i]);
+                    acc[2] += static_cast<double>(d2) * xn[i] * xn[i];
+                }
+                st4n(sv.x, j0, cnt, vec, xn); st4n(sv.r, j0, cnt, vec, rn);
+            }
+        }
+        if (m > 0)
+        {
+            float rr[6];
+            double a0 = 0.0, a1 = 0.0, a2 = 0.0;
+#pragma unroll
+            for (int k = 0; k < 6; ++k)
+            {
+                rr[k] = 0.0f;
+                if (k >= m) continue;
+                const int64_t j = cbase + k;
+                const float bj = sv.b[j];
+                const float d2 = __fmul_rn(lm_diag(sv.jtj[j], dmin, dmax), inv_radius);
+                float xj, rj;
+                if (INIT) { xj = 0.0f; rj = bj; }
+                else
+                {
+                    const float vj = sv.p[j];
+                    xj = __fmaf_rn(alpha, vj, sv.x[j]);
+                    rj = __fmaf_rn(-alpha, sv.z[j], sv.r[j]);
+                }
+                sv.x[j] = xj; sv.r[j] = rj; rr[k] = rj;
+                a1 -= static_cast<double>(xj) * (static_cast<double>(bj) + rj);
+                a2 += static_cast<double>(d2) * xj * xj;
+            }
+#pragma unroll
+            for (int i = 0; i < 6; ++i)
+            {
+                if (i >= m) continue;
+                double ssum = 0.0;
+#pragma unroll
+                for (int k = 0; k < 6; ++k) if (k < m) ssum += Mi[i * m + k] * static_cast<double>(rr[k]);
+                sv.z[cbase + i] = static_cast<float>(ssum);
+                a0 += static_cast<double>(rr[i]) * ssum;
+            }
+            acc[0] += a0; acc[1] += a1; acc[2] += a2;
+        }
+        step_partials<3>(acc, upd_site.partials, red_smem);
+        grid.sync();
+        if (tid < 32)
+        {
+            double tot[3];
+            step_totals<3>(upd_site.partials, tot);
+            if (tid == 0)
+            {
+                epilogue_update(&s_ctl, tot[0], tot[1], tot[2], INIT);
+                if (blockIdx.x == 0) { upd_site.out[0] = tot[0]; upd_site.out[1] = tot[1]; upd_site.out[2] = tot[2]; *ctl = s_ctl; }
+            }
+        }
+        __syncthreads();
+        if (s_ctl.done) return;
+    }
+
+    // ------------------------------------------------------------------ C: direction of the next iteration (k_cg_dir4)
+    const float beta = static_cast<float>(s_ctl.beta);
+    for (int k = 0; k < K; ++k)
+    {
+        const int64_t item = gt + k * T;
+        if (item >= items) break;
+        const int64_t v0 = 4 * item;
+        const int cnt = n - v0 < 4 ? static_cast<int>(n - v0) : 4;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+        {
+            const int64_t j0 = h * n + v0;
+            const bool vec = cnt == 4 && (h == 0 || (n & 3) == 0);      // albedo unknowns n + 4i: 16 B aligned when n is
+            float p[4], s4[4], ps[4];
+            ld4n(sv.s, j0, cnt, vec, s4);
+            if (beta != 0.0f) ld4n(sv.p, j0, cnt, vec, p);      // first iteration: p may hold anything
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+            {
+                const float z = (i < cnt) ? slot(k, 4 * h + i) : 0.0f;
+                p[i] = (beta == 0.0f) ? z : __fmaf_rn(beta, p[i], z);
+                ps[i] = __fmul_rn(s4[i], p[i]);
+            }
+            st4n(sv.p, j0, cnt, vec, p); st4n(sv.ps, j0, cnt, vec, ps);
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 6; ++k)
+    {
+        if (k >= m) break;
+        const int64_t j = cbase + k;
+        const float p = (beta == 0.0f) ? sv.z[j] : __fmaf_rn(beta, sv.p[j], sv.z[j]);
+        sv.p[j] = p; sv.ps[j] = __fmul_rn(sv.s[j], p);
+    }
 }
 
 // ---- multi-GPU exchange buffers ---------------------------------------------------------------------------------

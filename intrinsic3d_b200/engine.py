@@ -34,7 +34,7 @@ EXPORTED_SYMBOLS = [
     "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh", "i3d_extract_mesh_colored", "i3d_mode_colors",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
-    "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_normal_equations",
+    "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_pcg_vectors", "i3d_debug_get_normal_equations",
     "i3d_debug_apply_operator", "i3d_debug_fusion_num_voxels", "i3d_debug_get_fusion_volume", "i3d_debug_get_frames",
 ]
 KEYFRAME_CHUNK = 32       # I3D_KEYFRAME_CHUNK of include/i3d_c_api.h: frames scored per device pass
@@ -469,6 +469,13 @@ class Engine:
         cs = np.zeros(U, np.float64)
         self._check(self.L.i3d_debug_get_step(self.h, _p(st, C.c_double), _p(fm, C.c_uint8), _p(cs, C.c_double)))
         return st, fm, cs
+
+    def debug_pcg_vectors(self):
+        """(x, p): the PCG iterate and search direction (float32 [U], Jacobi-scaled) as the last LM trial's solve left them."""
+        U = 2 * self.n + 6 * self.F + 9
+        x, p = np.empty(U, np.float32), np.empty(U, np.float32)
+        self._check(self.L.i3d_debug_get_pcg_vectors(self.h, _p(x, C.c_float), _p(p, C.c_float)))
+        return x, p
 
     def debug_normal_equations(self):
         """b = J'^T f, Jacobi scale s, jtj = s^2 colnorm^2 (float32 [U]) and the raw E_g camera sums cam_acc (float32 [33F + 43])."""
