@@ -706,7 +706,7 @@ int check_frame_limit(I3DEngine* e, int F, int K)
     CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->device));
     cudaFuncAttributes fa_acc{}, fa_app{};
     CK(cudaFuncGetAttributes(&fa_acc, k_eg_accum));
-    CK(cudaFuncGetAttributes(&fa_app, k_eg_apply<APPLY_CG>));
+    CK(cudaFuncGetAttributes(&fa_app, k_eg_apply));
     const size_t lim = static_cast<size_t>(optin);
     auto fits = [&](int f) { return fa_acc.sharedSizeBytes + accum_smem_bytes(f, K) <= lim && fa_app.sharedSizeBytes + apply_smem_bytes(f, K) <= lim; };
     if (fits(F)) return 0;
@@ -723,20 +723,20 @@ void launch_eg_apply(I3DEngine* e, const GridView& g, const RegView& rv, const E
     if (rows.n_active > 0)
     {
         KernelTimer kt(e, "k_eg_apply", 0);     // the dominant kernel: every launch is timed (roofline = true average)
-        pdl_launch(e, k_eg_apply<APPLY_CG>, blocks_for(rows.n_active), kThreads, apply_smem_bytes(e->F, rows.K), g, rows, rv, sv, sv.ps, e->ctl.p, 1, e->site(SITE_EG_APPLY));
+        pdl_launch(e, k_eg_apply, blocks_for(rows.n_active), kThreads, apply_smem_bytes(e->F, rows.K), g, rows, rv, sv, sv.ps, e->ctl.p, e->site(SITE_EG_APPLY));
     }
     e->launches += 1;
 }
 
 void launch_operator(I3DEngine* e, const GridView& g, const RegView& rv, const EgRows& rows, const SolveVecs& sv, const Shard& sh, const float* vin,
-                     float dmin, float dmax, int is_cg_iteration, bool sample_timing = false)
+                     float dmin, float dmax, int is_cg_iteration)
 {
     launch_eg_apply(e, g, rv, rows, sv);
     e->launches += 1;
     {
         KernelTimer kt(e, "k_op_partial");
-        pdl_launch(e, (k_op_partial<APPLY_CG, 4>), blocks_for(static_cast<size_t>((e->held_count() + 3) / 4)), kThreads, 0, 
-            g, rv, sv, sh, e->held_count(), vin, sv.ps, e->type_w.p, dmin, dmax, e->ctl.p, 1, e->site(SITE_OP_POST), e->site(SITE_EG_APPLY).out, is_cg_iteration);
+        pdl_launch(e, k_op_partial, blocks_for(static_cast<size_t>((e->held_count() + 3) / 4)), kThreads, 0,
+            g, rv, sv, sh, e->held_count(), vin, sv.ps, e->type_w.p, dmin, dmax, e->ctl.p, e->site(SITE_OP_POST), e->site(SITE_EG_APPLY).out, is_cg_iteration);
     }
     if (e->world > 1)
     {
@@ -912,8 +912,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     e->row_frame.ensure(S + 1); e->row_res.ensure(S + 1); e->row_wraw.ensure(S + 1);
     e->ea_w.ensure(3 * static_cast<size_t>(n)); e->lap.ensure(n);
     // set unconditionally: the default limit is 48 KB minus the kernel's static shared memory, not 48 KB
-    CK(cudaFuncSetAttribute(k_eg_apply<APPLY_CG>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(apply_smem_bytes(F, K))));
-    CK(cudaFuncSetAttribute(k_eg_apply<APPLY_MODEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(apply_smem_bytes(F, K))));
+    CK(cudaFuncSetAttribute(k_eg_apply, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(apply_smem_bytes(F, K))));
     const EgRows rows = eg_rows(e);
     CamView cv{e->cam, e->pose_ctx.p, F};
     if (n_active > 0)
@@ -967,12 +966,11 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     // ------------------------------------------------------------------ LM loop (TrustRegionMinimizer + LevenbergMarquardtStrategy)
     Timer t_solve(e, "solve", 3);
     const float dmin = static_cast<float>(P.min_lm_diagonal), dmax = static_cast<float>(std::min(P.max_lm_diagonal, 3.0e38));
-    // voxel unknowns: 4 per thread (16 B accesses) in the single-GPU identity layout, 1 per thread through the held list when sharded
     // voxel unknowns of the held hull: 4 per thread (16 B accesses); the first F + 2 threads take one camera block each
     const unsigned upd_blocks = blocks_for(static_cast<size_t>((sh.held_voxel_unknowns() + 3) / 4 + F + 2));
     auto launch_update = [&](bool init, int refresh) {
-        if (init) pdl_launch(e, (k_cg_update<true, 4>), upd_blocks, kThreads, 0, sv, sh, e->minv.p, dmin, dmax, e->ctl.p, refresh, e->site(SITE_UPDATE));
-        else pdl_launch(e, (k_cg_update<false, 4>), upd_blocks, kThreads, 0, sv, sh, e->minv.p, dmin, dmax, e->ctl.p, refresh, e->site(SITE_UPDATE));
+        if (init) pdl_launch(e, k_cg_update<true>, upd_blocks, kThreads, 0, sv, sh, e->minv.p, dmin, dmax, e->ctl.p, refresh, e->site(SITE_UPDATE));
+        else pdl_launch(e, k_cg_update<false>, upd_blocks, kThreads, 0, sv, sh, e->minv.p, dmin, dmax, e->ctl.p, refresh, e->site(SITE_UPDATE));
         e->launches += 1;
     };
     const unsigned vec_blocks = blocks_for(static_cast<size_t>(hc));
@@ -1001,7 +999,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
                 dir_ready = true;
                 continue;
             }
-            launch_operator(e, g, rv, rows, sv, sh, sv.p, dmin, dmax, 1, enq == 1);
+            launch_operator(e, g, rv, rows, sv, sh, sv.p, dmin, dmax, 1);
             if (refresh)
             {
                 // exact residual: x += alpha p ; r = b - A x   (needs the operator's qg consumed first: do the plain update

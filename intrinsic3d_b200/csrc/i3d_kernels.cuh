@@ -1436,6 +1436,17 @@ k_finish_problem(GridView g, RegView rv, SolveVecs sv, Shard sh, int64_t count, 
 // LevenbergMarquardtStrategy: diag = clamp(colnorm^2(J'), min, max); D^2 = diag / radius
 __device__ __forceinline__ float lm_diag(float jtj, float dmin, float dmax) { return fminf(fmaxf(jtj, dmin), dmax); }
 
+// Camera block blk of the block-Jacobi preconditioner: blk < F the pose of frame blk (6 unknowns), F the intrinsics (4), F + 1 the
+// distortion (5).  base = its first unknown; its inverse is minv[moff, moff + m * m).
+struct CamBlock { int m; int64_t base; size_t moff; };
+__device__ __forceinline__ CamBlock cam_block(int blk, int F, int64_t n)
+{
+    const int64_t c0 = 2 * n + 6 * static_cast<int64_t>(F);
+    if (blk < F) return {6, 2 * n + 6 * static_cast<int64_t>(blk), 36 * static_cast<size_t>(blk)};
+    if (blk == F) return {4, c0, 36 * static_cast<size_t>(F)};
+    return {5, c0 + 4, 36 * static_cast<size_t>(F) + 16};
+}
+
 // Block-Jacobi preconditioner blocks of the camera parameters (BlockJacobiPreconditioner + Invert):
 // M_f = S G_f S * w_g + D^2, inverted by Cholesky in double.  One thread per block (F poses + intrinsics + distortion).
 __device__ inline bool chol_inverse(int m, double* A /* m*m in, L out */, double* inv)
@@ -1478,10 +1489,9 @@ __global__ void k_cam_precond(SolveVecs sv, const float* __restrict__ cam_acc, c
     const CamAccLayout lay{F};
     const double wg = type_w[0];
     const double inv_radius = ctl->inv_radius;
-    int m; const float* tri; int64_t base; double* out;
-    if (t < F) { m = 6; tri = cam_acc + lay.pose_stride() * t + 12; base = 2 * sv.n + 6 * static_cast<int64_t>(t); out = minv + 36 * static_cast<size_t>(t); }
-    else if (t == F) { m = 4; tri = cam_acc + lay.tail() + 18; base = 2 * sv.n + 6 * static_cast<int64_t>(F); out = minv + 36 * static_cast<size_t>(F); }
-    else { m = 5; tri = cam_acc + lay.tail() + 18 + 10; base = 2 * sv.n + 6 * static_cast<int64_t>(F) + 4; out = minv + 36 * static_cast<size_t>(F) + 16; }
+    const CamBlock cb = cam_block(t, F, sv.n);
+    const int m = cb.m; const int64_t base = cb.base; double* out = minv + cb.moff;
+    const float* tri = cam_acc + (t < F ? lay.pose_stride() * t + 12 : lay.tail() + (t == F ? 18 : 18 + 10));
     double A[36];
     int k = 0;
     for (int r = 0; r < m; ++r)
@@ -1499,9 +1509,8 @@ __global__ void k_cam_precond(SolveVecs sv, const float* __restrict__ cam_acc, c
 // ----------------------------------------------------------------------------------------------
 // k5: the CGNR operator  q = J'^T (J' p) + D^2 p   (CgnrLinearOperator::RightMultiply), split in
 //   k_eg_apply   E_g rows: one pass over J, fused J p and J^T (.) with atomics into qg; also the E_r row values of the input vector
-//   k_op_post    regulariser rows (gather form) + D^2 + Jacobi scale, p.q partials
+//   k_op_partial regulariser rows (gather form), p.q partials
 // ----------------------------------------------------------------------------------------------
-enum { APPLY_CG = 0, APPLY_MODEL = 1 };
 
 // unknown-space indices of the 14 voxel columns of voxel v's E_g rows: the sdf stencil in the reference's parameter order
 // (as gather_stencil), then the 4 albedo entries
@@ -1523,7 +1532,7 @@ __device__ __forceinline__ void eg_voxel_unknowns(const GridView& g, int64_t v, 
 // same tiles at 124 registers and 2 blocks per SM (the index re-read alone, at 2 blocks, cost 0.412); parking the indices in
 // shared memory as well (0.408), 128-thread blocks x 6 (0.427) and an L2 prefetch of the next row (0.380) did not help.
 //   u_k = J_k . ps          (ps = s o p, the Jacobi-scaled input)
-//   APPLY_CG   : qg[cols] += sum_k w_k u_k J_k ; partial p.q += w_k u_k^2
+//   qg[cols] += sum_k w_k u_k J_k ; partial p.q += w_k u_k^2
 //       voxel columns          : per-thread sums over the K rows, one global atomic per column per voxel
 //       intrinsics/distortion  : per-thread sums, one warp reduce-scatter at the end
 //       pose columns           : the K contributions of a thread (6 floats each) are parked in shared memory; after the row
@@ -1531,20 +1540,18 @@ __device__ __forceinline__ void eg_voxel_unknowns(const GridView& g, int64_t v, 
 //                                and for each does one 6-value butterfly all-reduce -> 6 shared-memory atomics.
 //                                (A first version reduced per row slot: ~20 passes per warp, 49 % of the kernel's
 //                                instructions were shuffle/select traffic; profiles/r01_summary.md.)
-//   APPLY_MODEL: partial model_cost_change += -w_k u_k (r_k + u_k/2)          (TrustRegionMinimizer::ComputeTrustRegionStep)
 // Contributions are added in double.  A double sum of B float addends is exact, and so independent of the atomics' order, when
 // all addends of one entry lie within about 2^(29 - log2 B) of each other; where they do not, only the final rounding to float
 // hides the order.  Measured: the full C3 scene (1.31 M active voxels, 5101 blocks, 200 frames) gives bit-identical results from
 // run to run over three GN iterations (tests/test_gpu_round2.py::test_c3_run_to_run_bit_identical).
 // (A bulk-async / mbarrier staged variant was measured slower: the kernel is issue-bound, not latency-bound.)
-template <int MODE>
 __global__ void __launch_bounds__(kThreads, 3)
-k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __restrict__ ps, const CgCtl* __restrict__ ctl, int respect_done, ReduceSite site)
+k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __restrict__ ps, const CgCtl* __restrict__ ctl, ReduceSite site)
 {
     pdl_prologue();
     // [6F + 9] camera accumulators (double) | [14][kThreads] ps of the voxel columns | [K][6][kThreads] parked pose contributions
     extern __shared__ double s_dyn_d[];
-    if (respect_done && ctl->done) return;
+    if (ctl->done) return;
     const int ncam = 6 * sv.F + 9;
     double* s_cam = s_dyn_d;
     float* s_pv = reinterpret_cast<float*>(s_dyn_d + ((ncam + 15) & ~15));
@@ -1553,8 +1560,7 @@ k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __res
     // the intrinsics / distortion entries of ps, the same for every row
     __shared__ float s_pt[9];
     if (threadIdx.x < 9) s_pt[threadIdx.x] = ps[2 * n + 6 * static_cast<int64_t>(sv.F) + threadIdx.x];
-    if (MODE == APPLY_CG)
-        for (int i = threadIdx.x; i < ncam; i += blockDim.x) s_cam[i] = 0.0;
+    for (int i = threadIdx.x; i < ncam; i += blockDim.x) s_cam[i] = 0.0;
     __syncthreads();
     const int tid = threadIdx.x, lane = tid & 31;
     const int a = blockIdx.x * blockDim.x + tid;
@@ -1622,91 +1628,79 @@ k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __res
             for (int m = 0; m < 8; m += 4) { u0 += jr[20 + m] * s_pt[m]; u1 += jr[21 + m] * s_pt[m + 1]; u2 += jr[22 + m] * s_pt[m + 2]; u3 += jr[23 + m] * s_pt[m + 3]; }
             u0 += jr[28] * s_pt[8];
             const float u = (u0 + u1) + (u2 + u3);
-            if (MODE == APPLY_CG)
-            {
-                const float wu = w * u;
-                acc[0] += static_cast<double>(wu) * static_cast<double>(u);
+            const float wu = w * u;
+            acc[0] += static_cast<double>(wu) * static_cast<double>(u);
 #pragma unroll
-                for (int m = 0; m < 14; ++m) out[m] += wu * jr[m];
+            for (int m = 0; m < 14; ++m) out[m] += wu * jr[m];
 #pragma unroll
-                for (int c = 0; c < 6; ++c) s_jp[(k * 6 + c) * kThreads + tid] = wu * jr[14 + c];
+            for (int c = 0; c < 6; ++c) s_jp[(k * 6 + c) * kThreads + tid] = wu * jr[14 + c];
 #pragma unroll
-                for (int m = 0; m < 9; ++m) tail[m] += wu * jr[20 + m];
-            }
-            else
-            {
-                const double r = rows.row_res[slot];
-                acc[0] -= static_cast<double>(w) * static_cast<double>(u) * (r + 0.5 * static_cast<double>(u));
-            }
+            for (int m = 0; m < 9; ++m) tail[m] += wu * jr[20 + m];
         }
     }
-    if (MODE == APPLY_CG)
+    // ---- pose columns: walk over the distinct frames of the warp's 32 x K rows
+    // (measured alternative, slower: reducing a slot straight from registers when all 32 rows of the warp share its frame and
+    // parking only mixed slots — 0.305 vs 0.289 ms per launch at C3: the uniformity test costs more than the walk it saves)
+    unsigned todo = 0u;                       // bit k: slot k of this lane still has to be added
+#pragma unroll
+    for (int k = 0; k < I3D_MAX_OBS; ++k) if (fk[k] >= 0) todo |= 1u << k;
+    while (true)
     {
-        // ---- pose columns: walk over the distinct frames of the warp's 32 x K rows
-        // (measured alternative, slower: reducing a slot straight from registers when all 32 rows of the warp share its frame and
-        // parking only mixed slots — 0.305 vs 0.289 ms per launch at C3: the uniformity test costs more than the walk it saves)
-        unsigned todo = 0u;                       // bit k: slot k of this lane still has to be added
+        const unsigned pending = __ballot_sync(0xffffffffu, todo != 0u);
+        if (pending == 0u) break;
+        const int leader = __ffs(pending) - 1;
+        const int mine_f = (todo != 0u) ? fk_select(fk, __ffs(todo) - 1) : -1;
+        const int f0 = __shfl_sync(0xffffffffu, mine_f, leader);
+        float r8[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
 #pragma unroll
-        for (int k = 0; k < I3D_MAX_OBS; ++k) if (fk[k] >= 0) todo |= 1u << k;
-        while (true)
+        for (int k = 0; k < I3D_MAX_OBS; ++k)
         {
-            const unsigned pending = __ballot_sync(0xffffffffu, todo != 0u);
-            if (pending == 0u) break;
-            const int leader = __ffs(pending) - 1;
-            const int mine_f = (todo != 0u) ? fk_select(fk, __ffs(todo) - 1) : -1;
-            const int f0 = __shfl_sync(0xffffffffu, mine_f, leader);
-            float r8[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
-#pragma unroll
-            for (int k = 0; k < I3D_MAX_OBS; ++k)
+            if (k >= rows.K) break;
+            if (((todo >> k) & 1u) && fk[k] == f0)
             {
-                if (k >= rows.K) break;
-                if (((todo >> k) & 1u) && fk[k] == f0)
-                {
 #pragma unroll
-                    for (int c = 0; c < 6; ++c) r8[c] = s_jp[(k * 6 + c) * kThreads + tid];
-                    todo &= ~(1u << k);
-                }
+                for (int c = 0; c < 6; ++c) r8[c] = s_jp[(k * 6 + c) * kThreads + tid];
+                todo &= ~(1u << k);
             }
-            // 8 -> 1 value per lane in three halving exchanges (offsets 16, 8, 4), then an all-reduce over the remaining two
-            // lane bits: 4 + 2 + 1 + 1 + 1 = 9 shuffles (a plain all-reduce of the 6 values needs 30)
-            rs_step<4, 16, 8>(r8, lane);
-            rs_step<2, 8, 8>(r8, lane);
-            rs_step<1, 4, 8>(r8, lane);
-            float val = r8[0];
-            val += __shfl_xor_sync(0xffffffffu, val, 2);
-            val += __shfl_xor_sync(0xffffffffu, val, 1);
-            const int id = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
-            if ((lane & 3) == 0 && id < 6 && val != 0.0f) atomicAdd(s_cam + 6 * f0 + id, static_cast<double>(val));
         }
-        if (any)
-        {
-            uint32_t idx[14];      // read again (L1 hits) rather than held in 14 registers across the row loop
-            eg_voxel_unknowns(g, rows.act[a], idx);
-#pragma unroll
-            for (int m = 0; m < 14; ++m) atomicAdd(sv.qgd + idx[m], static_cast<double>(out[m]));
-        }
-        {
-            float vv[32];
-#pragma unroll
-            for (int m = 0; m < 9; ++m) vv[m] = tail[m];
-#pragma unroll
-            for (int m = 9; m < 32; ++m) vv[m] = 0.0f;
-            warp_reduce_scatter<32>(vv, lane);
-            if (lane < 9 && vv[0] != 0.0f) atomicAdd(s_cam + 6 * sv.F + lane, static_cast<double>(vv[0]));
-        }
-        __syncthreads();
-        // block partial rounded to float, then summed over blocks in double: exact while the partials of one entry stay within
-        // about 2^(29 - log2 B) of each other, B = contributing blocks (see the kernel's comment for what was measured)
-        for (int i = tid; i < ncam; i += blockDim.x) { const float vv = static_cast<float>(s_cam[i]); if (vv != 0.0f) atomicAdd(sv.qgd + 2 * sv.n + i, static_cast<double>(vv)); }
+        // 8 -> 1 value per lane in three halving exchanges (offsets 16, 8, 4), then an all-reduce over the remaining two
+        // lane bits: 4 + 2 + 1 + 1 + 1 = 9 shuffles (a plain all-reduce of the 6 values needs 30)
+        rs_step<4, 16, 8>(r8, lane);
+        rs_step<2, 8, 8>(r8, lane);
+        rs_step<1, 4, 8>(r8, lane);
+        float val = r8[0];
+        val += __shfl_xor_sync(0xffffffffu, val, 2);
+        val += __shfl_xor_sync(0xffffffffu, val, 1);
+        const int id = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
+        if ((lane & 3) == 0 && id < 6 && val != 0.0f) atomicAdd(s_cam + 6 * f0 + id, static_cast<double>(val));
     }
+    if (any)
+    {
+        uint32_t idx[14];      // read again (L1 hits) rather than held in 14 registers across the row loop
+        eg_voxel_unknowns(g, rows.act[a], idx);
+#pragma unroll
+        for (int m = 0; m < 14; ++m) atomicAdd(sv.qgd + idx[m], static_cast<double>(out[m]));
+    }
+    {
+        float vv[32];
+#pragma unroll
+        for (int m = 0; m < 9; ++m) vv[m] = tail[m];
+#pragma unroll
+        for (int m = 9; m < 32; ++m) vv[m] = 0.0f;
+        warp_reduce_scatter<32>(vv, lane);
+        if (lane < 9 && vv[0] != 0.0f) atomicAdd(s_cam + 6 * sv.F + lane, static_cast<double>(vv[0]));
+    }
+    __syncthreads();
+    // block partial rounded to float, then summed over blocks in double: exact while the partials of one entry stay within
+    // about 2^(29 - log2 B) of each other, B = contributing blocks (see the kernel's comment for what was measured)
+    for (int i = tid; i < ncam; i += blockDim.x) { const float vv = static_cast<float>(s_cam[i]); if (vv != 0.0f) atomicAdd(sv.qgd + 2 * sv.n + i, static_cast<double>(vv)); }
     grid_reduce<1>(acc, site);
 }
 
 // ---- scalar epilogues of the PCG iteration (ConjugateGradientsSolver::Solve restated).  Single GPU: run by the last
 // block of the producing kernel; multi GPU: run by k_epilogue after the allreduce of the partial sums.
-__device__ __forceinline__ void epilogue_operator(CgCtl* ctl, double total, int mode, int is_cg_iteration)
+__device__ __forceinline__ void epilogue_operator(CgCtl* ctl, double total, int is_cg_iteration)
 {
-    if (mode == APPLY_MODEL) { ctl->model_cost_change = total; return; }
     if (!is_cg_iteration) return;
     ctl->pq = total;
     if (total <= 0.0 || isinf(total)) { ctl->done = 1; ctl->status = 2; ctl->it += 1; ctl->alpha = 0.0; }
@@ -1752,130 +1746,231 @@ __device__ __forceinline__ void epilogue_update(CgCtl* ctl, double rho_new, doub
     if (stop) ctl->done = 1;
 }
 
-enum { EPI_OPERATOR_CG = 0, EPI_OPERATOR_NOCG = 1, EPI_MODEL = 2, EPI_UPDATE = 3, EPI_UPDATE_INIT = 4 };
+enum { EPI_OPERATOR_CG, EPI_UPDATE, EPI_UPDATE_INIT };
 // multi-GPU: scalars[] holds the ALLREDUCED sums
 __global__ void k_epilogue(CgCtl* __restrict__ ctl, const double* __restrict__ scalars, int kind, int respect_done)
 {
     pdl_prologue();
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
     if (respect_done && kind != EPI_UPDATE_INIT && ctl->done) return;
-    if (kind == EPI_OPERATOR_CG) epilogue_operator(ctl, scalars[0], APPLY_CG, 1);
-    else if (kind == EPI_MODEL) epilogue_operator(ctl, scalars[0], APPLY_MODEL, 0);
+    if (kind == EPI_OPERATOR_CG) epilogue_operator(ctl, scalars[0], 1);
     else if (kind == EPI_UPDATE) epilogue_update(ctl, scalars[0], scalars[1], scalars[2], false);
     else if (kind == EPI_UPDATE_INIT) epilogue_update(ctl, scalars[0], scalars[1], scalars[2], true);
+}
+
+// ---- per-unknown arithmetic of a PCG iteration, shared by the kernel chain (k_op_partial, k_cg_update, k_cg_dir4) and the
+// cooperative k_cg_step.  Every float operation is written with an explicit-rounding intrinsic, so both paths round each one alike
+// whatever the compiler would contract.  Ownership enters as a type: the chain kernels pass their Shard (a sharded rank adds only
+// the rows of the voxels it owns), k_cg_step passes OwnAll (single GPU), which costs nothing.
+struct OwnAll
+{
+    __device__ __forceinline__ bool owns_voxel(int64_t) const { return true; }
+};
+
+// D_j^2 = lm_diag(jtj_j) / radius, in float
+__device__ __forceinline__ float cg_d2(float jtj, float dmin, float dmax, float inv_radius) { return __fmul_rn(lm_diag(jtj, dmin, dmax), inv_radius); }
+
+// Regulariser rows touching sdf unknown v in gather form, raw weights:  wr (-6 t_v + sum_o t_nbr(o)) + ws ps_v  over the E_r rows
+// (t = their values for the input vector, from k_eg_apply) and the E_s row of the voxels this rank owns; adds the rows' share of
+// p.q to acc.  nbr(o) = neighbour o of v, -1 for none.  Rounding: -6 t_v + t_nbr(0) is one FMA when `fuse0` and rounds the product
+// first otherwise; both paths pass fuse0 for the first two unknowns of each group of four.  Kept so that results stay byte-identical.
+template <class Own, class Nbr>
+__device__ __forceinline__ float reg_sdf(const RegView& rv, const float* __restrict__ tr, const float* __restrict__ ps, int64_t v, Nbr nbr,
+                                         const Own& own, float wr, float ws, bool fuse0, double& acc)
+{
+    float reg = 0.0f;
+    const bool ov = own.owns_voxel(v);
+    if (rv.use_er)
+    {
+        const float t0 = ov ? tr[v] : 0.0f;
+        const int32_t nb0 = nbr(0);
+        const bool has0 = nb0 >= 0 && own.owns_voxel(nb0);
+        float tt;
+        if (fuse0 && has0) tt = __fmaf_rn(t0, -6.0f, tr[nb0]);
+        else { tt = __fmul_rn(t0, -6.0f); if (has0) tt = __fadd_rn(tt, tr[nb0]); }
+#pragma unroll
+        for (int o = 1; o < 6; ++o) { const int32_t nb = nbr(o); if (nb >= 0 && own.owns_voxel(nb)) tt = __fadd_rn(tt, tr[nb]); }
+        reg = __fmaf_rn(wr, tt, reg);
+        acc += static_cast<double>(wr) * t0 * t0;
+    }
+    const uint8_t fl = rv.flags[v];
+    if (rv.use_es && ov && (fl & FL_ACTIVE) && (fl & FL_ES_JAC))
+    {
+        const float u = ps[v];
+        reg = __fmaf_rn(ws, u, reg);
+        acc += static_cast<double>(ws) * u * u;
+    }
+    return reg;
+}
+
+// Regulariser rows touching albedo unknown n + v in gather form, raw weights:  wa sum_d [w(d, v) (ps_v - ps_{v+e_d}) +
+// w(d, v-e_d) (ps_v - ps_{v-e_d})]  over the E_a pairs this rank owns (the pair {v, v + e_d} is stored at (d, v) and belongs to the
+// owner of v); adds the pairs' share of p.q to acc.  nbr(2d) = v + e_d, nbr(2d + 1) = v - e_d.
+template <class Own, class Nbr>
+__device__ __forceinline__ float reg_albedo(const RegView& rv, const float* __restrict__ ps, int64_t n, int64_t v, Nbr nbr, const Own& own,
+                                            float wa, double& acc)
+{
+    float reg = 0.0f;
+    if (!rv.use_ea) return reg;
+    const float pa = ps[n + v];
+    const bool ov = own.owns_voxel(v);
+#pragma unroll
+    for (int d = 0; d < 3; ++d)
+    {
+        const float wp = ov ? rv.ea_w[static_cast<int64_t>(d) * n + v] : 0.0f;
+        if (wp != 0.0f)
+        {
+            const float du = __fsub_rn(pa, ps[n + nbr(2 * d)]);
+            reg = __fmaf_rn(__fmul_rn(wa, wp), du, reg);
+            acc += static_cast<double>(wa) * wp * du * du;
+        }
+        const int32_t m = nbr(2 * d + 1);
+        if (m >= 0 && own.owns_voxel(m))
+        {
+            const float wm = rv.ea_w[static_cast<int64_t>(d) * n + m];
+            if (wm != 0.0f) reg = __fmaf_rn(__fmul_rn(wa, wm), __fsub_rn(pa, ps[n + m]), reg);
+        }
+    }
+    return reg;
+}
+
+// Operator finish of unknown j: the E_g part (summed in double by k_eg_apply) rounded once, plus the regulariser rows.  qg_j is zero
+// before it and is left at zero when this sum is zero.
+__device__ __forceinline__ float op_qg(double qgd, float reg) { return __fadd_rn(static_cast<float>(qgd), reg); }
+
+// The operator output q_j = s_j qg_j + D_j^2 v_j.  Rounding: fma(s, qg, D^2 v) for the unknowns the update takes in 16 B groups of
+// four (`vec`), fma(D^2, v, s qg) for the others (the last 2n % 4 voxel unknowns, unaligned groups of a shard, the camera blocks).
+// Kept so that results stay byte-identical.
+__device__ __forceinline__ float op_q(float s, float qg, float d2, float v, bool vec)
+{
+    return vec ? __fmaf_rn(s, qg, __fmul_rn(d2, v)) : __fmaf_rn(d2, v, __fmul_rn(s, qg));
+}
+
+// x and r of one unknown after the operator output q = A v:  x += alpha v, r -= alpha q;  refresh (v = x, already advanced by
+// k_x_update, every residual_reset_period iterations): r = b - q, the exact residual
+__device__ __forceinline__ void cg_xr(float b, float q, float v, float x0, float r0, float alpha, bool refresh, float& x, float& r)
+{
+    x = refresh ? x0 : __fmaf_rn(alpha, v, x0);
+    r = refresh ? __fsub_rn(b, q) : __fmaf_rn(-alpha, q, r0);
+}
+
+// z = r / (jtj + D^2), the preconditioner of a voxel unknown; adds rho = r.z, 2Q = -x.(b + r) and x.D^2 x to acc when `owned`
+__device__ __forceinline__ float cg_z(float x, float r, float b, float jt, float d2, bool owned, double (&acc)[3])
+{
+    const float z = __fdiv_rn(r, __fadd_rn(jt, d2));
+    if (owned)
+    {
+        acc[0] += static_cast<double>(r) * z;
+        acc[1] -= static_cast<double>(x) * (static_cast<double>(b) + r);
+        acc[2] += static_cast<double>(d2) * x * x;
+    }
+    return z;
+}
+
+// Camera block cb: x and r of its unknowns (INIT: x = 0, r = b; otherwise the operator output is q(j, D_j^2, v_j)), then z = M^-1 r
+// in double with the block's inverse from k_cam_precond.  Returns the block's rho, 2Q and x.D^2 x in a.
+template <bool INIT, class Q>
+__device__ __forceinline__ void cam_block_update(const SolveVecs& sv, const CamBlock& cb, const double* __restrict__ minv, float dmin, float dmax,
+                                                 float inv_radius, float alpha, bool refresh, Q q, double (&a)[3])
+{
+    const double* Mi = minv + cb.moff;
+    float rr[6];
+    a[0] = 0.0; a[1] = 0.0; a[2] = 0.0;
+#pragma unroll
+    for (int k = 0; k < 6; ++k)
+    {
+        rr[k] = 0.0f;
+        if (k >= cb.m) continue;
+        const int64_t j = cb.base + k;
+        const float b = sv.b[j];
+        const float d2 = cg_d2(sv.jtj[j], dmin, dmax, inv_radius);
+        float x = 0.0f, r = b;
+        if (!INIT)
+        {
+            const float v = refresh ? sv.x[j] : sv.p[j];
+            const float qj = q(j, d2, v);
+            cg_xr(b, qj, v, sv.x[j], sv.r[j], alpha, refresh, x, r);
+        }
+        sv.x[j] = x; sv.r[j] = r; rr[k] = r;
+        a[1] -= static_cast<double>(x) * (static_cast<double>(b) + r);
+        a[2] += static_cast<double>(d2) * x * x;
+    }
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+    {
+        if (i >= cb.m) continue;
+        double ssum = 0.0;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) if (k < cb.m) ssum += Mi[i * cb.m + k] * static_cast<double>(rr[k]);
+        sv.z[cb.base + i] = static_cast<float>(ssum);
+        a[0] += static_cast<double>(rr[i]) * ssum;
+    }
+}
+
+// The next direction p = z + beta p and ps = s o p.  beta == 0 (the first iteration): p = z, whatever p holds.
+__device__ __forceinline__ void cg_dir(float z, float p, float s, float beta, float& p_out, float& ps_out)
+{
+    p_out = (beta == 0.0f) ? z : __fmaf_rn(beta, p, z);
+    ps_out = __fmul_rn(s, p_out);
 }
 
 // Per-unknown part of the operator: adds the regulariser rows OWNED by this rank (gather form) into qg, in place:
 //     qg[j] += qgd[j] (k_eg_apply's E_g part, rounded once; qgd is cleared) + sum over owned E_r / E_s / E_a rows touching j
 //     (raw, Jacobi scale applied by the consumer)
 // The operator output  q_j = s_j * qg_j(total) + D_j^2 p_j  is never materialised: k_cg_update forms it on the fly.
-// MODE APPLY_CG   : partial p.q += (owned regulariser rows)^2 + D^2 p^2 (owned unknowns); last block: alpha = rho / pq.
-// MODE APPLY_MODEL: partial model_cost_change of the owned regulariser rows (qg untouched).
-template <int MODE, int VEC>
+// Partial p.q += (owned regulariser rows)^2 + D^2 p^2 (owned unknowns); last block: alpha = rho / pq.
+// 4 consecutive unknowns per thread (unrolled: the gathers of the four are independent and overlap).
 __global__ void __launch_bounds__(kThreads)
 k_op_partial(GridView g, RegView rv, SolveVecs sv, Shard sh, int64_t count, const float* __restrict__ pin, const float* __restrict__ ps,
-             const double* __restrict__ type_w, float dmin, float dmax, CgCtl* __restrict__ ctl, int respect_done,
+             const double* __restrict__ type_w, float dmin, float dmax, CgCtl* __restrict__ ctl,
              ReduceSite site, const double* __restrict__ eg_partial /* site.out of k_eg_apply */, int is_cg_iteration)
 {
     pdl_prologue();
-    if (respect_done && ctl->done) return;
-    const int64_t tbase = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) * VEC;
+    if (ctl->done) return;
+    const int64_t tbase = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) * 4;
     double acc[1] = {0.0};
     const int64_t n = g.n;
     const float wr = static_cast<float>(type_w[1]), ws = static_cast<float>(type_w[2]), wa = static_cast<float>(type_w[3]);
     const float inv_radius = static_cast<float>(ctl->inv_radius);
-    // VEC consecutive unknowns per thread (unrolled: the gathers of the VEC elements are independent and overlap)
-    float regs[VEC]; int64_t js[VEC];
+    float regs[4]; int64_t js[4];
 #pragma unroll
-    for (int e = 0; e < VEC; ++e) { regs[e] = 0.0f; js[e] = 0; }
+    for (int e = 0; e < 4; ++e) { regs[e] = 0.0f; js[e] = 0; }
 #pragma unroll
-    for (int e = 0; e < VEC; ++e)
+    for (int e = 0; e < 4; ++e)
     {
         const int64_t t = tbase + e;
         if (t >= count) break;
         const int64_t j = sh.unknown(t, sv.n);
         float reg = 0.0f;
-        if (j < n)
-        {
-            const int64_t v = j;
-            const uint8_t fl = rv.flags[v];
-            const bool own = sh.owns_voxel(v);
-            if (rv.use_er)
-            {
-                const float t0 = own ? sv.tr[v] : 0.0f;
-                float tt = -6.0f * t0;
-#pragma unroll
-                for (int o = 0; o < 6; ++o) { const int32_t nb = g.nbr[static_cast<int64_t>(o) * n + v]; if (nb >= 0 && sh.owns_voxel(nb)) tt += sv.tr[nb]; }
-                reg += wr * tt;
-                if (MODE == APPLY_CG) acc[0] += static_cast<double>(wr) * t0 * t0;
-                else if (own) acc[0] -= static_cast<double>(wr) * t0 * (rv.lap[v] + 0.5 * static_cast<double>(t0));
-            }
-            if (rv.use_es && own && (fl & FL_ACTIVE) && (fl & FL_ES_JAC))
-            {
-                const float u = ps[v];
-                reg += ws * u;
-                if (MODE == APPLY_CG) acc[0] += static_cast<double>(ws) * u * u;
-                else acc[0] -= static_cast<double>(ws) * u * ((g.sdf[v] - g.sdf0[v]) + 0.5 * static_cast<double>(u));
-            }
-        }
+        if (j < n) reg = reg_sdf(rv, sv.tr, ps, j, [&](int o) { return g.nbr[static_cast<int64_t>(o) * n + j]; }, sh, wr, ws, e < 2, acc[0]);
         else if (j < 2 * n)
         {
             const int64_t v = j - n;
-            if (rv.use_ea)
-            {
-                const float pa = ps[j];
-                const bool own = sh.owns_voxel(v);
-#pragma unroll
-                for (int d = 0; d < 3; ++d)
-                {
-                    // the pair {v, v + e_d} is stored at (d, v): it belongs to the rank that owns v
-                    const float wp = own ? rv.ea_w[static_cast<int64_t>(d) * n + v] : 0.0f;
-                    if (wp != 0.0f)
-                    {
-                        const int32_t b = g.nbr[static_cast<int64_t>(2 * d) * n + v];
-                        const float du = pa - ps[n + b];
-                        reg += wa * wp * du;
-                        if (MODE == APPLY_CG) acc[0] += static_cast<double>(wa) * wp * du * du;
-                        else acc[0] -= static_cast<double>(wa) * wp * du * ((g.albedo[v] - g.albedo[b]) + 0.5 * static_cast<double>(du));
-                    }
-                    const int32_t m = g.nbr[static_cast<int64_t>(2 * d + 1) * n + v];
-                    if (m >= 0 && sh.owns_voxel(m))
-                    {
-                        const float wm = rv.ea_w[static_cast<int64_t>(d) * n + m];
-                        if (wm != 0.0f) reg += wa * wm * (pa - ps[n + m]);
-                    }
-                }
-            }
+            reg = reg_albedo(rv, ps, n, v, [&](int o) { return g.nbr[static_cast<int64_t>(o) * n + v]; }, sh, wa, acc[0]);
         }
-        if (MODE == APPLY_CG)
+        regs[e] = reg; js[e] = j;       // the read-modify-write of qg is deferred so that the gathers of the next element can start
+        if (sh.owns_unknown(j, n))
         {
-            regs[e] = reg; js[e] = j;       // the read-modify-write of qg is deferred so that the gathers of the next element can start
-            if (sh.owns_unknown(j, n))
-            {
-                const float pj = pin[j];
-                const float d2 = lm_diag(sv.jtj[j], dmin, dmax) * inv_radius;
-                acc[0] += static_cast<double>(d2) * pj * pj;
-            }
+            const float pj = pin[j];
+            const float d2 = cg_d2(sv.jtj[j], dmin, dmax, inv_radius);
+            acc[0] += static_cast<double>(d2) * pj * pj;
         }
     }
-    if (MODE == APPLY_CG)
-    {
 #pragma unroll
-        for (int e = 0; e < VEC; ++e)
-        {
-            if (tbase + e >= count) break;
-            const double eg = sv.qgd[js[e]];
-            if (eg != 0.0) sv.qgd[js[e]] = 0.0;
-            const float add = static_cast<float>(eg) + regs[e];
-            if (add != 0.0f) sv.qg[js[e]] += add;
-        }
+    for (int e = 0; e < 4; ++e)
+    {
+        if (tbase + e >= count) break;
+        const double eg = sv.qgd[js[e]];
+        if (eg != 0.0) sv.qgd[js[e]] = 0.0;
+        const float add = op_qg(eg, regs[e]);
+        if (add != 0.0f) sv.qg[js[e]] += add;
     }
     if (grid_reduce<1>(acc, site) && threadIdx.x == 0)
     {
         // fold the E_g partial in so that site.out[0] is this rank's complete partial sum
         const double total = site.out[0] + eg_partial[0];
         site.out[0] = total;
-        if (!sh.defer) epilogue_operator(ctl, total, MODE, is_cg_iteration);
+        if (!sh.defer) epilogue_operator(ctl, total, is_cg_iteration);
     }
 }
 
@@ -1918,9 +2013,8 @@ __device__ __forceinline__ void st4(float* __restrict__ p, int64_t j, const floa
 // refreshing), and qg_j is reset to zero for the next application.
 // INIT: x = 0, r = b.  Epilogue: Q-based termination test and beta for the next iteration.
 // The first F + 2 threads handle one camera block each (serial 6x6 work, scheduled first so that it overlaps the streaming
-// part); the remaining threads handle the voxel unknowns: VEC = 4 consecutive unknowns per thread with 16 B accesses in the
-// single-GPU identity layout, VEC = 1 through the held list when sharded.
-template <bool INIT, int VEC>
+// part); the remaining threads handle 4 consecutive voxel unknowns each, with 16 B accesses where Shard::vec4 allows.
+template <bool INIT>
 __global__ void __launch_bounds__(kThreads)
 k_cg_update(SolveVecs sv, Shard sh, const double* __restrict__ minv, float dmin, float dmax, CgCtl* __restrict__ ctl, int refresh, ReduceSite site)
 {
@@ -1928,17 +2022,15 @@ k_cg_update(SolveVecs sv, Shard sh, const double* __restrict__ minv, float dmin,
     if (!INIT && ctl->done) return;
     const int64_t t0 = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
     const int64_t ncb = sv.F + 2;
-    const int64_t n2 = 2 * sv.n;
     const int64_t nvox = sh.held_voxel_unknowns();
-    const bool is_cam = t0 < ncb;
     double acc[3] = {0.0, 0.0, 0.0};      // rho = r.z, 2Q = -x.(b + r), x.D^2 x
     const float alpha = INIT ? 0.0f : static_cast<float>(ctl->alpha);
     const float inv_radius = static_cast<float>(ctl->inv_radius);
-    if (!is_cam)
+    if (t0 >= ncb)
     {
-        const int64_t e0 = (t0 - ncb) * VEC;
+        const int64_t e0 = (t0 - ncb) * 4;
         int64_t j0 = 0;
-        if (VEC == 4 && sh.vec4(e0, sv.n, &j0))
+        if (sh.vec4(e0, sv.n, &j0))
         {
             float bj[4], jt[4], sj[4], qg[4], vj[4], xo[4], ro[4], xn[4], rn[4], zn[4];
             ld4(sv.b, j0, bj); ld4(sv.jtj, j0, jt);
@@ -1950,21 +2042,10 @@ k_cg_update(SolveVecs sv, Shard sh, const double* __restrict__ minv, float dmin,
 #pragma unroll
             for (int i = 0; i < 4; ++i)
             {
-                const float d2 = lm_diag(jt[i], dmin, dmax) * inv_radius;
+                const float d2 = cg_d2(jt[i], dmin, dmax, inv_radius);
                 if (INIT) { xn[i] = 0.0f; rn[i] = bj[i]; }
-                else
-                {
-                    const float qj = sj[i] * qg[i] + d2 * vj[i];
-                    xn[i] = refresh ? xo[i] : (xo[i] + alpha * vj[i]);
-                    rn[i] = refresh ? (bj[i] - qj) : (ro[i] - alpha * qj);
-                }
-                zn[i] = rn[i] / (jt[i] + d2);
-                if (sh.owns_unknown(j0 + i, sv.n))
-                {
-                    acc[0] += static_cast<double>(rn[i]) * zn[i];
-                    acc[1] -= static_cast<double>(xn[i]) * (static_cast<double>(bj[i]) + rn[i]);
-                    acc[2] += static_cast<double>(d2) * xn[i] * xn[i];
-                }
+                else cg_xr(bj[i], op_q(sj[i], qg[i], d2, vj[i], true), vj[i], xo[i], ro[i], alpha, refresh, xn[i], rn[i]);
+                zn[i] = cg_z(xn[i], rn[i], bj[i], jt[i], d2, sh.owns_unknown(j0 + i, sv.n), acc);
             }
             st4(sv.x, j0, xn); st4(sv.r, j0, rn); st4(sv.z, j0, zn);
             if (!INIT) { const float zero[4] = {0.0f, 0.0f, 0.0f, 0.0f}; st4(sv.qg, j0, zero); }
@@ -1972,70 +2053,31 @@ k_cg_update(SolveVecs sv, Shard sh, const double* __restrict__ minv, float dmin,
         else
         {
 #pragma unroll 1
-            for (int64_t t = e0; t < e0 + VEC && t < nvox; ++t)
+            for (int64_t t = e0; t < e0 + 4 && t < nvox; ++t)
             {
                 const int64_t j = sh.unknown(t, sv.n);
                 const float bj = sv.b[j];
                 const float jt = sv.jtj[j];
-                const float d2 = lm_diag(jt, dmin, dmax) * inv_radius;
-                float xj, rj;
-                if (INIT) { xj = 0.0f; rj = bj; }
-                else
+                const float d2 = cg_d2(jt, dmin, dmax, inv_radius);
+                float xj = 0.0f, rj = bj;
+                if (!INIT)
                 {
                     const float vj = refresh ? sv.x[j] : sv.p[j];
-                    const float qj = sv.s[j] * sv.qg[j] + d2 * vj;
+                    const float qj = op_q(sv.s[j], sv.qg[j], d2, vj, false);
                     sv.qg[j] = 0.0f;
-                    // refresh: x was already advanced by k_x_update and q = A x (exact residual, every residual_reset_period iterations)
-                    xj = refresh ? sv.x[j] : (sv.x[j] + alpha * vj);
-                    rj = refresh ? (bj - qj) : (sv.r[j] - alpha * qj);
+                    cg_xr(bj, qj, vj, sv.x[j], sv.r[j], alpha, refresh, xj, rj);
                 }
-                const float zj = rj / (jt + d2);
+                const float zj = cg_z(xj, rj, bj, jt, d2, sh.owns_unknown(j, sv.n), acc);
                 sv.x[j] = xj; sv.r[j] = rj; sv.z[j] = zj;
-                if (sh.owns_unknown(j, sv.n))
-                {
-                    acc[0] += static_cast<double>(rj) * zj;
-                    acc[1] -= static_cast<double>(xj) * (static_cast<double>(bj) + rj);
-                    acc[2] += static_cast<double>(d2) * xj * xj;
-                }
             }
         }
     }
     else
     {
-        const int blk = static_cast<int>(t0);
-        int m; int64_t base; const double* Mi;
-        if (blk < sv.F) { m = 6; base = n2 + 6 * static_cast<int64_t>(blk); Mi = minv + 36 * static_cast<size_t>(blk); }
-        else if (blk == sv.F) { m = 4; base = n2 + 6 * static_cast<int64_t>(sv.F); Mi = minv + 36 * static_cast<size_t>(sv.F); }
-        else { m = 5; base = n2 + 6 * static_cast<int64_t>(sv.F) + 4; Mi = minv + 36 * static_cast<size_t>(sv.F) + 16; }
-        float rr[6];
-        double a0 = 0.0, a1 = 0.0, a2 = 0.0;
-        for (int k = 0; k < m; ++k)
-        {
-            const int64_t j = base + k;
-            const float bj = sv.b[j];
-            const float d2 = lm_diag(sv.jtj[j], dmin, dmax) * inv_radius;
-            float xj, rj;
-            if (INIT) { xj = 0.0f; rj = bj; }
-            else
-            {
-                const float vj = refresh ? sv.x[j] : sv.p[j];
-                const float qj = sv.s[j] * sv.qg[j] + d2 * vj;
-                sv.qg[j] = 0.0f;
-                xj = refresh ? sv.x[j] : (sv.x[j] + alpha * vj);
-                rj = refresh ? (bj - qj) : (sv.r[j] - alpha * qj);
-            }
-            sv.x[j] = xj; sv.r[j] = rj; rr[k] = rj;
-            a1 -= static_cast<double>(xj) * (static_cast<double>(bj) + rj);
-            a2 += static_cast<double>(d2) * xj * xj;
-        }
-        for (int i = 0; i < m; ++i)
-        {
-            double ssum = 0.0;
-            for (int k = 0; k < m; ++k) ssum += Mi[i * m + k] * static_cast<double>(rr[k]);
-            sv.z[base + i] = static_cast<float>(ssum);
-            a0 += static_cast<double>(rr[i]) * ssum;
-        }
-        if (sh.cam_owner) { acc[0] = a0; acc[1] = a1; acc[2] = a2; }
+        double a[3];
+        auto q = [&](int64_t j, float d2, float v) { const float qj = op_q(sv.s[j], sv.qg[j], d2, v, false); sv.qg[j] = 0.0f; return qj; };
+        cam_block_update<INIT>(sv, cam_block(static_cast<int>(t0), sv.F, sv.n), minv, dmin, dmax, inv_radius, alpha, refresh, q, a);
+        if (sh.cam_owner) { acc[0] = a[0]; acc[1] = a[1]; acc[2] = a[2]; }
     }
     if (grid_reduce<3>(acc, site) && threadIdx.x == 0 && !sh.defer) epilogue_update(ctl, site.out[0], site.out[1], site.out[2], INIT);
 }
@@ -2055,21 +2097,22 @@ k_cg_dir4(SolveVecs sv, Shard sh, int64_t count, const CgCtl* __restrict__ ctl)
         float z[4], p[4], s4[4], ps[4];
         ld4(sv.z, j0, z); ld4(sv.p, j0, p); ld4(sv.s, j0, s4);
 #pragma unroll
-        for (int i = 0; i < 4; ++i) { p[i] = (beta == 0.0f) ? z[i] : z[i] + beta * p[i]; ps[i] = s4[i] * p[i]; }      // first iteration: p may hold anything
+        for (int i = 0; i < 4; ++i) cg_dir(z[i], p[i], s4[i], beta, p[i], ps[i]);
         st4(sv.p, j0, p); st4(sv.ps, j0, ps);
     }
     else
         for (int64_t t = e0; t < e0 + 4 && t < count; ++t)
         {
             const int64_t j = sh.unknown(t, sv.n);
-            const float p = (beta == 0.0f) ? sv.z[j] : sv.z[j] + beta * sv.p[j];
-            sv.p[j] = p; sv.ps[j] = sv.s[j] * p;
+            float p, ps;
+            cg_dir(sv.z[j], sv.p[j], sv.s[j], beta, p, ps);
+            sv.p[j] = p; sv.ps[j] = ps;
         }
 }
 
 // ---- the per-unknown half of a PCG iteration as ONE cooperative grid (single GPU) ------------------------------------------
-// k_cg_step<false> = k_op_partial<APPLY_CG> + k_cg_update<false, 4> + the next k_cg_dir4;  k_cg_step<true> = k_cg_update<true, 4> +
-// the first k_cg_dir4.  Those kernels exist only because alpha and beta need grid-wide sums; here each sum is a grid barrier:
+// k_cg_step<false> = k_op_partial + k_cg_update<false> + the next k_cg_dir4;  k_cg_step<true> = k_cg_update<true> + the first
+// k_cg_dir4.  Those kernels exist only because alpha and beta need grid-wide sums; here each sum is a grid barrier:
 //   A  operator finish: q_j = s_j (float(qgd_j) + reg_j) + D_j^2 p_j (qgd cleared, qg never written), partial p.q   | barrier, alpha
 //   B  update: x, r, z (z kept on chip), partials rho, 2Q, x.D^2 x; camera blocks z = M^-1 r                        | barrier, beta
 //   C  direction: p = z + beta p, ps = s o p
@@ -2078,15 +2121,11 @@ k_cg_dir4(SolveVecs sv, Shard sh, int64_t count, const CgCtl* __restrict__ ctl)
 // grid is sized to full residency, T = blocks * 256 threads, and the launcher refuses the fused path when K = ceil(items / T) slots do
 // not fit (the whole unknown vector is on chip: 4 B per unknown, ~121 KB per SM at C3).  The camera blocks are taken by the last F + 2
 // threads of the grid, which park their <= 6 values of q, then z, in their own entries of z (a scratch vector on this path).
-// Every float operation per unknown is the one of the kernels it replaces, rounded as their compiled code rounds it: the operations
-// are written with explicit-rounding intrinsics, because the compiler fuses multiply-adds differently in different kernels (the chain's
-// k_op_partial fuses -6 t0 + tr[nb_0] in two of its four unrolled elements, k_cg_update's q differs between its 16 B path and its
-// scalar/camera path).  The double partial sums are decomposed differently
-// (block partials, then every block sums all partials in one fixed order, so the scalar epilogues run on identical inputs in every
-// block on a shared-memory copy of the control block; block 0 stores it).  ctl->done is read once, before the first barrier: the grid
-// leaves together.
-// sm_90a, -Xptxas -v: <false> 80 registers and 8 B of spill (predicates saved around the slow-path division calls, once per thread),
-// <true> 74 registers, no spill; 3 blocks of 256 threads per SM (396 blocks on 132 SMs).  At C3: 0.20 ms per iteration against
+// The per-unknown arithmetic is the chain's (the functions above), so the results are bit-equal to it; only the decomposition of the
+// double partial sums differs (block partials, then every block sums all partials in one fixed order, so the scalar epilogues run on
+// identical inputs in every block on a shared-memory copy of the control block; block 0 stores it).  ctl->done is read once, before
+// the first barrier: the grid leaves together.
+// sm_90a, -Xptxas -v: <false> 80 registers, <true> 74 registers, no spill; 3 blocks of 256 threads per SM (396 blocks on 132 SMs).  At C3: 0.20 ms per iteration against
 // 0.27 ms for the three kernels it replaces (H100 80GB HBM3, 700 W limit).
 constexpr int kStepThreads = 256;
 constexpr int kStepSlots = 8;       // unknowns of one work item: sdf and albedo of 4 voxels
@@ -2146,22 +2185,14 @@ k_cg_step(GridView g, RegView rv, SolveVecs sv, int64_t items, int K, const doub
     const int64_t T = static_cast<int64_t>(gridDim.x) * blockDim.x;
     const int64_t gt = blockIdx.x * static_cast<int64_t>(blockDim.x) + tid;
     const float inv_radius = static_cast<float>(s_ctl.inv_radius);
-    const int64_t tail0 = (2 * n) & ~int64_t(3);     // first unknown k_cg_update takes on its scalar path
+    const int64_t tail0 = (2 * n) & ~int64_t(3);     // the voxel unknowns below tail0 form whole 16 B groups of four (op_q)
     auto slot = [&](int k, int u) -> float& { return s_slot[(k * kStepSlots + u) * blockDim.x + tid]; };
 
-    // camera block of this thread (poses f < F: 6, intrinsics: 4, distortion: 5 unknowns)
+    // camera block of this thread (m = 0: none)
     const int64_t cblk = T - 1 - gt;
-    int m = 0; int64_t cbase = 0; const double* Mi = nullptr;
-    if (cblk < sv.F + 2)
-    {
-        const int blk = static_cast<int>(cblk);
-        const int64_t n2 = 2 * n;
-        if (blk < sv.F) { m = 6; cbase = n2 + 6 * static_cast<int64_t>(blk); Mi = minv + 36 * static_cast<size_t>(blk); }
-        else if (blk == sv.F) { m = 4; cbase = n2 + 6 * static_cast<int64_t>(sv.F); Mi = minv + 36 * static_cast<size_t>(sv.F); }
-        else { m = 5; cbase = n2 + 6 * static_cast<int64_t>(sv.F) + 4; Mi = minv + 36 * static_cast<size_t>(sv.F) + 16; }
-    }
+    const CamBlock cb = cblk < sv.F + 2 ? cam_block(static_cast<int>(cblk), sv.F, n) : CamBlock{0, 0, 0};
 
-    // ------------------------------------------------------------------ A: operator finish (k_op_partial<APPLY_CG>)
+    // ------------------------------------------------------------------ A: operator finish
     if (!INIT)
     {
         double acc[1] = {0.0};
@@ -2183,53 +2214,9 @@ k_cg_step(GridView g, RegView rv, SolveVecs sv, int64_t items, int K, const doub
                 int32_t nb[6];
 #pragma unroll
                 for (int o = 0; o < 6; ++o) nb[o] = (rv.use_er || rv.use_ea) ? g.nbr[static_cast<int64_t>(o) * n + v] : -1;
-                // sdf unknown v
-                float reg = 0.0f;
-                if (rv.use_er)
-                {
-                    const float t0 = sv.tr[v];
-                    // the chain's k_op_partial fuses -6 t0 + tr[nb_0] into one FMA for the voxels v % 4 < 2 (the first two of
-                    // its four unrolled elements) and rounds the product for the other two
-                    float tt;
-                    if (i < 2 && nb[0] >= 0) tt = __fmaf_rn(t0, -6.0f, sv.tr[nb[0]]);
-                    else { tt = __fmul_rn(t0, -6.0f); if (nb[0] >= 0) tt = __fadd_rn(tt, sv.tr[nb[0]]); }
-#pragma unroll
-                    for (int o = 1; o < 6; ++o) if (nb[o] >= 0) tt = __fadd_rn(tt, sv.tr[nb[o]]);
-                    reg = __fmaf_rn(wr, tt, reg);
-                    acc[0] += static_cast<double>(wr) * t0 * t0;
-                }
-                const uint8_t fl = rv.flags[v];
-                if (rv.use_es && (fl & FL_ACTIVE) && (fl & FL_ES_JAC))
-                {
-                    const float u = ps[v];
-                    reg = __fmaf_rn(ws, u, reg);
-                    acc[0] += static_cast<double>(ws) * u * u;
-                }
-                regs[0][i] = reg;
-                // albedo unknown n + v
-                reg = 0.0f;
-                if (rv.use_ea)
-                {
-                    const float pa = ps[n + v];
-#pragma unroll
-                    for (int d = 0; d < 3; ++d)
-                    {
-                        const float wp = rv.ea_w[static_cast<int64_t>(d) * n + v];
-                        if (wp != 0.0f)
-                        {
-                            const float du = __fsub_rn(pa, ps[n + nb[2 * d]]);
-                            reg = __fmaf_rn(__fmul_rn(wa, wp), du, reg);
-                            acc[0] += static_cast<double>(wa) * wp * du * du;
-                        }
-                        const int32_t mm = nb[2 * d + 1];
-                        if (mm >= 0)
-                        {
-                            const float wm = rv.ea_w[static_cast<int64_t>(d) * n + mm];
-                            if (wm != 0.0f) reg = __fmaf_rn(__fmul_rn(wa, wm), __fsub_rn(pa, ps[n + mm]), reg);
-                        }
-                    }
-                }
-                regs[1][i] = reg;
+                auto nbr = [&](int o) { return nb[o]; };
+                regs[0][i] = reg_sdf(rv, sv.tr, ps, v, nbr, OwnAll{}, wr, ws, i < 2, acc[0]);
+                regs[1][i] = reg_albedo(rv, ps, n, v, nbr, OwnAll{}, wa, acc[0]);
             }
 #pragma unroll
             for (int h = 0; h < 2; ++h)
@@ -2254,30 +2241,25 @@ k_cg_step(GridView g, RegView rv, SolveVecs sv, int64_t items, int K, const doub
                 {
                     if (i >= cnt) continue;
                     if (eg[i] != 0.0) sv.qgd[j0 + i] = 0.0;
-                    // qg_j as k_op_partial leaves it (qg is zero on entry): its update is skipped when the sum is zero
-                    const float add = __fadd_rn(static_cast<float>(eg[i]), regs[h][i]);
-                    const float qg = (add != 0.0f) ? add : 0.0f;
-                    const float d2 = __fmul_rn(lm_diag(jt[i], dmin, dmax), inv_radius);
+                    const float add = op_qg(eg[i], regs[h][i]);
+                    const float d2 = cg_d2(jt[i], dmin, dmax, inv_radius);
                     acc[0] += static_cast<double>(d2) * pj[i] * pj[i];
-                    // k_cg_update's q: fma(s, qg, D^2 p) on its 16 B path, fma(D^2, p, s qg) on its scalar tail (the last 2n % 4
-                    // unknowns) and for the camera blocks
-                    slot(k, 4 * h + i) = (j0 + i < tail0) ? __fmaf_rn(sj[i], qg, __fmul_rn(d2, pj[i])) : __fmaf_rn(d2, pj[i], __fmul_rn(sj[i], qg));
+                    slot(k, 4 * h + i) = op_q(sj[i], (add != 0.0f) ? add : 0.0f, d2, pj[i], j0 + i < tail0);
                 }
             }
         }
 #pragma unroll
         for (int k = 0; k < 6; ++k)
         {
-            if (k >= m) break;
-            const int64_t j = cbase + k;
+            if (k >= cb.m) break;
+            const int64_t j = cb.base + k;
             const double eg = sv.qgd[j];
             if (eg != 0.0) sv.qgd[j] = 0.0;
-            const float add = __fadd_rn(static_cast<float>(eg), 0.0f);
-            const float qg = (add != 0.0f) ? add : 0.0f;
+            const float add = op_qg(eg, 0.0f);
             const float pj = sv.p[j];
-            const float d2 = __fmul_rn(lm_diag(sv.jtj[j], dmin, dmax), inv_radius);
+            const float d2 = cg_d2(sv.jtj[j], dmin, dmax, inv_radius);
             acc[0] += static_cast<double>(d2) * pj * pj;
-            sv.z[j] = __fmaf_rn(d2, pj, __fmul_rn(sv.s[j], qg));
+            sv.z[j] = op_q(sv.s[j], (add != 0.0f) ? add : 0.0f, d2, pj, false);
         }
         step_partials<1>(acc, op_site.partials, red_smem);
         grid.sync();
@@ -2288,7 +2270,7 @@ k_cg_step(GridView g, RegView rv, SolveVecs sv, int64_t items, int K, const doub
             if (tid == 0)
             {
                 const double total = tot[0] + eg_partial[0];
-                epilogue_operator(&s_ctl, total, APPLY_CG, 1);
+                epilogue_operator(&s_ctl, total, 1);
                 if (blockIdx.x == 0) { op_site.out[0] = total; if (s_ctl.done) *ctl = s_ctl; }
             }
         }
@@ -2296,7 +2278,7 @@ k_cg_step(GridView g, RegView rv, SolveVecs sv, int64_t items, int K, const doub
         if (s_ctl.done) return;
     }
 
-    // ------------------------------------------------------------------ B: update (k_cg_update)
+    // ------------------------------------------------------------------ B: update
     {
         double acc[3] = {0.0, 0.0, 0.0};      // rho = r.z, 2Q = -x.(b + r), x.D^2 x
         const float alpha = INIT ? 0.0f : static_cast<float>(s_ctl.alpha);
@@ -2317,59 +2299,20 @@ k_cg_step(GridView g, RegView rv, SolveVecs sv, int64_t items, int K, const doub
 #pragma unroll
                 for (int i = 0; i < 4; ++i)
                 {
-                    const float d2 = __fmul_rn(lm_diag(jt[i], dmin, dmax), inv_radius);
+                    const float d2 = cg_d2(jt[i], dmin, dmax, inv_radius);
                     if (INIT) { xn[i] = 0.0f; rn[i] = bj[i]; }
-                    else
-                    {
-                        const float qj = (i < cnt) ? slot(k, 4 * h + i) : 0.0f;
-                        xn[i] = __fmaf_rn(alpha, vj[i], xo[i]);
-                        rn[i] = __fmaf_rn(-alpha, qj, ro[i]);
-                    }
+                    else cg_xr(bj[i], (i < cnt) ? slot(k, 4 * h + i) : 0.0f, vj[i], xo[i], ro[i], alpha, false, xn[i], rn[i]);
                     if (i >= cnt) continue;
-                    const float zn = __fdiv_rn(rn[i], __fadd_rn(jt[i], d2));
-                    slot(k, 4 * h + i) = zn;
-                    acc[0] += static_cast<double>(rn[i]) * zn;
-                    acc[1] -= static_cast<double>(xn[i]) * (static_cast<double>(bj[i]) + rn[i]);
-                    acc[2] += static_cast<double>(d2) * xn[i] * xn[i];
+                    slot(k, 4 * h + i) = cg_z(xn[i], rn[i], bj[i], jt[i], d2, true, acc);
                 }
                 st4n(sv.x, j0, cnt, vec, xn); st4n(sv.r, j0, cnt, vec, rn);
             }
         }
-        if (m > 0)
+        if (cb.m > 0)
         {
-            float rr[6];
-            double a0 = 0.0, a1 = 0.0, a2 = 0.0;
-#pragma unroll
-            for (int k = 0; k < 6; ++k)
-            {
-                rr[k] = 0.0f;
-                if (k >= m) continue;
-                const int64_t j = cbase + k;
-                const float bj = sv.b[j];
-                const float d2 = __fmul_rn(lm_diag(sv.jtj[j], dmin, dmax), inv_radius);
-                float xj, rj;
-                if (INIT) { xj = 0.0f; rj = bj; }
-                else
-                {
-                    const float vj = sv.p[j];
-                    xj = __fmaf_rn(alpha, vj, sv.x[j]);
-                    rj = __fmaf_rn(-alpha, sv.z[j], sv.r[j]);
-                }
-                sv.x[j] = xj; sv.r[j] = rj; rr[k] = rj;
-                a1 -= static_cast<double>(xj) * (static_cast<double>(bj) + rj);
-                a2 += static_cast<double>(d2) * xj * xj;
-            }
-#pragma unroll
-            for (int i = 0; i < 6; ++i)
-            {
-                if (i >= m) continue;
-                double ssum = 0.0;
-#pragma unroll
-                for (int k = 0; k < 6; ++k) if (k < m) ssum += Mi[i * m + k] * static_cast<double>(rr[k]);
-                sv.z[cbase + i] = static_cast<float>(ssum);
-                a0 += static_cast<double>(rr[i]) * ssum;
-            }
-            acc[0] += a0; acc[1] += a1; acc[2] += a2;
+            double a[3];
+            cam_block_update<INIT>(sv, cb, minv, dmin, dmax, inv_radius, alpha, false, [&](int64_t j, float, float) { return sv.z[j]; }, a);
+            acc[0] += a[0]; acc[1] += a[1]; acc[2] += a[2];
         }
         step_partials<3>(acc, upd_site.partials, red_smem);
         grid.sync();
@@ -2387,7 +2330,7 @@ k_cg_step(GridView g, RegView rv, SolveVecs sv, int64_t items, int K, const doub
         if (s_ctl.done) return;
     }
 
-    // ------------------------------------------------------------------ C: direction of the next iteration (k_cg_dir4)
+    // ------------------------------------------------------------------ C: direction of the next iteration
     const float beta = static_cast<float>(s_ctl.beta);
     for (int k = 0; k < K; ++k)
     {
@@ -2404,22 +2347,18 @@ k_cg_step(GridView g, RegView rv, SolveVecs sv, int64_t items, int K, const doub
             ld4n(sv.s, j0, cnt, vec, s4);
             if (beta != 0.0f) ld4n(sv.p, j0, cnt, vec, p);      // first iteration: p may hold anything
 #pragma unroll
-            for (int i = 0; i < 4; ++i)
-            {
-                const float z = (i < cnt) ? slot(k, 4 * h + i) : 0.0f;
-                p[i] = (beta == 0.0f) ? z : __fmaf_rn(beta, p[i], z);
-                ps[i] = __fmul_rn(s4[i], p[i]);
-            }
+            for (int i = 0; i < 4; ++i) cg_dir((i < cnt) ? slot(k, 4 * h + i) : 0.0f, p[i], s4[i], beta, p[i], ps[i]);
             st4n(sv.p, j0, cnt, vec, p); st4n(sv.ps, j0, cnt, vec, ps);
         }
     }
 #pragma unroll
     for (int k = 0; k < 6; ++k)
     {
-        if (k >= m) break;
-        const int64_t j = cbase + k;
-        const float p = (beta == 0.0f) ? sv.z[j] : __fmaf_rn(beta, sv.p[j], sv.z[j]);
-        sv.p[j] = p; sv.ps[j] = __fmul_rn(sv.s[j], p);
+        if (k >= cb.m) break;
+        const int64_t j = cb.base + k;
+        float p, ps;
+        cg_dir(sv.z[j], sv.p[j], sv.s[j], beta, p, ps);
+        sv.p[j] = p; sv.ps[j] = ps;
     }
 }
 
@@ -2553,11 +2492,7 @@ k_xchg_pull(P2PView pp, unsigned int seq, ShareView sh, float* __restrict__ v0, 
             // the scalar epilogue of the operator (alpha = rho / p.q) by the one thread that just summed p.q.  It can only SET `done`
             // (p.q <= 0: the solve stops and this application is discarded), so blocks of this launch that read `done` later and skip
             // their unpacking are harmless.
-            if (t == sh.n_shared + n_extra_f && epilogue_kind >= 0)
-            {
-                if (epilogue_kind == EPI_OPERATOR_CG) epilogue_operator(ctl, a, APPLY_CG, 1);
-                else if (epilogue_kind == EPI_MODEL) epilogue_operator(ctl, a, APPLY_MODEL, 0);
-            }
+            if (t == sh.n_shared + n_extra_f && epilogue_kind == EPI_OPERATOR_CG) epilogue_operator(ctl, a, 1);
         }
     }
 }
@@ -2582,8 +2517,7 @@ __global__ void k_xchg_scalars(P2PView pp, unsigned int seq, double* __restrict_
     __syncwarp();
     if (lane == 0 && kind >= 0)
     {
-        if (kind == EPI_OPERATOR_CG) epilogue_operator(ctl, vals[0], APPLY_CG, 1);
-        else if (kind == EPI_MODEL) epilogue_operator(ctl, vals[0], APPLY_MODEL, 0);
+        if (kind == EPI_OPERATOR_CG) epilogue_operator(ctl, vals[0], 1);
         else if (kind == EPI_UPDATE) epilogue_update(ctl, vals[0], vals[1], vals[2], false);
         else if (kind == EPI_UPDATE_INIT) epilogue_update(ctl, vals[0], vals[1], vals[2], true);
     }

@@ -12,7 +12,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(HERE, "..", "intrinsic3d_b200", "libi3d_b200.so")
-DEFAULT = ["k_eg_rowsILi0", "k_eg_rowsILi1", "k_eg_applyILi0", "k_eg_accum", "k_select_obsILi5", "k_op_partialILi0", "k_cg_updateILb0", "k_cg_dir4", "k_xchg_pull", "k_reg_build"]
+DEFAULT = ["k_eg_rowsILi0", "k_eg_rowsILi1", "k_eg_apply", "k_eg_accum", "k_select_obsILi5", "k_op_partial", "k_cg_updateILb0", "k_cg_dir4", "k_xchg_pull", "k_reg_build"]
 
 
 def main():
