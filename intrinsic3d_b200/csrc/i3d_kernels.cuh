@@ -82,10 +82,6 @@ __device__ __forceinline__ void pdl_prologue()
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 
-#ifndef I3D_BUILD_MIN_BLOCKS
-#define I3D_BUILD_MIN_BLOCKS 2
-#endif
-
 struct FrameView
 {
     int F, W, H;
@@ -640,9 +636,6 @@ __device__ __forceinline__ bool frame_may_see(const float c[3], float rad, const
 // canonical top-K of oracle.cpp).  Neighbouring threads are neighbouring voxels, so for a given frame the 32
 // depth taps of a warp fall on neighbouring pixels, and the per-frame pose (R|t) is warp-uniform (shared memory
 // broadcast).  Frames that provably see no voxel of the warp's cluster are skipped (frame_may_see).
-#ifndef I3D_SELECT_PIPELINE
-#define I3D_SELECT_PIPELINE 1
-#endif
 template <int KMAX>
 __global__ void __launch_bounds__(kThreads)
 k_select_obs(GridView g, FrameView fr, const float* __restrict__ Rt, SelectCam cam, CullView cull, int n_active, int stride,
@@ -735,13 +728,9 @@ k_select_obs(GridView g, FrameView fr, const float* __restrict__ Rt, SelectCam c
             const int f = 32 * j + __ffs(m) - 1;
             m &= m - 1;
             if (f >= fr.F) continue;
-#if I3D_SELECT_PIPELINE
             const ObsProbe nxt = obs_probe(pt, s_rt + 12 * f, cam, fr.depth + img * f, fr.W, fr.H);
             if (pend_f >= 0) insert(obs_finish(pend, nrm, s_rt + 12 * pend_f, cam), pend_f);
             pend = nxt; pend_f = f;
-#else
-            insert(observation_weight(pt, nrm, s_rt + 12 * f, cam, fr.depth + img * f, fr.W, fr.H), f);
-#endif
         }
     }
     if (pend_f >= 0) insert(obs_finish(pend, nrm, s_rt + 12 * pend_f, cam), pend_f);
@@ -888,9 +877,6 @@ struct CamAccLayout
 // warp-broadcast loads and the 16 luminance taps of a warp fall on neighbouring pixels.
 enum { ROWS_BUILD = 0, ROWS_COST = 1 };
 constexpr int kRowThreads = 128;       // block size of the global-memory variant of k_eg_rows (256 for the staged variant)
-#ifndef I3D_ROWS_STAGE_POSE
-#define I3D_ROWS_STAGE_POSE 1          // 0: never stage the pose table (A/B switch)
-#endif
 
 // ---- bulk-async copy (cp.async.bulk, the non-tensor TMA path) + mbarrier, used to stage the per-frame pose table ----------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -1613,7 +1599,6 @@ k_eg_apply(GridView g, EgRows rows, RegView rv, SolveVecs sv, const float* __res
             const float* pp = ps + 2 * n + 6 * static_cast<int64_t>(f);
             // four independent partial sums instead of one 29-long dependent FMA chain
             float u0 = 0.0f, u1 = 0.0f, u2 = 0.0f, u3 = 0.0f;
-#pragma unroll
             const float* pv = s_pv + tid;
 #pragma unroll
             for (int m = 0; m < 12; m += 4)
