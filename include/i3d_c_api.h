@@ -205,6 +205,27 @@ int         i3d_mode_colors(I3DEngine* e, int32_t sdf_source, int32_t color_mode
  * pointer may be NULL.  Fails when no mesh of the current grid has been extracted. */
 int         i3d_download_mesh(I3DEngine* e, float* xyz, uint8_t* rgb, int32_t* faces);
 
+/* ---- rendering the surface into the keyframes (DESIGN.md §6m) ---- */
+uint64_t    i3d_sizeof_render_params(void);
+uint64_t    i3d_sizeof_render_stats(void);
+/* sdf_source 1, every plane, photometric pairs on. */
+void        i3d_default_render_params(I3DRenderParams* p);
+/* Ray-casts the zero level set of params->sdf_source into the frames ids[0..n) of the resident camera state at the current pyramid level:
+ * W x H of the installed frames, the float R | t of the frame scans and their intrinsics * pyr_scale with the five distortion
+ * coefficients.  stats[n] (may be NULL) compares each view with its frame's depth and luminance.  The requested planes stay resident for
+ * i3d_download_render.  Reads the grid, camera, SH and frames only.  Fails, writing nothing, without grid, frames or camera, for n <= 0,
+ * n > 65535 or an id out of [0, F), a bad source or plane mask, shading / intensity planes or photometric pairs without per-voxel SH,
+ * intrinsics (after pyr_scale) that are not finite with fx, fy > 0, distortion that is not finite, and for world > 1.  A frame whose pose
+ * is not finite renders as a view without hits.  Device time: i3d_phase_ms("render"), of which the occupancy bitmap (built on the first
+ * render after a voxel-set change)
+ * is i3d_phase_ms("render_bricks"); lattice samples evaluated: i3d_phase_count("render_samples"). */
+int         i3d_render_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DRenderParams* params, I3DRenderStats* stats);
+/* The planes of the last render, float32 [n][H][W] (normal [n][H][W][3]).  Any pointer may be NULL.  Fails for a plane that was not
+ * rendered, and when no render of the current voxel set and frames exists.  The planes are those of the state at render time: a later
+ * i3d_set_camera, i3d_upload_voxel_params or i3d_gn_iteration neither updates nor drops them (render again to see the new state), as the
+ * resident mesh of i3d_extract_mesh; a change of the voxel set or of the frames drops them. */
+int         i3d_download_render(I3DEngine* e, float* depth, float* normal, float* albedo, float* shading, float* intensity);
+
 /* ---- keyframe selection and the RGB-D image pyramid: the inputs of fusion and refinement (DESIGN.md §6i) ---- */
 /* Frames scored per device pass by i3d_keyframe_scores: bounds its scratch memory (I3D_KEYFRAME_CHUNK * W * H * 3 bytes). */
 #define I3D_KEYFRAME_CHUNK 32
@@ -309,6 +330,8 @@ int         i3d_debug_get_fusion_volume(I3DEngine* e, int32_t* xyz, float* sdf, 
 /* The frames of the current level as the device holds them: lum[F][H][W], depth[F][H][W], bgr[F][H][W][3] (fails when asked for colours
  * that are not resident at this size).  Any pointer may be NULL. */
 int         i3d_debug_get_frames(I3DEngine* e, float* lum, float* depth, uint8_t* bgr);
+/* on = 1 (default): i3d_render_keyframes jumps over empty 8^3 bricks; 0: it evaluates every lattice sample.  The results are the same. */
+int         i3d_debug_set_render_skip(I3DEngine* e, int on);
 
 #ifdef __cplusplus
 }

@@ -203,6 +203,37 @@ enum
     I3D_MESH_COLOR_COUNT
 };
 
+/* ---- rendering the surface into the keyframes (DESIGN.md §6m) ---- */
+/* Planes of a render (bit mask of I3DRenderParams::planes). */
+enum
+{
+    I3D_RENDER_DEPTH = 1,                 /* camera z of the hit, 0 = no hit */
+    I3D_RENDER_NORMAL = 2,                /* unit sdf gradient at the hit, world frame, [3] per pixel; (0,0,0) = none */
+    I3D_RENDER_ALBEDO = 4,                /* trilinear albedo at the hit */
+    I3D_RENDER_SHADING = 8,               /* shading(normal, per-voxel SH) at the hit, 0 where undefined */
+    I3D_RENDER_INTENSITY = 16,            /* albedo * shading, 0 where undefined */
+    I3D_RENDER_ALL = 31
+};
+
+typedef struct I3DRenderParams
+{
+    int32_t sdf_source;                   /* 0 = sdf0, 1 = sdf_refined, as in I3DMeshParams */
+    int32_t planes;                       /* I3D_RENDER_* mask; 0 = statistics only (no plane buffers) */
+    int32_t photometric;                  /* 1 = photometric pairs (needs the per-voxel SH); 0 = geometry only */
+    int32_t reserved;
+} I3DRenderParams;
+
+/* Per-view comparison of a render with its keyframe.  Sums are double, in a fixed order: a view's numbers depend only on that view. */
+typedef struct I3DRenderStats
+{
+    int64_t num_hit;                      /* pixels whose ray hit the surface */
+    int64_t num_observed;                 /* pixels with input depth > 0 */
+    int64_t depth_count;                  /* hit and observed */
+    int64_t photo_count;                  /* hit, shading defined and observed (0 when photometric = 0) */
+    double  depth_abs, depth_sq;          /* sum |z_r - z_obs|, sum (z_r - z_obs)^2 over the depth pairs (metres) */
+    double  photo_abs, photo_sq;          /* sum |I_r - I_obs|, sum (I_r - I_obs)^2 over the photometric pairs (I_obs: the frame's luminance) */
+} I3DRenderStats;
+
 #ifdef __cplusplus
 }
 #endif

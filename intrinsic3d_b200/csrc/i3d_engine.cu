@@ -33,6 +33,7 @@
 #include "i3d_fusion.cuh"
 #include "i3d_frames.cuh"
 #include "i3d_mesh.h"
+#include "i3d_render.h"
 
 #include <cub/device/device_radix_sort.cuh>
 
@@ -227,6 +228,16 @@ struct I3DEngine
     cudaEvent_t ms_ev[16] = {};        // begin / end of up to 8 device-only segments of one extraction (MeshSegments)
     bool ms_ev_ready = false;
     Dev<uchar4> vis_rgb;               // per-voxel colours of the last colour pass (i3d_vis.cuh): scratch that only grows
+    // keyframe renderer (i3d_render.cuh): the voxel box and brick bitmap of the current voxel set (built on the first render after a
+    // change), scratch that only grows, and the resident planes of the last render
+    bool rd_skip = true;               // i3d_debug_set_render_skip
+    bool rd_box_ready = false, rd_have_bricks = false;
+    int rd_box[6] = {}, rd_blo[3] = {}, rd_bdim[3] = {};
+    Dev<int> rd_box_d; Dev<uint32_t> rd_bits;
+    Dev<float> rd_rt; Dev<int32_t> rd_ids; Dev<double> rd_partials, rd_sums; Dev<unsigned long long> rd_samples;
+    Dev<float> rd_depth, rd_normal, rd_albedo, rd_shading, rd_intensity;
+    bool have_render = false;
+    int rd_n = 0, rd_planes = 0;
     // shard (multi-GPU)
     int64_t shard_begin = 0, shard_end = -1;
     int rank = 0, world = 1;
@@ -327,10 +338,11 @@ int rebuild_topology(I3DEngine* e)
 }
 
 // Forgets everything derived from the voxel set: the per-voxel SH and the lighting estimate, the last iteration, the shard state and
-// range, and the resident mesh.  Every change of the voxel set calls it.
+// range, the resident mesh, and the renderer's voxel box, brick bitmap and planes.  Every change of the voxel set calls it.
 void forget_voxel_set(I3DEngine* e)
 {
     e->have_sh = false; e->sv_S = 0; e->sv_x = nullptr; e->have_iter = false; e->have_mesh = false;
+    e->rd_box_ready = false; e->rd_have_bricks = false; e->have_render = false;
     e->shard_ready = false; e->shard_begin = 0; e->shard_end = -1;
 }
 
@@ -359,11 +371,12 @@ int install_grid(I3DEngine* e, int64_t m, Fill&& fill)
 
 // Installs F frames of W x H as the engine's luminance / depth planes at scale pyr_scale: `fill` writes e->lum / e->depth (sized here) on
 // e->stream.  The one place that knows what a frame change invalidates: a new frame count drops the camera and the last iteration, a new
-// size drops the colour planes, and the depth tiles of the frame culling are rebuilt.
+// size drops the colour planes, the depth tiles of the frame culling are rebuilt, and the planes of the last render are dropped.
 template <class Fill>
 void install_frames(I3DEngine* e, int32_t F, int32_t W, int32_t H, double pyr_scale, Fill&& fill)
 {
     const size_t cnt = static_cast<size_t>(F) * W * H;
+    e->have_render = false;
     if (F != e->F) { e->have_cam = false; e->have_iter = false; }     // the unknown space of the last iteration no longer matches
     if (F != e->F || W != e->W || H != e->H) e->have_color = false;
     e->F = F; e->W = W; e->H = H; e->pyr_scale = pyr_scale;
@@ -1347,6 +1360,124 @@ int extract_mesh(I3DEngine* e, const I3DMeshParams& prm, int32_t color_mode, I3D
     return 0;
 }
 
+// Bits of the renderer's brick bitmap above which i3d_render_keyframes marches every lattice sample instead (128 MiB)
+constexpr int64_t kRenderBrickCap = 1ll << 30;
+
+// The voxel box and (when it fits under kRenderBrickCap) the brick bitmap of the current voxel set, timed as "render_bricks"; built
+// once per voxel set, dropped by forget_voxel_set.
+void render_bricks(I3DEngine* e)
+{
+    if (e->rd_box_ready) return;
+    cudaStream_t st = e->stream;
+    Timer t(e, "render_bricks");
+    const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
+    e->rd_box_d.ensure(6);
+    CK(cudaMemcpyAsync(e->rd_box_d.p, init, sizeof(init), cudaMemcpyHostToDevice, st));
+    render::bounds(e->n, e->x.p, e->y.p, e->z.p, e->rd_box_d.p, st);
+    CK(cudaMemcpyAsync(e->rd_box, e->rd_box_d.p, sizeof(e->rd_box), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    int64_t bits = 1;
+    for (int d = 0; d < 3; ++d)
+    {
+        e->rd_blo[d] = e->rd_box[d];
+        e->rd_bdim[d] = ((e->rd_box[3 + d] - e->rd_box[d]) >> 3) + 1;
+        bits *= e->rd_bdim[d];
+    }
+    e->rd_have_bricks = bits <= kRenderBrickCap;
+    if (e->rd_have_bricks)
+    {
+        const size_t words = static_cast<size_t>((bits + 31) >> 5);
+        e->rd_bits.ensure(words);
+        CK(cudaMemsetAsync(e->rd_bits.p, 0, words * sizeof(uint32_t), st));
+        render::bricks(e->n, e->x.p, e->y.p, e->z.p, e->rd_blo, e->rd_bdim, e->rd_bits.p, st);
+    }
+    t.stop();
+    e->rd_box_ready = true;
+}
+
+// Renders frames ids[0..n) (validated by the caller): the frame-scan camera of every frame, the voxel box / bitmap when the voxel set
+// changed, the march and the fixed-order finish of the statistics.  Refuses, before it writes anything, intrinsics (after pyr_scale) that
+// are not finite with fx, fy > 0 and distortion that is not finite.  Writes only the rd_* state and the resident planes.
+int render_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DRenderParams& P, I3DRenderStats* stats)
+{
+    cudaStream_t st = e->stream;
+    const int F = e->F, W = e->W, H = e->H;
+    double hc9[9];
+    CK(cudaMemcpyAsync(hc9, e->cam + 6 * static_cast<size_t>(F), 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    const SelectCam sc = select_cam(e, hc9, 0.0f);
+    if (!(std::isfinite(sc.fx) && sc.fx > 0.0f && std::isfinite(sc.fy) && sc.fy > 0.0f && std::isfinite(sc.cx) && std::isfinite(sc.cy)))
+        return fail(e, "i3d_render_keyframes: the camera needs finite intrinsics with fx, fy > 0 (fx %g, fy %g, cx %g, cy %g after pyr_scale %g)",
+                    sc.fx, sc.fy, sc.cx, sc.cy, e->pyr_scale);
+    for (int k = 0; k < 5; ++k)
+        if (!std::isfinite(sc.d[k])) return fail(e, "i3d_render_keyframes: distortion coefficient %d is not finite", k);
+    begin_timing(e, {"render", "render_bricks", "render_samples"});
+    e->have_render = false;
+    const size_t img = static_cast<size_t>(n) * W * H;
+    const int planes = P.planes;
+    if (planes & I3D_RENDER_DEPTH) e->rd_depth.ensure(img);
+    if (planes & I3D_RENDER_NORMAL) e->rd_normal.ensure(3 * img);
+    if (planes & I3D_RENDER_ALBEDO) e->rd_albedo.ensure(img);
+    if (planes & I3D_RENDER_SHADING) e->rd_shading.ensure(img);
+    if (planes & I3D_RENDER_INTENSITY) e->rd_intensity.ensure(img);
+    const int tiles_x = (W + kRenderTile - 1) / kRenderTile, tiles_y = (H + kRenderTile - 1) / kRenderTile;
+    e->rd_partials.ensure(static_cast<size_t>(n) * tiles_x * tiles_y * kRenderStats);
+    e->rd_sums.ensure(static_cast<size_t>(n) * kRenderStats);
+    e->rd_ids.ensure(n); e->rd_rt.ensure(12 * static_cast<size_t>(F)); e->rd_samples.ensure(1);
+    CK(cudaMemcpyAsync(e->rd_ids.p, ids, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(e->rd_samples.p, 0, sizeof(unsigned long long), st));
+    k_pose_mats<<<blocks_for(F, 64), 64, 0, st>>>(F, e->cam, e->rd_rt.p);
+    RenderCam cam;
+    cam.fx = sc.fx; cam.fy = sc.fy; cam.cx = sc.cx; cam.cy = sc.cy; cam.dist_zero = sc.dist_zero;
+    for (int k = 0; k < 5; ++k) cam.d[k] = sc.d[k];
+    {
+        Timer t(e, "render");
+        render_bricks(e);
+        RenderGrid rg;
+        rg.g = e->grid_view(P.sdf_source == 0 ? e->sdf0.p : e->sdf, e->alb);
+        rg.keys = e->up_keys.p; rg.vals = e->up_vals.p; rg.mask = e->hash_cap - 1;
+        rg.sh_has = P.photometric ? e->sh_has.p : nullptr;
+        if (!P.photometric) rg.g.sh = nullptr;
+        for (int d = 0; d < 3; ++d)
+        {
+            rg.lo[d] = static_cast<float>(e->rd_box[d]) * e->voxel_size;
+            rg.hi[d] = static_cast<float>(e->rd_box[3 + d]) * e->voxel_size;
+            rg.blo[d] = e->rd_blo[d]; rg.bdim[d] = e->rd_bdim[d];
+        }
+        rg.bricks = (e->rd_skip && e->rd_have_bricks) ? e->rd_bits.p : nullptr;
+        RenderViews rv;
+        rv.n = n; rv.W = W; rv.H = H; rv.tiles_x = tiles_x; rv.tiles_y = tiles_y;
+        rv.ids = e->rd_ids.p; rv.Rt = e->rd_rt.p; rv.depth = e->depth.p; rv.lum = e->lum.p;
+        rv.out_depth = (planes & I3D_RENDER_DEPTH) ? e->rd_depth.p : nullptr;
+        rv.out_normal = (planes & I3D_RENDER_NORMAL) ? e->rd_normal.p : nullptr;
+        rv.out_albedo = (planes & I3D_RENDER_ALBEDO) ? e->rd_albedo.p : nullptr;
+        rv.out_shading = (planes & I3D_RENDER_SHADING) ? e->rd_shading.p : nullptr;
+        rv.out_intensity = (planes & I3D_RENDER_INTENSITY) ? e->rd_intensity.p : nullptr;
+        rv.partials = e->rd_partials.p; rv.samples = e->rd_samples.p; rv.photometric = P.photometric ? 1 : 0;
+        render::march(rg, cam, rv, st);
+        render::finish(n, tiles_x * tiles_y, e->rd_partials.p, e->rd_sums.p, st);
+    }
+    std::vector<double> sums(static_cast<size_t>(n) * kRenderStats);
+    unsigned long long samples = 0;
+    CK(cudaMemcpyAsync(sums.data(), e->rd_sums.p, sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&samples, e->rd_samples.p, sizeof(samples), cudaMemcpyDeviceToHost, st));
+    collect_kernel_times(e);
+    CK(cudaGetLastError());
+    e->phases["render_samples"].count = static_cast<int64_t>(samples);
+    if (stats)
+        for (int i = 0; i < n; ++i)
+        {
+            const double* s = sums.data() + static_cast<size_t>(i) * kRenderStats;
+            I3DRenderStats r;
+            r.num_hit = static_cast<int64_t>(s[0]); r.num_observed = static_cast<int64_t>(s[1]);
+            r.depth_count = static_cast<int64_t>(s[2]); r.photo_count = static_cast<int64_t>(s[3]);
+            r.depth_abs = s[4]; r.depth_sq = s[5]; r.photo_abs = s[6]; r.photo_sq = s[7];
+            stats[i] = r;
+        }
+    e->have_render = true; e->rd_n = n; e->rd_planes = planes;
+    return 0;
+}
+
 } // namespace
 
 // =================================================================================================
@@ -2197,6 +2328,67 @@ int i3d_download_mesh(I3DEngine* e, float* xyz, uint8_t* rgb, int32_t* faces)
         CK(cudaStreamSynchronize(st));
         return 0;
     });
+}
+
+// ---- rendering the surface into the keyframes (i3d_render.cuh, DESIGN.md §6m) ----------------------
+uint64_t i3d_sizeof_render_params(void) { return sizeof(I3DRenderParams); }
+uint64_t i3d_sizeof_render_stats(void) { return sizeof(I3DRenderStats); }
+
+void i3d_default_render_params(I3DRenderParams* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    p->sdf_source = 1; p->planes = I3D_RENDER_ALL; p->photometric = 1;
+}
+
+int i3d_render_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DRenderParams* params, I3DRenderStats* stats)
+{
+    static const char* who = "i3d_render_keyframes";
+    if (!e) return 1;
+    if (!params) return fail(e, "%s: params is NULL", who);
+    if (e->world > 1) return fail(e, "%s: rendering runs on one GPU (world = %d)", who, e->world);
+    if (e->n <= 0) return fail(e, "%s: no grid", who);
+    if (e->F <= 0) return fail(e, "%s: no frames", who);
+    if (!e->have_cam) return fail(e, "%s: camera not set", who);
+    if (n <= 0 || !ids) return fail(e, "%s: need n > 0 frame ids (n = %d)", who, n);
+    if (n > kRenderMaxViews) return fail(e, "%s: %d views exceed the %d of one call", who, n, kRenderMaxViews);
+    for (int32_t k = 0; k < n; ++k)
+        if (ids[k] < 0 || ids[k] >= e->F) return fail(e, "%s: frame id %d (entry %d) is out of range [0, %d)", who, ids[k], k, e->F);
+    if (check_sdf_source(e, who, params->sdf_source)) return 1;
+    if (params->planes < 0 || params->planes > I3D_RENDER_ALL) return fail(e, "%s: planes must be a mask in [0, %d], got %d", who, I3D_RENDER_ALL, params->planes);
+    if (params->photometric != 0 && params->photometric != 1) return fail(e, "%s: photometric must be 0 or 1, got %d", who, params->photometric);
+    if ((params->planes & (I3D_RENDER_SHADING | I3D_RENDER_INTENSITY)) && !params->photometric)
+        return fail(e, "%s: the shading and intensity planes need photometric = 1", who);
+    if (params->photometric && !e->have_sh)
+        return fail(e, "%s: shading, intensity and photometric pairs need the per-voxel SH of the current grid (i3d_set_sh or i3d_estimate_lighting)", who);
+    return guarded(e, [&]() { return render_keyframes(e, n, ids, *params, stats); });
+}
+
+int i3d_download_render(I3DEngine* e, float* depth, float* normal, float* albedo, float* shading, float* intensity)
+{
+    if (!e) return 1;
+    if (!e->have_render) return fail(e, "i3d_download_render: no render (call i3d_render_keyframes after the last change of the grid or frames)");
+    const struct { float* dst; int bit; const char* name; } want[5] = {{depth, I3D_RENDER_DEPTH, "depth"}, {normal, I3D_RENDER_NORMAL, "normal"},
+        {albedo, I3D_RENDER_ALBEDO, "albedo"}, {shading, I3D_RENDER_SHADING, "shading"}, {intensity, I3D_RENDER_INTENSITY, "intensity"}};
+    for (const auto& w : want)
+        if (w.dst && !(e->rd_planes & w.bit)) return fail(e, "i3d_download_render: the %s plane was not rendered", w.name);
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t img = static_cast<size_t>(e->rd_n) * e->W * e->H * sizeof(float);
+        if (depth) CK(cudaMemcpyAsync(depth, e->rd_depth.p, img, cudaMemcpyDeviceToHost, st));
+        if (normal) CK(cudaMemcpyAsync(normal, e->rd_normal.p, 3 * img, cudaMemcpyDeviceToHost, st));
+        if (albedo) CK(cudaMemcpyAsync(albedo, e->rd_albedo.p, img, cudaMemcpyDeviceToHost, st));
+        if (shading) CK(cudaMemcpyAsync(shading, e->rd_shading.p, img, cudaMemcpyDeviceToHost, st));
+        if (intensity) CK(cudaMemcpyAsync(intensity, e->rd_intensity.p, img, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    });
+}
+
+int i3d_debug_set_render_skip(I3DEngine* e, int on)
+{
+    if (!e) return 1;
+    e->rd_skip = on != 0;
+    return 0;
 }
 
 // ---- keyframe selection and the RGB-D pyramid (i3d_frames.cuh, DESIGN.md §6i) --------------------

@@ -207,3 +207,29 @@ class I3DMeshInfo(C.Structure, _Dictable):
         ("ms_clean", C.c_double),
         ("ms_components", C.c_double),
     ]
+
+
+# I3D_RENDER_* plane bits of include/i3d_types.h
+RENDER_PLANES = {"depth": 1, "normal": 2, "albedo": 4, "shading": 8, "intensity": 16}
+
+
+class I3DRenderParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("sdf_source", C.c_int32),
+        ("planes", C.c_int32),
+        ("photometric", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
+class I3DRenderStats(C.Structure, _Dictable):
+    _fields_ = [
+        ("num_hit", C.c_int64),
+        ("num_observed", C.c_int64),
+        ("depth_count", C.c_int64),
+        ("photo_count", C.c_int64),
+        ("depth_abs", C.c_double),
+        ("depth_sq", C.c_double),
+        ("photo_abs", C.c_double),
+        ("photo_sq", C.c_double),
+    ]

@@ -11,8 +11,8 @@ import os
 
 import numpy as np
 
-from .ctypes_defs import (I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo, I3DMeshParams,
-                          I3DParams)
+from .ctypes_defs import (RENDER_PLANES, I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo,
+                          I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("I3D_LIB", os.path.join(_HERE, "libi3d_b200.so"))   # I3D_LIB: A/B builds of the same library
@@ -32,6 +32,8 @@ EXPORTED_SYMBOLS = [
     "i3d_sensor_frames_begin", "i3d_sensor_frames_add", "i3d_sensor_num_frames", "i3d_sensor_keyframe_scores", "i3d_fusion_integrate_sensor",
     "i3d_select_rgbd_frames",
     "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh", "i3d_extract_mesh_colored", "i3d_mode_colors",
+    "i3d_sizeof_render_params", "i3d_sizeof_render_stats", "i3d_default_render_params", "i3d_render_keyframes", "i3d_download_render",
+    "i3d_debug_set_render_skip",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
     "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_pcg_vectors", "i3d_debug_get_normal_equations",
@@ -86,6 +88,14 @@ def load_library():
     L.i3d_mode_colors.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_uint8)]
     L.i3d_sensor_num_frames.restype = C.c_int32
     L.i3d_sensor_num_frames.argtypes = [C.c_void_p]
+    L.i3d_sizeof_render_params.restype = C.c_uint64
+    L.i3d_sizeof_render_stats.restype = C.c_uint64
+    if L.i3d_sizeof_render_params() != C.sizeof(I3DRenderParams) or L.i3d_sizeof_render_stats() != C.sizeof(I3DRenderStats):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (render structs)")
+    L.i3d_render_keyframes.restype = C.c_int
+    L.i3d_render_keyframes.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(I3DRenderParams), C.POINTER(I3DRenderStats)]
+    L.i3d_download_render.restype = C.c_int
+    L.i3d_download_render.argtypes = [C.c_void_p] + [C.POINTER(C.c_float)] * 5
     _LIB = L
     return L
 
@@ -334,6 +344,35 @@ class Engine:
         rgb = np.empty((n, 3), np.uint8)
         self._check(self.L.i3d_mode_colors(self.h, src, m, _p(rgb, C.c_uint8)))
         return rgb
+
+    # ---- rendering the surface into the keyframes (DESIGN.md §6m) -------------------------------------------------------------
+    def render_keyframes(self, ids, source: str = "refined", planes=("depth", "normal", "albedo", "shading", "intensity"),
+                         photometric: bool = True):
+        """Ray-casts the zero level set of `source` ("fused": sdf0, "refined") into the frames `ids` with the engine's current camera,
+        at the size of the installed frames.  Returns a dict with the requested planes, float32 [n, H, W] (normal [n, H, W, 3]), and
+        stats: one dict per view (I3DRenderStats: hit / observed pixel counts, depth pairs and photometric pairs with their sums of
+        |error| and error^2).  planes=() gives the statistics only.  photometric=False skips the shading and the photometric pairs, so
+        no per-voxel SH is needed.  Device time: phase_ms("render")."""
+        src = self._mesh_source(source)
+        mask = 0
+        for p in planes:
+            if p not in RENDER_PLANES:
+                raise ValueError(f"plane must be one of {sorted(RENDER_PLANES)}, got {p!r}")
+            mask |= RENDER_PLANES[p]
+        ids, n = self._ids(ids)
+        prm = I3DRenderParams(src, mask, 1 if photometric else 0, 0)
+        stats = (I3DRenderStats * max(n, 1))()
+        self._check(self.L.i3d_render_keyframes(self.h, C.c_int32(n), _p(ids, C.c_int32), C.byref(prm), stats))
+        W, H = self.frame_size
+        out = {p: np.empty((n, H, W, 3) if p == "normal" else (n, H, W), np.float32) for p in RENDER_PLANES if RENDER_PLANES[p] & mask}
+        if out:
+            self._check(self.L.i3d_download_render(self.h, *(_p(out.get(p), C.c_float) for p in RENDER_PLANES)))
+        out["stats"] = [stats[i].as_dict() for i in range(n)]
+        return out
+
+    def set_render_skip(self, on: bool):
+        """True (default): the renderer jumps over empty 8^3 bricks; False: it evaluates every lattice sample (same results)."""
+        self._check(self.L.i3d_debug_set_render_skip(self.h, C.c_int(1 if on else 0)))
 
     # ---- keyframe selection and the RGB-D pyramid (KeyframeSelection::estimateBlur, Pyramid::create) ----------------------
     def keyframe_scores(self, bgr):
