@@ -226,6 +226,36 @@ int         i3d_render_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, co
  * resident mesh of i3d_extract_mesh; a change of the voxel set or of the frames drops them. */
 int         i3d_download_render(I3DEngine* e, float* depth, float* normal, float* albedo, float* shading, float* intensity);
 
+/* ---- tracking sensor frames against the surface: point-to-plane ICP over the depth pyramid (DESIGN.md §6n) ---- */
+/* Frames tracked per device pass: bounds the scratch memory (I3D_TRACK_CHUNK prediction, pyramid and normal planes at depth size). */
+#define I3D_TRACK_CHUNK 32
+uint64_t    i3d_sizeof_track_params(void);
+uint64_t    i3d_sizeof_track_info(void);
+/* sdf_source 0, 3 levels, iterations {10, 5, 4, 0}, max_distance 0.05 m, min_normal_cos cos(20 deg), min_correspondences 100. */
+void        i3d_default_track_params(I3DTrackParams* p);
+/* Frame-to-model tracking of the stored sensor frames ids[0..n) (distinct ids) against params->sdf_source of the current grid.  Per frame:
+ * the surface rendered at the input pose with the store's depth camera (the prediction), the depth pyramid of the stored depth, and
+ * Gauss-Newton iterations of point-to-plane ICP, coarsest level first, every iteration enqueued without host synchronisation.
+ * pose_in / pose_out: world -> camera, double [n][12] (R row-major | t), the Rt layout of fusion and render; info[n] may be NULL.
+ * Reads the grid, the store and the renderer's voxel box; writes only its own buffers, pose_out and info.  A frame's result does not depend
+ * on the other frames of the call.  Fails, writing nothing, without grid or stored frames, for n <= 0 or n > 65535, an id out of range or
+ * repeated, a non-finite input pose, num_levels outside 1..4 or a level built from a level under 3 px, negative iterations, max_distance
+ * not finite and > 0, min_normal_cos outside [-1, 1], min_correspondences < 6, a bad sdf_source, and world > 1.
+ * Device time: i3d_phase_ms("track") for the call, of which "track_predict", "track_pyramid" and "track_icp";
+ * i3d_phase_count("track_correspondences") = rows of every evaluated system. */
+int         i3d_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params,
+                                    double* pose_out, I3DTrackInfo* info);
+/* Parity hook: sums [n][29] = the last evaluated system of each frame of the last call (21 upper-triangle entries of J^T J row by row,
+ * 6 of J^T r, sum r^2, rows) and pose_cam_to_world [n][12] = its pose state (R row-major | t, camera -> world) after the last solve.
+ * Either pointer may be NULL.  Fails before a tracking call. */
+int         i3d_debug_get_track_system(I3DEngine* e, double* sums, double* pose_cam_to_world);
+/* Parity hook: the planes of the last pass (the last I3D_TRACK_CHUNK frames or fewer) of the last call, for the frames of that pass:
+ * depth [m][H_l][W_l] and camera-frame normals [m][H_l][W_l][3] of pyramid level `level`, the prediction depth [m][H][W] and world
+ * normals [m][H][W][3], and mask uint8 [m][H][W] (1 = a correspondence of the last level-0 system).  Any pointer may be NULL.  m is
+ * returned in *frames (may be NULL).  Fails before a tracking call and for a level that call did not build. */
+int         i3d_debug_get_track_planes(I3DEngine* e, int32_t level, float* depth, float* normal, float* pred_depth, float* pred_normal,
+                                       uint8_t* mask, int32_t* frames);
+
 /* ---- keyframe selection and the RGB-D image pyramid: the inputs of fusion and refinement (DESIGN.md §6i) ---- */
 /* Frames scored per device pass by i3d_keyframe_scores: bounds its scratch memory (I3D_KEYFRAME_CHUNK * W * H * 3 bytes). */
 #define I3D_KEYFRAME_CHUNK 32

@@ -234,6 +234,37 @@ typedef struct I3DRenderStats
     double  photo_abs, photo_sq;          /* sum |I_r - I_obs|, sum (I_r - I_obs)^2 over the photometric pairs (I_obs: the frame's luminance) */
 } I3DRenderStats;
 
+/* ---- tracking sensor frames against the surface: point-to-plane ICP over the depth pyramid (DESIGN.md §6n) ---- */
+/* Per-frame outcome of a tracking call (I3DTrackInfo::status). */
+enum
+{
+    I3D_TRACK_OK = 0,                     /* every scheduled update applied */
+    I3D_TRACK_FEW_CORRESPONDENCES = 1,    /* a system had fewer than min_correspondences rows: frozen there */
+    I3D_TRACK_NOT_POSITIVE_DEFINITE = 2,  /* the Cholesky factorisation of a system failed: frozen there */
+    I3D_TRACK_NON_FINITE = 3              /* a system, its update or the updated pose was not finite: frozen there */
+};
+
+typedef struct I3DTrackParams
+{
+    int32_t sdf_source;                   /* 0 = sdf0, 1 = sdf_refined, as in I3DMeshParams / I3DRenderParams */
+    int32_t num_levels;                   /* depth pyramid levels, 1..4 */
+    int32_t iterations[4];                /* Gauss-Newton iterations per level, level 0 first; the coarsest level runs first */
+    float   max_distance;                 /* correspondence gate |p - q|, metres */
+    float   min_normal_cos;               /* correspondence gate n_in . n_model; -1 = off */
+    int32_t min_correspondences;          /* fewer rows at a solve freeze the frame (>= 6) */
+    int32_t reserved;
+} I3DTrackParams;
+
+typedef struct I3DTrackInfo
+{
+    int32_t        status;                /* I3D_TRACK_* */
+    int32_t        iterations;            /* updates applied before the frame froze or finished */
+    int64_t        correspondences;       /* rows of the last evaluated system */
+    double         residual_sq;           /* sum of squared point-to-plane residuals of that system (metres^2) */
+    double         update_norm;           /* |xi| of the last applied update (0 without one) */
+    I3DRenderStats initial;               /* the prediction render against the frame's depth, at the input pose */
+} I3DTrackInfo;
+
 #ifdef __cplusplus
 }
 #endif

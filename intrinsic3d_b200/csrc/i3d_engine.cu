@@ -34,6 +34,7 @@
 #include "i3d_frames.cuh"
 #include "i3d_mesh.h"
 #include "i3d_render.h"
+#include "i3d_track.h"
 
 #include <cub/device/device_radix_sort.cuh>
 
@@ -238,6 +239,12 @@ struct I3DEngine
     Dev<float> rd_depth, rd_normal, rd_albedo, rd_shading, rd_intensity;
     bool have_render = false;
     int rd_n = 0, rd_planes = 0;
+    // frame-to-model tracker (i3d_track.cuh): per-call state of n frames, and the chunk's prediction, pyramid, normal and mask planes
+    // (scratch that only grows; the planes of the last chunk stay for i3d_debug_get_track_planes)
+    Dev<float> tr_rt; Dev<int32_t> tr_ids; Dev<double> tr_pose_in; Dev<TrackState> tr_state;
+    Dev<double> tr_sys, tr_sums, tr_partials, tr_rd_partials, tr_rd_sums; Dev<unsigned long long> tr_counters;
+    Dev<float> tr_pdepth, tr_pnrm, tr_depth[kTrackMaxLevels], tr_nrm[kTrackMaxLevels]; Dev<uint8_t> tr_mask;
+    int tr_n = 0, tr_levels = 0, tr_last_m = 0, tr_W[kTrackMaxLevels] = {}, tr_H[kTrackMaxLevels] = {};
     // shard (multi-GPU)
     int64_t shard_begin = 0, shard_end = -1;
     int rank = 0, world = 1;
@@ -1478,6 +1485,142 @@ int render_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DRende
     return 0;
 }
 
+// Tracks the stored frames ids[0..n) (validated by the caller; Wl / Hl: the pyramid sizes) in passes of I3D_TRACK_CHUNK frames.  Per pass:
+// the prediction (render::march at the input poses with the depth camera, geometry only), the depth pyramid (k_frames_depthdown chain on
+// the gathered store depth) with its normals, then every Gauss-Newton iteration of every level, coarsest first, with no host
+// synchronisation; one read-back at the end.  Writes only the tr_* state, pose_out and info.
+int track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl,
+                        const int* Hl, double* pose_out, I3DTrackInfo* info)
+{
+    cudaStream_t st = e->stream;
+    const I3DFusionCamera& dc = e->sn_dcam;
+    const int L = P.num_levels, W = dc.width, H = dc.height, C = std::min<int>(n, I3D_TRACK_CHUNK);
+    const size_t img = static_cast<size_t>(W) * H;
+    const int tiles_x = (W + kRenderTile - 1) / kRenderTile, tiles_y = (H + kRenderTile - 1) / kRenderTile;
+    static_assert(kRenderTile == kTrackTile, "the prediction and the rows share the level-0 tile grid");
+    begin_timing(e, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences"});
+    e->tr_n = 0;
+    e->tr_ids.ensure(n); e->tr_pose_in.ensure(12 * static_cast<size_t>(n)); e->tr_state.ensure(n);
+    e->tr_sys.ensure(static_cast<size_t>(n) * kTrackVals); e->tr_rd_sums.ensure(static_cast<size_t>(n) * kRenderStats);
+    e->tr_rt.ensure(12 * static_cast<size_t>(e->sn_F)); e->tr_counters.ensure(2);
+    e->tr_rd_partials.ensure(static_cast<size_t>(C) * tiles_x * tiles_y * kRenderStats);
+    e->tr_partials.ensure(static_cast<size_t>(C) * tiles_x * tiles_y * kTrackVals); e->tr_sums.ensure(static_cast<size_t>(C) * kTrackVals);
+    e->tr_pdepth.ensure(C * img); e->tr_pnrm.ensure(3 * C * img); e->tr_mask.ensure(C * img);
+    for (int l = 0; l < L; ++l)
+    {
+        const size_t c = static_cast<size_t>(C) * Wl[l] * Hl[l];
+        e->tr_depth[l].ensure(c); e->tr_nrm[l].ensure(3 * c);
+    }
+    // the input poses in float, scattered by sensor id: the march reads Rt + 12 * id
+    std::vector<float> hrt(12 * static_cast<size_t>(e->sn_F), 0.0f);
+    for (int k = 0; k < n; ++k)
+        for (int i = 0; i < 12; ++i) hrt[12 * static_cast<size_t>(ids[k]) + i] = static_cast<float>(pose_in[12 * static_cast<size_t>(k) + i]);
+    CK(cudaMemcpyAsync(e->tr_ids.p, ids, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(e->tr_pose_in.p, pose_in, 12 * static_cast<size_t>(n) * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(e->tr_rt.p, hrt.data(), hrt.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(e->tr_counters.p, 0, 2 * sizeof(unsigned long long), st));
+    int total_iters = 0;
+    for (int l = 0; l < L; ++l) total_iters += P.iterations[l];
+    TrackCam cam[kTrackMaxLevels];
+    for (int l = 0; l < L; ++l)
+    {
+        const double s = std::ldexp(1.0, -l);       // the pyramid scale, as select_cam applies pyr_scale
+        cam[l] = TrackCam{Wl[l], Hl[l], static_cast<float>(dc.fx * s), static_cast<float>(dc.fy * s), static_cast<float>(dc.cx * s),
+                          static_cast<float>(dc.cy * s)};
+    }
+    Timer whole(e, "track");
+    render_bricks(e);
+    RenderGrid rg;
+    rg.g = e->grid_view(P.sdf_source == 0 ? e->sdf0.p : e->sdf, e->alb);
+    rg.g.sh = nullptr;
+    rg.keys = e->up_keys.p; rg.vals = e->up_vals.p; rg.mask = e->hash_cap - 1; rg.sh_has = nullptr;
+    for (int d = 0; d < 3; ++d)
+    {
+        rg.lo[d] = static_cast<float>(e->rd_box[d]) * e->voxel_size;
+        rg.hi[d] = static_cast<float>(e->rd_box[3 + d]) * e->voxel_size;
+        rg.blo[d] = e->rd_blo[d]; rg.bdim[d] = e->rd_bdim[d];
+    }
+    rg.bricks = (e->rd_skip && e->rd_have_bricks) ? e->rd_bits.p : nullptr;
+    RenderCam rcam{};
+    rcam.fx = dc.fx; rcam.fy = dc.fy; rcam.cx = dc.cx; rcam.cy = dc.cy; rcam.dist_zero = 1;
+    track::init(n, e->tr_pose_in.p, e->tr_state.p, st);
+    const float max_dist_sq = P.max_distance * P.max_distance;
+    int m = 0;
+    for (int c0 = 0; c0 < n; c0 += C)
+    {
+        m = std::min(C, n - c0);
+        const int32_t* ids_d = e->tr_ids.p + c0;
+        {
+            Timer t(e, "track_predict");
+            RenderViews rv{};
+            rv.n = m; rv.W = W; rv.H = H; rv.tiles_x = tiles_x; rv.tiles_y = tiles_y;
+            rv.ids = ids_d; rv.Rt = e->tr_rt.p; rv.depth = e->sn_depth.p; rv.lum = nullptr;
+            rv.out_depth = e->tr_pdepth.p; rv.out_normal = e->tr_pnrm.p;
+            rv.partials = e->tr_rd_partials.p; rv.samples = e->tr_counters.p + 1; rv.photometric = 0;
+            render::march(rg, rcam, rv, st);
+            render::finish(m, tiles_x * tiles_y, e->tr_rd_partials.p, e->tr_rd_sums.p + static_cast<size_t>(c0) * kRenderStats, st);
+        }
+        {
+            Timer t(e, "track_pyramid");
+            track::gather(m, W, H, ids_d, e->sn_depth.p, e->tr_depth[0].p, st);
+            for (int l = 1; l < L; ++l)
+            {
+                const dim3 grid((Wl[l] + 31) / 32, (Hl[l] + 7) / 8, m);
+                k_frames_depthdown<<<grid, dim3(32, 8), 0, st>>>(m, Wl[l - 1], Hl[l - 1], e->tr_depth[l - 1].p, e->tr_depth[l].p);
+            }
+            for (int l = 0; l < L; ++l) track::normals(m, cam[l], e->tr_depth[l].p, e->tr_nrm[l].p, st);
+        }
+        {
+            Timer t(e, "track_icp");
+            CK(cudaMemsetAsync(e->tr_mask.p, 0, m * img, st));
+            TrackRows tr{};
+            tr.pcam = cam[0]; tr.pdepth = e->tr_pdepth.p; tr.pnrm = e->tr_pnrm.p; tr.ids = ids_d; tr.rt_in = e->tr_rt.p;
+            tr.state = e->tr_state.p + c0; tr.max_dist_sq = max_dist_sq; tr.min_cos = P.min_normal_cos;
+            tr.use_cos = P.min_normal_cos > -1.0f ? 1 : 0; tr.partials = e->tr_partials.p;
+            auto system = [&](int l, int solve) {
+                tr.cam = cam[l]; tr.depth = e->tr_depth[l].p; tr.nrm = e->tr_nrm[l].p; tr.mask = l == 0 ? e->tr_mask.p : nullptr;
+                tr.tiles_x = (Wl[l] + kTrackTile - 1) / kTrackTile; tr.tiles_y = (Hl[l] + kTrackTile - 1) / kTrackTile;
+                {
+                    Timer tk(e, "k_track_rows", 1);
+                    track::rows(m, tr, st);
+                }
+                track::finish(m, tr.tiles_x * tr.tiles_y, e->tr_partials.p, e->tr_sums.p, st);
+                track::solve(m, e->tr_sums.p, e->tr_state.p + c0, e->tr_sys.p + static_cast<size_t>(c0) * kTrackVals, P.min_correspondences, solve,
+                             e->tr_counters.p, st);
+            };
+            for (int l = L - 1; l >= 0; --l)
+                for (int it = 0; it < P.iterations[l]; ++it) system(l, 1);
+            if (total_iters == 0) system(0, 0);        // no update: the level-0 system at the input pose
+        }
+    }
+    std::vector<TrackState> hs(n);
+    std::vector<double> rs(static_cast<size_t>(n) * kRenderStats);
+    unsigned long long counters[2] = {0, 0};
+    CK(cudaMemcpyAsync(hs.data(), e->tr_state.p, n * sizeof(TrackState), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(rs.data(), e->tr_rd_sums.p, rs.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(counters, e->tr_counters.p, sizeof(counters), cudaMemcpyDeviceToHost, st));
+    whole.stop();
+    collect_kernel_times(e);
+    CK(cudaGetLastError());
+    e->phases["track_correspondences"].count = static_cast<int64_t>(counters[0]);
+    for (int k = 0; k < n; ++k)
+    {
+        std::memcpy(pose_out + 12 * static_cast<size_t>(k), hs[k].w2c, 12 * sizeof(double));
+        if (!info) continue;
+        I3DTrackInfo r{};
+        r.status = hs[k].status; r.iterations = hs[k].iterations; r.correspondences = hs[k].correspondences;
+        r.residual_sq = hs[k].residual_sq; r.update_norm = hs[k].update_norm;
+        const double* s = rs.data() + static_cast<size_t>(k) * kRenderStats;
+        r.initial.num_hit = static_cast<int64_t>(s[0]); r.initial.num_observed = static_cast<int64_t>(s[1]);
+        r.initial.depth_count = static_cast<int64_t>(s[2]); r.initial.photo_count = static_cast<int64_t>(s[3]);
+        r.initial.depth_abs = s[4]; r.initial.depth_sq = s[5]; r.initial.photo_abs = s[6]; r.initial.photo_sq = s[7];
+        info[k] = r;
+    }
+    e->tr_n = n; e->tr_levels = L; e->tr_last_m = m;
+    for (int l = 0; l < L; ++l) { e->tr_W[l] = Wl[l]; e->tr_H[l] = Hl[l]; }
+    return 0;
+}
+
 } // namespace
 
 // =================================================================================================
@@ -2389,6 +2532,94 @@ int i3d_debug_set_render_skip(I3DEngine* e, int on)
     if (!e) return 1;
     e->rd_skip = on != 0;
     return 0;
+}
+
+// ---- tracking sensor frames against the surface (i3d_track.cuh, DESIGN.md §6n) -------------------
+uint64_t i3d_sizeof_track_params(void) { return sizeof(I3DTrackParams); }
+uint64_t i3d_sizeof_track_info(void) { return sizeof(I3DTrackInfo); }
+
+void i3d_default_track_params(I3DTrackParams* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    p->sdf_source = 0; p->num_levels = 3;
+    p->iterations[0] = 10; p->iterations[1] = 5; p->iterations[2] = 4; p->iterations[3] = 0;
+    p->max_distance = 0.05f; p->min_normal_cos = static_cast<float>(std::cos(20.0 * M_PI / 180.0));
+    p->min_correspondences = 100;
+}
+
+int i3d_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params, double* pose_out,
+                            I3DTrackInfo* info)
+{
+    static const char* who = "i3d_track_sensor_frames";
+    if (!e) return 1;
+    if (!params || !pose_in || !pose_out) return fail(e, "%s: params, pose_in and pose_out must not be NULL", who);
+    if (e->world > 1) return fail(e, "%s: tracking runs on one GPU (world = %d)", who, e->world);
+    if (e->n <= 0) return fail(e, "%s: no grid", who);
+    if (check_sensor_ids(e, who, n, ids)) return 1;
+    if (n > kRenderMaxViews) return fail(e, "%s: %d frames exceed the %d of one call", who, n, kRenderMaxViews);
+    {
+        std::vector<uint8_t> seen(e->sn_F, 0);
+        for (int32_t k = 0; k < n; ++k)
+        {
+            if (seen[ids[k]]) return fail(e, "%s: frame id %d is repeated (entry %d); each frame has one pose", who, ids[k], k);
+            seen[ids[k]] = 1;
+        }
+    }
+    for (int64_t i = 0; i < 12 * static_cast<int64_t>(n); ++i)
+        if (!std::isfinite(pose_in[i])) return fail(e, "%s: the input pose of entry %d is not finite", who, static_cast<int>(i / 12));
+    const I3DTrackParams& P = *params;
+    if (check_sdf_source(e, who, P.sdf_source)) return 1;
+    if (P.num_levels < 1 || P.num_levels > kTrackMaxLevels) return fail(e, "%s: num_levels must be in 1..%d, got %d", who, kTrackMaxLevels, P.num_levels);
+    int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
+    Wl[0] = e->sn_dcam.width; Hl[0] = e->sn_dcam.height;
+    for (int l = 1; l < P.num_levels; ++l)
+    {
+        if (Wl[l - 1] < 3 || Hl[l - 1] < 3)
+            return fail(e, "%s: level %d would be built from a %d x %d level; downsampling needs at least 3 px on each axis", who, l, Wl[l - 1], Hl[l - 1]);
+        Wl[l] = Wl[l - 1] / 2; Hl[l] = Hl[l - 1] / 2;
+    }
+    for (int l = 0; l < kTrackMaxLevels; ++l)
+        if (P.iterations[l] < 0) return fail(e, "%s: iterations[%d] = %d is negative", who, l, P.iterations[l]);
+    if (!(std::isfinite(P.max_distance) && P.max_distance > 0.0f)) return fail(e, "%s: max_distance must be finite and > 0, got %g", who, P.max_distance);
+    if (!(P.min_normal_cos >= -1.0f && P.min_normal_cos <= 1.0f)) return fail(e, "%s: min_normal_cos must be in [-1, 1], got %g", who, P.min_normal_cos);
+    if (P.min_correspondences < 6) return fail(e, "%s: min_correspondences must be >= 6, got %d", who, P.min_correspondences);
+    return guarded(e, [&]() { return track_sensor_frames(e, n, ids, pose_in, P, Wl, Hl, pose_out, info); });
+}
+
+int i3d_debug_get_track_system(I3DEngine* e, double* sums, double* pose_cam_to_world)
+{
+    if (!e) return 1;
+    if (e->tr_n <= 0) return fail(e, "i3d_debug_get_track_system: no tracking call");
+    return guarded(e, [&]() {
+        const int n = e->tr_n;
+        if (sums) CK(cudaMemcpyAsync(sums, e->tr_sys.p, static_cast<size_t>(n) * kTrackVals * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+        std::vector<TrackState> hs(pose_cam_to_world ? n : 0);
+        if (pose_cam_to_world) CK(cudaMemcpyAsync(hs.data(), e->tr_state.p, n * sizeof(TrackState), cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaStreamSynchronize(e->stream));
+        for (size_t k = 0; k < hs.size(); ++k) std::memcpy(pose_cam_to_world + 12 * k, hs[k].T, 12 * sizeof(double));
+        return 0;
+    });
+}
+
+int i3d_debug_get_track_planes(I3DEngine* e, int32_t level, float* depth, float* normal, float* pred_depth, float* pred_normal, uint8_t* mask,
+                               int32_t* frames)
+{
+    if (!e) return 1;
+    if (e->tr_n <= 0) return fail(e, "i3d_debug_get_track_planes: no tracking call");
+    if (level < 0 || level >= e->tr_levels) return fail(e, "i3d_debug_get_track_planes: level %d was not built (%d levels)", level, e->tr_levels);
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t m = static_cast<size_t>(e->tr_last_m);
+        const size_t lv = m * e->tr_W[level] * e->tr_H[level], img = m * e->tr_W[0] * e->tr_H[0];
+        if (depth) CK(cudaMemcpyAsync(depth, e->tr_depth[level].p, lv * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (normal) CK(cudaMemcpyAsync(normal, e->tr_nrm[level].p, 3 * lv * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (pred_depth) CK(cudaMemcpyAsync(pred_depth, e->tr_pdepth.p, img * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (pred_normal) CK(cudaMemcpyAsync(pred_normal, e->tr_pnrm.p, 3 * img * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (mask) CK(cudaMemcpyAsync(mask, e->tr_mask.p, img, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (frames) *frames = static_cast<int32_t>(m);
+        return 0;
+    });
 }
 
 // ---- keyframe selection and the RGB-D pyramid (i3d_frames.cuh, DESIGN.md §6i) --------------------

@@ -1,0 +1,331 @@
+/*
+ * i3d_track.cuh — frame-to-model tracking on the device (DESIGN.md §6n): point-to-plane ICP of stored depth frames against the surface
+ * rendered at their input poses, over the depth pyramid, with per-frame 6 x 6 normal equations solved in double.
+ *
+ *   k_track_init     one thread per frame: T_cw = inverse of the input pose, its float copy, the returned pose = the input
+ *   k_track_gather   the chunk's stored depth planes side by side (level 0 of its pyramid)
+ *   k_track_normals  camera-frame normals by the computeNormals(K, depth, 0.3) rule of k_fuse_normals, frames in gridDim.y
+ *   k_track_rows     one thread per pixel, 16 x 16 tiles, frames in gridDim.z: association, gates, the point-to-plane row and its
+ *                    29 products, reduced per tile (fixed warp shuffle tree, then the warps in order)
+ *   k_track_finish   per (frame, value) the frame's tiles summed in order
+ *   k_track_solve    one thread per frame: Cholesky of the 6 x 6 system in a fixed order, xi = -A^-1 b, T_cw <- [Rodrigues(w) | v] T_cw
+ *
+ * Compiled in its own translation unit, i3d_track.cu, and launched through the host wrappers declared in i3d_track.h.  Every float
+ * operation is explicitly rounded and every double operation is an explicit __d*_rn (no FMA contraction), so tests/track_ref.py restates
+ * the planes, masks and sums exactly.  A frame's bytes depend only on that frame.
+ */
+#pragma once
+#include "i3d_grid.cuh"
+#include "i3d_track.h"
+
+namespace i3d
+{
+
+#define DM(a, b) __dmul_rn((a), (b))
+#define DA(a, b) __dadd_rn((a), (b))
+#define DS(a, b) __dsub_rn((a), (b))
+
+// R (row-major 3 x 3) times v, sums left to right, plus t when given
+__device__ __forceinline__ void tr_xform(const float* R, const float* t, const float v[3], float out[3])
+{
+#pragma unroll
+    for (int d = 0; d < 3; ++d)
+    {
+        const float s = FA(FA(FM(R[3 * d], v[0]), FM(R[3 * d + 1], v[1])), FM(R[3 * d + 2], v[2]));
+        out[d] = t ? FA(s, t[d]) : s;
+    }
+}
+
+// world -> camera of T_cw (R | t): R^T | -(R^T t), in double
+__device__ __forceinline__ void tr_inverse(const double* T, double* out)
+{
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+    {
+#pragma unroll
+        for (int j = 0; j < 3; ++j) out[3 * i + j] = T[3 * j + i];
+        out[9 + i] = -DA(DA(DM(T[i], T[9]), DM(T[3 + i], T[10])), DM(T[6 + i], T[11]));
+    }
+}
+
+__global__ void k_track_init(int n, const double* __restrict__ pose_in, TrackState* __restrict__ state)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const double* P = pose_in + 12 * static_cast<int64_t>(k);
+    TrackState& s = state[k];
+    tr_inverse(P, s.T);                 // the inverse of R | t has the same form: R^T | -(R^T t)
+#pragma unroll
+    for (int i = 0; i < 12; ++i) { s.w2c[i] = P[i]; s.Tf[i] = __double2float_rn(s.T[i]); }
+    s.status = 0; s.iterations = 0; s.frozen = 0; s.pad = 0;
+    s.correspondences = 0; s.residual_sq = 0.0; s.update_norm = 0.0;
+}
+
+__global__ void k_track_gather(int n, int W, int H, const int32_t* __restrict__ ids, const float* __restrict__ src, float* __restrict__ dst)
+{
+    const int64_t img = static_cast<int64_t>(W) * H;
+    const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    if (i >= img) return;
+    const int k = blockIdx.y;
+    dst[k * img + i] = src[static_cast<int64_t>(ids[k]) * img + i];
+}
+
+// computeVertexMap (processing.cpp:49-69) as k_fuse_normals evaluates it: (x0 d, y0 d, d), x0 = (x - cx) * (1 / fx)
+__device__ __forceinline__ void tr_vertex(const float* __restrict__ depth, int W, int x, int y, float fxi, float fyi, float cx, float cy, float v[3])
+{
+    const float d = depth[static_cast<int64_t>(y) * W + x];
+    v[0] = FM(FM(FS(static_cast<float>(x), cx), fxi), d);
+    v[1] = FM(FM(FS(static_cast<float>(y), cy), fyi), d);
+    v[2] = d;
+}
+
+// The rule of k_fuse_normals (computeNormals(vertex_map, 0.3), processing.cpp:72-118) for frame blockIdx.y: central tangents,
+// n = (t_y x t_x).normalized(); zero where undefined
+__global__ void k_track_normals(TrackCam cam, const float* __restrict__ depth_all, float* __restrict__ nrm_all)
+{
+    const int W = cam.W, H = cam.H;
+    const int64_t img = static_cast<int64_t>(W) * H;
+    const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    if (i >= img) return;
+    const float* depth = depth_all + blockIdx.y * img;
+    float* nrm = nrm_all + 3 * blockIdx.y * img;
+    const int y = static_cast<int>(i / W), x = static_cast<int>(i - static_cast<int64_t>(y) * W);
+    float n[3] = {0.0f, 0.0f, 0.0f};
+    if (x >= 1 && y >= 1 && x < W - 1 && y < H - 1 && depth[i] != 0.0f)
+    {
+        const float fxi = FD(1.0f, cam.fx), fyi = FD(1.0f, cam.fy);
+        float vx0[3], vx1[3], vy0[3], vy1[3];
+        tr_vertex(depth, W, x - 1, y, fxi, fyi, cam.cx, cam.cy, vx0);
+        tr_vertex(depth, W, x + 1, y, fxi, fyi, cam.cx, cam.cy, vx1);
+        tr_vertex(depth, W, x, y - 1, fxi, fyi, cam.cx, cam.cy, vy0);
+        tr_vertex(depth, W, x, y + 1, fxi, fyi, cam.cx, cam.cy, vy1);
+        if (vx0[2] != 0.0f && vx1[2] != 0.0f && vy0[2] != 0.0f && vy1[2] != 0.0f)
+        {
+            const float tx[3] = {FS(vx1[0], vx0[0]), FS(vx1[1], vx0[1]), FS(vx1[2], vx0[2])};
+            const float ty[3] = {FS(vy1[0], vy0[0]), FS(vy1[1], vy0[1]), FS(vy1[2], vy0[2])};
+            const float lx = __fsqrt_rn(FA(FA(FM(tx[0], tx[0]), FM(tx[1], tx[1])), FM(tx[2], tx[2])));
+            const float ly = __fsqrt_rn(FA(FA(FM(ty[0], ty[0]), FM(ty[1], ty[1])), FM(ty[2], ty[2])));
+            if (lx < 0.3f && ly < 0.3f)
+            {
+                float c[3] = {FS(FM(ty[1], tx[2]), FM(ty[2], tx[1])), FS(FM(ty[2], tx[0]), FM(ty[0], tx[2])), FS(FM(ty[0], tx[1]), FM(ty[1], tx[0]))};
+                const float sq = FA(FA(FM(c[0], c[0]), FM(c[1], c[1])), FM(c[2], c[2]));
+                if (sq > 0.0f) { const float l = __fsqrt_rn(sq); c[0] = FD(c[0], l); c[1] = FD(c[1], l); c[2] = FD(c[2], l); }
+                n[0] = c[0]; n[1] = c[1]; n[2] = c[2];
+            }
+        }
+    }
+    nrm[3 * i] = n[0]; nrm[3 * i + 1] = n[1]; nrm[3 * i + 2] = n[2];
+}
+
+// The correspondence of pixel (u, v) of frame z at the current pose (DESIGN.md §6n): p (world), q (model point), n_m (model normal)
+__device__ __forceinline__ bool tr_associate(const TrackRows& tr, int z, int u, int v, const float* Tf, float p[3], float q[3], float nm[3])
+{
+    const int64_t pix = (static_cast<int64_t>(z) * tr.cam.H + v) * tr.cam.W + u;
+    const float d = tr.depth[pix];
+    if (!(d > 0.0f)) return false;
+    const float vc[3] = {FM(FD(FS(__int2float_rn(u), tr.cam.cx), tr.cam.fx), d), FM(FD(FS(__int2float_rn(v), tr.cam.cy), tr.cam.fy), d), d};
+    tr_xform(Tf, Tf + 9, vc, p);
+    // projection into the prediction (level 0, input pose R0 | t0), pixel int(x + 0.5f) (nv::round, Q35)
+    const float* R0 = tr.rt_in + 12 * static_cast<int64_t>(tr.ids[z]);
+    float pc[3];
+    tr_xform(R0, R0 + 9, p, pc);
+    if (!(pc[2] > 0.0f)) return false;
+    const TrackCam& c0 = tr.pcam;
+    const float tu = FA(FA(FM(c0.fx, FD(pc[0], pc[2])), c0.cx), 0.5f), tv = FA(FA(FM(c0.fy, FD(pc[1], pc[2])), c0.cy), 0.5f);
+    if (!(tu > -1.0f && tu < static_cast<float>(c0.W) && tv > -1.0f && tv < static_cast<float>(c0.H))) return false;
+    const int iu = __float2int_rz(tu), iv = __float2int_rz(tv);
+    const int64_t pp = (static_cast<int64_t>(z) * c0.H + iv) * c0.W + iu;
+    const float zm = tr.pdepth[pp];
+    if (!(zm > 0.0f)) return false;
+    nm[0] = tr.pnrm[3 * pp]; nm[1] = tr.pnrm[3 * pp + 1]; nm[2] = tr.pnrm[3 * pp + 2];
+    if (nm[0] == 0.0f && nm[1] == 0.0f && nm[2] == 0.0f) return false;
+    // q = o0 + z_m R0^T (x', y', 1), o0 = -R0^T t0, as the march built the ray of that pixel
+    const float xn = FD(FS(__int2float_rn(iu), c0.cx), c0.fx), yn = FD(FS(__int2float_rn(iv), c0.cy), c0.fy);
+    float dsq = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+    {
+        const float o = -FA(FA(FM(R0[k], R0[9]), FM(R0[3 + k], R0[10])), FM(R0[6 + k], R0[11]));
+        const float dir = FA(FA(FM(R0[k], xn), FM(R0[3 + k], yn)), R0[6 + k]);
+        q[k] = FA(o, FM(zm, dir));
+        const float e = FS(p[k], q[k]);
+        dsq = FA(dsq, FM(e, e));
+    }
+    if (!(dsq <= tr.max_dist_sq)) return false;
+    if (tr.use_cos)
+    {
+        const float* nc = tr.nrm + 3 * pix;
+        float nin[3];
+        tr_xform(Tf, nullptr, nc, nin);
+        const float dot = FA(FA(FM(nin[0], nm[0]), FM(nin[1], nm[1])), FM(nin[2], nm[2]));
+        if (!(dot >= tr.min_cos)) return false;
+    }
+    return true;
+}
+
+// One thread per pixel of frame blockIdx.z at the rows launch's level
+__global__ void __launch_bounds__(kTrackTile * kTrackTile) k_track_rows(TrackRows tr)
+{
+    __shared__ double warp_sums[kTrackTile * kTrackTile / 32][kTrackVals];
+    const int u = blockIdx.x * kTrackTile + threadIdx.x, v = blockIdx.y * kTrackTile + threadIdx.y, z = blockIdx.z;
+    const int tid = threadIdx.y * kTrackTile + threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const TrackState& s = tr.state[z];
+    const bool frozen = s.frozen != 0;
+    double J[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, r = 0.0, cnt = 0.0;
+    if (u < tr.cam.W && v < tr.cam.H && !frozen)
+    {
+        float Tf[12];
+#pragma unroll
+        for (int i = 0; i < 12; ++i) Tf[i] = s.Tf[i];
+        float p[3], q[3], nm[3];
+        const bool ok = tr_associate(tr, z, u, v, Tf, p, q, nm);
+        if (tr.mask) tr.mask[(static_cast<int64_t>(z) * tr.cam.H + v) * tr.cam.W + u] = ok ? 1 : 0;
+        if (ok)
+        {
+            double pd[3], nd[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) { pd[k] = static_cast<double>(p[k]); nd[k] = static_cast<double>(nm[k]); }
+            r = DA(DA(DM(nd[0], DS(pd[0], static_cast<double>(q[0]))), DM(nd[1], DS(pd[1], static_cast<double>(q[1])))),
+                   DM(nd[2], DS(pd[2], static_cast<double>(q[2]))));
+            J[0] = DS(DM(pd[1], nd[2]), DM(pd[2], nd[1]));
+            J[1] = DS(DM(pd[2], nd[0]), DM(pd[0], nd[2]));
+            J[2] = DS(DM(pd[0], nd[1]), DM(pd[1], nd[0]));
+            J[3] = nd[0]; J[4] = nd[1]; J[5] = nd[2];
+            cnt = 1.0;
+        }
+    }
+    else if (u < tr.cam.W && v < tr.cam.H && tr.mask)
+        tr.mask[(static_cast<int64_t>(z) * tr.cam.H + v) * tr.cam.W + u] = 0;
+    // the 29 products, each summed over the warp by a fixed shuffle tree as it is formed; lane 0 keeps the warp's sums
+    int j = 0;
+#pragma unroll
+    for (int a = 0; a < 6; ++a)
+    {
+#pragma unroll
+        for (int b = a; b < 6; ++b, ++j)
+        {
+            double x = DM(J[a], J[b]);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) x = DA(x, __shfl_down_sync(0xffffffffu, x, o));
+            if (lane == 0) warp_sums[warp][j] = x;
+        }
+    }
+#pragma unroll
+    for (int a = 0; a < 8; ++a, ++j)
+    {
+        double x = a < 6 ? DM(J[a], r) : (a == 6 ? DM(r, r) : cnt);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) x = DA(x, __shfl_down_sync(0xffffffffu, x, o));
+        if (lane == 0) warp_sums[warp][j] = x;
+    }
+    __syncthreads();
+    if (tid < kTrackVals)
+    {
+        double t = warp_sums[0][tid];
+#pragma unroll
+        for (int w = 1; w < kTrackTile * kTrackTile / 32; ++w) t = DA(t, warp_sums[w][tid]);
+        const int64_t tile = (static_cast<int64_t>(z) * tr.tiles_y + blockIdx.y) * tr.tiles_x + blockIdx.x;
+        tr.partials[tile * kTrackVals + tid] = t;
+    }
+}
+
+// One thread per (frame, value): the frame's tiles summed in order
+__global__ void k_track_finish(int n, int tiles, const double* __restrict__ partials, double* __restrict__ sums)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n * kTrackVals) return;
+    const int f = i / kTrackVals, j = i % kTrackVals;
+    const double* p = partials + static_cast<int64_t>(f) * tiles * kTrackVals + j;
+    double s = 0.0;
+    for (int t = 0; t < tiles; ++t) s = DA(s, p[static_cast<int64_t>(t) * kTrackVals]);
+    sums[i] = s;
+}
+
+// One thread per frame.  Records the system; with solve = 1: freezes on too few rows or a non-finite system, factors A = L L^T
+// (j = 0..5: d = A_jj - sum_k<j L_jk^2, in k order; L_jj = sqrt(d), refused unless d > 0; L_ij = (A_ij - sum_k<j L_ik L_jk) / L_jj), solves
+// L y = -b, L^T xi = y, and applies T_cw <- [Rodrigues(w) | v] T_cw (xi = (w, v)).
+__global__ void k_track_solve(int n, const double* __restrict__ sums, TrackState* __restrict__ state, double* __restrict__ sys, int min_corr,
+                              int solve, unsigned long long* rows)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    TrackState& s = state[k];
+    if (s.frozen) return;
+    const double* S = sums + static_cast<int64_t>(k) * kTrackVals;
+    double* out = sys + static_cast<int64_t>(k) * kTrackVals;
+    bool finite = true;
+    for (int i = 0; i < kTrackVals; ++i) { out[i] = S[i]; finite = finite && isfinite(S[i]); }
+    s.correspondences = static_cast<long long>(S[28]);
+    s.residual_sq = S[27];
+    atomicAdd(rows, static_cast<unsigned long long>(s.correspondences));
+    if (!solve) return;
+    if (s.correspondences < min_corr) { s.status = 1; s.frozen = 1; return; }
+    if (!finite) { s.status = 3; s.frozen = 1; return; }
+    double A[6][6], L[6][6], b[6], y[6], x[6];
+    int j = 0;
+    for (int a = 0; a < 6; ++a)
+        for (int c = a; c < 6; ++c, ++j) { A[a][c] = S[j]; A[c][a] = S[j]; }
+    for (int a = 0; a < 6; ++a) b[a] = S[21 + a];
+    for (int c = 0; c < 6; ++c)
+    {
+        double d = A[c][c];
+        for (int m = 0; m < c; ++m) d = DS(d, DM(L[c][m], L[c][m]));
+        if (!(d > 0.0)) { s.status = 2; s.frozen = 1; return; }
+        L[c][c] = __dsqrt_rn(d);
+        for (int i = c + 1; i < 6; ++i)
+        {
+            double t = A[i][c];
+            for (int m = 0; m < c; ++m) t = DS(t, DM(L[i][m], L[c][m]));
+            L[i][c] = __ddiv_rn(t, L[c][c]);
+        }
+    }
+    for (int i = 0; i < 6; ++i)
+    {
+        double t = -b[i];
+        for (int m = 0; m < i; ++m) t = DS(t, DM(L[i][m], y[m]));
+        y[i] = __ddiv_rn(t, L[i][i]);
+    }
+    for (int i = 5; i >= 0; --i)
+    {
+        double t = y[i];
+        for (int m = i + 1; m < 6; ++m) t = DS(t, DM(L[m][i], x[m]));
+        x[i] = __ddiv_rn(t, L[i][i]);
+    }
+    // Rodrigues: R = I + (sin th / th) K + ((1 - cos th) / th^2) K^2, K = [w]x; R = I for th = 0
+    const double th2 = DA(DA(DM(x[0], x[0]), DM(x[1], x[1])), DM(x[2], x[2]));
+    const double th = __dsqrt_rn(th2);
+    double R[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
+    if (th > 0.0)
+    {
+        const double sa = __ddiv_rn(sin(th), th), sb = __ddiv_rn(DS(1.0, cos(th)), th2);
+        const double K[9] = {0.0, -x[2], x[1], x[2], 0.0, -x[0], -x[1], x[0], 0.0};
+        for (int a = 0; a < 3; ++a)
+            for (int c = 0; c < 3; ++c)
+            {
+                const double k2 = DA(DA(DM(K[3 * a], K[c]), DM(K[3 * a + 1], K[3 + c])), DM(K[3 * a + 2], K[6 + c]));
+                R[3 * a + c] = DA(DA(R[3 * a + c], DM(sa, K[3 * a + c])), DM(sb, k2));
+            }
+    }
+    double T[12];
+    for (int a = 0; a < 3; ++a)
+    {
+        for (int c = 0; c < 3; ++c) T[3 * a + c] = DA(DA(DM(R[3 * a], s.T[c]), DM(R[3 * a + 1], s.T[3 + c])), DM(R[3 * a + 2], s.T[6 + c]));
+        T[9 + a] = DA(DA(DA(DM(R[3 * a], s.T[9]), DM(R[3 * a + 1], s.T[10])), DM(R[3 * a + 2], s.T[11])), x[3 + a]);
+    }
+    bool ok = true;
+    for (int i = 0; i < 6; ++i) ok = ok && isfinite(x[i]);
+    for (int i = 0; i < 12; ++i) ok = ok && isfinite(T[i]);
+    if (!ok) { s.status = 3; s.frozen = 1; return; }
+    for (int i = 0; i < 12; ++i) { s.T[i] = T[i]; s.Tf[i] = __double2float_rn(T[i]); }
+    tr_inverse(T, s.w2c);
+    double un = 0.0;
+    for (int i = 0; i < 6; ++i) un = DA(un, DM(x[i], x[i]));
+    s.update_norm = __dsqrt_rn(un);
+    s.iterations += 1;
+}
+
+#undef DM
+#undef DA
+#undef DS
+
+} // namespace i3d

@@ -233,3 +233,35 @@ class I3DRenderStats(C.Structure, _Dictable):
         ("photo_abs", C.c_double),
         ("photo_sq", C.c_double),
     ]
+
+
+TRACK_LEVELS = 4          # entries of I3DTrackParams::iterations
+TRACK_STATUS = {0: "tracked", 1: "too few correspondences", 2: "not positive definite", 3: "non-finite"}
+
+
+class I3DTrackParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("sdf_source", C.c_int32),
+        ("num_levels", C.c_int32),
+        ("iterations", C.c_int32 * TRACK_LEVELS),
+        ("max_distance", C.c_float),
+        ("min_normal_cos", C.c_float),
+        ("min_correspondences", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
+class I3DTrackInfo(C.Structure, _Dictable):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("iterations", C.c_int32),
+        ("correspondences", C.c_int64),
+        ("residual_sq", C.c_double),
+        ("update_norm", C.c_double),
+        ("initial", I3DRenderStats),
+    ]
+
+    def as_dict(self):
+        out = _Dictable.as_dict(self)
+        out["initial"] = self.initial.as_dict()
+        return out

@@ -12,7 +12,7 @@ import os
 import numpy as np
 
 from .ctypes_defs import (RENDER_PLANES, I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo,
-                          I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats)
+                          I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats, I3DTrackInfo, I3DTrackParams, TRACK_LEVELS)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("I3D_LIB", os.path.join(_HERE, "libi3d_b200.so"))   # I3D_LIB: A/B builds of the same library
@@ -34,6 +34,8 @@ EXPORTED_SYMBOLS = [
     "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh", "i3d_extract_mesh_colored", "i3d_mode_colors",
     "i3d_sizeof_render_params", "i3d_sizeof_render_stats", "i3d_default_render_params", "i3d_render_keyframes", "i3d_download_render",
     "i3d_debug_set_render_skip",
+    "i3d_sizeof_track_params", "i3d_sizeof_track_info", "i3d_default_track_params", "i3d_track_sensor_frames", "i3d_debug_get_track_system",
+    "i3d_debug_get_track_planes",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
     "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_pcg_vectors", "i3d_debug_get_normal_equations",
@@ -96,6 +98,17 @@ def load_library():
     L.i3d_render_keyframes.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(I3DRenderParams), C.POINTER(I3DRenderStats)]
     L.i3d_download_render.restype = C.c_int
     L.i3d_download_render.argtypes = [C.c_void_p] + [C.POINTER(C.c_float)] * 5
+    L.i3d_sizeof_track_params.restype = C.c_uint64
+    L.i3d_sizeof_track_info.restype = C.c_uint64
+    if L.i3d_sizeof_track_params() != C.sizeof(I3DTrackParams) or L.i3d_sizeof_track_info() != C.sizeof(I3DTrackInfo):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (track structs)")
+    L.i3d_track_sensor_frames.restype = C.c_int
+    L.i3d_track_sensor_frames.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(I3DTrackParams),
+                                          C.POINTER(C.c_double), C.POINTER(I3DTrackInfo)]
+    L.i3d_debug_get_track_system.restype = C.c_int
+    L.i3d_debug_get_track_system.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    L.i3d_debug_get_track_planes.restype = C.c_int
+    L.i3d_debug_get_track_planes.argtypes = [C.c_void_p, C.c_int32] + [C.POINTER(C.c_float)] * 4 + [C.POINTER(C.c_uint8), C.POINTER(C.c_int32)]
     _LIB = L
     return L
 
@@ -119,6 +132,12 @@ def default_lighting_params() -> I3DLightingParams:
 def default_fusion_params() -> I3DFusionParams:
     p = I3DFusionParams()
     load_library().i3d_default_fusion_params(C.byref(p))
+    return p
+
+
+def default_track_params() -> I3DTrackParams:
+    p = I3DTrackParams()
+    load_library().i3d_default_track_params(C.byref(p))
     return p
 
 
@@ -446,6 +465,62 @@ class Engine:
         w2c = np.ascontiguousarray(pose_world_to_cam, np.float32)
         assert c2w.shape == (n, 12) and w2c.shape == (n, 12)
         self._check(self.L.i3d_fusion_integrate_sensor(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(c2w, C.c_float), _p(w2c, C.c_float)))
+
+    # ---- tracking stored frames against the surface (DESIGN.md §6n) --------------------------------------------------------------
+    def track_sensor_frames(self, ids, pose_w2c, source: str = "fused", **params):
+        """Point-to-plane ICP of the stored frames `ids` (distinct) against the surface of `source` ("fused": sdf0, "refined"), over the
+        depth pyramid, starting from pose_w2c float64 [len(ids), 12] (world -> camera, R row-major | t).  params: fields of
+        I3DTrackParams (num_levels, iterations (up to 4 values, level 0 first), max_distance, min_normal_cos, min_correspondences);
+        the rest keep default_track_params().  Returns (poses float64 [n, 12] world -> camera, infos: one dict per frame).
+        Device time: phase_ms("track")."""
+        p = default_track_params()
+        p.sdf_source = self._mesh_source(source)
+        for k, v in params.items():
+            if k == "iterations":
+                v = list(v) + [0] * (TRACK_LEVELS - len(v))
+                if len(v) != TRACK_LEVELS:
+                    raise ValueError(f"iterations takes at most {TRACK_LEVELS} values")
+                for i, x in enumerate(v):
+                    p.iterations[i] = int(x)
+            elif k in ("num_levels", "min_correspondences"):
+                setattr(p, k, int(v))
+            elif k in ("max_distance", "min_normal_cos"):
+                setattr(p, k, float(v))
+            else:
+                raise ValueError(f"unknown tracking parameter {k!r}")
+        ids, n = self._ids(ids)
+        pose = np.ascontiguousarray(pose_w2c, np.float64)
+        if pose.shape != (n, 12):
+            raise ValueError(f"pose_w2c must be [{n}, 12], got {pose.shape}")
+        out = np.empty((max(n, 1), 12), np.float64)
+        infos = (I3DTrackInfo * max(n, 1))()
+        self._check(self.L.i3d_track_sensor_frames(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(pose, C.c_double), C.byref(p),
+                                                   _p(out, C.c_double), infos))
+        return out[:n], [infos[i].as_dict() for i in range(n)]
+
+    def debug_track_system(self, n):
+        """(sums float64 [n, 29], pose camera -> world float64 [n, 12]) of the last tracking call of n frames."""
+        sums, pose = np.empty((n, 29), np.float64), np.empty((n, 12), np.float64)
+        self._check(self.L.i3d_debug_get_track_system(self.h, _p(sums, C.c_double), _p(pose, C.c_double)))
+        return sums, pose
+
+    def debug_track_planes(self, level, frames):
+        """The last pass's planes of the last tracking call (`frames` = its frame count): dict of depth / normal at pyramid `level`,
+        pred_depth / pred_normal of the prediction and the level-0 correspondence mask."""
+        dc = self._sensor_cams[0]
+        W, H = dc.width, dc.height
+        Wl, Hl = W, H
+        for _ in range(level):
+            Wl, Hl = Wl // 2, Hl // 2
+        out = dict(depth=np.empty((frames, Hl, Wl), np.float32), normal=np.empty((frames, Hl, Wl, 3), np.float32),
+                   pred_depth=np.empty((frames, H, W), np.float32), pred_normal=np.empty((frames, H, W, 3), np.float32),
+                   mask=np.empty((frames, H, W), np.uint8))
+        m = C.c_int32(0)
+        self._check(self.L.i3d_debug_get_track_planes(self.h, C.c_int32(int(level)), _p(out["depth"], C.c_float), _p(out["normal"], C.c_float),
+                                                      _p(out["pred_depth"], C.c_float), _p(out["pred_normal"], C.c_float),
+                                                      _p(out["mask"], C.c_uint8), C.byref(m)))
+        assert m.value == frames, (m.value, frames)
+        return out
 
     def select_rgbd_frames(self, ids):
         """The stored frames `ids` (any order, repeats allowed) become the level-0 keyframes of the frame store, their depth resized to the
