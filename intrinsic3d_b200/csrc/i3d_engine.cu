@@ -21,7 +21,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <map>
 #include <string>
 #include <vector>
 
@@ -32,6 +31,7 @@
 #include "i3d_gridops.cuh"
 #include "i3d_fusion.cuh"
 #include "i3d_frames.cuh"
+#include "i3d_host.h"
 #include "i3d_mesh.h"
 #include "i3d_render.h"
 #include "i3d_track.h"
@@ -76,38 +76,10 @@ struct NcclApi
 NcclApi g_nccl;
 enum { NCCL_UINT8 = 1, NCCL_FLOAT32 = 7, NCCL_FLOAT64 = 8, NCCL_SUM = 0 };
 
-struct CudaError { cudaError_t code; const char* what; int line; };
 struct NcclError { int code; int line; };
-
-#define CK(call)                                                                  \
-    do {                                                                          \
-        cudaError_t _e = (call);                                                  \
-        if (_e != cudaSuccess) throw CudaError{_e, #call, __LINE__};              \
-    } while (0)
-
-template <class T>
-struct Dev
-{
-    T* p = nullptr;
-    size_t cap = 0;
-    ~Dev() { release(); }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    void ensure(size_t count)
-    {
-        if (count <= cap) return;
-        release();
-        CK(cudaMalloc(&p, std::max<size_t>(count, 1) * sizeof(T)));
-        cap = count;
-    }
-    void swap(Dev& o) { std::swap(p, o.p); std::swap(cap, o.cap); }
-};
-
-inline unsigned blocks_for(size_t n, int threads = kThreads) { return static_cast<unsigned>((n + threads - 1) / threads); }
 
 enum Site { SITE_BUILD = 0, SITE_REG, SITE_FINISH, SITE_EG_APPLY, SITE_OP_POST, SITE_UPDATE, SITE_CAND, SITE_EG_COST, SITE_REG_COST, SITE_COUNT };
 constexpr int kSiteVals = 9;
-
-struct Phase { double ms = 0.0; int64_t count = 0; };
 } // namespace
 
 struct I3DEngine
@@ -170,15 +142,9 @@ struct I3DEngine
     Dev<float> dbg_v;            // input vector of i3d_debug_apply_operator
     I3DParams last_params{};
     bool have_iter = false;
-    std::map<std::string, Phase> phases;
-    // event pairs of the phase and kernel timers (Timer) of the current call, resolved by collect_kernel_times()
-    std::vector<cudaEvent_t> ev_pool;
-    struct TimedLaunch { int a, b; const char* name; };
-    std::vector<TimedLaunch> timed;
-    size_t ev_used = 0;
+    Timing timing;               // the phase and kernel timers of every entry point
     int64_t launches = 0;        // kernels launched during the last i3d_gn_iteration (counted by pdl_launch; other entry points do not count)
     int64_t host_syncs = 0;      // cudaStreamSynchronize calls of the last i3d_gn_iteration
-    int timer_level = 0;         // 0: phases + the roofline kernels (sampled); 1: every kernel of the iteration (i3d_debug_set_kernel_timers)
     Dev<IterDev> iter_dev;       // device-resident result / LM state of the current iteration
     int last_cg_iterations = 4, prev_cg_iterations = 4;  // PCG iteration counts of the previous two solves: their maximum sizes the first launch batch
     bool pcg_fused = true;       // k_cg_step where it applies (I3D_PCG_FUSED=0 at engine creation: the four-kernel chain)
@@ -217,34 +183,9 @@ struct I3DEngine
     int sn_cap = 0, sn_F = 0;
     I3DFusionCamera sn_dcam{}, sn_ccam{};
     Dev<float> sn_depth; Dev<uint8_t> sn_bgr; Dev<int32_t> sn_ids;
-    // surface extraction (i3d_mesh.cuh): scratch that only grows, and the resident mesh of the last i3d_extract_mesh
-    bool have_mesh = false;
-    int64_t mesh_V = 0, mesh_F = 0;
-    float* mesh_vpos = nullptr; uint8_t* mesh_vcol = nullptr; int3* mesh_faces = nullptr;
-    Dev<uint8_t> ms_case, ms_keep, ms_cub; Dev<int32_t> ms_cnt, ms_sel; Dev<int64_t> ms_off; Dev<unsigned long long> ms_cubes, ms_best;
-    Dev<float> ms_cpos, ms_vpos, ms_vpos2; Dev<uint8_t> ms_ccol, ms_vcol, ms_vcol2;
-    Dev<uint32_t> ms_klo, ms_klo2; Dev<unsigned long long> ms_khi, ms_khi2;
-    Dev<int32_t> ms_perm, ms_perm2, ms_first, ms_fid, ms_head, ms_seg, ms_cvid, ms_parent, ms_used, ms_newid;
-    Dev<int3> ms_faces, ms_faces2; Dev<unsigned> ms_ccount, ms_cminf;
-    cudaEvent_t ms_ev[16] = {};        // begin / end of up to 8 device-only segments of one extraction (MeshSegments)
-    bool ms_ev_ready = false;
-    Dev<uchar4> vis_rgb;               // per-voxel colours of the last colour pass (i3d_vis.cuh): scratch that only grows
-    // keyframe renderer (i3d_render.cuh): the voxel box and brick bitmap of the current voxel set (built on the first render after a
-    // change), scratch that only grows, and the resident planes of the last render
-    bool rd_skip = true;               // i3d_debug_set_render_skip
-    bool rd_box_ready = false, rd_have_bricks = false;
-    int rd_box[6] = {}, rd_blo[3] = {}, rd_bdim[3] = {};
-    Dev<int> rd_box_d; Dev<uint32_t> rd_bits;
-    Dev<float> rd_rt; Dev<int32_t> rd_ids; Dev<double> rd_partials, rd_sums; Dev<unsigned long long> rd_samples;
-    Dev<float> rd_depth, rd_normal, rd_albedo, rd_shading, rd_intensity;
-    bool have_render = false;
-    int rd_n = 0, rd_planes = 0;
-    // frame-to-model tracker (i3d_track.cuh): per-call state of n frames, and the chunk's prediction, pyramid, normal and mask planes
-    // (scratch that only grows; the planes of the last chunk stay for i3d_debug_get_track_planes)
-    Dev<float> tr_rt; Dev<int32_t> tr_ids; Dev<double> tr_pose_in; Dev<TrackState> tr_state;
-    Dev<double> tr_sys, tr_sums, tr_partials, tr_rd_partials, tr_rd_sums; Dev<unsigned long long> tr_counters;
-    Dev<float> tr_pdepth, tr_pnrm, tr_depth[kTrackMaxLevels], tr_nrm[kTrackMaxLevels]; Dev<uint8_t> tr_mask;
-    int tr_n = 0, tr_levels = 0, tr_last_m = 0, tr_W[kTrackMaxLevels] = {}, tr_H[kTrackMaxLevels] = {};
+    MeshState mesh;                    // surface extraction (i3d_mesh.cu)
+    RenderState render;                // keyframe renderer (i3d_render.cu)
+    TrackScratch track;                // frame-to-model tracker (i3d_render.cu)
     // shard (multi-GPU)
     int64_t shard_begin = 0, shard_end = -1;
     int rank = 0, world = 1;
@@ -317,7 +258,8 @@ int guarded(I3DEngine* e, Fn&& fn)
     }
     catch (const CudaError& ce)
     {
-        return fail(e, "CUDA error %d (%s) at i3d_engine.cu:%d: %s", static_cast<int>(ce.code), cudaGetErrorString(ce.code), ce.line, ce.what);
+        const char* file = std::strrchr(ce.file, '/') ? std::strrchr(ce.file, '/') + 1 : ce.file;     // the file name, without its directory
+        return fail(e, "CUDA error %d (%s) at %s:%d: %s", static_cast<int>(ce.code), cudaGetErrorString(ce.code), file, ce.line, ce.what);
     }
     catch (const NcclError& ne) { return fail(e, "NCCL error %d (%s) at i3d_engine.cu:%d", ne.code, g_nccl.GetErrorString ? g_nccl.GetErrorString(ne.code) : "?", ne.line); }
     catch (const std::exception& ex) { return fail(e, "exception: %s", ex.what()); }
@@ -348,8 +290,8 @@ int rebuild_topology(I3DEngine* e)
 // range, the resident mesh, and the renderer's voxel box, brick bitmap and planes.  Every change of the voxel set calls it.
 void forget_voxel_set(I3DEngine* e)
 {
-    e->have_sh = false; e->sv_S = 0; e->sv_x = nullptr; e->have_iter = false; e->have_mesh = false;
-    e->rd_box_ready = false; e->rd_have_bricks = false; e->have_render = false;
+    e->have_sh = false; e->sv_S = 0; e->sv_x = nullptr; e->have_iter = false; e->mesh.have_mesh = false;
+    e->render.box_ready = false; e->render.have_bricks = false; e->render.have_render = false;
     e->shard_ready = false; e->shard_begin = 0; e->shard_end = -1;
 }
 
@@ -383,7 +325,7 @@ template <class Fill>
 void install_frames(I3DEngine* e, int32_t F, int32_t W, int32_t H, double pyr_scale, Fill&& fill)
 {
     const size_t cnt = static_cast<size_t>(F) * W * H;
-    e->have_render = false;
+    e->render.have_render = false;
     if (F != e->F) { e->have_cam = false; e->have_iter = false; }     // the unknown space of the last iteration no longer matches
     if (F != e->F || W != e->W || H != e->H) e->have_color = false;
     e->F = F; e->W = W; e->H = H; e->pyr_scale = pyr_scale;
@@ -612,44 +554,6 @@ CullView cull_view(const I3DEngine* e, unsigned long long* stats)
     return CullView{e->tile_min.p, e->tile_max.p, no_cull ? 0 : 1, stats};
 }
 
-// Brackets stream work (a phase, or one kernel launch) with two events from the pool; resolved without extra synchronisation by
-// collect_kernel_times().  `level` 0 = always recorded: the phases and the roofline kernels (k_eg_rows, k_eg_apply, k_select_obs);
-// level 1 = only when i3d_debug_set_kernel_timers(e, 1) asked for the per-kernel table.  (An event record between two kernels makes
-// the second one wait for the first one's completion the ordinary way: no programmatic overlap across it.)
-struct Timer
-{
-    I3DEngine* e; int a = -1, b = -1; const char* name;
-    Timer(I3DEngine* eng, const char* nm, int level = 0) : e(eng), name(nm)
-    {
-        if (level <= e->timer_level && e->ev_used + 2 <= e->ev_pool.size()) { a = static_cast<int>(e->ev_used++); b = static_cast<int>(e->ev_used++); cudaEventRecord(e->ev_pool[a], e->stream); }
-    }
-    void stop()
-    {
-        if (a >= 0) { cudaEventRecord(e->ev_pool[b], e->stream); e->timed.push_back({a, b, name}); a = -1; }
-    }
-    ~Timer() { stop(); }
-};
-
-// Starts the timing of one call: the event pool is free again, and the phases the call owns start from zero
-void begin_timing(I3DEngine* e, std::initializer_list<const char*> owned)
-{
-    e->timed.clear(); e->ev_used = 0;
-    for (const char* nm : owned) e->phases.erase(nm);
-}
-
-void collect_kernel_times(I3DEngine* e)
-{
-    cudaStreamSynchronize(e->stream);
-    for (const auto& t : e->timed)
-    {
-        float ms = 0.f;
-        if (cudaEventElapsedTime(&ms, e->ev_pool[t.a], e->ev_pool[t.b]) == cudaSuccess) { Phase& p = e->phases[t.name]; p.ms += ms; p.count += 1; }
-    }
-    e->timed.clear(); e->ev_used = 0;
-    e->phases["launches"].count = e->launches;
-    e->phases["host_syncs"].count = e->host_syncs;
-}
-
 #define NK(call)                                                            \
     do {                                                                    \
         int _r = (call);                                                    \
@@ -777,7 +681,7 @@ int check_frame_limit(I3DEngine* e, int F, int K)
 void launch_eg_apply(I3DEngine* e, const GridView& g, const RegView& rv, const EgRows& rows, const SolveVecs& sv)
 {
     if (rows.n_active == 0) return;
-    Timer kt(e, "k_eg_apply");     // the dominant kernel: every launch is timed (roofline = true average)
+    Timer kt(e->timing, e->stream, "k_eg_apply");     // the dominant kernel: every launch is timed (roofline = true average)
     pdl_launch(e, k_eg_apply, blocks_for(rows.n_active), kThreads, apply_smem_bytes(e->F, rows.K), g, rows, rv, sv, sv.ps, e->ctl.p, e->site(SITE_EG_APPLY));
 }
 
@@ -786,13 +690,13 @@ void launch_operator(I3DEngine* e, const GridView& g, const RegView& rv, const E
 {
     launch_eg_apply(e, g, rv, rows, sv);
     {
-        Timer kt(e, "k_op_partial", 1);
+        Timer kt(e->timing, e->stream, "k_op_partial", 1);
         pdl_launch(e, k_op_partial, blocks_for(static_cast<size_t>((e->held_count() + 3) / 4)), kThreads, 0,
             g, rv, sv, sh, e->held_count(), vin, sv.ps, e->type_w.p, dmin, dmax, e->ctl.p, e->site(SITE_OP_POST), e->site(SITE_EG_APPLY).out, is_cg_iteration);
     }
     if (e->world > 1)
     {
-        Timer kt(e, "exchange", 1);
+        Timer kt(e->timing, e->stream, "exchange", 1);
         exchange(e, sv.qg, nullptr, sv.qg + 2 * e->n, 6 * e->F + 9, e->site(SITE_OP_POST).out, 1, 1, is_cg_iteration ? EPI_OPERATOR_CG : -1);
     }
 }
@@ -861,7 +765,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     if (check_frame_limit(e, e->F, K) != 0) return 1;
     e->K = K;
     e->last_params = P;
-    e->phases.clear(); begin_timing(e, {}); e->launches = 0; e->host_syncs = 0;        // the iteration owns every phase
+    e->timing.phases.clear(); begin_timing(e->timing, {}); e->launches = 0; e->host_syncs = 0;        // the iteration owns every phase
     const int64_t n = e->n;
     const int F = e->F;
     const bool multi = e->world > 1;
@@ -872,11 +776,11 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     const int64_t own = sh.own_end - sh.own_begin;
     const int64_t hc = e->held_count();
     const size_t U = static_cast<size_t>(e->U());
-    Timer t_total(e, "total");
+    Timer t_total(e->timing, e->stream, "total");
     auto sync = [&]() { CK(cudaStreamSynchronize(st)); e->host_syncs += 1; };
 
     // ------------------------------------------------------------------ activity, compaction of the rows this rank owns
-    Timer t_sel(e, "select");
+    Timer t_sel(e->timing, e->stream, "select");
     e->flags.ensure(n);
     GridView g = e->grid_view(e->sdf, e->alb);
     // flags over the range this rank reads (own voxels + 4 stencil rings); compaction of the owned rows over the owned range
@@ -921,7 +825,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
         const size_t smem = 12 * static_cast<size_t>(F) * sizeof(float);
         auto kern = (K <= 5) ? k_select_obs<5> : k_select_obs<I3D_MAX_OBS>;
         if (smem > 48 * 1024) CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-        Timer kt(e, "k_select_obs");
+        Timer kt(e->timing, e->stream, "k_select_obs");
         static const bool want_stats = std::getenv("I3D_CULL_STATS") != nullptr;
         e->cull_stats.ensure(2);
         if (want_stats) CK(cudaMemsetAsync(e->cull_stats.p, 0, 2 * sizeof(unsigned long long), st));
@@ -939,7 +843,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     t_sel.stop();
 
     // ------------------------------------------------------------------ k2 build
-    Timer t_build(e, "build");
+    Timer t_build(e->timing, e->stream, "build");
     e->Jt.ensure(EgRows::kTiles * S + 1); e->Jtail.ensure(S + 1);
     e->row_frame.ensure(S + 1); e->row_res.ensure(S + 1); e->row_wraw.ensure(S + 1);
     e->ea_w.ensure(3 * static_cast<size_t>(n)); e->lap.ensure(n);
@@ -950,13 +854,13 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     if (n_active > 0)
     {
         {
-            Timer kt(e, "k_eg_build");
+            Timer kt(e->timing, e->stream, "k_eg_build");
             launch_eg_rows<ROWS_BUILD>(e, g, cv, rows, e->obs_frame.p, e->obs_w.p);
         }
         const size_t smem = accum_smem_bytes(F, K);
         if (smem > 48 * 1024) CK(cudaFuncSetAttribute(k_eg_accum, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
         {
-            Timer kt(e, "k_eg_accum", 1);
+            Timer kt(e->timing, e->stream, "k_eg_accum", 1);
             pdl_launch(e, k_eg_accum, blocks_for(static_cast<size_t>(n_active)), kThreads, smem, g, rows, F, e->v_bgd.p, e->v_cgd.p, e->cam_accd.p, e->site(SITE_BUILD));
         }
         pdl_launch(e, k_acc_to_float, blocks_for(std::max(U, static_cast<size_t>(lay.size()))), kThreads, 0, static_cast<int64_t>(U), lay.size(),
@@ -992,7 +896,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     }
 
     // ------------------------------------------------------------------ LM loop (TrustRegionMinimizer + LevenbergMarquardtStrategy)
-    Timer t_solve(e, "solve");
+    Timer t_solve(e->timing, e->stream, "solve");
     const float dmin = static_cast<float>(P.min_lm_diagonal), dmax = static_cast<float>(std::min(P.max_lm_diagonal, 3.0e38));
     // voxel unknowns of the held hull: 4 per thread (16 B accesses); the first F + 2 threads take one camera block each
     const unsigned upd_blocks = blocks_for(static_cast<size_t>((sh.held_voxel_unknowns() + 3) / 4 + F + 2));
@@ -1013,14 +917,14 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
             const bool refresh = (enq % P.residual_reset_period == 0);
             if (!dir_ready)
             {
-                Timer kt(e, "k_cg_dir", 1);
+                Timer kt(e->timing, e->stream, "k_cg_dir", 1);
                 pdl_launch(e, k_cg_dir4, blocks_for(static_cast<size_t>((hc + 3) / 4)), kThreads, 0, sv, sh, hc, e->ctl.p);
             }
             dir_ready = false;
             if (fused && !refresh)
             {
                 launch_eg_apply(e, g, rv, rows, sv);
-                Timer kt(e, "k_cg_update", 1);        // k_cg_step is timed in k_cg_update's place
+                Timer kt(e->timing, e->stream, "k_cg_update", 1);        // k_cg_step is timed in k_cg_update's place
                 launch_cg_step<false>(e, g, rv, sv, dmin, dmax);
                 dir_ready = true;
                 continue;
@@ -1039,7 +943,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
             }
             else
             {
-                Timer kt(e, "k_cg_update", 1);
+                Timer kt(e->timing, e->stream, "k_cg_update", 1);
                 launch_update(false, 0);
             }
             if (multi) allreduce_scalars(e, e->site(SITE_UPDATE).out, 3, EPI_UPDATE, 1);
@@ -1048,7 +952,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     // candidate point + candidate cost + the trust-region decision, all stream-ordered behind the PCG.  The model cost change comes
     // from the PCG's own scalars (k_lm_decide): no extra pass over the Jacobian.
     auto enqueue_decision = [&]() {
-        Timer t_cand(e, "candidate");
+        Timer t_cand(e->timing, e->stream, "candidate");
         CK(cudaMemsetAsync(e->red_out.p + SITE_CAND * kSiteVals, 0, 3 * kSiteVals * sizeof(double), st));
         pdl_launch(e, k_candidate, vec_blocks, kThreads, 0, g, sv, sh, hc, 0, e->cam, e->c_sdf, e->c_alb, e->c_cam, e->v_delta.p, e->ctl.p, e->site(SITE_CAND));
         GridView gc = e->grid_view(e->c_sdf, e->c_alb);
@@ -1056,7 +960,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
         CamView cvc{e->c_cam, e->pose_ctx_c.p, F};
         if (n_active > 0)
         {
-            Timer kt(e, "k_eg_cost");
+            Timer kt(e->timing, e->stream, "k_eg_cost");
             launch_eg_rows<ROWS_COST>(e, gc, cvc, rows, nullptr, nullptr);
         }
         pdl_launch(e, k_reg_cost, blocks_for(static_cast<size_t>(own)), kThreads, 0, gc, rv, sh, e->c_sdf, e->c_alb, e->site(SITE_REG_COST));
@@ -1067,7 +971,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
     IterDev h{};
     for (int it = 1; it <= P.lm_steps; ++it)
     {
-        Timer t_pcg(e, "pcg");
+        Timer t_pcg(e->timing, e->stream, "pcg");
         pdl_launch(e, k_lm_begin, 1, 32, 0, e->iter_dev.p, e->ctl.p, e->fail_flag.p, P);
         pdl_launch(e, k_cam_precond, blocks_for(static_cast<size_t>(F) + 2, 64), 64, 0, sv, e->cam_acc.p, e->type_w.p, e->ctl.p, dmin, dmax, e->minv.p, e->fail_flag.p);
         if (fused) launch_cg_step<true>(e, g, rv, sv, dmin, dmax);
@@ -1088,7 +992,7 @@ int gn_iteration_impl(I3DEngine* e, const I3DParams& P, I3DIterInfo& info)
             sync();
             CK(cudaGetLastError());
             if (!h.pcg_unfinished || h.state != LM_RUNNING) break;
-            Timer t_more(e, "pcg");
+            Timer t_more(e->timing, e->stream, "pcg");
             enqueue_pcg(2);
         }
         if (h.info.lm_iterations >= 1)
@@ -1179,35 +1083,7 @@ int setup_shard(I3DEngine* e)
     return 0;
 }
 
-// ---- surface extraction (i3d_mesh.cuh, DESIGN.md §6j) ----------------------------------------------
-// runs one CUB-style device call twice: temp-size query, then the call on e->ms_cub (grown, never shrunk)
-template <class Fn>
-void cub_call(I3DEngine* e, Fn&& fn)
-{
-    size_t bytes = 0;
-    CK(fn(static_cast<void*>(nullptr), bytes));
-    e->ms_cub.ensure(bytes);
-    CK(fn(static_cast<void*>(e->ms_cub.p), bytes));
-}
-
-// Device time per stage of one extraction: event pairs around device-only segments, each credited to a stage.  The host round trips
-// that read counts back fall between segments, so they are not counted.
-struct MeshSegments
-{
-    I3DEngine* e; int used = 0; int stage[8];
-    void begin(int s) { CK(cudaEventRecord(e->ms_ev[2 * used], e->stream)); stage[used] = s; }
-    void end() { CK(cudaEventRecord(e->ms_ev[2 * used + 1], e->stream)); ++used; }
-};
-
-template <class T>
-T read_back(I3DEngine* e, const T* d)
-{
-    T h{};
-    CK(cudaMemcpyAsync(&h, d, sizeof(T), cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
-    return h;
-}
-
+// ---- surface extraction, rendering and tracking (i3d_mesh.cu, i3d_render.cu) ----------------------
 // The sdf a mesh is cut from, or a colour mode reads: 0 = sdf0, 1 = the refined sdf
 int check_sdf_source(I3DEngine* e, const char* who, int32_t sdf_source)
 {
@@ -1226,189 +1102,44 @@ int check_color_mode(I3DEngine* e, const char* who, int32_t mode)
     return 0;
 }
 
-// The colour pass (i3d_vis.cuh) of a mode other than I3D_MESH_COLOR_VOXEL into e->vis_rgb, timed as phase "mesh_colorize".  The
-// geometric modes read the sdf the mesh is cut from.  Writes nothing but e->vis_rgb.
+// The colour pass of a mode other than I3D_MESH_COLOR_VOXEL into e->mesh.vis_rgb; the geometric modes read the sdf the mesh is cut from
 void colorize(I3DEngine* e, int32_t sdf_source, int32_t mode)
 {
-    begin_timing(e, {"mesh_colorize"});
-    e->vis_rgb.ensure(static_cast<size_t>(e->n));
-    {
-        Timer t(e, "mesh_colorize");
-        mesh::colorize(e->grid_view(sdf_source == 0 ? e->sdf0.p : e->sdf, e->alb), e->sv_grid, e->sv_x, e->sv_S, mode, e->vis_rgb.p, e->stream);
-    }
-    collect_kernel_times(e);
-    CK(cudaGetLastError());
+    mesh::colorize(e->mesh, e->timing, e->grid_view(sdf_source == 0 ? e->sdf0.p : e->sdf, e->alb), e->sv_grid, e->sv_x, e->sv_S, mode, e->stream);
 }
 
-// Marching cubes over the resident grid, welding, degenerate-face removal and (optionally) the largest component.  Every count is
-// read back before the buffers of the next stage are sized.  Reads the grid; writes only the ms_* scratch and the resident mesh (and,
-// for a colour mode other than the voxel colours, e->vis_rgb, which then colours the mesh).
+// The extraction of the surface of prm.sdf_source, coloured by the voxel colours or by a colour mode (validated by the caller)
 int extract_mesh(I3DEngine* e, const I3DMeshParams& prm, int32_t color_mode, I3DMeshInfo* info)
 {
-    cudaStream_t st = e->stream;
-    const int64_t n = e->n;
-    e->have_mesh = false;
-    if (!e->ms_ev_ready) { for (auto& ev : e->ms_ev) CK(cudaEventCreate(&ev)); e->ms_ev_ready = true; }
     if (color_mode != I3D_MESH_COLOR_VOXEL) colorize(e, prm.sdf_source, color_mode);
-    I3DMeshInfo inf{};
     MeshGrid g;
-    g.n = n; g.x = e->x.p; g.y = e->y.p; g.z = e->z.p; g.sdf = prm.sdf_source == 0 ? e->sdf0.p : e->sdf; g.weight = e->weight.p;
-    g.rgb = color_mode == I3D_MESH_COLOR_VOXEL ? e->rgb.p : e->vis_rgb.p;
+    g.n = e->n; g.x = e->x.p; g.y = e->y.p; g.z = e->z.p; g.sdf = prm.sdf_source == 0 ? e->sdf0.p : e->sdf; g.weight = e->weight.p;
+    g.rgb = color_mode == I3D_MESH_COLOR_VOXEL ? e->rgb.p : e->mesh.vis_rgb.p;
     g.nbr = e->nbr.p; g.keys = e->up_keys.p; g.vals = e->up_vals.p; g.mask = e->hash_cap - 1; g.voxel_size = e->voxel_size;
-
-    enum { CLASSIFY, EMIT, WELD, CLEAN, COMPONENTS };
-    MeshSegments seg{e};
-
-    // 1. cube cases and per-voxel triangle counts -> face offsets
-    e->ms_case.ensure(n); e->ms_cnt.ensure(n); e->ms_off.ensure(n); e->ms_cubes.ensure(1); e->ms_sel.ensure(1); e->ms_best.ensure(1);
-    seg.begin(CLASSIFY);
-    CK(cudaMemsetAsync(e->ms_cubes.p, 0, sizeof(unsigned long long), st));
-    mesh::classify(g, e->ms_case.p, e->ms_cnt.p, e->ms_cubes.p, st);
-    cub_call(e, [&](void* t, size_t& b) { return mesh::face_offsets(t, b, e->ms_cnt.p, e->ms_off.p, static_cast<int>(n), st); });
-    seg.end();
-    inf.num_cubes = static_cast<int64_t>(read_back(e, e->ms_cubes.p));
-    const int64_t F0 = read_back(e, e->ms_off.p + (n - 1)) + read_back(e, e->ms_cnt.p + (n - 1));
-    inf.num_faces_raw = F0;
-    // corner and vertex ids are int32 (as the PLY's indices); element offsets into the interleaved arrays are computed in int64
-    if (3 * F0 > INT_MAX) return fail(e, "i3d_extract_mesh: %lld triangles exceed the int32 corner indices of the mesh", static_cast<long long>(F0));
-    const int32_t M = static_cast<int32_t>(3 * F0);
-    float* vpos = nullptr; uint8_t* vcol = nullptr; int3* faces = nullptr;
-    int64_t V = 0, F = 0;
-    if (M > 0)
-    {
-        // 2. the triangle soup, corner by corner
-        e->ms_cpos.ensure(3 * static_cast<size_t>(M)); e->ms_ccol.ensure(3 * static_cast<size_t>(M));
-        e->ms_klo.ensure(M); e->ms_klo2.ensure(M); e->ms_khi.ensure(M); e->ms_khi2.ensure(M); e->ms_perm.ensure(M); e->ms_perm2.ensure(M);
-        seg.begin(EMIT);
-        mesh::emit(g, e->ms_case.p, e->ms_cnt.p, e->ms_off.p, MeshCorners{e->ms_cpos.p, e->ms_ccol.p, e->ms_klo.p, e->ms_khi.p}, st);
-        seg.end();
-
-        // 3. welding: stable sort of the corner indices by position (z bits, then x|y bits), segment heads, ids by first appearance
-        e->ms_first.ensure(M); e->ms_fid.ensure(M); e->ms_head.ensure(M); e->ms_seg.ensure(M); e->ms_cvid.ensure(M);
-        seg.begin(WELD);
-        mesh::iota(M, e->ms_perm2.p, st);
-        cub_call(e, [&](void* t, size_t& b) { return mesh::sort_z(t, b, e->ms_klo.p, e->ms_klo2.p, e->ms_perm2.p, e->ms_perm.p, M, st); });
-        mesh::gather_key_hi(M, e->ms_perm.p, e->ms_khi.p, e->ms_khi2.p, st);
-        cub_call(e, [&](void* t, size_t& b) { return mesh::sort_xy(t, b, e->ms_khi2.p, e->ms_khi.p, e->ms_perm.p, e->ms_perm2.p, M, st); });
-        mesh::weld_heads(M, e->ms_perm2.p, e->ms_khi.p, e->ms_klo.p, e->ms_first.p, e->ms_head.p, st);
-        cub_call(e, [&](void* t, size_t& b) { return mesh::exclusive_sum(t, b, e->ms_first.p, e->ms_fid.p, M, st); });
-        cub_call(e, [&](void* t, size_t& b) { return mesh::inclusive_max(t, b, e->ms_head.p, e->ms_seg.p, M, st); });
-        seg.end();
-        const int64_t Vw = read_back(e, e->ms_fid.p + (M - 1)) + read_back(e, e->ms_first.p + (M - 1));
-        e->ms_vpos.ensure(3 * static_cast<size_t>(Vw)); e->ms_vcol.ensure(3 * static_cast<size_t>(Vw));
-        seg.begin(WELD);
-        mesh::weld_assign(M, e->ms_perm2.p, e->ms_seg.p, e->ms_fid.p, e->ms_cpos.p, e->ms_ccol.p, e->ms_cvid.p, e->ms_vpos.p, e->ms_vcol.p, st);
-        seg.end();
-        inf.num_vertices_welded = Vw;
-
-        // 4. degenerate faces, survivors kept in order; the vertices stay
-        const int32_t F0i = static_cast<int32_t>(F0);
-        const int3* faces0 = reinterpret_cast<const int3*>(e->ms_cvid.p);
-        e->ms_keep.ensure(F0); e->ms_faces.ensure(F0);
-        seg.begin(CLEAN);
-        mesh::face_clean(F0i, faces0, e->ms_vpos.p, e->ms_keep.p, st);
-        cub_call(e, [&](void* t, size_t& b) { return mesh::select_faces(t, b, faces0, e->ms_keep.p, e->ms_faces.p, e->ms_sel.p, F0i, st); });
-        seg.end();
-        const int32_t F1 = read_back(e, e->ms_sel.p);
-        inf.num_faces_clean = F1;
-        vpos = e->ms_vpos.p; vcol = e->ms_vcol.p; faces = e->ms_faces.p; V = Vw; F = F1;
-
-        // 5. the largest face-connected component, then only the vertices it uses
-        if (prm.largest_component_only)
-        {
-            const int32_t Vi = static_cast<int32_t>(Vw);
-            e->ms_parent.ensure(Vw); e->ms_ccount.ensure(Vw); e->ms_cminf.ensure(Vw); e->ms_used.ensure(Vw); e->ms_newid.ensure(Vw);
-            e->ms_faces2.ensure(std::max<int32_t>(F1, 1));
-            int32_t F2 = 0, V2 = 0;
-            if (F1 > 0)
-            {
-                seg.begin(COMPONENTS);
-                mesh::iota(Vi, e->ms_parent.p, st);
-                mesh::cc_union(F1, e->ms_faces.p, e->ms_parent.p, st);
-                mesh::cc_flatten(Vi, e->ms_parent.p, st);
-                CK(cudaMemsetAsync(e->ms_ccount.p, 0, Vw * sizeof(unsigned), st));
-                CK(cudaMemsetAsync(e->ms_cminf.p, 0xFF, Vw * sizeof(unsigned), st));
-                CK(cudaMemsetAsync(e->ms_best.p, 0, sizeof(unsigned long long), st));
-                mesh::cc_count(F1, e->ms_faces.p, e->ms_parent.p, e->ms_ccount.p, e->ms_cminf.p, st);
-                mesh::cc_best(Vi, e->ms_ccount.p, e->ms_cminf.p, e->ms_best.p, st);
-                mesh::cc_keep(F1, e->ms_faces.p, e->ms_parent.p, e->ms_best.p, e->ms_keep.p, st);
-                cub_call(e, [&](void* t, size_t& b) { return mesh::select_faces(t, b, e->ms_faces.p, e->ms_keep.p, e->ms_faces2.p, e->ms_sel.p, F1, st); });
-                seg.end();
-                F2 = read_back(e, e->ms_sel.p);
-                seg.begin(COMPONENTS);
-                CK(cudaMemsetAsync(e->ms_used.p, 0, Vw * sizeof(int32_t), st));
-                if (F2 > 0) mesh::mark_used(F2, e->ms_faces2.p, e->ms_used.p, st);
-                cub_call(e, [&](void* t, size_t& b) { return mesh::exclusive_sum(t, b, e->ms_used.p, e->ms_newid.p, Vi, st); });
-                seg.end();
-                V2 = read_back(e, e->ms_newid.p + (Vi - 1)) + read_back(e, e->ms_used.p + (Vi - 1));
-                e->ms_vpos2.ensure(3 * static_cast<size_t>(V2)); e->ms_vcol2.ensure(3 * static_cast<size_t>(V2));
-                seg.begin(COMPONENTS);
-                mesh::compact_vertices(Vi, e->ms_used.p, e->ms_newid.p, e->ms_vpos.p, e->ms_vcol.p, e->ms_vpos2.p, e->ms_vcol2.p, st);
-                if (F2 > 0) mesh::remap_faces(F2, e->ms_newid.p, e->ms_faces2.p, st);
-                seg.end();
-            }
-            vpos = e->ms_vpos2.p; vcol = e->ms_vcol2.p; faces = e->ms_faces2.p; V = V2; F = F2;
-        }
-    }
-    CK(cudaStreamSynchronize(st));
-    CK(cudaGetLastError());
-    double ms[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
-    for (int k = 0; k < seg.used; ++k)
-    {
-        float t = 0.f;
-        CK(cudaEventElapsedTime(&t, e->ms_ev[2 * k], e->ms_ev[2 * k + 1]));
-        ms[seg.stage[k]] += t;
-    }
-    inf.ms_classify = ms[CLASSIFY]; inf.ms_emit = ms[EMIT]; inf.ms_weld = ms[WELD]; inf.ms_clean = ms[CLEAN]; inf.ms_components = ms[COMPONENTS];
-    inf.num_faces = F; inf.num_vertices = V;
-    e->mesh_vpos = vpos; e->mesh_vcol = vcol; e->mesh_faces = faces; e->mesh_V = V; e->mesh_F = F;
-    e->have_mesh = true;
-    if (info) *info = inf;
+    std::string err;
+    if (mesh::extract(e->mesh, g, prm.largest_component_only != 0, info, err, e->stream)) return fail(e, "%s", err.c_str());
     return 0;
 }
 
-// Bits of the renderer's brick bitmap above which i3d_render_keyframes marches every lattice sample instead (128 MiB)
-constexpr int64_t kRenderBrickCap = 1ll << 30;
-
-// The voxel box and (when it fits under kRenderBrickCap) the brick bitmap of the current voxel set, timed as "render_bricks"; built
-// once per voxel set, dropped by forget_voxel_set.
-void render_bricks(I3DEngine* e)
+// The grid as the renderer marches it, without its voxel box (the render module adds it): the sdf of sdf_source, and the per-voxel SH
+// only for photometric outputs
+RenderGrid render_grid(const I3DEngine* e, int32_t sdf_source, bool photometric)
 {
-    if (e->rd_box_ready) return;
-    cudaStream_t st = e->stream;
-    Timer t(e, "render_bricks");
-    const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
-    e->rd_box_d.ensure(6);
-    CK(cudaMemcpyAsync(e->rd_box_d.p, init, sizeof(init), cudaMemcpyHostToDevice, st));
-    render::bounds(e->n, e->x.p, e->y.p, e->z.p, e->rd_box_d.p, st);
-    CK(cudaMemcpyAsync(e->rd_box, e->rd_box_d.p, sizeof(e->rd_box), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    int64_t bits = 1;
-    for (int d = 0; d < 3; ++d)
-    {
-        e->rd_blo[d] = e->rd_box[d];
-        e->rd_bdim[d] = ((e->rd_box[3 + d] - e->rd_box[d]) >> 3) + 1;
-        bits *= e->rd_bdim[d];
-    }
-    e->rd_have_bricks = bits <= kRenderBrickCap;
-    if (e->rd_have_bricks)
-    {
-        const size_t words = static_cast<size_t>((bits + 31) >> 5);
-        e->rd_bits.ensure(words);
-        CK(cudaMemsetAsync(e->rd_bits.p, 0, words * sizeof(uint32_t), st));
-        render::bricks(e->n, e->x.p, e->y.p, e->z.p, e->rd_blo, e->rd_bdim, e->rd_bits.p, st);
-    }
-    t.stop();
-    e->rd_box_ready = true;
+    RenderGrid rg{};
+    rg.g = e->grid_view(sdf_source == 0 ? e->sdf0.p : e->sdf, e->alb);
+    if (!photometric) rg.g.sh = nullptr;
+    rg.keys = e->up_keys.p; rg.vals = e->up_vals.p; rg.mask = e->hash_cap - 1;
+    rg.sh_has = photometric ? e->sh_has.p : nullptr;
+    return rg;
 }
 
-// Renders frames ids[0..n) (validated by the caller): the frame-scan camera of every frame, the voxel box / bitmap when the voxel set
-// changed, the march and the fixed-order finish of the statistics.  Refuses, before it writes anything, intrinsics (after pyr_scale) that
-// are not finite with fx, fy > 0 and distortion that is not finite.  Writes only the rd_* state and the resident planes.
+// Renders frames ids[0..n) (validated by the caller) with the camera of the frame scans: k_pose_mats' float poses and select_cam's
+// intrinsics.  Refuses, before it writes anything, intrinsics (after pyr_scale) that are not finite with fx, fy > 0 and distortion that
+// is not finite.
 int render_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DRenderParams& P, I3DRenderStats* stats)
 {
     cudaStream_t st = e->stream;
-    const int F = e->F, W = e->W, H = e->H;
+    const int F = e->F;
     double hc9[9];
     CK(cudaMemcpyAsync(hc9, e->cam + 6 * static_cast<size_t>(F), 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -1418,210 +1149,23 @@ int render_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DRende
                     sc.fx, sc.fy, sc.cx, sc.cy, e->pyr_scale);
     for (int k = 0; k < 5; ++k)
         if (!std::isfinite(sc.d[k])) return fail(e, "i3d_render_keyframes: distortion coefficient %d is not finite", k);
-    begin_timing(e, {"render", "render_bricks", "render_samples"});
-    e->have_render = false;
-    const size_t img = static_cast<size_t>(n) * W * H;
-    const int planes = P.planes;
-    if (planes & I3D_RENDER_DEPTH) e->rd_depth.ensure(img);
-    if (planes & I3D_RENDER_NORMAL) e->rd_normal.ensure(3 * img);
-    if (planes & I3D_RENDER_ALBEDO) e->rd_albedo.ensure(img);
-    if (planes & I3D_RENDER_SHADING) e->rd_shading.ensure(img);
-    if (planes & I3D_RENDER_INTENSITY) e->rd_intensity.ensure(img);
-    const int tiles_x = (W + kRenderTile - 1) / kRenderTile, tiles_y = (H + kRenderTile - 1) / kRenderTile;
-    e->rd_partials.ensure(static_cast<size_t>(n) * tiles_x * tiles_y * kRenderStats);
-    e->rd_sums.ensure(static_cast<size_t>(n) * kRenderStats);
-    e->rd_ids.ensure(n); e->rd_rt.ensure(12 * static_cast<size_t>(F)); e->rd_samples.ensure(1);
-    CK(cudaMemcpyAsync(e->rd_ids.p, ids, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(e->rd_samples.p, 0, sizeof(unsigned long long), st));
-    k_pose_mats<<<blocks_for(F, 64), 64, 0, st>>>(F, e->cam, e->rd_rt.p);
     RenderCam cam;
     cam.fx = sc.fx; cam.fy = sc.fy; cam.cx = sc.cx; cam.cy = sc.cy; cam.dist_zero = sc.dist_zero;
     for (int k = 0; k < 5; ++k) cam.d[k] = sc.d[k];
-    {
-        Timer t(e, "render");
-        render_bricks(e);
-        RenderGrid rg;
-        rg.g = e->grid_view(P.sdf_source == 0 ? e->sdf0.p : e->sdf, e->alb);
-        rg.keys = e->up_keys.p; rg.vals = e->up_vals.p; rg.mask = e->hash_cap - 1;
-        rg.sh_has = P.photometric ? e->sh_has.p : nullptr;
-        if (!P.photometric) rg.g.sh = nullptr;
-        for (int d = 0; d < 3; ++d)
-        {
-            rg.lo[d] = static_cast<float>(e->rd_box[d]) * e->voxel_size;
-            rg.hi[d] = static_cast<float>(e->rd_box[3 + d]) * e->voxel_size;
-            rg.blo[d] = e->rd_blo[d]; rg.bdim[d] = e->rd_bdim[d];
-        }
-        rg.bricks = (e->rd_skip && e->rd_have_bricks) ? e->rd_bits.p : nullptr;
-        RenderViews rv;
-        rv.n = n; rv.W = W; rv.H = H; rv.tiles_x = tiles_x; rv.tiles_y = tiles_y;
-        rv.ids = e->rd_ids.p; rv.Rt = e->rd_rt.p; rv.depth = e->depth.p; rv.lum = e->lum.p;
-        rv.out_depth = (planes & I3D_RENDER_DEPTH) ? e->rd_depth.p : nullptr;
-        rv.out_normal = (planes & I3D_RENDER_NORMAL) ? e->rd_normal.p : nullptr;
-        rv.out_albedo = (planes & I3D_RENDER_ALBEDO) ? e->rd_albedo.p : nullptr;
-        rv.out_shading = (planes & I3D_RENDER_SHADING) ? e->rd_shading.p : nullptr;
-        rv.out_intensity = (planes & I3D_RENDER_INTENSITY) ? e->rd_intensity.p : nullptr;
-        rv.partials = e->rd_partials.p; rv.samples = e->rd_samples.p; rv.photometric = P.photometric ? 1 : 0;
-        render::march(rg, cam, rv, st);
-        render::finish(n, tiles_x * tiles_y, e->rd_partials.p, e->rd_sums.p, st);
-    }
-    std::vector<double> sums(static_cast<size_t>(n) * kRenderStats);
-    unsigned long long samples = 0;
-    CK(cudaMemcpyAsync(sums.data(), e->rd_sums.p, sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&samples, e->rd_samples.p, sizeof(samples), cudaMemcpyDeviceToHost, st));
-    collect_kernel_times(e);
-    CK(cudaGetLastError());
-    e->phases["render_samples"].count = static_cast<int64_t>(samples);
-    if (stats)
-        for (int i = 0; i < n; ++i)
-        {
-            const double* s = sums.data() + static_cast<size_t>(i) * kRenderStats;
-            I3DRenderStats r;
-            r.num_hit = static_cast<int64_t>(s[0]); r.num_observed = static_cast<int64_t>(s[1]);
-            r.depth_count = static_cast<int64_t>(s[2]); r.photo_count = static_cast<int64_t>(s[3]);
-            r.depth_abs = s[4]; r.depth_sq = s[5]; r.photo_abs = s[6]; r.photo_sq = s[7];
-            stats[i] = r;
-        }
-    e->have_render = true; e->rd_n = n; e->rd_planes = planes;
-    return 0;
-}
-
-// Tracks the stored frames ids[0..n) (validated by the caller; Wl / Hl: the pyramid sizes) in passes of I3D_TRACK_CHUNK frames.  Per pass:
-// the prediction (render::march at the input poses with the depth camera, geometry only), the depth pyramid (k_frames_depthdown chain on
-// the gathered store depth) with its normals, then every Gauss-Newton iteration of every level, coarsest first, with no host
-// synchronisation; one read-back at the end.  Writes only the tr_* state, pose_out and info.
-int track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl,
-                        const int* Hl, double* pose_out, I3DTrackInfo* info)
-{
-    cudaStream_t st = e->stream;
-    const I3DFusionCamera& dc = e->sn_dcam;
-    const int L = P.num_levels, W = dc.width, H = dc.height, C = std::min<int>(n, I3D_TRACK_CHUNK);
-    const size_t img = static_cast<size_t>(W) * H;
-    const int tiles_x = (W + kRenderTile - 1) / kRenderTile, tiles_y = (H + kRenderTile - 1) / kRenderTile;
-    static_assert(kRenderTile == kTrackTile, "the prediction and the rows share the level-0 tile grid");
-    begin_timing(e, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences"});
-    e->tr_n = 0;
-    e->tr_ids.ensure(n); e->tr_pose_in.ensure(12 * static_cast<size_t>(n)); e->tr_state.ensure(n);
-    e->tr_sys.ensure(static_cast<size_t>(n) * kTrackVals); e->tr_rd_sums.ensure(static_cast<size_t>(n) * kRenderStats);
-    e->tr_rt.ensure(12 * static_cast<size_t>(e->sn_F)); e->tr_counters.ensure(2);
-    e->tr_rd_partials.ensure(static_cast<size_t>(C) * tiles_x * tiles_y * kRenderStats);
-    e->tr_partials.ensure(static_cast<size_t>(C) * tiles_x * tiles_y * kTrackVals); e->tr_sums.ensure(static_cast<size_t>(C) * kTrackVals);
-    e->tr_pdepth.ensure(C * img); e->tr_pnrm.ensure(3 * C * img); e->tr_mask.ensure(C * img);
-    for (int l = 0; l < L; ++l)
-    {
-        const size_t c = static_cast<size_t>(C) * Wl[l] * Hl[l];
-        e->tr_depth[l].ensure(c); e->tr_nrm[l].ensure(3 * c);
-    }
-    // the input poses in float, scattered by sensor id: the march reads Rt + 12 * id
-    std::vector<float> hrt(12 * static_cast<size_t>(e->sn_F), 0.0f);
-    for (int k = 0; k < n; ++k)
-        for (int i = 0; i < 12; ++i) hrt[12 * static_cast<size_t>(ids[k]) + i] = static_cast<float>(pose_in[12 * static_cast<size_t>(k) + i]);
-    CK(cudaMemcpyAsync(e->tr_ids.p, ids, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->tr_pose_in.p, pose_in, 12 * static_cast<size_t>(n) * sizeof(double), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->tr_rt.p, hrt.data(), hrt.size() * sizeof(float), cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(e->tr_counters.p, 0, 2 * sizeof(unsigned long long), st));
-    int total_iters = 0;
-    for (int l = 0; l < L; ++l) total_iters += P.iterations[l];
-    TrackCam cam[kTrackMaxLevels];
-    for (int l = 0; l < L; ++l)
-    {
-        const double s = std::ldexp(1.0, -l);       // the pyramid scale, as select_cam applies pyr_scale
-        cam[l] = TrackCam{Wl[l], Hl[l], static_cast<float>(dc.fx * s), static_cast<float>(dc.fy * s), static_cast<float>(dc.cx * s),
-                          static_cast<float>(dc.cy * s)};
-    }
-    Timer whole(e, "track");
-    render_bricks(e);
-    RenderGrid rg;
-    rg.g = e->grid_view(P.sdf_source == 0 ? e->sdf0.p : e->sdf, e->alb);
-    rg.g.sh = nullptr;
-    rg.keys = e->up_keys.p; rg.vals = e->up_vals.p; rg.mask = e->hash_cap - 1; rg.sh_has = nullptr;
-    for (int d = 0; d < 3; ++d)
-    {
-        rg.lo[d] = static_cast<float>(e->rd_box[d]) * e->voxel_size;
-        rg.hi[d] = static_cast<float>(e->rd_box[3 + d]) * e->voxel_size;
-        rg.blo[d] = e->rd_blo[d]; rg.bdim[d] = e->rd_bdim[d];
-    }
-    rg.bricks = (e->rd_skip && e->rd_have_bricks) ? e->rd_bits.p : nullptr;
-    RenderCam rcam{};
-    rcam.fx = dc.fx; rcam.fy = dc.fy; rcam.cx = dc.cx; rcam.cy = dc.cy; rcam.dist_zero = 1;
-    track::init(n, e->tr_pose_in.p, e->tr_state.p, st);
-    const float max_dist_sq = P.max_distance * P.max_distance;
-    int m = 0;
-    for (int c0 = 0; c0 < n; c0 += C)
-    {
-        m = std::min(C, n - c0);
-        const int32_t* ids_d = e->tr_ids.p + c0;
-        {
-            Timer t(e, "track_predict");
-            RenderViews rv{};
-            rv.n = m; rv.W = W; rv.H = H; rv.tiles_x = tiles_x; rv.tiles_y = tiles_y;
-            rv.ids = ids_d; rv.Rt = e->tr_rt.p; rv.depth = e->sn_depth.p; rv.lum = nullptr;
-            rv.out_depth = e->tr_pdepth.p; rv.out_normal = e->tr_pnrm.p;
-            rv.partials = e->tr_rd_partials.p; rv.samples = e->tr_counters.p + 1; rv.photometric = 0;
-            render::march(rg, rcam, rv, st);
-            render::finish(m, tiles_x * tiles_y, e->tr_rd_partials.p, e->tr_rd_sums.p + static_cast<size_t>(c0) * kRenderStats, st);
-        }
-        {
-            Timer t(e, "track_pyramid");
-            track::gather(m, W, H, ids_d, e->sn_depth.p, e->tr_depth[0].p, st);
-            for (int l = 1; l < L; ++l)
-            {
-                const dim3 grid((Wl[l] + 31) / 32, (Hl[l] + 7) / 8, m);
-                k_frames_depthdown<<<grid, dim3(32, 8), 0, st>>>(m, Wl[l - 1], Hl[l - 1], e->tr_depth[l - 1].p, e->tr_depth[l].p);
-            }
-            for (int l = 0; l < L; ++l) track::normals(m, cam[l], e->tr_depth[l].p, e->tr_nrm[l].p, st);
-        }
-        {
-            Timer t(e, "track_icp");
-            CK(cudaMemsetAsync(e->tr_mask.p, 0, m * img, st));
-            TrackRows tr{};
-            tr.pcam = cam[0]; tr.pdepth = e->tr_pdepth.p; tr.pnrm = e->tr_pnrm.p; tr.ids = ids_d; tr.rt_in = e->tr_rt.p;
-            tr.state = e->tr_state.p + c0; tr.max_dist_sq = max_dist_sq; tr.min_cos = P.min_normal_cos;
-            tr.use_cos = P.min_normal_cos > -1.0f ? 1 : 0; tr.partials = e->tr_partials.p;
-            auto system = [&](int l, int solve) {
-                tr.cam = cam[l]; tr.depth = e->tr_depth[l].p; tr.nrm = e->tr_nrm[l].p; tr.mask = l == 0 ? e->tr_mask.p : nullptr;
-                tr.tiles_x = (Wl[l] + kTrackTile - 1) / kTrackTile; tr.tiles_y = (Hl[l] + kTrackTile - 1) / kTrackTile;
-                {
-                    Timer tk(e, "k_track_rows", 1);
-                    track::rows(m, tr, st);
-                }
-                track::finish(m, tr.tiles_x * tr.tiles_y, e->tr_partials.p, e->tr_sums.p, st);
-                track::solve(m, e->tr_sums.p, e->tr_state.p + c0, e->tr_sys.p + static_cast<size_t>(c0) * kTrackVals, P.min_correspondences, solve,
-                             e->tr_counters.p, st);
-            };
-            for (int l = L - 1; l >= 0; --l)
-                for (int it = 0; it < P.iterations[l]; ++it) system(l, 1);
-            if (total_iters == 0) system(0, 0);        // no update: the level-0 system at the input pose
-        }
-    }
-    std::vector<TrackState> hs(n);
-    std::vector<double> rs(static_cast<size_t>(n) * kRenderStats);
-    unsigned long long counters[2] = {0, 0};
-    CK(cudaMemcpyAsync(hs.data(), e->tr_state.p, n * sizeof(TrackState), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(rs.data(), e->tr_rd_sums.p, rs.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(counters, e->tr_counters.p, sizeof(counters), cudaMemcpyDeviceToHost, st));
-    whole.stop();
-    collect_kernel_times(e);
-    CK(cudaGetLastError());
-    e->phases["track_correspondences"].count = static_cast<int64_t>(counters[0]);
-    for (int k = 0; k < n; ++k)
-    {
-        std::memcpy(pose_out + 12 * static_cast<size_t>(k), hs[k].w2c, 12 * sizeof(double));
-        if (!info) continue;
-        I3DTrackInfo r{};
-        r.status = hs[k].status; r.iterations = hs[k].iterations; r.correspondences = hs[k].correspondences;
-        r.residual_sq = hs[k].residual_sq; r.update_norm = hs[k].update_norm;
-        const double* s = rs.data() + static_cast<size_t>(k) * kRenderStats;
-        r.initial.num_hit = static_cast<int64_t>(s[0]); r.initial.num_observed = static_cast<int64_t>(s[1]);
-        r.initial.depth_count = static_cast<int64_t>(s[2]); r.initial.photo_count = static_cast<int64_t>(s[3]);
-        r.initial.depth_abs = s[4]; r.initial.depth_sq = s[5]; r.initial.photo_abs = s[6]; r.initial.photo_sq = s[7];
-        info[k] = r;
-    }
-    e->tr_n = n; e->tr_levels = L; e->tr_last_m = m;
-    for (int l = 0; l < L; ++l) { e->tr_W[l] = Wl[l]; e->tr_H[l] = Hl[l]; }
+    e->render.rt.ensure(12 * static_cast<size_t>(F));
+    k_pose_mats<<<blocks_for(F, 64), 64, 0, st>>>(F, e->cam, e->render.rt.p);
+    render::keyframes(e->render, e->timing, render_grid(e, P.sdf_source, P.photometric != 0), cam, e->render.rt.p, n, ids, e->W, e->H, e->depth.p,
+                      e->lum.p, P.planes, P.photometric != 0, stats, st);
     return 0;
 }
 
 } // namespace
+
+void i3d::frames_depthdown(int n, int W, int H, const float* src, float* dst, cudaStream_t st)
+{
+    const dim3 grid((W / 2 + 31) / 32, (H / 2 + 7) / 8, std::min(n, 65535));
+    k_frames_depthdown<<<grid, dim3(32, 8), 0, st>>>(n, W, H, src, dst);
+}
 
 // =================================================================================================
 // C-ABI
@@ -1661,8 +1205,8 @@ int i3d_engine_create(int device, I3DEngine** out)
     { const char* v = std::getenv("I3D_PCG_FUSED"); e->pcg_fused = !(v && v[0] == '0'); }
     const int rc = guarded(e, [&]() {
         CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-        e->ev_pool.resize(4096);
-        for (auto& ev : e->ev_pool) CK(cudaEventCreate(&ev));
+        e->timing.pool.resize(4096);
+        for (auto& ev : e->timing.pool) CK(cudaEventCreate(&ev));
         return 0;
     });
     if (rc != 0) { g_create_error = e->error; delete e; return rc; }
@@ -1678,8 +1222,8 @@ void i3d_engine_destroy(I3DEngine* e)
     for (size_t r = 0; r < e->peer_base.size(); ++r)
         if (static_cast<int>(r) != e->rank && e->peer_base[r]) cudaIpcCloseMemHandle(e->peer_base[r]);
     if (e->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
-    for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
-    if (e->ms_ev_ready) for (auto& ev : e->ms_ev) cudaEventDestroy(ev);
+    for (auto& ev : e->timing.pool) cudaEventDestroy(ev);
+    if (e->mesh.ev_ready) for (auto& ev : e->mesh.ev) cudaEventDestroy(ev);
     cudaStreamDestroy(e->stream);
     delete e;
 }
@@ -1776,11 +1320,13 @@ int i3d_gn_iteration(I3DEngine* e, const I3DParams* params, I3DIterInfo* info)
     if (!e || !params || !info) return 1;
     return guarded(e, [&]() {
         const int rc = gn_iteration_impl(e, *params, *info);
-        collect_kernel_times(e);
+        collect_kernel_times(e->timing, e->stream);
+        e->timing.phases["launches"].count = e->launches;
+        e->timing.phases["host_syncs"].count = e->host_syncs;
         // the reference's three phase timers (NLSSolver::ProblemInfo::time_add/time_build, SolverInfo::time_solve)
-        info->time_add = (e->phases["select"].ms + e->phases["build"].ms) * 1e-3;
+        info->time_add = (e->timing.phases["select"].ms + e->timing.phases["build"].ms) * 1e-3;
         info->time_build = 0.0;
-        info->time_solve = e->phases["solve"].ms * 1e-3;
+        info->time_solve = e->timing.phases["solve"].ms * 1e-3;
         return rc;
     });
 }
@@ -1831,14 +1377,14 @@ int i3d_estimate_lighting(I3DEngine* e, const I3DLightingParams* params, I3DLigh
     return guarded(e, [&]() {
         cudaStream_t st = e->stream;
         const int64_t n = e->n;
-        begin_timing(e, {"light_subvolumes", "light_accumulate", "light_solve", "light_interpolate"});
+        begin_timing(e->timing, {"light_subvolumes", "light_accumulate", "light_solve", "light_interpolate"});
         const GridView g = e->grid_view(e->sdf, e->alb);
         SubvolGrid sg;
         sg.inv_size = 1.0f / P.subvolume_size;
         // ---- Subvolumes::compute ----
         e->sv_scalars.ensure(8);
         {
-            Timer t(e, "light_subvolumes");
+            Timer t(e->timing, e->stream, "light_subvolumes");
             const int init[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
             CK(cudaMemcpyAsync(e->sv_scalars.p, init, sizeof(init), cudaMemcpyHostToDevice, st));
             k_svsh_bounds<<<blocks_for(n), kThreads, 0, st>>>(n, e->x.p, e->y.p, e->z.p, e->voxel_size, sg.inv_size, e->sv_scalars.p);
@@ -1875,7 +1421,7 @@ int i3d_estimate_lighting(I3DEngine* e, const I3DLightingParams* params, I3DLigh
         // ---- data rows -> per-subvolume normal equations ----
         e->sv_acc.ensure(static_cast<size_t>(S) * kLightAcc);
         {
-            Timer t(e, "light_accumulate");
+            Timer t(e->timing, e->stream, "light_accumulate");
             CK(cudaMemsetAsync(e->sv_acc.p, 0, static_cast<size_t>(S) * kLightAcc * sizeof(double), st));
             k_svsh_accumulate<<<blocks_for(n), kThreads, 0, st>>>(g, sg, P.thres_shell, P.weighted != 0, e->sv_acc.p);
         }
@@ -1893,7 +1439,7 @@ int i3d_estimate_lighting(I3DEngine* e, const I3DLightingParams* params, I3DLigh
             e->sv_x = W.x;
         }
         {
-            Timer t(e, "light_solve");
+            Timer t(e->timing, e->stream, "light_solve");
             CK(cudaMemsetAsync(e->sv_info.p, 0, sizeof(I3DLightingInfo), st));
             k_svsh_solve<<<1, kLightSolveThreads, 0, st>>>(W, P);
         }
@@ -1904,16 +1450,16 @@ int i3d_estimate_lighting(I3DEngine* e, const I3DLightingParams* params, I3DLigh
         {
             // ---- computeVoxelShCoeffs ----
             e->sh.ensure(9 * static_cast<size_t>(n)); e->sh_has.ensure(static_cast<size_t>(n));
-            Timer t(e, "light_interpolate");
+            Timer t(e->timing, e->stream, "light_interpolate");
             k_svsh_interpolate<<<blocks_for(n), kThreads, 0, st>>>(g, sg, P.thres_shell, e->sv_x, e->sh.p, e->sh_has.p);
             t.stop();
             e->have_sh = true;
         }
-        collect_kernel_times(e);
+        collect_kernel_times(e->timing, e->stream);
         CK(cudaGetLastError());
-        info->time_accumulate = (e->phases["light_subvolumes"].ms + e->phases["light_accumulate"].ms) * 1e-3;
-        info->time_solve = e->phases["light_solve"].ms * 1e-3;
-        info->time_interpolate = e->phases["light_interpolate"].ms * 1e-3;
+        info->time_accumulate = (e->timing.phases["light_subvolumes"].ms + e->timing.phases["light_accumulate"].ms) * 1e-3;
+        info->time_solve = e->timing.phases["light_solve"].ms * 1e-3;
+        info->time_interpolate = e->timing.phases["light_interpolate"].ms * 1e-3;
         return 0;
     });
 }
@@ -1975,7 +1521,7 @@ int i3d_recompute_colors(I3DEngine* e, const float* pose_world_to_cam, float max
     return guarded(e, [&]() {
         cudaStream_t st = e->stream;
         const int F = e->F, K = max_num_observations;
-        begin_timing(e, {"recolor"});
+        begin_timing(e->timing, {"recolor"});
         double hc9[9];
         CK(cudaMemcpyAsync(hc9, e->cam + 6 * static_cast<size_t>(F), 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
@@ -1983,7 +1529,7 @@ int i3d_recompute_colors(I3DEngine* e, const float* pose_world_to_cam, float max
         e->recolor_counts.ensure(2);
         CK(cudaMemsetAsync(e->recolor_counts.p, 0, 2 * sizeof(unsigned long long), st));
         {
-            Timer t(e, "recolor");
+            Timer t(e->timing, e->stream, "recolor");
             if (pose_world_to_cam) CK(cudaMemcpyAsync(e->Rt.p, pose_world_to_cam, 12 * static_cast<size_t>(F) * sizeof(float), cudaMemcpyHostToDevice, st));
             else k_pose_mats<<<blocks_for(F, 64), 64, 0, st>>>(F, e->cam, e->Rt.p);
             const size_t smem = 12 * static_cast<size_t>(F) * sizeof(float);
@@ -1995,7 +1541,7 @@ int i3d_recompute_colors(I3DEngine* e, const float* pose_world_to_cam, float max
         }
         unsigned long long hcnt[2] = {0, 0};
         CK(cudaMemcpyAsync(hcnt, e->recolor_counts.p, sizeof(hcnt), cudaMemcpyDeviceToHost, st));
-        collect_kernel_times(e);
+        collect_kernel_times(e->timing, e->stream);
         CK(cudaGetLastError());
         if (num_recolored) *num_recolored = static_cast<int64_t>(hcnt[0]);
         if (num_observations) *num_observations = static_cast<int64_t>(hcnt[1]);
@@ -2025,10 +1571,10 @@ int i3d_clear_voxels_outside_thin_shell(I3DEngine* e, double thres_shell, int64_
     return guarded(e, [&]() {
         cudaStream_t st = e->stream;
         const int64_t n = e->n;
-        begin_timing(e, {"prune"});
+        begin_timing(e->timing, {"prune"});
         int m = 0;
         {
-            Timer t(e, "prune");
+            Timer t(e->timing, e->stream, "prune");
             const GridView g = e->grid_view(e->sdf, e->alb);
             e->flags.ensure(static_cast<size_t>(n));
             CK(cudaMemsetAsync(e->flags.p, 0, static_cast<size_t>(n), st));
@@ -2048,14 +1594,14 @@ int i3d_clear_voxels_outside_thin_shell(I3DEngine* e, double thres_shell, int64_
                 // then fails and Intrinsic3D::refine skips the level): same state, not an error
                 e->n = 0;
                 forget_voxel_set(e);
-                collect_kernel_times(e);
+                collect_kernel_times(e->timing, e->stream);
                 if (num_voxels_out) *num_voxels_out = 0;
                 return 0;
             }
             if (install_grid(e, m, [&](const VoxelArrays& out) { k_gather_voxels<<<blocks_for(static_cast<size_t>(m)), kThreads, 0, st>>>(m, e->act.p, g, out); }))
                 return fail(e, "i3d_clear_voxels_outside_thin_shell: internal error (duplicate voxels)");
         }
-        collect_kernel_times(e);
+        collect_kernel_times(e->timing, e->stream);
         if (num_voxels_out) *num_voxels_out = m;
         return 0;
     });
@@ -2068,16 +1614,16 @@ int i3d_upsample_grid(I3DEngine* e, int64_t* num_voxels_out)
     return guarded(e, [&]() {
         cudaStream_t st = e->stream;
         const int64_t n = e->n, m = 8 * n;
-        begin_timing(e, {"upsample"});
+        begin_timing(e->timing, {"upsample"});
         {
-            Timer t(e, "upsample");
+            Timer t(e->timing, e->stream, "upsample");
             const GridView g = e->grid_view(e->sdf, e->alb);
             if (install_grid(e, m, [&](const VoxelArrays& out) { k_upsample<<<blocks_for(static_cast<size_t>(m)), kThreads, 0, st>>>(g, e->up_keys.p, e->up_vals.p, e->hash_cap - 1, out); }))
                 return fail(e, "i3d_upsample_grid: internal error (duplicate voxels)");
             // SparseVoxelGrid::create(voxelSize * 0.5f): truncation = 5 * voxel size (src/sparse_voxel_grid.cpp:48)
             e->voxel_size = e->voxel_size * 0.5f; e->truncation = e->voxel_size * 5.0f;
         }
-        collect_kernel_times(e);
+        collect_kernel_times(e->timing, e->stream);
         if (num_voxels_out) *num_voxels_out = m;
         return 0;
     });
@@ -2138,7 +1684,7 @@ int i3d_fusion_begin(I3DEngine* e, const I3DFusionParams* params)
         fuse_reset_table(e, cap);
         e->fu_n = 0;
         // the fusion phases add up over the calls until i3d_fusion_finish
-        begin_timing(e, {"fusion_prep", "fusion_alloc", "fusion_integrate", "fusion_correct", "fusion_finish", "fusion_growths", "fusion_sweeps"});
+        begin_timing(e->timing, {"fusion_prep", "fusion_alloc", "fusion_integrate", "fusion_correct", "fusion_finish", "fusion_growths", "fusion_sweeps"});
         e->fu_active = true;
         return 0;
     });
@@ -2160,7 +1706,7 @@ static int fuse_frames(I3DEngine* e, const char* who, int32_t n, const I3DFusion
     const FuseCam dc{depth_cam.width, depth_cam.height, depth_cam.fx, depth_cam.fy, depth_cam.cx, depth_cam.cy};
     const FuseCam cc{color_cam.width, color_cam.height, color_cam.fx, color_cam.fy, color_cam.cx, color_cam.cy};
     const FuseConst c = fuse_const(P);
-    begin_timing(e, {});                 // the fusion phases were reset by i3d_fusion_begin
+    begin_timing(e->timing, {});                 // the fusion phases were reset by i3d_fusion_begin
     for (int f = 0; f < n; ++f)
     {
         const size_t src = static_cast<size_t>(ids ? ids[f] : f);
@@ -2169,7 +1715,7 @@ static int fuse_frames(I3DEngine* e, const char* who, int32_t n, const I3DFusion
         std::memcpy(fr.R_wc, pose_world_to_cam + 12 * f, 9 * sizeof(float)); std::memcpy(fr.t_wc, pose_world_to_cam + 12 * f + 9, 3 * sizeof(float));
         fuse_frustum_bounds(depth_cam, P.depth_min, P.depth_max, P.voxel_size, fr.R_cw, fr.t_cw, fr.bounds);
         {
-            Timer t(e, "fusion_prep");
+            Timer t(e->timing, e->stream, "fusion_prep");
             k_fuse_erode<<<blocks_for(dimg), kThreads, 0, st>>>(dc.W, dc.H, P.discont_window_size, depth + dimg * src, e->fu_depth.p);
             if (want_normals) k_fuse_normals<<<blocks_for(dimg), kThreads, 0, st>>>(dc, e->fu_depth.p, e->fu_nrm.p);
         }
@@ -2177,12 +1723,12 @@ static int fuse_frames(I3DEngine* e, const char* who, int32_t n, const I3DFusion
         for (int attempt = 0;; ++attempt)
         {
             {
-                Timer t(e, "fusion_alloc");
+                Timer t(e->timing, e->stream, "fusion_alloc");
                 CK(cudaMemsetAsync(e->fu_ctl.p + 1, 0, sizeof(int), st));
                 k_fuse_alloc<<<blocks_for(dimg), kThreads, 0, st>>>(dc, fr, c, e->fu_depth.p, fuse_table(e), fuse_volume(e), attempt == 0 ? 1 : 0);
                 CK(cudaMemcpyAsync(ctl, e->fu_ctl.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
             }
-            collect_kernel_times(e);         // synchronises: ctl is on the host
+            collect_kernel_times(e->timing, e->stream);         // synchronises: ctl is on the host
             CK(cudaGetLastError());
             e->fu_n = ctl[0];
             if (ctl[1] & 2)
@@ -2194,17 +1740,17 @@ static int fuse_frames(I3DEngine* e, const char* who, int32_t n, const I3DFusion
             while (static_cast<uint64_t>(e->fu_n) * 4 > cap) cap <<= 1;
             if (cap > (1ull << 31)) return fail(e, "%s: more than 2^30 allocated voxels; the fusion is ended", who);
             fuse_grow_table(e, cap);
-            e->phases["fusion_growths"].count += 1;
+            e->timing.phases["fusion_growths"].count += 1;
         }
         {
-            Timer t(e, "fusion_integrate");
+            Timer t(e->timing, e->stream, "fusion_integrate");
             if (e->fu_n > 0)
                 k_fuse_integrate<<<blocks_for(static_cast<size_t>(e->fu_n)), kThreads, 0, st>>>(e->fu_n, dc, cc, fr, c, e->fu_depth.p,
                                                                                                 want_normals ? e->fu_nrm.p : nullptr,
                                                                                                 bgr + cimg * src, fuse_volume(e));
         }
     }
-    collect_kernel_times(e);
+    collect_kernel_times(e->timing, e->stream);
     CK(cudaGetLastError());
     return 0;
 }
@@ -2283,20 +1829,20 @@ int i3d_sensor_keyframe_scores(I3DEngine* e, double* scores)
         const int tx = (W + kBlurTileW - 1) / kBlurTileW, ty = (H + kBlurTileH - 1) / kBlurTileH;
         const int chunk = std::min<int>(F, I3D_KEYFRAME_CHUNK);
         e->kf_partials.ensure(static_cast<size_t>(chunk) * tx * ty * 4); e->kf_scores.ensure(F);
-        begin_timing(e, {"keyframe_scores", "keyframe_chunks"});
+        begin_timing(e->timing, {"keyframe_scores", "keyframe_chunks"});
         {
             // the chunks share the partials buffer in stream order: no host synchronisation between them
-            Timer t(e, "keyframe_scores");
+            Timer t(e->timing, e->stream, "keyframe_scores");
             for (int f0 = 0; f0 < F; f0 += chunk)
             {
                 const int n = std::min(chunk, F - f0);
                 k_blur_partials<<<dim3(tx, ty, n), dim3(32, 8), 0, st>>>(n, W, H, e->sn_bgr.p + img * f0, e->kf_partials.p);
                 k_blur_finish<<<(n + 3) / 4, 128, 0, st>>>(n, tx * ty, e->kf_partials.p, e->kf_scores.p + f0);
-                e->phases["keyframe_chunks"].count += 1;
+                e->timing.phases["keyframe_chunks"].count += 1;
             }
         }
         CK(cudaMemcpyAsync(scores, e->kf_scores.p, F * sizeof(double), cudaMemcpyDeviceToHost, st));
-        collect_kernel_times(e);
+        collect_kernel_times(e->timing, e->stream);
         CK(cudaGetLastError());
         return 0;
     });
@@ -2337,9 +1883,9 @@ int i3d_select_rgbd_frames(I3DEngine* e, int32_t n, const int32_t* ids)
         const int W = cc.width, H = cc.height;
         const size_t cnt = static_cast<size_t>(n) * W * H, dimg = static_cast<size_t>(dc.width) * dc.height, cimg = static_cast<size_t>(W) * H * 3;
         e->st_lum.ensure(cnt); e->st_depth.ensure(cnt); e->st_bgr.ensure(3 * cnt);
-        begin_timing(e, {"sensor_select", "resize_depth"});
+        begin_timing(e->timing, {"sensor_select", "resize_depth"});
         {
-            Timer t(e, "sensor_select");
+            Timer t(e->timing, e->stream, "sensor_select");
             for (int32_t k = 0; k < n; ++k)
                 CK(cudaMemcpyAsync(e->st_bgr.p + cimg * k, e->sn_bgr.p + cimg * ids[k], cimg, cudaMemcpyDeviceToDevice, st));
             if (dc.width == W && dc.height == H)
@@ -2353,13 +1899,13 @@ int i3d_select_rgbd_frames(I3DEngine* e, int32_t n, const int32_t* ids)
                 e->sn_ids.ensure(n);
                 CK(cudaMemcpyAsync(e->sn_ids.p, ids, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
                 const ResizeCams rc{dc.width, dc.height, dc.fx, dc.fy, dc.cx, dc.cy, W, H, cc.fx, cc.fy, cc.cx, cc.cy};
-                Timer tr(e, "resize_depth");
+                Timer tr(e->timing, e->stream, "resize_depth");
                 k_resize_depth<<<dim3((W + 31) / 32, (H + 7) / 8, std::min(n, 65535)), dim3(32, 8), 0, st>>>(n, e->sn_ids.p, rc, e->sn_depth.p,
                                                                                                            e->st_depth.p);
             }
             k_frames_lum0<<<blocks_for(cnt), kThreads, 0, st>>>(cnt, e->st_bgr.p, e->st_lum.p);
         }
-        collect_kernel_times(e);
+        collect_kernel_times(e->timing, e->stream);
         CK(cudaGetLastError());
         e->st_F = n; e->st_W = W; e->st_H = H;
         return 0;
@@ -2374,10 +1920,10 @@ int i3d_fusion_finish(I3DEngine* e, int64_t* num_voxels_out)
     return guarded(e, [&]() {
         cudaStream_t st = e->stream;
         const int64_t n = e->fu_n;
-        begin_timing(e, {});                 // the fusion phases were reset by i3d_fusion_begin
+        begin_timing(e->timing, {});                 // the fusion phases were reset by i3d_fusion_begin
         if (n > 0)
         {
-            Timer t(e, "fusion_correct");
+            Timer t(e->timing, e->stream, "fusion_correct");
             e->fu_sdf2.ensure(e->fu_sdf.cap); e->fu_w2.ensure(e->fu_w.cap);
             for (int it = 0; it < e->fu_p.correct_sdf_iterations; ++it)
             {
@@ -2389,13 +1935,13 @@ int i3d_fusion_finish(I3DEngine* e, int64_t* num_voxels_out)
                 e->fu_sdf.swap(e->fu_sdf2); e->fu_w.swap(e->fu_w2);
                 CK(cudaMemcpyAsync(&changed, e->fu_ctl.p + 2, sizeof(int), cudaMemcpyDeviceToHost, st));
                 CK(cudaStreamSynchronize(st));
-                e->phases["fusion_sweeps"].count += 1;
+                e->timing.phases["fusion_sweeps"].count += 1;
                 if (!changed) break;
             }
         }
         int m = 0;
         {
-            Timer t(e, "fusion_finish");
+            Timer t(e->timing, e->stream, "fusion_finish");
             if (n > 0) m = fuse_sort(e, true);
             if (m > 0)
             {
@@ -2410,7 +1956,7 @@ int i3d_fusion_finish(I3DEngine* e, int64_t* num_voxels_out)
                 forget_voxel_set(e);
             }
         }
-        collect_kernel_times(e);
+        collect_kernel_times(e->timing, e->stream);
         e->fu_n = 0;
         if (num_voxels_out) *num_voxels_out = m;
         return 0;
@@ -2448,7 +1994,7 @@ int i3d_mode_colors(I3DEngine* e, int32_t sdf_source, int32_t color_mode, uint8_
     if (check_color_mode(e, "i3d_mode_colors", color_mode)) return 1;
     return guarded(e, [&]() {
         const uchar4* src = e->rgb.p;
-        if (color_mode != I3D_MESH_COLOR_VOXEL) { colorize(e, sdf_source, color_mode); src = e->vis_rgb.p; }
+        if (color_mode != I3D_MESH_COLOR_VOXEL) { colorize(e, sdf_source, color_mode); src = e->mesh.vis_rgb.p; }
         e->up_rgb.ensure(3 * static_cast<size_t>(e->n));
         k_interleave_rgb<<<blocks_for(e->n), kThreads, 0, e->stream>>>(e->n, src, e->up_rgb.p);
         CK(cudaMemcpyAsync(rgb, e->up_rgb.p, 3 * static_cast<size_t>(e->n), cudaMemcpyDeviceToHost, e->stream));
@@ -2461,13 +2007,13 @@ int i3d_mode_colors(I3DEngine* e, int32_t sdf_source, int32_t color_mode, uint8_
 int i3d_download_mesh(I3DEngine* e, float* xyz, uint8_t* rgb, int32_t* faces)
 {
     if (!e) return 1;
-    if (!e->have_mesh) return fail(e, "i3d_download_mesh: no mesh (call i3d_extract_mesh after the last change of the voxel set)");
+    if (!e->mesh.have_mesh) return fail(e, "i3d_download_mesh: no mesh (call i3d_extract_mesh after the last change of the voxel set)");
     return guarded(e, [&]() {
         cudaStream_t st = e->stream;
-        const size_t V = static_cast<size_t>(e->mesh_V), F = static_cast<size_t>(e->mesh_F);
-        if (xyz && V) CK(cudaMemcpyAsync(xyz, e->mesh_vpos, 3 * V * sizeof(float), cudaMemcpyDeviceToHost, st));
-        if (rgb && V) CK(cudaMemcpyAsync(rgb, e->mesh_vcol, 3 * V, cudaMemcpyDeviceToHost, st));
-        if (faces && F) CK(cudaMemcpyAsync(faces, e->mesh_faces, F * sizeof(int3), cudaMemcpyDeviceToHost, st));
+        const size_t V = static_cast<size_t>(e->mesh.mesh_V), F = static_cast<size_t>(e->mesh.mesh_F);
+        if (xyz && V) CK(cudaMemcpyAsync(xyz, e->mesh.mesh_vpos, 3 * V * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (rgb && V) CK(cudaMemcpyAsync(rgb, e->mesh.mesh_vcol, 3 * V, cudaMemcpyDeviceToHost, st));
+        if (faces && F) CK(cudaMemcpyAsync(faces, e->mesh.mesh_faces, F * sizeof(int3), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         return 0;
     });
@@ -2509,19 +2055,19 @@ int i3d_render_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DR
 int i3d_download_render(I3DEngine* e, float* depth, float* normal, float* albedo, float* shading, float* intensity)
 {
     if (!e) return 1;
-    if (!e->have_render) return fail(e, "i3d_download_render: no render (call i3d_render_keyframes after the last change of the grid or frames)");
+    if (!e->render.have_render) return fail(e, "i3d_download_render: no render (call i3d_render_keyframes after the last change of the grid or frames)");
     const struct { float* dst; int bit; const char* name; } want[5] = {{depth, I3D_RENDER_DEPTH, "depth"}, {normal, I3D_RENDER_NORMAL, "normal"},
         {albedo, I3D_RENDER_ALBEDO, "albedo"}, {shading, I3D_RENDER_SHADING, "shading"}, {intensity, I3D_RENDER_INTENSITY, "intensity"}};
     for (const auto& w : want)
-        if (w.dst && !(e->rd_planes & w.bit)) return fail(e, "i3d_download_render: the %s plane was not rendered", w.name);
+        if (w.dst && !(e->render.planes & w.bit)) return fail(e, "i3d_download_render: the %s plane was not rendered", w.name);
     return guarded(e, [&]() {
         cudaStream_t st = e->stream;
-        const size_t img = static_cast<size_t>(e->rd_n) * e->W * e->H * sizeof(float);
-        if (depth) CK(cudaMemcpyAsync(depth, e->rd_depth.p, img, cudaMemcpyDeviceToHost, st));
-        if (normal) CK(cudaMemcpyAsync(normal, e->rd_normal.p, 3 * img, cudaMemcpyDeviceToHost, st));
-        if (albedo) CK(cudaMemcpyAsync(albedo, e->rd_albedo.p, img, cudaMemcpyDeviceToHost, st));
-        if (shading) CK(cudaMemcpyAsync(shading, e->rd_shading.p, img, cudaMemcpyDeviceToHost, st));
-        if (intensity) CK(cudaMemcpyAsync(intensity, e->rd_intensity.p, img, cudaMemcpyDeviceToHost, st));
+        const size_t img = static_cast<size_t>(e->render.n) * e->W * e->H * sizeof(float);
+        if (depth) CK(cudaMemcpyAsync(depth, e->render.depth.p, img, cudaMemcpyDeviceToHost, st));
+        if (normal) CK(cudaMemcpyAsync(normal, e->render.normal.p, 3 * img, cudaMemcpyDeviceToHost, st));
+        if (albedo) CK(cudaMemcpyAsync(albedo, e->render.albedo.p, img, cudaMemcpyDeviceToHost, st));
+        if (shading) CK(cudaMemcpyAsync(shading, e->render.shading.p, img, cudaMemcpyDeviceToHost, st));
+        if (intensity) CK(cudaMemcpyAsync(intensity, e->render.intensity.p, img, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         return 0;
     });
@@ -2530,7 +2076,7 @@ int i3d_download_render(I3DEngine* e, float* depth, float* normal, float* albedo
 int i3d_debug_set_render_skip(I3DEngine* e, int on)
 {
     if (!e) return 1;
-    e->rd_skip = on != 0;
+    e->render.skip = on != 0;
     return 0;
 }
 
@@ -2583,18 +2129,22 @@ int i3d_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const d
     if (!(std::isfinite(P.max_distance) && P.max_distance > 0.0f)) return fail(e, "%s: max_distance must be finite and > 0, got %g", who, P.max_distance);
     if (!(P.min_normal_cos >= -1.0f && P.min_normal_cos <= 1.0f)) return fail(e, "%s: min_normal_cos must be in [-1, 1], got %g", who, P.min_normal_cos);
     if (P.min_correspondences < 6) return fail(e, "%s: min_correspondences must be >= 6, got %d", who, P.min_correspondences);
-    return guarded(e, [&]() { return track_sensor_frames(e, n, ids, pose_in, P, Wl, Hl, pose_out, info); });
+    return guarded(e, [&]() {
+        track::sensor_frames(e->track, e->render, e->timing, render_grid(e, P.sdf_source, false), e->sn_dcam, e->sn_depth.p, e->sn_F, n, ids, pose_in, P,
+                             Wl, Hl, pose_out, info, e->stream);
+        return 0;
+    });
 }
 
 int i3d_debug_get_track_system(I3DEngine* e, double* sums, double* pose_cam_to_world)
 {
     if (!e) return 1;
-    if (e->tr_n <= 0) return fail(e, "i3d_debug_get_track_system: no tracking call");
+    if (e->track.n <= 0) return fail(e, "i3d_debug_get_track_system: no tracking call");
     return guarded(e, [&]() {
-        const int n = e->tr_n;
-        if (sums) CK(cudaMemcpyAsync(sums, e->tr_sys.p, static_cast<size_t>(n) * kTrackVals * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+        const int n = e->track.n;
+        if (sums) CK(cudaMemcpyAsync(sums, e->track.sys.p, static_cast<size_t>(n) * kTrackVals * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
         std::vector<TrackState> hs(pose_cam_to_world ? n : 0);
-        if (pose_cam_to_world) CK(cudaMemcpyAsync(hs.data(), e->tr_state.p, n * sizeof(TrackState), cudaMemcpyDeviceToHost, e->stream));
+        if (pose_cam_to_world) CK(cudaMemcpyAsync(hs.data(), e->track.state.p, n * sizeof(TrackState), cudaMemcpyDeviceToHost, e->stream));
         CK(cudaStreamSynchronize(e->stream));
         for (size_t k = 0; k < hs.size(); ++k) std::memcpy(pose_cam_to_world + 12 * k, hs[k].T, 12 * sizeof(double));
         return 0;
@@ -2605,17 +2155,17 @@ int i3d_debug_get_track_planes(I3DEngine* e, int32_t level, float* depth, float*
                                int32_t* frames)
 {
     if (!e) return 1;
-    if (e->tr_n <= 0) return fail(e, "i3d_debug_get_track_planes: no tracking call");
-    if (level < 0 || level >= e->tr_levels) return fail(e, "i3d_debug_get_track_planes: level %d was not built (%d levels)", level, e->tr_levels);
+    if (e->track.n <= 0) return fail(e, "i3d_debug_get_track_planes: no tracking call");
+    if (level < 0 || level >= e->track.levels) return fail(e, "i3d_debug_get_track_planes: level %d was not built (%d levels)", level, e->track.levels);
     return guarded(e, [&]() {
         cudaStream_t st = e->stream;
-        const size_t m = static_cast<size_t>(e->tr_last_m);
-        const size_t lv = m * e->tr_W[level] * e->tr_H[level], img = m * e->tr_W[0] * e->tr_H[0];
-        if (depth) CK(cudaMemcpyAsync(depth, e->tr_depth[level].p, lv * sizeof(float), cudaMemcpyDeviceToHost, st));
-        if (normal) CK(cudaMemcpyAsync(normal, e->tr_nrm[level].p, 3 * lv * sizeof(float), cudaMemcpyDeviceToHost, st));
-        if (pred_depth) CK(cudaMemcpyAsync(pred_depth, e->tr_pdepth.p, img * sizeof(float), cudaMemcpyDeviceToHost, st));
-        if (pred_normal) CK(cudaMemcpyAsync(pred_normal, e->tr_pnrm.p, 3 * img * sizeof(float), cudaMemcpyDeviceToHost, st));
-        if (mask) CK(cudaMemcpyAsync(mask, e->tr_mask.p, img, cudaMemcpyDeviceToHost, st));
+        const size_t m = static_cast<size_t>(e->track.last_m);
+        const size_t lv = m * e->track.W[level] * e->track.H[level], img = m * e->track.W[0] * e->track.H[0];
+        if (depth) CK(cudaMemcpyAsync(depth, e->track.depth[level].p, lv * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (normal) CK(cudaMemcpyAsync(normal, e->track.nrm[level].p, 3 * lv * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (pred_depth) CK(cudaMemcpyAsync(pred_depth, e->track.pdepth.p, img * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (pred_normal) CK(cudaMemcpyAsync(pred_normal, e->track.pnrm.p, 3 * img * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (mask) CK(cudaMemcpyAsync(mask, e->track.mask.p, img, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         if (frames) *frames = static_cast<int32_t>(m);
         return 0;
@@ -2634,20 +2184,20 @@ int i3d_keyframe_scores(I3DEngine* e, int32_t F, int32_t W, int32_t H, const uin
         const int tx = (W + kBlurTileW - 1) / kBlurTileW, ty = (H + kBlurTileH - 1) / kBlurTileH;
         const int chunk = std::min<int>(F, I3D_KEYFRAME_CHUNK);
         e->kf_bgr.ensure(img * chunk); e->kf_partials.ensure(static_cast<size_t>(chunk) * tx * ty * 4); e->kf_scores.ensure(chunk);
-        begin_timing(e, {"keyframe_scores", "keyframe_chunks"});
+        begin_timing(e->timing, {"keyframe_scores", "keyframe_chunks"});
         for (int f0 = 0; f0 < F; f0 += chunk)
         {
             const int n = std::min(chunk, F - f0);
             CK(cudaMemcpyAsync(e->kf_bgr.p, bgr + img * f0, img * n, cudaMemcpyHostToDevice, st));
             {
-                Timer t(e, "keyframe_scores");
+                Timer t(e->timing, e->stream, "keyframe_scores");
                 k_blur_partials<<<dim3(tx, ty, n), dim3(32, 8), 0, st>>>(n, W, H, e->kf_bgr.p, e->kf_partials.p);
                 k_blur_finish<<<(n + 3) / 4, 128, 0, st>>>(n, tx * ty, e->kf_partials.p, e->kf_scores.p);
             }
             CK(cudaMemcpyAsync(scores + f0, e->kf_scores.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
-            collect_kernel_times(e);          // synchronises: the chunk buffer is free again
+            collect_kernel_times(e->timing, e->stream);          // synchronises: the chunk buffer is free again
             CK(cudaGetLastError());
-            e->phases["keyframe_chunks"].count += 1;
+            e->timing.phases["keyframe_chunks"].count += 1;
         }
         return 0;
     });
@@ -2690,9 +2240,9 @@ int i3d_use_rgbd_level(I3DEngine* e, int32_t lvl, int32_t* W_out, int32_t* H_out
         cudaStream_t st = e->stream;
         const int F = e->st_F;
         const size_t cnt = static_cast<size_t>(F) * W * H;
-        begin_timing(e, {"frames_level"});
+        begin_timing(e->timing, {"frames_level"});
         install_frames(e, F, W, H, std::ldexp(1.0, -lvl), [&]() {
-            Timer t(e, "frames_level");
+            Timer t(e->timing, e->stream, "frames_level");
             if (lvl == 0)
             {
                 CK(cudaMemcpyAsync(e->lum.p, e->st_lum.p, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -2724,7 +2274,7 @@ int i3d_use_rgbd_level(I3DEngine* e, int32_t lvl, int32_t* W_out, int32_t* H_out
             CK(cudaMemcpyAsync(e->color.p, e->st_bgr.p, 3 * cnt, cudaMemcpyDeviceToDevice, st));
             e->have_color = true;
         }
-        collect_kernel_times(e);
+        collect_kernel_times(e->timing, e->stream);
         CK(cudaGetLastError());
         if (W_out) *W_out = W;
         if (H_out) *H_out = H;
@@ -2833,20 +2383,20 @@ int i3d_set_shard(I3DEngine* e, int64_t voxel_begin, int64_t voxel_end)
 
 double i3d_phase_ms(const I3DEngine* e, const char* name)
 {
-    auto it = e->phases.find(name);
-    return it == e->phases.end() ? 0.0 : it->second.ms;
+    auto it = e->timing.phases.find(name);
+    return it == e->timing.phases.end() ? 0.0 : it->second.ms;
 }
 int64_t i3d_phase_count(const I3DEngine* e, const char* name)
 {
-    auto it = e->phases.find(name);
-    return it == e->phases.end() ? 0 : it->second.count;
+    auto it = e->timing.phases.find(name);
+    return it == e->timing.phases.end() ? 0 : it->second.count;
 }
 
 int64_t i3d_debug_num_slots(const I3DEngine* e) { return e->have_iter ? static_cast<int64_t>(e->K) * e->stride : 0; }
 int i3d_debug_set_kernel_timers(I3DEngine* e, int level)
 {
     if (!e) return 1;
-    e->timer_level = level > 0 ? 1 : 0;
+    e->timing.level = level > 0 ? 1 : 0;
     return 0;
 }
 
@@ -3005,9 +2555,9 @@ int i3d_debug_apply_operator(I3DEngine* e, const float* v, float* q)
         CK(cudaMemcpyAsync(e->ctl.p, &running, sizeof(CgCtl), cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(e->dbg_v.p, v, U * sizeof(float), cudaMemcpyHostToDevice, st));
         CK(cudaMemsetAsync(e->v_qg.p, 0, U * sizeof(float), st));
-        const int timer_level = e->timer_level;
+        const int timer_level = e->timing.level;
         const int64_t launches = e->launches;
-        e->timer_level = -1;                       // keep the last iteration's kernel table
+        e->timing.level = -1;                       // keep the last iteration's kernel table
         GridView g = e->grid_view(e->sdf, e->alb);
         const RegView rv = reg_view(e, e->last_params);
         const EgRows rows = eg_rows(e);
@@ -3016,7 +2566,7 @@ int i3d_debug_apply_operator(I3DEngine* e, const float* v, float* q)
         const int64_t hc = e->held_count();
         pdl_launch(e, k_scale_vec, blocks_for(static_cast<size_t>(hc)), kThreads, 0, sv, sh, hc, e->dbg_v.p, 1.0f, sv.ps, e->ctl.p, 0);
         launch_operator(e, g, rv, rows, sv, sh, e->dbg_v.p, 0.0f, 0.0f, 0);
-        e->timer_level = timer_level;
+        e->timing.level = timer_level;
         e->launches = launches;
         std::vector<float> qg(U), s(U);
         CK(cudaMemcpyAsync(qg.data(), e->v_qg.p, U * sizeof(float), cudaMemcpyDeviceToHost, st));

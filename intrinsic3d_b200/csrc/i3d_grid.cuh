@@ -1,8 +1,9 @@
 /*
  * i3d_grid.cuh — what every device module of the engine shares about the grid: the neighbour-table slots, the block size, the device
  * hash (coordinates -> voxel index), the explicitly rounded float operations, the grid view with the per-voxel operators both modules
- * evaluate (surface normal, intensity) and the subvolume table of the lighting.  No kernels: i3d_kernels.cuh (the engine's module) and
- * i3d_mesh.cuh / i3d_vis.cuh (the surface extraction's module) both include it.
+ * evaluate (surface normal, intensity), the normal rule of a depth plane (fusion and tracking) and the subvolume table of the lighting.
+ * No kernels: i3d_kernels.cuh (the engine's module), i3d_mesh.cuh / i3d_vis.cuh (the surface extraction's module) and i3d_render.cuh /
+ * i3d_track.cuh (the renderer's module) all include it.
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -84,6 +85,48 @@ __device__ __forceinline__ bool surface_normal_f(const GridView& g, int64_t v, f
     if (len != 0.0f) { g0 = FD(g0, len); g1 = FD(g1, len); g2 = FD(g2, len); }
     nrm[0] = g0; nrm[1] = g1; nrm[2] = g2;
     return !(g0 == 0.0f && g1 == 0.0f && g2 == 0.0f);
+}
+
+// ----------------------------------------------------------------------------------------------
+// normals of a depth plane (k_fuse_normals, k_track_normals)
+// ----------------------------------------------------------------------------------------------
+// computeNormals(vertex_map, 0.3) (processing.cpp:72-118) at pixel i of a W x H depth plane, with the vertex map evaluated on the fly as
+// computeVertexMap (:49-69) builds it: (x0 d, y0 d, d), x0 = (x - cx) * (1 / fx).  Central tangents, n = (t_y x t_x).normalized(); zero
+// where undefined.
+__device__ __forceinline__ float3 depth_normal(const float* __restrict__ depth, int W, int H, float fx, float fy, float cx, float cy, int64_t i)
+{
+    const int y = static_cast<int>(i / W), x = static_cast<int>(i - static_cast<int64_t>(y) * W);
+    float n[3] = {0.0f, 0.0f, 0.0f};
+    if (x >= 1 && y >= 1 && x < W - 1 && y < H - 1 && depth[i] != 0.0f)
+    {
+        const float fxi = FD(1.0f, fx), fyi = FD(1.0f, fy);
+        auto vertex = [&](int u, int v, float out[3]) {
+            const float d = depth[static_cast<int64_t>(v) * W + u];
+            out[0] = FM(FM(FS(static_cast<float>(u), cx), fxi), d);
+            out[1] = FM(FM(FS(static_cast<float>(v), cy), fyi), d);
+            out[2] = d;
+        };
+        float vx0[3], vx1[3], vy0[3], vy1[3];
+        vertex(x - 1, y, vx0);
+        vertex(x + 1, y, vx1);
+        vertex(x, y - 1, vy0);
+        vertex(x, y + 1, vy1);
+        if (vx0[2] != 0.0f && vx1[2] != 0.0f && vy0[2] != 0.0f && vy1[2] != 0.0f)
+        {
+            const float tx[3] = {FS(vx1[0], vx0[0]), FS(vx1[1], vx0[1]), FS(vx1[2], vx0[2])};
+            const float ty[3] = {FS(vy1[0], vy0[0]), FS(vy1[1], vy0[1]), FS(vy1[2], vy0[2])};
+            const float lx = __fsqrt_rn(FA(FA(FM(tx[0], tx[0]), FM(tx[1], tx[1])), FM(tx[2], tx[2])));
+            const float ly = __fsqrt_rn(FA(FA(FM(ty[0], ty[0]), FM(ty[1], ty[1])), FM(ty[2], ty[2])));
+            if (lx < 0.3f && ly < 0.3f)
+            {
+                float c[3] = {FS(FM(ty[1], tx[2]), FM(ty[2], tx[1])), FS(FM(ty[2], tx[0]), FM(ty[0], tx[2])), FS(FM(ty[0], tx[1]), FM(ty[1], tx[0]))};
+                const float sq = FA(FA(FM(c[0], c[0]), FM(c[1], c[1])), FM(c[2], c[2]));
+                if (sq > 0.0f) { const float l = __fsqrt_rn(sq); c[0] = FD(c[0], l); c[1] = FD(c[1], l); c[2] = FD(c[2], l); }
+                n[0] = c[0]; n[1] = c[1]; n[2] = c[2];
+            }
+        }
+    }
+    return make_float3(n[0], n[1], n[2]);
 }
 
 // nv::intensity(unsigned char r, g, b) (src/color_util.cpp:41-46)

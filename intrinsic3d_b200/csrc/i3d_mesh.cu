@@ -1,8 +1,10 @@
 /*
- * i3d_mesh.cu — the surface-extraction kernels (i3d_mesh.cuh), the colour modes they can take their colours from (i3d_vis.cuh) and
- * their CUB passes, compiled as a translation unit of their own, and the host wrappers of i3d_mesh.h that launch them.  Keeping them
- * out of i3d_engine.cu leaves the engine's device module as it is.
+ * i3d_mesh.cu — the surface extraction: its kernels (i3d_mesh.cuh), the colour modes it can take its colours from (i3d_vis.cuh), their
+ * CUB passes and the host code that sequences them (i3d_mesh.h).  Keeping them out of i3d_engine.cu leaves the engine's device module
+ * as it is.
  */
+#include <climits>
+
 #include "i3d_mesh.cuh"
 #include "i3d_vis.cuh"
 
@@ -18,99 +20,190 @@ namespace
 {
 struct AddI64 { __device__ __forceinline__ int64_t operator()(int64_t a, int64_t b) const { return a + b; } };
 struct MaxI32 { __device__ __forceinline__ int32_t operator()(int32_t a, int32_t b) const { return a > b ? a : b; } };
-inline unsigned blocks(int64_t n) { return static_cast<unsigned>((n + kThreads - 1) / kThreads); }
+
+// runs one CUB device call twice: temp-size query, then the call on ms.cub (grown, never shrunk)
+template <class Fn>
+void cub_call(MeshState& ms, Fn&& fn)
+{
+    size_t bytes = 0;
+    CK(fn(static_cast<void*>(nullptr), bytes));
+    ms.cub.ensure(bytes);
+    CK(fn(static_cast<void*>(ms.cub.p), bytes));
+}
+
+// Device time per stage of one extraction: event pairs around device-only segments, each credited to a stage.  The host round trips
+// that read counts back fall between segments, so they are not counted.
+struct MeshSegments
+{
+    MeshState& ms; cudaStream_t st; int used = 0; int stage[8];
+    void begin(int s) { CK(cudaEventRecord(ms.ev[2 * used], st)); stage[used] = s; }
+    void end() { CK(cudaEventRecord(ms.ev[2 * used + 1], st)); ++used; }
+};
+
+template <class T>
+T read_back(const T* d, cudaStream_t st)
+{
+    T h{};
+    CK(cudaMemcpyAsync(&h, d, sizeof(T), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return h;
+}
 } // namespace
 
-void colorize(const GridView& g, const SubvolGrid& sg, const double* sub_sh, int S, int mode, uchar4* out, cudaStream_t st)
+void colorize(MeshState& ms, Timing& tm, const GridView& g, const SubvolGrid& sg, const double* sub_sh, int S, int mode, cudaStream_t st)
 {
-    switch (mode)
+    begin_timing(tm, {"mesh_colorize"});
+    ms.vis_rgb.ensure(static_cast<size_t>(g.n));
     {
-    case I3D_MESH_COLOR_NORMALS: k_vis_colors<I3D_MESH_COLOR_NORMALS><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
-    case I3D_MESH_COLOR_LAPLACIAN: k_vis_colors<I3D_MESH_COLOR_LAPLACIAN><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
-    case I3D_MESH_COLOR_INTENSITY: k_vis_colors<I3D_MESH_COLOR_INTENSITY><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
-    case I3D_MESH_COLOR_INTENSITY_GRAD: k_vis_colors<I3D_MESH_COLOR_INTENSITY_GRAD><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
-    case I3D_MESH_COLOR_ALBEDO: k_vis_colors<I3D_MESH_COLOR_ALBEDO><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
-    case I3D_MESH_COLOR_SHADING_SV: k_vis_colors<I3D_MESH_COLOR_SHADING_SV><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
-    case I3D_MESH_COLOR_SHADING_SV_CONST: k_vis_colors<I3D_MESH_COLOR_SHADING_SV_CONST><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
-    case I3D_MESH_COLOR_CHROMACITY: k_vis_colors<I3D_MESH_COLOR_CHROMACITY><<<blocks(g.n), kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
-    default: break;     // the engine validates the mode before it calls
+        Timer t(tm, st, "mesh_colorize");
+        uchar4* out = ms.vis_rgb.p;
+        const unsigned nb = blocks_for(g.n);
+        switch (mode)
+        {
+        case I3D_MESH_COLOR_NORMALS: k_vis_colors<I3D_MESH_COLOR_NORMALS><<<nb, kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+        case I3D_MESH_COLOR_LAPLACIAN: k_vis_colors<I3D_MESH_COLOR_LAPLACIAN><<<nb, kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+        case I3D_MESH_COLOR_INTENSITY: k_vis_colors<I3D_MESH_COLOR_INTENSITY><<<nb, kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+        case I3D_MESH_COLOR_INTENSITY_GRAD: k_vis_colors<I3D_MESH_COLOR_INTENSITY_GRAD><<<nb, kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+        case I3D_MESH_COLOR_ALBEDO: k_vis_colors<I3D_MESH_COLOR_ALBEDO><<<nb, kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+        case I3D_MESH_COLOR_SHADING_SV: k_vis_colors<I3D_MESH_COLOR_SHADING_SV><<<nb, kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+        case I3D_MESH_COLOR_SHADING_SV_CONST: k_vis_colors<I3D_MESH_COLOR_SHADING_SV_CONST><<<nb, kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+        case I3D_MESH_COLOR_CHROMACITY: k_vis_colors<I3D_MESH_COLOR_CHROMACITY><<<nb, kThreads, 0, st>>>(g, sg, sub_sh, S, out); break;
+        default: break;
+        }
     }
+    collect_kernel_times(tm, st);
+    CK(cudaGetLastError());
 }
 
-void classify(const MeshGrid& g, uint8_t* cube_case, int32_t* tri_count, unsigned long long* num_cubes, cudaStream_t st)
+int extract(MeshState& ms, const MeshGrid& g, bool largest_component_only, I3DMeshInfo* info, std::string& error, cudaStream_t st)
 {
-    k_mesh_classify<<<blocks(g.n), kThreads, 0, st>>>(g, cube_case, tri_count, num_cubes);
+    const int64_t n = g.n;
+    ms.have_mesh = false;
+    if (!ms.ev_ready) { for (auto& ev : ms.ev) CK(cudaEventCreate(&ev)); ms.ev_ready = true; }
+    I3DMeshInfo inf{};
+
+    enum { CLASSIFY, EMIT, WELD, CLEAN, COMPONENTS };
+    MeshSegments seg{ms, st};
+
+    // 1. cube cases and per-voxel triangle counts -> face offsets (int64 exclusive scan of the counts)
+    ms.cases.ensure(n); ms.cnt.ensure(n); ms.off.ensure(n); ms.cubes.ensure(1); ms.sel.ensure(1); ms.best.ensure(1);
+    seg.begin(CLASSIFY);
+    CK(cudaMemsetAsync(ms.cubes.p, 0, sizeof(unsigned long long), st));
+    k_mesh_classify<<<blocks_for(n), kThreads, 0, st>>>(g, ms.cases.p, ms.cnt.p, ms.cubes.p);
+    cub_call(ms, [&](void* t, size_t& b) {
+        return cub::DeviceScan::ExclusiveScan(t, b, static_cast<const int32_t*>(ms.cnt.p), ms.off.p, AddI64(), static_cast<int64_t>(0), static_cast<int>(n), st);
+    });
+    seg.end();
+    inf.num_cubes = static_cast<int64_t>(read_back(ms.cubes.p, st));
+    const int64_t F0 = read_back(ms.off.p + (n - 1), st) + read_back(ms.cnt.p + (n - 1), st);
+    inf.num_faces_raw = F0;
+    // corner and vertex ids are int32 (as the PLY's indices); element offsets into the interleaved arrays are computed in int64
+    if (3 * F0 > INT_MAX)
+    {
+        error = "i3d_extract_mesh: " + std::to_string(static_cast<long long>(F0)) + " triangles exceed the int32 corner indices of the mesh";
+        return 1;
+    }
+    const int32_t M = static_cast<int32_t>(3 * F0);
+    float* vpos = nullptr; uint8_t* vcol = nullptr; int3* faces = nullptr;
+    int64_t V = 0, F = 0;
+    if (M > 0)
+    {
+        // 2. the triangle soup, corner by corner
+        ms.cpos.ensure(3 * static_cast<size_t>(M)); ms.ccol.ensure(3 * static_cast<size_t>(M));
+        ms.klo.ensure(M); ms.klo2.ensure(M); ms.khi.ensure(M); ms.khi2.ensure(M); ms.perm.ensure(M); ms.perm2.ensure(M);
+        seg.begin(EMIT);
+        k_mesh_emit<<<blocks_for(n), kThreads, 0, st>>>(g, ms.cases.p, ms.cnt.p, ms.off.p, MeshCorners{ms.cpos.p, ms.ccol.p, ms.klo.p, ms.khi.p});
+        seg.end();
+
+        // 3. welding: stable sort of the corner indices by position (z bits, then x|y bits), segment heads, ids by first appearance
+        ms.first.ensure(M); ms.fid.ensure(M); ms.head.ensure(M); ms.seg.ensure(M); ms.cvid.ensure(M);
+        seg.begin(WELD);
+        k_mesh_iota<<<blocks_for(M), kThreads, 0, st>>>(M, ms.perm2.p);
+        cub_call(ms, [&](void* t, size_t& b) {
+            return cub::DeviceRadixSort::SortPairs(t, b, static_cast<const uint32_t*>(ms.klo.p), ms.klo2.p, static_cast<const int32_t*>(ms.perm2.p), ms.perm.p,
+                                                   M, 0, 32, st);
+        });
+        k_gather_key_hi<<<blocks_for(M), kThreads, 0, st>>>(M, ms.perm.p, ms.khi.p, ms.khi2.p);
+        cub_call(ms, [&](void* t, size_t& b) {
+            return cub::DeviceRadixSort::SortPairs(t, b, static_cast<const unsigned long long*>(ms.khi2.p), ms.khi.p, static_cast<const int32_t*>(ms.perm.p),
+                                                   ms.perm2.p, M, 0, 64, st);
+        });
+        k_weld_heads<<<blocks_for(M), kThreads, 0, st>>>(M, ms.perm2.p, ms.khi.p, ms.klo.p, ms.first.p, ms.head.p);
+        cub_call(ms, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, static_cast<const int32_t*>(ms.first.p), ms.fid.p, M, st); });
+        cub_call(ms, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveScan(t, b, static_cast<const int32_t*>(ms.head.p), ms.seg.p, MaxI32(), M, st); });
+        seg.end();
+        const int64_t Vw = read_back(ms.fid.p + (M - 1), st) + read_back(ms.first.p + (M - 1), st);
+        ms.vpos.ensure(3 * static_cast<size_t>(Vw)); ms.vcol.ensure(3 * static_cast<size_t>(Vw));
+        seg.begin(WELD);
+        k_weld_assign<<<blocks_for(M), kThreads, 0, st>>>(M, ms.perm2.p, ms.seg.p, ms.fid.p, ms.cpos.p, ms.ccol.p, ms.cvid.p, ms.vpos.p, ms.vcol.p);
+        seg.end();
+        inf.num_vertices_welded = Vw;
+
+        // 4. degenerate faces, survivors kept in order; the vertices stay
+        const int32_t F0i = static_cast<int32_t>(F0);
+        const int3* faces0 = reinterpret_cast<const int3*>(ms.cvid.p);
+        ms.keep.ensure(F0); ms.faces.ensure(F0);
+        seg.begin(CLEAN);
+        k_face_clean<<<blocks_for(F0i), kThreads, 0, st>>>(F0i, faces0, ms.vpos.p, ms.keep.p);
+        cub_call(ms, [&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, faces0, static_cast<const uint8_t*>(ms.keep.p), ms.faces.p, ms.sel.p, F0i, st); });
+        seg.end();
+        const int32_t F1 = read_back(ms.sel.p, st);
+        inf.num_faces_clean = F1;
+        vpos = ms.vpos.p; vcol = ms.vcol.p; faces = ms.faces.p; V = Vw; F = F1;
+
+        // 5. the largest face-connected component, then only the vertices it uses
+        if (largest_component_only)
+        {
+            const int32_t Vi = static_cast<int32_t>(Vw);
+            ms.parent.ensure(Vw); ms.ccount.ensure(Vw); ms.cminf.ensure(Vw); ms.used.ensure(Vw); ms.newid.ensure(Vw);
+            ms.faces2.ensure(std::max<int32_t>(F1, 1));
+            int32_t F2 = 0, V2 = 0;
+            if (F1 > 0)
+            {
+                seg.begin(COMPONENTS);
+                k_mesh_iota<<<blocks_for(Vi), kThreads, 0, st>>>(Vi, ms.parent.p);
+                k_cc_union<<<blocks_for(F1), kThreads, 0, st>>>(F1, ms.faces.p, ms.parent.p);
+                k_cc_flatten<<<blocks_for(Vi), kThreads, 0, st>>>(Vi, ms.parent.p);
+                CK(cudaMemsetAsync(ms.ccount.p, 0, Vw * sizeof(unsigned), st));
+                CK(cudaMemsetAsync(ms.cminf.p, 0xFF, Vw * sizeof(unsigned), st));
+                CK(cudaMemsetAsync(ms.best.p, 0, sizeof(unsigned long long), st));
+                k_cc_count<<<blocks_for(F1), kThreads, 0, st>>>(F1, ms.faces.p, ms.parent.p, ms.ccount.p, ms.cminf.p);
+                k_cc_best<<<blocks_for(Vi), kThreads, 0, st>>>(Vi, ms.ccount.p, ms.cminf.p, ms.best.p);
+                k_cc_keep<<<blocks_for(F1), kThreads, 0, st>>>(F1, ms.faces.p, ms.parent.p, ms.best.p, ms.keep.p);
+                cub_call(ms, [&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, static_cast<const int3*>(ms.faces.p), static_cast<const uint8_t*>(ms.keep.p), ms.faces2.p, ms.sel.p, F1, st); });
+                seg.end();
+                F2 = read_back(ms.sel.p, st);
+                seg.begin(COMPONENTS);
+                CK(cudaMemsetAsync(ms.used.p, 0, Vw * sizeof(int32_t), st));
+                if (F2 > 0) k_mark_used<<<blocks_for(F2), kThreads, 0, st>>>(F2, ms.faces2.p, ms.used.p);
+                cub_call(ms, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, static_cast<const int32_t*>(ms.used.p), ms.newid.p, Vi, st); });
+                seg.end();
+                V2 = read_back(ms.newid.p + (Vi - 1), st) + read_back(ms.used.p + (Vi - 1), st);
+                ms.vpos2.ensure(3 * static_cast<size_t>(V2)); ms.vcol2.ensure(3 * static_cast<size_t>(V2));
+                seg.begin(COMPONENTS);
+                k_compact_vertices<<<blocks_for(Vi), kThreads, 0, st>>>(Vi, ms.used.p, ms.newid.p, ms.vpos.p, ms.vcol.p, ms.vpos2.p, ms.vcol2.p);
+                if (F2 > 0) k_remap_faces<<<blocks_for(F2), kThreads, 0, st>>>(F2, ms.newid.p, ms.faces2.p);
+                seg.end();
+            }
+            vpos = ms.vpos2.p; vcol = ms.vcol2.p; faces = ms.faces2.p; V = V2; F = F2;
+        }
+    }
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
+    double t_ms[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int k = 0; k < seg.used; ++k)
+    {
+        float t = 0.f;
+        CK(cudaEventElapsedTime(&t, ms.ev[2 * k], ms.ev[2 * k + 1]));
+        t_ms[seg.stage[k]] += t;
+    }
+    inf.ms_classify = t_ms[CLASSIFY]; inf.ms_emit = t_ms[EMIT]; inf.ms_weld = t_ms[WELD]; inf.ms_clean = t_ms[CLEAN]; inf.ms_components = t_ms[COMPONENTS];
+    inf.num_faces = F; inf.num_vertices = V;
+    ms.mesh_vpos = vpos; ms.mesh_vcol = vcol; ms.mesh_faces = faces; ms.mesh_V = V; ms.mesh_F = F;
+    ms.have_mesh = true;
+    if (info) *info = inf;
+    return 0;
 }
-cudaError_t face_offsets(void* tmp, size_t& bytes, const int32_t* tri_count, int64_t* face_off, int n, cudaStream_t st)
-{
-    return cub::DeviceScan::ExclusiveScan(tmp, bytes, tri_count, face_off, AddI64(), static_cast<int64_t>(0), n, st);
-}
-void emit(const MeshGrid& g, const uint8_t* cube_case, const int32_t* tri_count, const int64_t* face_off, const MeshCorners& out, cudaStream_t st)
-{
-    k_mesh_emit<<<blocks(g.n), kThreads, 0, st>>>(g, cube_case, tri_count, face_off, out);
-}
-void iota(int32_t m, int32_t* out, cudaStream_t st) { k_mesh_iota<<<blocks(m), kThreads, 0, st>>>(m, out); }
-cudaError_t sort_z(void* tmp, size_t& bytes, const uint32_t* key_lo, uint32_t* key_lo_sorted, const int32_t* perm_in, int32_t* perm_out, int32_t m,
-                   cudaStream_t st)
-{
-    return cub::DeviceRadixSort::SortPairs(tmp, bytes, key_lo, key_lo_sorted, perm_in, perm_out, m, 0, 32, st);
-}
-void gather_key_hi(int32_t m, const int32_t* perm, const unsigned long long* key_hi, unsigned long long* out, cudaStream_t st)
-{
-    k_gather_key_hi<<<blocks(m), kThreads, 0, st>>>(m, perm, key_hi, out);
-}
-cudaError_t sort_xy(void* tmp, size_t& bytes, const unsigned long long* key_hi, unsigned long long* key_hi_sorted, const int32_t* perm_in,
-                    int32_t* perm_out, int32_t m, cudaStream_t st)
-{
-    return cub::DeviceRadixSort::SortPairs(tmp, bytes, key_hi, key_hi_sorted, perm_in, perm_out, m, 0, 64, st);
-}
-void weld_heads(int32_t m, const int32_t* perm, const unsigned long long* hi_sorted, const uint32_t* key_lo, int32_t* is_first, int32_t* head_pos,
-                cudaStream_t st)
-{
-    k_weld_heads<<<blocks(m), kThreads, 0, st>>>(m, perm, hi_sorted, key_lo, is_first, head_pos);
-}
-cudaError_t exclusive_sum(void* tmp, size_t& bytes, const int32_t* in, int32_t* out, int32_t m, cudaStream_t st)
-{
-    return cub::DeviceScan::ExclusiveSum(tmp, bytes, in, out, m, st);
-}
-cudaError_t inclusive_max(void* tmp, size_t& bytes, const int32_t* in, int32_t* out, int32_t m, cudaStream_t st)
-{
-    return cub::DeviceScan::InclusiveScan(tmp, bytes, in, out, MaxI32(), m, st);
-}
-void weld_assign(int32_t m, const int32_t* perm, const int32_t* seg_head, const int32_t* first_id, const float* cpos, const uint8_t* ccol,
-                 int32_t* corner_vid, float* vpos, uint8_t* vcol, cudaStream_t st)
-{
-    k_weld_assign<<<blocks(m), kThreads, 0, st>>>(m, perm, seg_head, first_id, cpos, ccol, corner_vid, vpos, vcol);
-}
-void face_clean(int32_t f, const int3* faces, const float* vpos, uint8_t* keep, cudaStream_t st)
-{
-    k_face_clean<<<blocks(f), kThreads, 0, st>>>(f, faces, vpos, keep);
-}
-cudaError_t select_faces(void* tmp, size_t& bytes, const int3* in, const uint8_t* keep, int3* out, int32_t* num_selected, int32_t f, cudaStream_t st)
-{
-    return cub::DeviceSelect::Flagged(tmp, bytes, in, keep, out, num_selected, f, st);
-}
-void cc_union(int32_t f, const int3* faces, int32_t* parent, cudaStream_t st) { k_cc_union<<<blocks(f), kThreads, 0, st>>>(f, faces, parent); }
-void cc_flatten(int32_t nv, int32_t* parent, cudaStream_t st) { k_cc_flatten<<<blocks(nv), kThreads, 0, st>>>(nv, parent); }
-void cc_count(int32_t f, const int3* faces, const int32_t* root, unsigned* count, unsigned* min_face, cudaStream_t st)
-{
-    k_cc_count<<<blocks(f), kThreads, 0, st>>>(f, faces, root, count, min_face);
-}
-void cc_best(int32_t nv, const unsigned* count, const unsigned* min_face, unsigned long long* best, cudaStream_t st)
-{
-    k_cc_best<<<blocks(nv), kThreads, 0, st>>>(nv, count, min_face, best);
-}
-void cc_keep(int32_t f, const int3* faces, const int32_t* root, const unsigned long long* best, uint8_t* keep, cudaStream_t st)
-{
-    k_cc_keep<<<blocks(f), kThreads, 0, st>>>(f, faces, root, best, keep);
-}
-void mark_used(int32_t f, const int3* faces, int32_t* used, cudaStream_t st) { k_mark_used<<<blocks(f), kThreads, 0, st>>>(f, faces, used); }
-void compact_vertices(int32_t nv, const int32_t* used, const int32_t* new_id, const float* vpos, const uint8_t* vcol, float* vpos_out,
-                      uint8_t* vcol_out, cudaStream_t st)
-{
-    k_compact_vertices<<<blocks(nv), kThreads, 0, st>>>(nv, used, new_id, vpos, vcol, vpos_out, vcol_out);
-}
-void remap_faces(int32_t f, const int32_t* new_id, int3* faces, cudaStream_t st) { k_remap_faces<<<blocks(f), kThreads, 0, st>>>(f, new_id, faces); }
 
 } // namespace mesh
 } // namespace i3d

@@ -1,15 +1,15 @@
 /*
- * i3d_mesh.h — host interface of the surface-extraction kernels (i3d_mesh.cuh, compiled in i3d_mesh.cu).  The kernels live in a
- * device module of their own, so the engine's module holds exactly the kernels of the refinement path; the engine (i3d_engine.cu)
- * owns the buffers and the stage order and calls these wrappers on its stream.  The CUB wrappers follow CUB's two-call convention:
- * with tmp == nullptr they only set `bytes`.
+ * i3d_mesh.h — the surface extraction (i3d_mesh.cuh) and its colour modes (i3d_vis.cuh), compiled in i3d_mesh.cu, a device module of
+ * its own: its state, and the two calls the engine (i3d_engine.cu) makes with the grid it builds and its stream.
  */
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
 
+#include "../../include/i3d_types.h"
 #include "i3d_grid.cuh"
+#include "i3d_host.h"
 
 namespace i3d
 {
@@ -36,42 +36,33 @@ struct MeshCorners
     unsigned long long* key_hi;    // x bits << 32 | y bits
 };
 
+// Surface-extraction state of an engine: scratch that only grows, the event pairs of the stage timings, the resident mesh of the last
+// extraction (pointers into the scratch) and the per-voxel colours of the last colour pass
+struct MeshState
+{
+    Dev<uint8_t> cases, keep, cub; Dev<int32_t> cnt, sel; Dev<int64_t> off; Dev<unsigned long long> cubes, best;
+    Dev<float> cpos, vpos, vpos2; Dev<uint8_t> ccol, vcol, vcol2;
+    Dev<uint32_t> klo, klo2; Dev<unsigned long long> khi, khi2;
+    Dev<int32_t> perm, perm2, first, fid, head, seg, cvid, parent, used, newid;
+    Dev<int3> faces, faces2; Dev<unsigned> ccount, cminf;
+    cudaEvent_t ev[16] = {};           // begin / end of up to 8 device-only segments of one extraction
+    bool ev_ready = false;
+    bool have_mesh = false;
+    int64_t mesh_V = 0, mesh_F = 0;
+    float* mesh_vpos = nullptr; uint8_t* mesh_vcol = nullptr; int3* mesh_faces = nullptr;
+    Dev<uchar4> vis_rgb;
+};
+
 namespace mesh
 {
-// 0. the per-voxel colours of a colour mode (i3d_vis.cuh; mode 1 .. I3D_MESH_COLOR_COUNT - 1) into out [n]; g.sdf is the sdf the mesh is
-// cut from, sg / sub_sh [S][9] the subvolumes and subvolume SH of the last lighting estimate (read by the shading modes only)
-void colorize(const GridView& g, const SubvolGrid& sg, const double* sub_sh, int S, int mode, uchar4* out, cudaStream_t st);
-// 1. cube cases, triangle counts, used-cube count; face offsets (int64 exclusive scan of the counts)
-void classify(const MeshGrid& g, uint8_t* cube_case, int32_t* tri_count, unsigned long long* num_cubes, cudaStream_t st);
-cudaError_t face_offsets(void* tmp, size_t& bytes, const int32_t* tri_count, int64_t* face_off, int n, cudaStream_t st);
-// 2. the triangle soup
-void emit(const MeshGrid& g, const uint8_t* cube_case, const int32_t* tri_count, const int64_t* face_off, const MeshCorners& out, cudaStream_t st);
-// 3. welding
-void iota(int32_t m, int32_t* out, cudaStream_t st);
-cudaError_t sort_z(void* tmp, size_t& bytes, const uint32_t* key_lo, uint32_t* key_lo_sorted, const int32_t* perm_in, int32_t* perm_out, int32_t m,
-                   cudaStream_t st);
-void gather_key_hi(int32_t m, const int32_t* perm, const unsigned long long* key_hi, unsigned long long* out, cudaStream_t st);
-cudaError_t sort_xy(void* tmp, size_t& bytes, const unsigned long long* key_hi, unsigned long long* key_hi_sorted, const int32_t* perm_in,
-                    int32_t* perm_out, int32_t m, cudaStream_t st);
-void weld_heads(int32_t m, const int32_t* perm, const unsigned long long* hi_sorted, const uint32_t* key_lo, int32_t* is_first, int32_t* head_pos,
-                cudaStream_t st);
-cudaError_t exclusive_sum(void* tmp, size_t& bytes, const int32_t* in, int32_t* out, int32_t m, cudaStream_t st);
-cudaError_t inclusive_max(void* tmp, size_t& bytes, const int32_t* in, int32_t* out, int32_t m, cudaStream_t st);
-void weld_assign(int32_t m, const int32_t* perm, const int32_t* seg_head, const int32_t* first_id, const float* cpos, const uint8_t* ccol,
-                 int32_t* corner_vid, float* vpos, uint8_t* vcol, cudaStream_t st);
-// 4. degenerate faces; order-keeping selection of flagged faces
-void face_clean(int32_t f, const int3* faces, const float* vpos, uint8_t* keep, cudaStream_t st);
-cudaError_t select_faces(void* tmp, size_t& bytes, const int3* in, const uint8_t* keep, int3* out, int32_t* num_selected, int32_t f, cudaStream_t st);
-// 5. largest component and the vertices it uses
-void cc_union(int32_t f, const int3* faces, int32_t* parent, cudaStream_t st);
-void cc_flatten(int32_t nv, int32_t* parent, cudaStream_t st);
-void cc_count(int32_t f, const int3* faces, const int32_t* root, unsigned* count, unsigned* min_face, cudaStream_t st);
-void cc_best(int32_t nv, const unsigned* count, const unsigned* min_face, unsigned long long* best, cudaStream_t st);
-void cc_keep(int32_t f, const int3* faces, const int32_t* root, const unsigned long long* best, uint8_t* keep, cudaStream_t st);
-void mark_used(int32_t f, const int3* faces, int32_t* used, cudaStream_t st);
-void compact_vertices(int32_t nv, const int32_t* used, const int32_t* new_id, const float* vpos, const uint8_t* vcol, float* vpos_out,
-                      uint8_t* vcol_out, cudaStream_t st);
-void remap_faces(int32_t f, const int32_t* new_id, int3* faces, cudaStream_t st);
+// The colour pass (i3d_vis.cuh) of mode 1 .. I3D_MESH_COLOR_COUNT - 1 (validated by the caller) into ms.vis_rgb [g.n], timed as phase
+// "mesh_colorize".  g.sdf is the sdf the mesh is cut from, sg / sub_sh [S][9] the subvolumes and subvolume SH of the last lighting
+// estimate (read by the shading modes only).  Writes nothing but ms.vis_rgb.
+void colorize(MeshState& ms, Timing& tm, const GridView& g, const SubvolGrid& sg, const double* sub_sh, int S, int mode, cudaStream_t st);
+// Marching cubes over g, welding, degenerate-face removal and (optionally) the largest component, into the resident mesh of ms.  Every
+// count is read back before the buffers of the next stage are sized; info (may be nullptr) gets the counts and stage times.  Returns
+// non-zero with the message in `error`, writing no info and leaving no mesh resident, when the triangles exceed the int32 corner indices.
+int extract(MeshState& ms, const MeshGrid& g, bool largest_component_only, I3DMeshInfo* info, std::string& error, cudaStream_t st);
 } // namespace mesh
 
 } // namespace i3d

@@ -1,39 +1,242 @@
 /*
- * i3d_render.cu — the keyframe renderer's kernels (i3d_render.cuh), compiled as a translation unit of their own, and the host wrappers of
- * i3d_render.h that launch them.  Keeping them out of i3d_engine.cu leaves the engine's device module as it is.
+ * i3d_render.cu — the keyframe renderer (i3d_render.cuh) and the frame-to-model tracker (i3d_track.cuh), which marches the renderer's kernel
+ * for its prediction: their kernels and the host code that sequences them (i3d_render.h, i3d_track.h).  Keeping them out of i3d_engine.cu
+ * leaves the engine's device module as it is.
  */
+#include <climits>
+#include <cmath>
+#include <cstring>
+
+#include "../../include/i3d_c_api.h"
 #include "i3d_render.cuh"
+#include "i3d_track.cuh"
 
 namespace i3d
 {
-namespace render
-{
 namespace
 {
-inline unsigned blocks(int64_t n) { return static_cast<unsigned>((n + kThreads - 1) / kThreads); }
-} // namespace
+// Bits of the renderer's brick bitmap above which the march visits every lattice sample instead (128 MiB)
+constexpr int64_t kRenderBrickCap = 1ll << 30;
 
-void bounds(int64_t n, const int32_t* x, const int32_t* y, const int32_t* z, int* box, cudaStream_t st)
+// Completes rg with the voxel box and (when it fits under kRenderBrickCap) the brick bitmap of its voxel set.  They are built, timed as
+// "render_bricks", on the first call after the voxel set changed.
+void add_voxel_box(RenderState& rs, Timing& tm, RenderGrid& rg, cudaStream_t st)
 {
-    k_render_bounds<<<blocks(n), kThreads, 0, st>>>(n, x, y, z, box);
-}
-
-void bricks(int64_t n, const int32_t* x, const int32_t* y, const int32_t* z, const int blo[3], const int bdim[3], uint32_t* bits, cudaStream_t st)
-{
-    const BrickBox bb{{blo[0], blo[1], blo[2]}, {bdim[0], bdim[1], bdim[2]}};
-    k_render_bricks<<<blocks(n), kThreads, 0, st>>>(n, x, y, z, bb, bits);
+    if (!rs.box_ready)
+    {
+        Timer t(tm, st, "render_bricks");
+        const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
+        rs.box_d.ensure(6);
+        CK(cudaMemcpyAsync(rs.box_d.p, init, sizeof(init), cudaMemcpyHostToDevice, st));
+        k_render_bounds<<<blocks_for(rg.g.n), kThreads, 0, st>>>(rg.g.n, rg.g.x, rg.g.y, rg.g.z, rs.box_d.p);
+        CK(cudaMemcpyAsync(rs.box, rs.box_d.p, sizeof(rs.box), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        int64_t bits = 1;
+        for (int d = 0; d < 3; ++d)
+        {
+            rs.blo[d] = rs.box[d];
+            rs.bdim[d] = ((rs.box[3 + d] - rs.box[d]) >> 3) + 1;
+            bits *= rs.bdim[d];
+        }
+        rs.have_bricks = bits <= kRenderBrickCap;
+        if (rs.have_bricks)
+        {
+            const size_t words = static_cast<size_t>((bits + 31) >> 5);
+            rs.bits.ensure(words);
+            CK(cudaMemsetAsync(rs.bits.p, 0, words * sizeof(uint32_t), st));
+            const BrickBox bb{{rs.blo[0], rs.blo[1], rs.blo[2]}, {rs.bdim[0], rs.bdim[1], rs.bdim[2]}};
+            k_render_bricks<<<blocks_for(rg.g.n), kThreads, 0, st>>>(rg.g.n, rg.g.x, rg.g.y, rg.g.z, bb, rs.bits.p);
+        }
+        t.stop();
+        rs.box_ready = true;
+    }
+    for (int d = 0; d < 3; ++d)
+    {
+        rg.lo[d] = static_cast<float>(rs.box[d]) * rg.g.voxel_size;
+        rg.hi[d] = static_cast<float>(rs.box[3 + d]) * rg.g.voxel_size;
+        rg.blo[d] = rs.blo[d]; rg.bdim[d] = rs.bdim[d];
+    }
+    rg.bricks = (rs.skip && rs.have_bricks) ? rs.bits.p : nullptr;
 }
 
 void march(const RenderGrid& rg, const RenderCam& cam, const RenderViews& rv, cudaStream_t st)
 {
-    const dim3 grid(rv.tiles_x, rv.tiles_y, rv.n), block(kRenderTile, kRenderTile);
-    k_render_march<<<grid, block, 0, st>>>(rg, cam, rv);
+    k_render_march<<<dim3(rv.tiles_x, rv.tiles_y, rv.n), dim3(kRenderTile, kRenderTile), 0, st>>>(rg, cam, rv);
 }
 
-void finish(int n, int tiles, const double* partials, double* out, cudaStream_t st)
+// out[n][V] = the fixed-order sums of the n views' partials [n][tiles][V]
+template <int V>
+void tile_sums(int n, int tiles, const double* partials, double* out, cudaStream_t st)
 {
-    k_render_finish<<<blocks(static_cast<int64_t>(n) * kRenderStats), kThreads, 0, st>>>(n, tiles, partials, out);
+    k_tile_sums<V><<<blocks_for(static_cast<size_t>(n) * V), kThreads, 0, st>>>(n, tiles, partials, out);
 }
 
-} // namespace render
+// One view's kRenderStats sums
+I3DRenderStats render_stats(const double* s)
+{
+    I3DRenderStats r;
+    r.num_hit = static_cast<int64_t>(s[0]); r.num_observed = static_cast<int64_t>(s[1]);
+    r.depth_count = static_cast<int64_t>(s[2]); r.photo_count = static_cast<int64_t>(s[3]);
+    r.depth_abs = s[4]; r.depth_sq = s[5]; r.photo_abs = s[6]; r.photo_sq = s[7];
+    return r;
+}
+} // namespace
+
+void render::keyframes(RenderState& rs, Timing& tm, RenderGrid rg, const RenderCam& cam, const float* Rt, int n, const int32_t* ids, int W, int H,
+                       const float* depth, const float* lum, int planes, bool photometric, I3DRenderStats* stats, cudaStream_t st)
+{
+    begin_timing(tm, {"render", "render_bricks", "render_samples"});
+    rs.have_render = false;
+    const size_t img = static_cast<size_t>(n) * W * H;
+    if (planes & I3D_RENDER_DEPTH) rs.depth.ensure(img);
+    if (planes & I3D_RENDER_NORMAL) rs.normal.ensure(3 * img);
+    if (planes & I3D_RENDER_ALBEDO) rs.albedo.ensure(img);
+    if (planes & I3D_RENDER_SHADING) rs.shading.ensure(img);
+    if (planes & I3D_RENDER_INTENSITY) rs.intensity.ensure(img);
+    const int tiles_x = (W + kRenderTile - 1) / kRenderTile, tiles_y = (H + kRenderTile - 1) / kRenderTile;
+    rs.partials.ensure(static_cast<size_t>(n) * tiles_x * tiles_y * kRenderStats);
+    rs.sums.ensure(static_cast<size_t>(n) * kRenderStats);
+    rs.ids.ensure(n); rs.samples.ensure(1);
+    CK(cudaMemcpyAsync(rs.ids.p, ids, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(rs.samples.p, 0, sizeof(unsigned long long), st));
+    {
+        Timer t(tm, st, "render");
+        add_voxel_box(rs, tm, rg, st);
+        RenderViews rv;
+        rv.n = n; rv.W = W; rv.H = H; rv.tiles_x = tiles_x; rv.tiles_y = tiles_y;
+        rv.ids = rs.ids.p; rv.Rt = Rt; rv.depth = depth; rv.lum = lum;
+        rv.out_depth = (planes & I3D_RENDER_DEPTH) ? rs.depth.p : nullptr;
+        rv.out_normal = (planes & I3D_RENDER_NORMAL) ? rs.normal.p : nullptr;
+        rv.out_albedo = (planes & I3D_RENDER_ALBEDO) ? rs.albedo.p : nullptr;
+        rv.out_shading = (planes & I3D_RENDER_SHADING) ? rs.shading.p : nullptr;
+        rv.out_intensity = (planes & I3D_RENDER_INTENSITY) ? rs.intensity.p : nullptr;
+        rv.partials = rs.partials.p; rv.samples = rs.samples.p; rv.photometric = photometric ? 1 : 0;
+        march(rg, cam, rv, st);
+        tile_sums<kRenderStats>(n, tiles_x * tiles_y, rs.partials.p, rs.sums.p, st);
+    }
+    std::vector<double> sums(static_cast<size_t>(n) * kRenderStats);
+    unsigned long long samples = 0;
+    CK(cudaMemcpyAsync(sums.data(), rs.sums.p, sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&samples, rs.samples.p, sizeof(samples), cudaMemcpyDeviceToHost, st));
+    collect_kernel_times(tm, st);
+    CK(cudaGetLastError());
+    tm.phases["render_samples"].count = static_cast<int64_t>(samples);
+    if (stats)
+        for (int i = 0; i < n; ++i) stats[i] = render_stats(sums.data() + static_cast<size_t>(i) * kRenderStats);
+    rs.have_render = true; rs.n = n; rs.planes = planes;
+}
+
+void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderGrid rg, const I3DFusionCamera& dc, const float* store_depth,
+                          int store_F, int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl,
+                          double* pose_out, I3DTrackInfo* info, cudaStream_t st)
+{
+    const int L = P.num_levels, W = dc.width, H = dc.height, C = std::min<int>(n, I3D_TRACK_CHUNK);
+    const size_t img = static_cast<size_t>(W) * H;
+    const int tiles_x = (W + kRenderTile - 1) / kRenderTile, tiles_y = (H + kRenderTile - 1) / kRenderTile;
+    static_assert(kRenderTile == kTrackTile, "the prediction and the rows share the level-0 tile grid");
+    begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences"});
+    ts.n = 0;
+    ts.ids.ensure(n); ts.pose_in.ensure(12 * static_cast<size_t>(n)); ts.state.ensure(n);
+    ts.sys.ensure(static_cast<size_t>(n) * kTrackVals); ts.rd_sums.ensure(static_cast<size_t>(n) * kRenderStats);
+    ts.rt.ensure(12 * static_cast<size_t>(store_F)); ts.counters.ensure(2);
+    ts.rd_partials.ensure(static_cast<size_t>(C) * tiles_x * tiles_y * kRenderStats);
+    ts.partials.ensure(static_cast<size_t>(C) * tiles_x * tiles_y * kTrackVals); ts.sums.ensure(static_cast<size_t>(C) * kTrackVals);
+    ts.pdepth.ensure(C * img); ts.pnrm.ensure(3 * C * img); ts.mask.ensure(C * img);
+    for (int l = 0; l < L; ++l)
+    {
+        const size_t c = static_cast<size_t>(C) * Wl[l] * Hl[l];
+        ts.depth[l].ensure(c); ts.nrm[l].ensure(3 * c);
+    }
+    // the input poses in float, scattered by sensor id: the march reads Rt + 12 * id
+    std::vector<float> hrt(12 * static_cast<size_t>(store_F), 0.0f);
+    for (int k = 0; k < n; ++k)
+        for (int i = 0; i < 12; ++i) hrt[12 * static_cast<size_t>(ids[k]) + i] = static_cast<float>(pose_in[12 * static_cast<size_t>(k) + i]);
+    CK(cudaMemcpyAsync(ts.ids.p, ids, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ts.pose_in.p, pose_in, 12 * static_cast<size_t>(n) * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ts.rt.p, hrt.data(), hrt.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(ts.counters.p, 0, 2 * sizeof(unsigned long long), st));
+    int total_iters = 0;
+    for (int l = 0; l < L; ++l) total_iters += P.iterations[l];
+    TrackCam cam[kTrackMaxLevels];
+    for (int l = 0; l < L; ++l)
+    {
+        const double s = std::ldexp(1.0, -l);       // the pyramid scale, as select_cam applies pyr_scale
+        cam[l] = TrackCam{Wl[l], Hl[l], static_cast<float>(dc.fx * s), static_cast<float>(dc.fy * s), static_cast<float>(dc.cx * s),
+                          static_cast<float>(dc.cy * s)};
+    }
+    Timer whole(tm, st, "track");
+    add_voxel_box(rs, tm, rg, st);
+    RenderCam rcam{};
+    rcam.fx = dc.fx; rcam.fy = dc.fy; rcam.cx = dc.cx; rcam.cy = dc.cy; rcam.dist_zero = 1;
+    k_track_init<<<blocks_for(n, 64), 64, 0, st>>>(n, ts.pose_in.p, ts.state.p);
+    const float max_dist_sq = P.max_distance * P.max_distance;
+    int m = 0;
+    for (int c0 = 0; c0 < n; c0 += C)
+    {
+        m = std::min(C, n - c0);
+        const int32_t* ids_d = ts.ids.p + c0;
+        {
+            Timer t(tm, st, "track_predict");
+            RenderViews rv{};
+            rv.n = m; rv.W = W; rv.H = H; rv.tiles_x = tiles_x; rv.tiles_y = tiles_y;
+            rv.ids = ids_d; rv.Rt = ts.rt.p; rv.depth = store_depth; rv.lum = nullptr;
+            rv.out_depth = ts.pdepth.p; rv.out_normal = ts.pnrm.p;
+            rv.partials = ts.rd_partials.p; rv.samples = ts.counters.p + 1; rv.photometric = 0;
+            march(rg, rcam, rv, st);
+            tile_sums<kRenderStats>(m, tiles_x * tiles_y, ts.rd_partials.p, ts.rd_sums.p + static_cast<size_t>(c0) * kRenderStats, st);
+        }
+        {
+            Timer t(tm, st, "track_pyramid");
+            k_track_gather<<<dim3(blocks_for(img), m), kThreads, 0, st>>>(m, W, H, ids_d, store_depth, ts.depth[0].p);
+            for (int l = 1; l < L; ++l) frames_depthdown(m, Wl[l - 1], Hl[l - 1], ts.depth[l - 1].p, ts.depth[l].p, st);
+            for (int l = 0; l < L; ++l)
+                k_track_normals<<<dim3(blocks_for(static_cast<size_t>(Wl[l]) * Hl[l]), m), kThreads, 0, st>>>(cam[l], ts.depth[l].p, ts.nrm[l].p);
+        }
+        {
+            Timer t(tm, st, "track_icp");
+            CK(cudaMemsetAsync(ts.mask.p, 0, m * img, st));
+            TrackRows tr{};
+            tr.pcam = cam[0]; tr.pdepth = ts.pdepth.p; tr.pnrm = ts.pnrm.p; tr.ids = ids_d; tr.rt_in = ts.rt.p;
+            tr.state = ts.state.p + c0; tr.max_dist_sq = max_dist_sq; tr.min_cos = P.min_normal_cos;
+            tr.use_cos = P.min_normal_cos > -1.0f ? 1 : 0; tr.partials = ts.partials.p;
+            auto system = [&](int l, int solve) {
+                tr.cam = cam[l]; tr.depth = ts.depth[l].p; tr.nrm = ts.nrm[l].p; tr.mask = l == 0 ? ts.mask.p : nullptr;
+                tr.tiles_x = (Wl[l] + kTrackTile - 1) / kTrackTile; tr.tiles_y = (Hl[l] + kTrackTile - 1) / kTrackTile;
+                {
+                    Timer tk(tm, st, "k_track_rows", 1);
+                    k_track_rows<<<dim3(tr.tiles_x, tr.tiles_y, m), dim3(kTrackTile, kTrackTile), 0, st>>>(tr);
+                }
+                tile_sums<kTrackVals>(m, tr.tiles_x * tr.tiles_y, ts.partials.p, ts.sums.p, st);
+                k_track_solve<<<blocks_for(m, 64), 64, 0, st>>>(m, ts.sums.p, ts.state.p + c0, ts.sys.p + static_cast<size_t>(c0) * kTrackVals,
+                                                                P.min_correspondences, solve, ts.counters.p);
+            };
+            for (int l = L - 1; l >= 0; --l)
+                for (int it = 0; it < P.iterations[l]; ++it) system(l, 1);
+            if (total_iters == 0) system(0, 0);        // no update: the level-0 system at the input pose
+        }
+    }
+    std::vector<TrackState> hs(n);
+    std::vector<double> rs_sums(static_cast<size_t>(n) * kRenderStats);
+    unsigned long long counters[2] = {0, 0};
+    CK(cudaMemcpyAsync(hs.data(), ts.state.p, n * sizeof(TrackState), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(rs_sums.data(), ts.rd_sums.p, rs_sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(counters, ts.counters.p, sizeof(counters), cudaMemcpyDeviceToHost, st));
+    whole.stop();
+    collect_kernel_times(tm, st);
+    CK(cudaGetLastError());
+    tm.phases["track_correspondences"].count = static_cast<int64_t>(counters[0]);
+    for (int k = 0; k < n; ++k)
+    {
+        std::memcpy(pose_out + 12 * static_cast<size_t>(k), hs[k].w2c, 12 * sizeof(double));
+        if (!info) continue;
+        I3DTrackInfo r{};
+        r.status = hs[k].status; r.iterations = hs[k].iterations; r.correspondences = hs[k].correspondences;
+        r.residual_sq = hs[k].residual_sq; r.update_norm = hs[k].update_norm;
+        r.initial = render_stats(rs_sums.data() + static_cast<size_t>(k) * kRenderStats);
+        info[k] = r;
+    }
+    ts.n = n; ts.levels = L; ts.last_m = m;
+    for (int l = 0; l < L; ++l) { ts.W[l] = Wl[l]; ts.H[l] = Hl[l]; }
+}
+
 } // namespace i3d

@@ -6,9 +6,9 @@
  *   k_render_bounds   the bounding box of the voxel coordinates (integer atomics)
  *   k_render_bricks   the occupancy bitmap of 8^3 bricks over that box (integer atomics)
  *   k_render_march    one thread per pixel, 16 x 16 tiles, views in gridDim.z: planes + per-tile statistic partials
- *   k_render_finish   the fixed-order sum of a view's partials
+ *   k_tile_sums       the fixed-order sum of a view's partials (also the tracker's)
  *
- * Compiled in its own translation unit, i3d_render.cu, and launched through the host wrappers declared in i3d_render.h.  Every float
+ * Compiled with the tracker in i3d_render.cu, which launches them (render::keyframes, i3d_render.h).  Every float
  * operation is explicitly rounded (no FMA contraction, IEEE division and square root), so the planes are byte-equal to tests/render_ref.py.
  * The statistics are double sums in a fixed order (tile tree, then tiles in order): a view's bytes depend only on that view.
  */
@@ -312,15 +312,17 @@ __global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march(Rend
     if ((tid & 31) == 0 && nsamp) atomicAdd(rv.samples, static_cast<unsigned long long>(nsamp));
 }
 
-// One thread per (view, statistic): the view's tiles summed in order
-__global__ void k_render_finish(int n, int tiles, const double* __restrict__ partials, double* __restrict__ out)
+// One thread per (view, value) of V per-tile values: the view's tiles summed in order.  V = kRenderStats (k_render_march's statistics),
+// kTrackVals (k_track_rows' systems).
+template <int V>
+__global__ void k_tile_sums(int n, int tiles, const double* __restrict__ partials, double* __restrict__ out)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n * kRenderStats) return;
-    const int view = i / kRenderStats, j = i % kRenderStats;
-    const double* p = partials + static_cast<int64_t>(view) * tiles * kRenderStats + j;
+    if (i >= n * V) return;
+    const int view = i / V, j = i % V;
+    const double* p = partials + static_cast<int64_t>(view) * tiles * V + j;
     double s = 0.0;
-    for (int t = 0; t < tiles; ++t) s = __dadd_rn(s, p[static_cast<int64_t>(t) * kRenderStats]);
+    for (int t = 0; t < tiles; ++t) s = __dadd_rn(s, p[static_cast<int64_t>(t) * V]);
     out[i] = s;
 }
 

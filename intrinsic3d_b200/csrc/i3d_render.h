@@ -1,14 +1,16 @@
 /*
- * i3d_render.h — host interface of the keyframe renderer (i3d_render.cuh, compiled in i3d_render.cu; DESIGN.md §6m).  The kernels live
- * in a device module of their own, so the engine's module holds exactly the kernels of the refinement path; the engine (i3d_engine.cu)
- * owns the buffers and calls these wrappers on its stream.
+ * i3d_render.h — the keyframe renderer (i3d_render.cuh, DESIGN.md §6m), compiled with the tracker that marches its kernel in i3d_render.cu,
+ * a device module of its own: the renderer's types and state, and the call the engine (i3d_engine.cu) makes with the grid and camera it
+ * builds and its stream.
  */
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
 
+#include "../../include/i3d_types.h"
 #include "i3d_grid.cuh"
+#include "i3d_host.h"
 
 namespace i3d
 {
@@ -54,16 +56,27 @@ struct RenderViews
     int photometric;
 };
 
+// Renderer state of an engine: the voxel box and brick bitmap of the current voxel set (built on the first render after a change; the
+// engine clears box_ready when the voxel set changes), scratch that only grows, and the resident planes of the last render
+struct RenderState
+{
+    bool skip = true;                  // i3d_debug_set_render_skip
+    bool box_ready = false, have_bricks = false;
+    int box[6] = {}, blo[3] = {}, bdim[3] = {};
+    Dev<int> box_d; Dev<uint32_t> bits;
+    Dev<float> rt; Dev<int32_t> ids; Dev<double> partials, sums; Dev<unsigned long long> samples;
+    Dev<float> depth, normal, albedo, shading, intensity;
+    bool have_render = false;
+    int n = 0, planes = 0;
+};
+
 namespace render
 {
-// 1. the bounding box of the voxel coordinates: box[0..2] = min (atomicMin), box[3..5] = max; box must hold INT_MAX / INT_MIN on entry
-void bounds(int64_t n, const int32_t* x, const int32_t* y, const int32_t* z, int* box, cudaStream_t st);
-// 2. the brick bitmap (zeroed by the caller)
-void bricks(int64_t n, const int32_t* x, const int32_t* y, const int32_t* z, const int blo[3], const int bdim[3], uint32_t* bits, cudaStream_t st);
-// 3. one thread per pixel, views in gridDim.z: the requested planes and the per-tile statistic partials
-void march(const RenderGrid& rg, const RenderCam& cam, const RenderViews& rv, cudaStream_t st);
-// 4. out[n][kRenderStats] = the fixed-order sums of the partials of each view
-void finish(int n, int tiles, const double* partials, double* out, cudaStream_t st);
+// Renders frames ids[0..n) (validated by the caller) of the W x H planes depth / lum with the poses Rt + 12 * id and the camera cam.  rg is
+// the grid without its voxel box, which is built here when the voxel set changed; then the march and the fixed-order finish of the
+// statistics, timed as phases "render", "render_bricks" and "render_samples".  Writes only rs and stats [n].
+void keyframes(RenderState& rs, Timing& tm, RenderGrid rg, const RenderCam& cam, const float* Rt, int n, const int32_t* ids, int W, int H,
+               const float* depth, const float* lum, int planes, bool photometric, I3DRenderStats* stats, cudaStream_t st);
 } // namespace render
 
 } // namespace i3d

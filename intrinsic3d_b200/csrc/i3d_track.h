@@ -1,13 +1,13 @@
 /*
- * i3d_track.h — host interface of the frame-to-model tracker (i3d_track.cuh, compiled in i3d_track.cu; DESIGN.md §6n).  The kernels live
- * in a device module of their own, so the engine's module holds exactly the kernels of the refinement path; the engine (i3d_engine.cu)
- * owns the buffers, renders the prediction with render::march and builds the depth pyramid with k_frames_depthdown, and calls these
- * wrappers on its stream.
+ * i3d_track.h — the frame-to-model tracker (i3d_track.cuh, DESIGN.md §6n), compiled with the renderer whose march it uses for the prediction
+ * in i3d_render.cu: the tracker's types and scratch, and the call the engine (i3d_engine.cu) makes with the grid it builds and its stream.
  */
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
+
+#include "i3d_render.h"
 
 namespace i3d
 {
@@ -48,21 +48,26 @@ struct TrackRows
     int tiles_x, tiles_y;
 };
 
+// Tracker scratch of an engine (grows only): the per-call state of n frames, and the chunk's prediction, pyramid, normal and mask planes.
+// The planes of the last chunk stay for i3d_debug_get_track_planes.
+struct TrackScratch
+{
+    Dev<float> rt; Dev<int32_t> ids; Dev<double> pose_in; Dev<TrackState> state;
+    Dev<double> sys, sums, partials, rd_partials, rd_sums; Dev<unsigned long long> counters;
+    Dev<float> pdepth, pnrm, depth[kTrackMaxLevels], nrm[kTrackMaxLevels]; Dev<uint8_t> mask;
+    int n = 0, levels = 0, last_m = 0, W[kTrackMaxLevels] = {}, H[kTrackMaxLevels] = {};
+};
+
 namespace track
 {
-// T_cw, its float copy and w2c from the input poses pose_in [n][12] (world -> camera); status and counts cleared
-void init(int n, const double* pose_in, TrackState* state, cudaStream_t st);
-// dst[k] = the stored depth plane ids[k] (W x H each)
-void gather(int n, int W, int H, const int32_t* ids, const float* src, float* dst, cudaStream_t st);
-// camera-frame normals of n depth planes by the computeNormals(K, depth, 0.3) rule of k_fuse_normals
-void normals(int n, const TrackCam& cam, const float* depth, float* nrm, cudaStream_t st);
-// per-tile partials of the chunk's systems at one level
-void rows(int n, const TrackRows& tr, cudaStream_t st);
-// sums[n][kTrackVals] = the fixed-order sums of each frame's partials
-void finish(int n, int tiles, const double* partials, double* sums, cudaStream_t st);
-// solve = 1: record, factor, solve and update every frame that is not frozen; 0: record the system only.  sys[n][kTrackVals] gets the
-// recorded sums; rows counts the recorded rows (integer atomics)
-void solve(int n, const double* sums, TrackState* state, double* sys, int min_corr, int solve, unsigned long long* rows, cudaStream_t st);
+// Tracks the stored frames ids[0..n) (validated by the caller; Wl / Hl: the pyramid sizes) of the store's depth planes store_depth
+// [store_F][dc] in passes of I3D_TRACK_CHUNK frames.  Per pass: the prediction (k_render_march at the input poses with the depth camera,
+// geometry only; rg is the grid without its voxel box, built in rs when the voxel set changed), the depth pyramid (frames_depthdown on
+// the gathered store depth) with its normals, then every Gauss-Newton iteration of every level, coarsest first, with no host
+// synchronisation; one read-back at the end.  Writes only ts, rs's voxel box, pose_out [n][12] and info [n].
+void sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderGrid rg, const I3DFusionCamera& dc, const float* store_depth, int store_F,
+                   int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out,
+                   I3DTrackInfo* info, cudaStream_t st);
 } // namespace track
 
 } // namespace i3d
