@@ -14,7 +14,7 @@
  * the 8 warps in order, then per frame a fixed-order pass over the tiles.  No atomics: a frame's score depends only on its own pixels.
  */
 #pragma once
-#include "i3d_kernels.cuh"
+#include "i3d_grid.cuh"
 
 namespace i3d
 {

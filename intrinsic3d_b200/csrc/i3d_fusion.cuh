@@ -19,8 +19,7 @@
  * (sort key fuse_order_key).
  */
 #pragma once
-#include "i3d_kernels.cuh"
-#include "i3d_gridops.cuh"
+#include "i3d_grid.cuh"
 
 namespace i3d
 {

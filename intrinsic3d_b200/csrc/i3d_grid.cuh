@@ -1,9 +1,10 @@
 /*
  * i3d_grid.cuh — what every device module of the engine shares about the grid: the neighbour-table slots, the block size, the device
  * hash (coordinates -> voxel index), the explicitly rounded float operations, the grid view with the per-voxel operators both modules
- * evaluate (surface normal, intensity), the normal rule of a depth plane (fusion and tracking) and the subvolume table of the lighting.
- * No kernels: i3d_kernels.cuh (the engine's module), i3d_mesh.cuh / i3d_vis.cuh (the surface extraction's module) and i3d_render.cuh /
- * i3d_track.cuh (the renderer's module) all include it.
+ * evaluate (surface normal, intensity), the voxel arrays a new voxel set is written into, the normal rule of a depth plane (fusion and
+ * tracking) and the subvolume table of the lighting.  No kernels: i3d_kernels.cuh (the engine's module), i3d_fusion.cuh (the fusion's),
+ * i3d_frames.cuh (the frames'), i3d_mesh.cuh / i3d_vis.cuh (the surface extraction's) and i3d_render.cuh / i3d_track.cuh (the
+ * renderer's) all include it.
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -67,6 +68,15 @@ struct GridView
     const int32_t* nbr;    // [12][n]
     const double* sh;      // [9][n]
     float voxel_size, truncation;
+};
+
+// the voxel arrays a new voxel set is written into (grid-level transitions, fusion)
+struct VoxelArrays
+{
+    int32_t* x; int32_t* y; int32_t* z;
+    double* sdf0; double* sdf; double* albedo;
+    float* weight;
+    uchar4* rgb;
 };
 
 // SDFOperators::computeSurfaceNormal (src/sdf/operators.cpp:58-77): float forward differences.

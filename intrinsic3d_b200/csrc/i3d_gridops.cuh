@@ -55,14 +55,6 @@ __global__ void k_shell_crossing(GridView g, const unsigned long long* __restric
     if (crossing) keep[v] = 2;               // distinct value: pass 2 must not feed back into other threads' pass-1 test
 }
 
-struct VoxelArrays
-{
-    int32_t* x; int32_t* y; int32_t* z;
-    double* sdf0; double* sdf; double* albedo;
-    float* weight;
-    uchar4* rgb;
-};
-
 __global__ void k_gather_voxels(int64_t m, const int32_t* __restrict__ list, GridView g, VoxelArrays out)
 {
     const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;

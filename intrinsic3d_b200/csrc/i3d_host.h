@@ -1,7 +1,6 @@
 /*
  * i3d_host.h — what every host translation unit of the engine shares: device buffers, the CUDA error check, launch sizes and the
- * phase timers, plus the launches of engine-module kernels that other modules need.  No kernels: it includes no .cuh that defines one,
- * so a module that includes it keeps its own device code.
+ * phase timers.  No kernels: it includes no .cuh that defines one, so a module that includes it keeps its own device code.
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -98,9 +97,5 @@ inline void collect_kernel_times(Timing& tm, cudaStream_t st)
     }
     tm.pending.clear(); tm.used = 0;
 }
-
-// ---- engine-module launches other modules use (defined in i3d_engine.cu) ----------------------
-// Pyramid::downsampleDepth (k_frames_depthdown) of n W x H depth planes into n (W / 2) x (H / 2) planes
-void frames_depthdown(int n, int W, int H, const float* src, float* dst, cudaStream_t st);
 
 } // namespace i3d

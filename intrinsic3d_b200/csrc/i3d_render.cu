@@ -8,6 +8,7 @@
 #include <cstring>
 
 #include "../../include/i3d_c_api.h"
+#include "i3d_frames.h"
 #include "i3d_render.cuh"
 #include "i3d_track.cuh"
 
@@ -188,7 +189,7 @@ void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderG
         {
             Timer t(tm, st, "track_pyramid");
             k_track_gather<<<dim3(blocks_for(img), m), kThreads, 0, st>>>(m, W, H, ids_d, store_depth, ts.depth[0].p);
-            for (int l = 1; l < L; ++l) frames_depthdown(m, Wl[l - 1], Hl[l - 1], ts.depth[l - 1].p, ts.depth[l].p, st);
+            for (int l = 1; l < L; ++l) frames::depthdown(m, Wl[l - 1], Hl[l - 1], ts.depth[l - 1].p, ts.depth[l].p, st);
             for (int l = 0; l < L; ++l)
                 k_track_normals<<<dim3(blocks_for(static_cast<size_t>(Wl[l]) * Hl[l]), m), kThreads, 0, st>>>(cam[l], ts.depth[l].p, ts.nrm[l].p);
         }

@@ -62,7 +62,7 @@ namespace track
 {
 // Tracks the stored frames ids[0..n) (validated by the caller; Wl / Hl: the pyramid sizes) of the store's depth planes store_depth
 // [store_F][dc] in passes of I3D_TRACK_CHUNK frames.  Per pass: the prediction (k_render_march at the input poses with the depth camera,
-// geometry only; rg is the grid without its voxel box, built in rs when the voxel set changed), the depth pyramid (frames_depthdown on
+// geometry only; rg is the grid without its voxel box, built in rs when the voxel set changed), the depth pyramid (frames::depthdown on
 // the gathered store depth) with its normals, then every Gauss-Newton iteration of every level, coarsest first, with no host
 // synchronisation; one read-back at the end.  Writes only ts, rs's voxel box, pose_out [n][12] and info [n].
 void sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderGrid rg, const I3DFusionCamera& dc, const float* store_depth, int store_F,
