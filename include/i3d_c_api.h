@@ -256,6 +256,34 @@ int         i3d_debug_get_track_system(I3DEngine* e, double* sums, double* pose_
 int         i3d_debug_get_track_planes(I3DEngine* e, int32_t level, float* depth, float* normal, float* pred_depth, float* pred_normal,
                                        uint8_t* mask, int32_t* frames);
 
+/* ---- tracking against the fusion in progress, and dense RGB-D odometry (DESIGN.md §6o) ---- */
+/* i3d_track_sensor_frames with the fusion volume in progress as the model: the prediction is marched through the fusion's own table (a
+ * cube is valid when its 8 corners exist with weight != 0; the value is the trilinear blend of the float Voxel::sdf) inside the box of the
+ * voxels with weight > 0, whose brick bitmap is rebuilt here.  Equal byte for byte to i3d_fusion_finish with correct_sdf_iterations = 0
+ * followed by i3d_track_sensor_frames(sdf_source 0).  params->sdf_source must be 0.  Writes only its own buffers, pose_out and info: the
+ * fusion volume, the grid, the renderer's state and the resident mesh and render are left as they were.  Fails, writing none of those,
+ * without a fusion in progress, when no voxel has weight > 0, and for every refusal of i3d_track_sensor_frames except "no grid".
+ * Device time as there, plus i3d_phase_ms("track_bricks") for the box and bitmap. */
+int         i3d_fusion_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params,
+                                           double* pose_out, I3DTrackInfo* info);
+/* Dense frame-to-model odometry: the stored frames ids[0..n) (repeats allowed), in list order, each tracked against the fusion in progress
+ * and then integrated into it.  Per frame:
+ *   1. the guess: pose_first (world -> camera [12]) for ids[0] when it is not NULL, which resets the motion state; otherwise the motion
+ *      state the fusion keeps (i3d_fusion_begin and every i3d_fusion_integrate* call clear it).  With two previous poses the guess is the
+ *      constant-velocity one, in double with camera -> world poses T: T(k) = T(k-1) . (T(k-2)^-1 . T(k-1)); with one, T(k-1).
+ *   2. no voxel with weight > 0: the frame is integrated at the guess, untracked (status I3D_TRACK_ANCHORED).
+ *   3. otherwise i3d_fusion_track_sensor_frames of that frame from the guess; at status I3D_TRACK_OK the frame is integrated at the
+ *      tracked pose (the float camera -> world and world -> camera of the double pose).  At any other status it is not integrated,
+ *      pose_out is the guess and the velocity becomes zero at the last integrated pose (the guess when the state has none).
+ * pose_out [n][12] world -> camera, info[n] may be NULL.  Calls chain: n frames in one call or in several with pose_first = NULL after
+ * the first give the same bytes.  Fails, leaving the fusion in progress and every state as it was, for the refusals of
+ * i3d_fusion_track_sensor_frames (repeated ids and n > 65535 allowed), a non-finite pose_first, and pose_first = NULL without a motion
+ * state.  A failure while fusing ends the fusion as i3d_fusion_integrate_sensor does.  Time: i3d_phase_ms("odometry") is the call's host
+ * wall time, of which the device times "odometry_predict" (box, bitmap, prediction) and "odometry_icp" (pyramid and ICP) and the fusion
+ * phases; i3d_phase_count("odometry_correspondences") = rows of every evaluated system. */
+int         i3d_fusion_track_and_integrate_sensor(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_first,
+                                                  const I3DTrackParams* params, double* pose_out, I3DTrackInfo* info);
+
 /* ---- keyframe selection and the RGB-D image pyramid: the inputs of fusion and refinement (DESIGN.md §6i) ---- */
 /* Frames scored per device pass by i3d_keyframe_scores: bounds its scratch memory (I3D_KEYFRAME_CHUNK * W * H * 3 bytes). */
 #define I3D_KEYFRAME_CHUNK 32

@@ -241,7 +241,8 @@ enum
     I3D_TRACK_OK = 0,                     /* every scheduled update applied */
     I3D_TRACK_FEW_CORRESPONDENCES = 1,    /* a system had fewer than min_correspondences rows: frozen there */
     I3D_TRACK_NOT_POSITIVE_DEFINITE = 2,  /* the Cholesky factorisation of a system failed: frozen there */
-    I3D_TRACK_NON_FINITE = 3              /* a system, its update or the updated pose was not finite: frozen there */
+    I3D_TRACK_NON_FINITE = 3,             /* a system, its update or the updated pose was not finite: frozen there */
+    I3D_TRACK_ANCHORED = 4                /* odometry: the volume had no integrated voxel; the frame was integrated at its guess untracked */
 };
 
 typedef struct I3DTrackParams

@@ -1788,30 +1788,23 @@ void i3d_default_track_params(I3DTrackParams* p)
     p->min_correspondences = 100;
 }
 
-int i3d_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params, double* pose_out,
-                            I3DTrackInfo* info)
+// The refusals of a call that tracks frames side by side: n <= 65535 and distinct ids
+static int check_track_batch(I3DEngine* e, const char* who, int32_t n, const int32_t* ids)
 {
-    static const char* who = "i3d_track_sensor_frames";
-    if (!e) return 1;
-    if (!params || !pose_in || !pose_out) return fail(e, "%s: params, pose_in and pose_out must not be NULL", who);
-    if (e->world > 1) return fail(e, "%s: tracking runs on one GPU (world = %d)", who, e->world);
-    if (e->n <= 0) return fail(e, "%s: no grid", who);
-    if (check_sensor_ids(e, who, n, ids)) return 1;
     if (n > kRenderMaxViews) return fail(e, "%s: %d frames exceed the %d of one call", who, n, kRenderMaxViews);
+    std::vector<uint8_t> seen(e->sensor.F, 0);
+    for (int32_t k = 0; k < n; ++k)
     {
-        std::vector<uint8_t> seen(e->sensor.F, 0);
-        for (int32_t k = 0; k < n; ++k)
-        {
-            if (seen[ids[k]]) return fail(e, "%s: frame id %d is repeated (entry %d); each frame has one pose", who, ids[k], k);
-            seen[ids[k]] = 1;
-        }
+        if (seen[ids[k]]) return fail(e, "%s: frame id %d is repeated (entry %d); each frame has one pose", who, ids[k], k);
+        seen[ids[k]] = 1;
     }
-    for (int64_t i = 0; i < 12 * static_cast<int64_t>(n); ++i)
-        if (!std::isfinite(pose_in[i])) return fail(e, "%s: the input pose of entry %d is not finite", who, static_cast<int>(i / 12));
-    const I3DTrackParams& P = *params;
-    if (check_sdf_source(e, who, P.sdf_source)) return 1;
+    return 0;
+}
+
+// The tracking parameters other than sdf_source; fills the pyramid sizes Wl / Hl
+static int check_track_params(I3DEngine* e, const char* who, const I3DTrackParams& P, int* Wl, int* Hl)
+{
     if (P.num_levels < 1 || P.num_levels > kTrackMaxLevels) return fail(e, "%s: num_levels must be in 1..%d, got %d", who, kTrackMaxLevels, P.num_levels);
-    int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
     Wl[0] = e->sensor.dcam.width; Hl[0] = e->sensor.dcam.height;
     for (int l = 1; l < P.num_levels; ++l)
     {
@@ -1824,11 +1817,88 @@ int i3d_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const d
     if (!(std::isfinite(P.max_distance) && P.max_distance > 0.0f)) return fail(e, "%s: max_distance must be finite and > 0, got %g", who, P.max_distance);
     if (!(P.min_normal_cos >= -1.0f && P.min_normal_cos <= 1.0f)) return fail(e, "%s: min_normal_cos must be in [-1, 1], got %g", who, P.min_normal_cos);
     if (P.min_correspondences < 6) return fail(e, "%s: min_correspondences must be >= 6, got %d", who, P.min_correspondences);
+    return 0;
+}
+
+static int check_finite_poses(I3DEngine* e, const char* who, int32_t n, const double* pose, const char* what)
+{
+    for (int64_t i = 0; i < 12 * static_cast<int64_t>(n); ++i)
+        if (!std::isfinite(pose[i])) return fail(e, "%s: %s of entry %d is not finite", who, what, static_cast<int>(i / 12));
+    return 0;
+}
+
+int i3d_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params, double* pose_out,
+                            I3DTrackInfo* info)
+{
+    static const char* who = "i3d_track_sensor_frames";
+    if (!e) return 1;
+    if (!params || !pose_in || !pose_out) return fail(e, "%s: params, pose_in and pose_out must not be NULL", who);
+    if (e->world > 1) return fail(e, "%s: tracking runs on one GPU (world = %d)", who, e->world);
+    if (e->n <= 0) return fail(e, "%s: no grid", who);
+    if (check_sensor_ids(e, who, n, ids)) return 1;
+    if (check_track_batch(e, who, n, ids)) return 1;
+    if (check_finite_poses(e, who, n, pose_in, "the input pose")) return 1;
+    const I3DTrackParams& P = *params;
+    if (check_sdf_source(e, who, P.sdf_source)) return 1;
+    int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
+    if (check_track_params(e, who, P, Wl, Hl)) return 1;
     return guarded(e, [&]() {
         track::sensor_frames(e->track, e->render, e->timing, render_grid(e, P.sdf_source, false), e->sensor.dcam, e->sensor.depth.p, e->sensor.F, n, ids, pose_in, P,
                              Wl, Hl, pose_out, info, e->stream);
         return 0;
     });
+}
+
+// The checks of the two calls that track against the fusion in progress, up to the poses
+static int check_fusion_track(I3DEngine* e, const char* who, int32_t n, const int32_t* ids, const I3DTrackParams* params, double* pose_out)
+{
+    if (!params || !pose_out) return fail(e, "%s: params and pose_out must not be NULL", who);
+    if (e->world > 1) return fail(e, "%s: tracking runs on one GPU (world = %d)", who, e->world);
+    if (!e->fusion.active) return fail(e, "%s: no fusion in progress (call i3d_fusion_begin first)", who);
+    return check_sensor_ids(e, who, n, ids);
+}
+
+int i3d_fusion_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params, double* pose_out,
+                                   I3DTrackInfo* info)
+{
+    static const char* who = "i3d_fusion_track_sensor_frames";
+    if (!e) return 1;
+    if (!pose_in) return fail(e, "%s: pose_in must not be NULL", who);
+    if (check_fusion_track(e, who, n, ids, params, pose_out)) return 1;
+    if (check_track_batch(e, who, n, ids)) return 1;
+    if (check_finite_poses(e, who, n, pose_in, "the input pose")) return 1;
+    const I3DTrackParams& P = *params;
+    if (P.sdf_source != 0) return fail(e, "%s: sdf_source must be 0 (the fusion volume holds one sdf), got %d", who, P.sdf_source);
+    int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
+    if (check_track_params(e, who, P, Wl, Hl)) return 1;
+    return guarded(e, [&]() {
+        if (track::fusion_frames(e->track, e->fusion, e->render.skip, e->timing, e->sensor, n, ids, pose_in, P, Wl, Hl, pose_out, info, e->stream))
+            return fail(e, "%s: the fusion volume has no voxel with weight > 0", who);
+        return 0;
+    });
+}
+
+int i3d_fusion_track_and_integrate_sensor(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_first, const I3DTrackParams* params,
+                                          double* pose_out, I3DTrackInfo* info)
+{
+    static const char* who = "i3d_fusion_track_and_integrate_sensor";
+    if (!e) return 1;
+    if (check_fusion_track(e, who, n, ids, params, pose_out)) return 1;
+    if (pose_first ? check_finite_poses(e, who, 1, pose_first, "pose_first") : 0) return 1;
+    if (!pose_first && e->fusion.motion == 0)
+        return fail(e, "%s: pose_first is NULL and the fusion has no motion state (a fusion begun or integrated since the last odometry call)", who);
+    const I3DTrackParams& P = *params;
+    if (P.sdf_source != 0) return fail(e, "%s: sdf_source must be 0 (the fusion volume holds one sdf), got %d", who, P.sdf_source);
+    int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
+    if (check_track_params(e, who, P, Wl, Hl)) return 1;
+    const int rc = guarded(e, [&]() {
+        std::string err;
+        if (track::odometry(e->track, e->fusion, e->render.skip, e->timing, e->sensor, n, ids, pose_first, P, Wl, Hl, pose_out, info, err, e->stream))
+            return fail(e, "%s: %s", who, err.c_str());
+        return 0;
+    });
+    if (rc != 0) e->fusion.active = false;
+    return rc;
 }
 
 int i3d_debug_get_track_system(I3DEngine* e, double* sums, double* pose_cam_to_world)

@@ -123,6 +123,7 @@ void fusion::begin(FusionState& fs, Timing& tm, const I3DFusionParams& P, cudaSt
     while (cap < static_cast<uint64_t>(P.initial_capacity)) cap <<= 1;
     fuse_reset_table(fs, cap, st);
     fs.n = 0;
+    fs.motion = 0;
     begin_timing(tm, {"fusion_prep", "fusion_alloc", "fusion_integrate", "fusion_correct", "fusion_finish", "fusion_growths", "fusion_sweeps"});
 }
 
@@ -150,6 +151,7 @@ int fusion::integrate(FusionState& fs, Timing& tm, int n, const I3DFusionCamera&
     const FuseCam dc{depth_cam.width, depth_cam.height, depth_cam.fx, depth_cam.fy, depth_cam.cx, depth_cam.cy};
     const FuseCam cc{color_cam.width, color_cam.height, color_cam.fx, color_cam.fy, color_cam.cx, color_cam.cy};
     const FuseConst c = fuse_const(P);
+    fs.motion = 0;
     begin_timing(tm, {});                        // the fusion phases were reset by begin
     for (int f = 0; f < n; ++f)
     {
@@ -246,6 +248,11 @@ int fusion::sort(FusionState& fs, bool valid_only, cudaStream_t st)
 void fusion::convert(const FusionState& fs, int m, const VoxelArrays& out, cudaStream_t st)
 {
     k_fuse_convert<<<blocks_for(static_cast<size_t>(m)), kThreads, 0, st>>>(m, fs.si.p, fuse_volume(fs), out);
+}
+
+FuseView fusion::view(const FusionState& fs)
+{
+    return FuseView{fs.keys.p, fs.vals.p, fs.cap - 1, fs.x.p, fs.y.p, fs.z.p, fs.sdf.p, fs.w.p, fs.n};
 }
 
 void fusion::download(FusionState& fs, int32_t* xyz, float* sdf, float* weight, uint8_t* rgb, cudaStream_t st)

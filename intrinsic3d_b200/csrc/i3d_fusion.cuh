@@ -19,14 +19,11 @@
  * (sort key fuse_order_key).
  */
 #pragma once
-#include "i3d_grid.cuh"
+#include "i3d_fusion_view.cuh"
 
 namespace i3d
 {
 
-// hash value of the fusion table: voxel index in the low 31 bits, bit 31 = "the 3x3x3 block around this voxel is complete"
-constexpr unsigned kFuseBlockBit = 0x80000000u;
-constexpr unsigned kFuseIndexMask = 0x7FFFFFFFu;
 constexpr int kFuseMaxProbe = 128;            // a longer linear probe means the table is too full: grow it
 constexpr int kFuseCoordLimit = (1 << 20) - 2; // centre voxels beyond this would put a block neighbour outside pack_key's range
 
@@ -260,19 +257,6 @@ __global__ void k_fuse_rehash(uint64_t old_cap, const unsigned long long* __rest
     uint64_t slot = mix64(key) & mask;
     while (atomicCAS(&keys[slot], kEmptyKey, key) != kEmptyKey) slot = (slot + 1) & mask;
     vals[slot] = ovals[s];
-}
-
-__device__ __forceinline__ int32_t fuse_find(const unsigned long long* __restrict__ keys, const unsigned* __restrict__ vals, uint64_t mask, int x, int y, int z)
-{
-    const unsigned long long key = pack_key(x, y, z);
-    uint64_t slot = mix64(key) & mask;
-    while (true)
-    {
-        const unsigned long long k = keys[slot];
-        if (k == key) return static_cast<int32_t>(vals[slot] & kFuseIndexMask);
-        if (k == kEmptyKey) return -1;
-        slot = (slot + 1) & mask;
-    }
 }
 
 // One Jacobi sweep of SDFAlgorithms::correctSDF (algorithms.cpp:260-337): every valid voxel compares its 26 neighbours in (k, j, i)

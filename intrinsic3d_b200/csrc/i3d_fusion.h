@@ -10,6 +10,7 @@
 #include <string>
 
 #include "../../include/i3d_types.h"
+#include "i3d_fusion_view.cuh"
 #include "i3d_grid.cuh"
 #include "i3d_host.h"
 
@@ -28,6 +29,10 @@ struct FusionState
     Dev<int> ctl;                      // [0] allocated voxels, [1] alloc status, [2] correctSDF "changed", [3] valid voxels
     Dev<float> depth_in, depth, nrm; Dev<uint8_t> bgr;      // host frames of i3d_fusion_integrate; the eroded depth and its normals
     Dev<unsigned long long> sk, sk2; Dev<int32_t> si, si2; Dev<uint8_t> cub;
+    // the odometry's motion state (track::odometry): the last `motion` (0..2) integrated camera -> world poses, R row-major | t in
+    // double, newest in motion_T[1]; begin and every integrate clear it
+    int motion = 0;
+    double motion_T[2][12] = {};
 };
 
 namespace fusion
@@ -50,6 +55,8 @@ void correct(FusionState& fs, Timing& tm, cudaStream_t st);
 int sort(FusionState& fs, bool valid_only, cudaStream_t st);
 // SDFAlgorithms::convert of the first m voxels of the order into out
 void convert(const FusionState& fs, int m, const VoxelArrays& out, cudaStream_t st);
+// The volume in progress, read-only, for a reader outside this module (i3d_fusion_view.cuh)
+FuseView view(const FusionState& fs);
 // The volume in canonical order, interleaved, into host buffers (each may be nullptr)
 void download(FusionState& fs, int32_t* xyz, float* sdf, float* weight, uint8_t* rgb, cudaStream_t st);
 } // namespace fusion

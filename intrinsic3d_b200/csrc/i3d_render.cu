@@ -3,9 +3,11 @@
  * for its prediction: their kernels and the host code that sequences them (i3d_render.h, i3d_track.h).  Keeping them out of i3d_engine.cu
  * leaves the engine's device module as it is.
  */
+#include <chrono>
 #include <climits>
 #include <cmath>
 #include <cstring>
+#include <optional>
 
 #include "../../include/i3d_c_api.h"
 #include "i3d_frames.h"
@@ -127,15 +129,25 @@ void render::keyframes(RenderState& rs, Timing& tm, RenderGrid rg, const RenderC
     rs.have_render = true; rs.n = n; rs.planes = planes;
 }
 
-void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderGrid rg, const I3DFusionCamera& dc, const float* store_depth,
-                          int store_F, int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl,
-                          double* pose_out, I3DTrackInfo* info, cudaStream_t st)
+namespace
+{
+// The phase names of one tracking pass (whole: nullptr = not timed as a whole)
+struct TrackPhases { const char* whole; const char* predict; const char* pyramid; const char* icp; const char* correspondences; };
+constexpr TrackPhases kTrackPhases{"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences"};
+constexpr TrackPhases kOdometryPhases{nullptr, "odometry_predict", "odometry_icp", "odometry_icp", "odometry_correspondences"};
+
+// The tracker's passes over ids[0..n), shared by the grid and the fusion volume: prepare() (false: stop, nothing tracked) runs once
+// after the uploads, predict(cam, rv) marches a chunk's prediction into rv.  pose_cw_out [n][12] (may be nullptr): the tracked
+// camera -> world poses.  Returns false when prepare() stopped the call.
+template <class Prepare, class Predict>
+bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&& prepare, Predict&& predict, const I3DFusionCamera& dc,
+                  const float* store_depth, int store_F, int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl,
+                  const int* Hl, double* pose_out, double* pose_cw_out, I3DTrackInfo* info, cudaStream_t st)
 {
     const int L = P.num_levels, W = dc.width, H = dc.height, C = std::min<int>(n, I3D_TRACK_CHUNK);
     const size_t img = static_cast<size_t>(W) * H;
     const int tiles_x = (W + kRenderTile - 1) / kRenderTile, tiles_y = (H + kRenderTile - 1) / kRenderTile;
     static_assert(kRenderTile == kTrackTile, "the prediction and the rows share the level-0 tile grid");
-    begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences"});
     ts.n = 0;
     ts.ids.ensure(n); ts.pose_in.ensure(12 * static_cast<size_t>(n)); ts.state.ensure(n);
     ts.sys.ensure(static_cast<size_t>(n) * kTrackVals); ts.rd_sums.ensure(static_cast<size_t>(n) * kRenderStats);
@@ -165,8 +177,9 @@ void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderG
         cam[l] = TrackCam{Wl[l], Hl[l], static_cast<float>(dc.fx * s), static_cast<float>(dc.fy * s), static_cast<float>(dc.cx * s),
                           static_cast<float>(dc.cy * s)};
     }
-    Timer whole(tm, st, "track");
-    add_voxel_box(rs, tm, rg, st);
+    std::optional<Timer> whole;
+    if (ph.whole) whole.emplace(tm, st, ph.whole);
+    if (!prepare()) return false;
     RenderCam rcam{};
     rcam.fx = dc.fx; rcam.fy = dc.fy; rcam.cx = dc.cx; rcam.cy = dc.cy; rcam.dist_zero = 1;
     k_track_init<<<blocks_for(n, 64), 64, 0, st>>>(n, ts.pose_in.p, ts.state.p);
@@ -177,24 +190,24 @@ void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderG
         m = std::min(C, n - c0);
         const int32_t* ids_d = ts.ids.p + c0;
         {
-            Timer t(tm, st, "track_predict");
+            Timer t(tm, st, ph.predict);
             RenderViews rv{};
             rv.n = m; rv.W = W; rv.H = H; rv.tiles_x = tiles_x; rv.tiles_y = tiles_y;
             rv.ids = ids_d; rv.Rt = ts.rt.p; rv.depth = store_depth; rv.lum = nullptr;
             rv.out_depth = ts.pdepth.p; rv.out_normal = ts.pnrm.p;
             rv.partials = ts.rd_partials.p; rv.samples = ts.counters.p + 1; rv.photometric = 0;
-            march(rg, rcam, rv, st);
+            predict(rcam, rv);
             tile_sums<kRenderStats>(m, tiles_x * tiles_y, ts.rd_partials.p, ts.rd_sums.p + static_cast<size_t>(c0) * kRenderStats, st);
         }
         {
-            Timer t(tm, st, "track_pyramid");
+            Timer t(tm, st, ph.pyramid);
             k_track_gather<<<dim3(blocks_for(img), m), kThreads, 0, st>>>(m, W, H, ids_d, store_depth, ts.depth[0].p);
             for (int l = 1; l < L; ++l) frames::depthdown(m, Wl[l - 1], Hl[l - 1], ts.depth[l - 1].p, ts.depth[l].p, st);
             for (int l = 0; l < L; ++l)
                 k_track_normals<<<dim3(blocks_for(static_cast<size_t>(Wl[l]) * Hl[l]), m), kThreads, 0, st>>>(cam[l], ts.depth[l].p, ts.nrm[l].p);
         }
         {
-            Timer t(tm, st, "track_icp");
+            Timer t(tm, st, ph.icp);
             CK(cudaMemsetAsync(ts.mask.p, 0, m * img, st));
             TrackRows tr{};
             tr.pcam = cam[0]; tr.pdepth = ts.pdepth.p; tr.pnrm = ts.pnrm.p; tr.ids = ids_d; tr.rt_in = ts.rt.p;
@@ -222,13 +235,14 @@ void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderG
     CK(cudaMemcpyAsync(hs.data(), ts.state.p, n * sizeof(TrackState), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(rs_sums.data(), ts.rd_sums.p, rs_sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(counters, ts.counters.p, sizeof(counters), cudaMemcpyDeviceToHost, st));
-    whole.stop();
+    if (whole) whole->stop();
     collect_kernel_times(tm, st);
     CK(cudaGetLastError());
-    tm.phases["track_correspondences"].count = static_cast<int64_t>(counters[0]);
+    tm.phases[ph.correspondences].count += static_cast<int64_t>(counters[0]);
     for (int k = 0; k < n; ++k)
     {
         std::memcpy(pose_out + 12 * static_cast<size_t>(k), hs[k].w2c, 12 * sizeof(double));
+        if (pose_cw_out) std::memcpy(pose_cw_out + 12 * static_cast<size_t>(k), hs[k].T, 12 * sizeof(double));
         if (!info) continue;
         I3DTrackInfo r{};
         r.status = hs[k].status; r.iterations = hs[k].iterations; r.correspondences = hs[k].correspondences;
@@ -238,6 +252,165 @@ void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderG
     }
     ts.n = n; ts.levels = L; ts.last_m = m;
     for (int l = 0; l < L; ++l) { ts.W[l] = Wl[l]; ts.H[l] = Hl[l]; }
+    return true;
+}
+
+
+// Completes lg from the fusion volume fv: the box of its voxels with weight > 0 and, when skip and it fits under kRenderBrickCap, their
+// brick bitmap; timed as `phase`.  The box read synchronises.  Returns false when no voxel has weight > 0.
+bool live_box(TrackScratch& ts, Timing& tm, const char* phase, const FuseView& fv, float voxel_size, bool skip, LiveGrid& lg, cudaStream_t st)
+{
+    Timer t(tm, st, phase);
+    int box[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
+    ts.live_box.ensure(6);
+    CK(cudaMemcpyAsync(ts.live_box.p, box, sizeof(box), cudaMemcpyHostToDevice, st));
+    if (fv.n > 0) k_live_bounds<<<blocks_for(fv.n), kThreads, 0, st>>>(fv.n, fv.x, fv.y, fv.z, fv.weight, ts.live_box.p);
+    CK(cudaMemcpyAsync(box, ts.live_box.p, sizeof(box), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (box[0] > box[3]) return false;
+    lg.v = fv; lg.voxel_size = voxel_size; lg.bricks = nullptr;
+    int64_t bits = 1;
+    for (int d = 0; d < 3; ++d)
+    {
+        lg.lo[d] = static_cast<float>(box[d]) * voxel_size;
+        lg.hi[d] = static_cast<float>(box[3 + d]) * voxel_size;
+        lg.blo[d] = box[d];
+        lg.bdim[d] = ((box[3 + d] - box[d]) >> 3) + 1;
+        bits *= lg.bdim[d];
+    }
+    if (skip && bits <= kRenderBrickCap)
+    {
+        const size_t words = static_cast<size_t>((bits + 31) >> 5);
+        ts.live_bits.ensure(words);
+        CK(cudaMemsetAsync(ts.live_bits.p, 0, words * sizeof(uint32_t), st));
+        const BrickBox bb{{lg.blo[0], lg.blo[1], lg.blo[2]}, {lg.bdim[0], lg.bdim[1], lg.bdim[2]}};
+        k_live_bricks<<<blocks_for(fv.n), kThreads, 0, st>>>(fv.n, fv.x, fv.y, fv.z, fv.weight, bb, ts.live_bits.p);
+        lg.bricks = ts.live_bits.p;
+    }
+    return true;
+}
+
+void march_live(const LiveGrid& lg, const RenderCam& cam, const RenderViews& rv, cudaStream_t st)
+{
+    k_render_march_live<<<dim3(rv.tiles_x, rv.tiles_y, rv.n), dim3(kRenderTile, kRenderTile), 0, st>>>(lg, cam, rv);
+}
+
+// Poses R row-major | t in double, every sum left to right as tests/test_odometry.py restates them.  The inverse is tr_inverse's.
+void pose_inverse(const double* T, double* out)
+{
+    for (int i = 0; i < 3; ++i)
+    {
+        for (int j = 0; j < 3; ++j) out[3 * i + j] = T[3 * j + i];
+        out[9 + i] = -((T[i] * T[9] + T[3 + i] * T[10]) + T[6 + i] * T[11]);
+    }
+}
+
+// A . B = [R_A R_B | R_A t_B + t_A]
+void pose_compose(const double* A, const double* B, double* out)
+{
+    for (int a = 0; a < 3; ++a)
+    {
+        for (int c = 0; c < 3; ++c) out[3 * a + c] = (A[3 * a] * B[c] + A[3 * a + 1] * B[3 + c]) + A[3 * a + 2] * B[6 + c];
+        out[9 + a] = ((A[3 * a] * B[9] + A[3 * a + 1] * B[10]) + A[3 * a + 2] * B[11]) + A[9 + a];
+    }
+}
+} // namespace
+
+void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderGrid rg, const I3DFusionCamera& dc, const float* store_depth,
+                          int store_F, int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl,
+                          double* pose_out, I3DTrackInfo* info, cudaStream_t st)
+{
+    begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences"});
+    track_passes(
+        ts, tm, kTrackPhases, [&]() { add_voxel_box(rs, tm, rg, st); return true; },
+        [&](const RenderCam& cam, const RenderViews& rv) { march(rg, cam, rv, st); }, dc, store_depth, store_F, n, ids, pose_in, P, Wl, Hl,
+        pose_out, nullptr, info, st);
+}
+
+int track::fusion_frames(TrackScratch& ts, const FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids,
+                         const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, cudaStream_t st)
+{
+    begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences", "track_bricks"});
+    LiveGrid lg{};
+    const bool ok = track_passes(
+        ts, tm, kTrackPhases, [&]() { return live_box(ts, tm, "track_bricks", fusion::view(fs), fs.p.voxel_size, skip, lg, st); },
+        [&](const RenderCam& cam, const RenderViews& rv) { march_live(lg, cam, rv, st); }, ss.dcam, ss.depth.p, ss.F, n, ids, pose_in, P, Wl, Hl,
+        pose_out, nullptr, info, st);
+    if (!ok) collect_kernel_times(tm, st);
+    return ok ? 0 : 1;
+}
+
+int track::odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids, const double* pose_first,
+                    const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, std::string& error, cudaStream_t st)
+{
+    const auto t0 = std::chrono::steady_clock::now();
+    for (const char* nm : {"odometry", "odometry_predict", "odometry_icp", "odometry_correspondences"}) tm.phases.erase(nm);
+    // the motion state, kept here while fusion::integrate (which clears fs's) runs
+    int motion = pose_first ? 0 : fs.motion;
+    double prev[12], last[12];
+    std::memcpy(prev, fs.motion_T[0], sizeof(prev)); std::memcpy(last, fs.motion_T[1], sizeof(last));
+    for (int k = 0; k < n; ++k)
+    {
+        // the guess: T_cw(k) = T_cw(k-1) . (T_cw(k-2)^-1 . T_cw(k-1)), or T_cw(k-1) with one previous pose
+        double T[12], W[12];
+        if (k == 0 && pose_first)
+        {
+            std::memcpy(W, pose_first, sizeof(W));
+            pose_inverse(W, T);
+        }
+        else
+        {
+            if (motion == 1) std::memcpy(T, last, sizeof(T));
+            else
+            {
+                double ip[12], d[12];
+                pose_inverse(prev, ip);
+                pose_compose(ip, last, d);
+                pose_compose(last, d, T);
+            }
+            pose_inverse(T, W);
+        }
+        begin_timing(tm, {});
+        I3DTrackInfo r{};
+        double Tt[12], Wt[12];
+        const double* Ti = nullptr;
+        const double* Wi = nullptr;
+        LiveGrid lg{};
+        if (!live_box(ts, tm, "odometry_predict", fusion::view(fs), fs.p.voxel_size, skip, lg, st))
+        {
+            collect_kernel_times(tm, st);
+            r.status = I3D_TRACK_ANCHORED;
+            Ti = T; Wi = W;
+        }
+        else
+        {
+            track_passes(
+                ts, tm, kOdometryPhases, []() { return true; }, [&](const RenderCam& cam, const RenderViews& rv) { march_live(lg, cam, rv, st); },
+                ss.dcam, ss.depth.p, ss.F, 1, ids + k, W, P, Wl, Hl, Wt, Tt, &r, st);
+            if (r.status == I3D_TRACK_OK) { Ti = Tt; Wi = Wt; }
+        }
+        if (Ti)
+        {
+            float c2w[12], w2c[12];
+            for (int i = 0; i < 12; ++i) { c2w[i] = static_cast<float>(Ti[i]); w2c[i] = static_cast<float>(Wi[i]); }
+            if (fusion::integrate(fs, tm, 1, ss.dcam, ss.depth.p, ss.ccam, ss.bgr.p, ids + k, c2w, w2c, error, st)) return 1;
+            std::memcpy(prev, last, sizeof(prev)); std::memcpy(last, Ti, sizeof(last));
+            motion = std::min(motion + 1, 2);
+        }
+        else
+        {
+            // not integrated: the velocity is zero from the last integrated pose (the guess when this state has none)
+            if (motion == 0) std::memcpy(last, T, sizeof(last));
+            motion = 1;
+        }
+        fs.motion = motion;
+        std::memcpy(fs.motion_T[0], prev, sizeof(prev)); std::memcpy(fs.motion_T[1], last, sizeof(last));
+        std::memcpy(pose_out + 12 * static_cast<size_t>(k), Wi ? Wi : W, 12 * sizeof(double));
+        if (info) info[k] = r;
+    }
+    tm.phases["odometry"].ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    tm.phases["odometry"].count += 1;
+    return 0;
 }
 
 } // namespace i3d

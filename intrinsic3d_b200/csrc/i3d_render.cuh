@@ -6,6 +6,8 @@
  *   k_render_bounds   the bounding box of the voxel coordinates (integer atomics)
  *   k_render_bricks   the occupancy bitmap of 8^3 bricks over that box (integer atomics)
  *   k_render_march    one thread per pixel, 16 x 16 tiles, views in gridDim.z: planes + per-tile statistic partials
+ *   k_live_bounds / k_live_bricks / k_render_march_live   the same three over the fusion volume in progress (DESIGN.md §6o): the voxels
+ *                     with weight > 0, and the cube rule by one fusion-hash probe per corner (the volume has no neighbour table)
  *   k_tile_sums       the fixed-order sum of a view's partials (also the tracker's)
  *
  * Compiled with the tracker in i3d_render.cu, which launches them (render::keyframes, i3d_render.h).  Every float
@@ -68,12 +70,53 @@ __device__ __forceinline__ int rd_cube(const RenderGrid& rg, const float p[3], R
     return (q.c[7] >= 0 && g.weight[q.c[7]] != 0.0f) ? RD_VALID : RD_INVALID;
 }
 
+// The same rule on the fusion volume in progress, which has no neighbour table: one probe of its hash per corner.  The base and brick
+// steps are rd_cube's above, written out again: sharing them changes that function's register allocation in k_render_march.
+__device__ __forceinline__ int rd_cube(const LiveGrid& lg, const float p[3], RdCube& q)
+{
+    const float vs = lg.voxel_size;
+#pragma unroll
+    for (int d = 0; d < 3; ++d)
+    {
+        const float gd = FD(p[d], vs);
+        const float fl = floorf(gd);
+        q.base[d] = __float2int_rz(fl);
+        q.f[d] = FS(gd, fl);
+    }
+    if (lg.bricks)
+    {
+        int b[3];
+#pragma unroll
+        for (int d = 0; d < 3; ++d)
+        {
+            b[d] = q.base[d] - lg.blo[d];
+            if (b[d] < 0) return RD_INVALID;
+            b[d] >>= 3;
+            if (b[d] >= lg.bdim[d]) return RD_INVALID;
+        }
+        const int64_t idx = (static_cast<int64_t>(b[2]) * lg.bdim[1] + b[1]) * lg.bdim[0] + b[0];
+        if (!((lg.bricks[idx >> 5] >> (idx & 31)) & 1u)) return RD_EMPTY_BRICK;
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+    {
+        const int32_t c = fuse_find(lg.v.keys, lg.v.vals, lg.v.mask, q.base[0] + (i & 1), q.base[1] + ((i >> 1) & 1), q.base[2] + ((i >> 2) & 1));
+        if (c < 0 || lg.v.weight[c] == 0.0f) return RD_INVALID;
+        q.c[i] = c;
+    }
+    return RD_VALID;
+}
+
+__device__ __forceinline__ float rd_float(double a) { return __double2float_rn(a); }
+__device__ __forceinline__ float rd_float(float a) { return a; }
+
 // Trilinear blend of float(a[c]) over the cube: along x, then y, then z.  s_out (optional) gets the 8 corner values.
-__device__ __forceinline__ float rd_trilinear(const double* __restrict__ a, const RdCube& q, float (*s_out)[8] = nullptr)
+template <class T>
+__device__ __forceinline__ float rd_trilinear(const T* __restrict__ a, const RdCube& q, float (*s_out)[8] = nullptr)
 {
     float s[8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) s[i] = __double2float_rn(a[q.c[i]]);
+    for (int i = 0; i < 8; ++i) s[i] = rd_float(a[q.c[i]]);
     if (s_out)
     {
 #pragma unroll
@@ -124,6 +167,16 @@ __device__ __forceinline__ bool rd_sh(const RenderGrid& rg, const RdCube& q, flo
     return true;
 }
 
+// What the march reads besides the cube rule: the voxel size, the surface's sdf, the albedo at a hit and the per-voxel SH.  The volume in
+// progress has only a float sdf.
+__device__ __forceinline__ float rd_voxel_size(const RenderGrid& rg) { return rg.g.voxel_size; }
+__device__ __forceinline__ float rd_voxel_size(const LiveGrid& lg) { return lg.voxel_size; }
+__device__ __forceinline__ const double* rd_sdf(const RenderGrid& rg) { return rg.g.sdf; }
+__device__ __forceinline__ const float* rd_sdf(const LiveGrid& lg) { return lg.v.sdf; }
+__device__ __forceinline__ float rd_albedo(const RenderGrid& rg, const RdCube& q) { return rd_trilinear(rg.g.albedo, q); }
+__device__ __forceinline__ float rd_albedo(const LiveGrid&, const RdCube&) { return 0.0f; }
+__device__ __forceinline__ bool rd_sh(const LiveGrid&, const RdCube&, float*) { return false; }
+
 // The point at ray parameter s
 __device__ __forceinline__ void rd_point(const float o[3], const float dn[3], float s, float p[3])
 {
@@ -134,8 +187,9 @@ __device__ __forceinline__ void rd_point(const float o[3], const float dn[3], fl
 // One thread per pixel (u, v) of view blockIdx.z.  Ray: the pixel centre through the inverse of observation_weight's projection, in
 // world coordinates; samples s_k = s0 + k * voxel_size / 2 from where the ray enters the voxel box (clipped to s >= 0) to where it
 // leaves it; the hit is the first pair of consecutive valid samples going from > 0 to <= 0 whose linearly interpolated crossing lies in a
-// valid cube.
-__global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march(RenderGrid rg, RenderCam cam, RenderViews rv)
+// valid cube.  G: the installed grid (RenderGrid) or the fusion volume in progress (LiveGrid).
+template <class G>
+__device__ __forceinline__ void rd_march(G rg, RenderCam cam, RenderViews rv)
 {
     __shared__ double red[kRenderStats][kRenderTile * kRenderTile];
     const int u = blockIdx.x * kRenderTile + threadIdx.x, v = blockIdx.y * kRenderTile + threadIdx.y, view = blockIdx.z;
@@ -194,8 +248,8 @@ __global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march(Rend
         bool finite = isfinite(s1);
 #pragma unroll
         for (int d = 0; d < 3; ++d) finite = finite && isfinite(o[d]) && isfinite(dn[d]);
-        const float h = FM(rg.g.voxel_size, 0.5f);
-        const double* sdf = rg.g.sdf;
+        const float h = FM(rd_voxel_size(rg), 0.5f);
+        const auto* sdf = rd_sdf(rg);
         RdCube q;
         float s_hit = 0.0f;
         bool hit = false;
@@ -220,7 +274,7 @@ __global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march(Rend
                     {
                         if (dn[d] == 0.0f) continue;
                         const int b0 = rg.blo[d] + ((q.base[d] - rg.blo[d]) & ~7);
-                        const float face = FM(__int2float_rn(dn[d] > 0.0f ? b0 + 8 : b0), rg.g.voxel_size);
+                        const float face = FM(__int2float_rn(dn[d] > 0.0f ? b0 + 8 : b0), rd_voxel_size(rg));
                         te = fminf(te, FD(FS(face, o[d]), dn[d]));
                     }
                     const float kf = floorf(FD(FS(te, s0), h));
@@ -256,7 +310,7 @@ __global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march(Rend
             float s8[8];
             rd_trilinear(sdf, q, &s8);
             rd_normal(s8, q.f, nrm);
-            alb = rd_trilinear(rg.g.albedo, q);
+            alb = rd_albedo(rg, q);
             if (rv.photometric)
             {
                 float sh[9];
@@ -312,6 +366,11 @@ __global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march(Rend
     if ((tid & 31) == 0 && nsamp) atomicAdd(rv.samples, static_cast<unsigned long long>(nsamp));
 }
 
+__global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march(RenderGrid rg, RenderCam cam, RenderViews rv) { rd_march(rg, cam, rv); }
+
+// The march of the fusion volume in progress (geometry only: albedo 0, no shading), for the tracker's prediction
+__global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march_live(LiveGrid lg, RenderCam cam, RenderViews rv) { rd_march(lg, cam, rv); }
+
 // One thread per (view, value) of V per-tile values: the view's tiles summed in order.  V = kRenderStats (k_render_march's statistics),
 // kTrackVals (k_track_rows' systems).
 template <int V>
@@ -326,13 +385,14 @@ __global__ void k_tile_sums(int n, int tiles, const double* __restrict__ partial
     out[i] = s;
 }
 
-// Min / max of the coordinates per warp (__reduce_*_sync), then per block in shared memory, then one integer atomic per block and value
-__global__ void __launch_bounds__(kThreads) k_render_bounds(int64_t n, const int32_t* __restrict__ x, const int32_t* __restrict__ y,
-                                                            const int32_t* __restrict__ z, int* box)
+// Min / max of the coordinates per warp (__reduce_*_sync), then per block in shared memory, then one integer atomic per block and value.
+// w: only the voxels with weight > 0 count (nullptr: all).
+__device__ __forceinline__ void rd_bounds(int64_t n, const int32_t* __restrict__ x, const int32_t* __restrict__ y, const int32_t* __restrict__ z,
+                                          const float* __restrict__ w, int* box)
 {
     __shared__ int part[6][kThreads / 32];
     const int64_t v = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-    const bool in = v < n;
+    const bool in = v < n && (!w || w[v] > 0.0f);
     int c[6];
     c[0] = in ? x[v] : INT_MAX; c[1] = in ? y[v] : INT_MAX; c[2] = in ? z[v] : INT_MAX;
     c[3] = in ? c[0] : INT_MIN; c[4] = in ? c[1] : INT_MIN; c[5] = in ? c[2] : INT_MIN;
@@ -353,16 +413,43 @@ __global__ void __launch_bounds__(kThreads) k_render_bounds(int64_t n, const int
     }
 }
 
+__global__ void __launch_bounds__(kThreads) k_render_bounds(int64_t n, const int32_t* __restrict__ x, const int32_t* __restrict__ y,
+                                                            const int32_t* __restrict__ z, int* box)
+{
+    rd_bounds(n, x, y, z, nullptr, box);
+}
+
+// The box of the fusion volume's voxels with weight > 0
+__global__ void __launch_bounds__(kThreads) k_live_bounds(int64_t n, const int32_t* __restrict__ x, const int32_t* __restrict__ y,
+                                                          const int32_t* __restrict__ z, const float* __restrict__ w, int* box)
+{
+    rd_bounds(n, x, y, z, w, box);
+}
+
 struct BrickBox { int lo[3], dim[3]; };
+
+// w: only the voxels with weight > 0 set their brick (nullptr: all)
+__device__ __forceinline__ void rd_bricks(int64_t n, const int32_t* __restrict__ x, const int32_t* __restrict__ y, const int32_t* __restrict__ z,
+                                          const float* __restrict__ w, const BrickBox& bb, uint32_t* __restrict__ bits)
+{
+    const int64_t v = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    if (v >= n) return;
+    if (w && !(w[v] > 0.0f)) return;
+    const int bx = (x[v] - bb.lo[0]) >> 3, by = (y[v] - bb.lo[1]) >> 3, bz = (z[v] - bb.lo[2]) >> 3;
+    const int64_t idx = (static_cast<int64_t>(bz) * bb.dim[1] + by) * bb.dim[0] + bx;
+    atomicOr(bits + (idx >> 5), 1u << (idx & 31));
+}
 
 __global__ void k_render_bricks(int64_t n, const int32_t* __restrict__ x, const int32_t* __restrict__ y, const int32_t* __restrict__ z, BrickBox bb,
                                 uint32_t* __restrict__ bits)
 {
-    const int64_t v = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-    if (v >= n) return;
-    const int bx = (x[v] - bb.lo[0]) >> 3, by = (y[v] - bb.lo[1]) >> 3, bz = (z[v] - bb.lo[2]) >> 3;
-    const int64_t idx = (static_cast<int64_t>(bz) * bb.dim[1] + by) * bb.dim[0] + bx;
-    atomicOr(bits + (idx >> 5), 1u << (idx & 31));
+    rd_bricks(n, x, y, z, nullptr, bb, bits);
+}
+
+__global__ void k_live_bricks(int64_t n, const int32_t* __restrict__ x, const int32_t* __restrict__ y, const int32_t* __restrict__ z,
+                              const float* __restrict__ w, BrickBox bb, uint32_t* __restrict__ bits)
+{
+    rd_bricks(n, x, y, z, w, bb, bits);
 }
 
 } // namespace i3d

@@ -9,6 +9,7 @@
 #include <stdint.h>
 
 #include "../../include/i3d_types.h"
+#include "i3d_fusion_view.cuh"
 #include "i3d_grid.cuh"
 #include "i3d_host.h"
 
@@ -34,6 +35,17 @@ struct RenderGrid
     GridView g;
     const unsigned long long* keys; const int32_t* vals; uint64_t mask;
     const uint8_t* sh_has;
+    float lo[3], hi[3];
+    const uint32_t* bricks;
+    int blo[3], bdim[3];
+};
+
+// The fusion volume in progress as the march reads it (k_render_march_live): the volume, and the box and bitmap of its voxels with
+// weight > 0 in RenderGrid's layout.  Built per call by the tracker (i3d_render.cu), never cached in RenderState.
+struct LiveGrid
+{
+    FuseView v;
+    float voxel_size;
     float lo[3], hi[3];
     const uint32_t* bricks;
     int blo[3], bdim[3];

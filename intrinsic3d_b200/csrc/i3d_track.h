@@ -7,6 +7,10 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <string>
+
+#include "i3d_frames.h"
+#include "i3d_fusion.h"
 #include "i3d_render.h"
 
 namespace i3d
@@ -55,6 +59,7 @@ struct TrackScratch
     Dev<float> rt; Dev<int32_t> ids; Dev<double> pose_in; Dev<TrackState> state;
     Dev<double> sys, sums, partials, rd_partials, rd_sums; Dev<unsigned long long> counters;
     Dev<float> pdepth, pnrm, depth[kTrackMaxLevels], nrm[kTrackMaxLevels]; Dev<uint8_t> mask;
+    Dev<int> live_box; Dev<uint32_t> live_bits;           // box and brick bitmap of the fusion volume in progress, rebuilt per use
     int n = 0, levels = 0, last_m = 0, W[kTrackMaxLevels] = {}, H[kTrackMaxLevels] = {};
 };
 
@@ -68,6 +73,18 @@ namespace track
 void sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderGrid rg, const I3DFusionCamera& dc, const float* store_depth, int store_F,
                    int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out,
                    I3DTrackInfo* info, cudaStream_t st);
+// sensor_frames with the prediction marched from the fusion volume in progress (k_render_march_live; fs unchanged) instead of a grid.  The
+// box and bitmap of the volume's voxels with weight > 0 are built first, timed as "track_bricks"; skip: march with the bitmap
+// (i3d_debug_set_render_skip).  Returns non-zero, having tracked nothing, when no voxel has weight > 0.
+int fusion_frames(TrackScratch& ts, const FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids,
+                  const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, cudaStream_t st);
+// Dense frame-to-model odometry over the stored frames ids[0..n) (validated by the caller; repeats allowed), in list order.  Per frame:
+// the guess (pose_first for ids[0] when given, which resets fs's motion state; else constant velocity from it), then with no voxel of
+// weight > 0 the frame is integrated at the guess (I3D_TRACK_ANCHORED), otherwise fusion_frames' tracking of that one frame (m = 1) and,
+// at status 0 only, fusion::integrate at the tracked pose.  Timed as "odometry" (host wall time of the call), "odometry_predict",
+// "odometry_icp" and the fusion phases.  Returns non-zero with the message in `error` when fusion::integrate fails.
+int odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids, const double* pose_first,
+             const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, std::string& error, cudaStream_t st);
 } // namespace track
 
 } // namespace i3d

@@ -236,7 +236,7 @@ class I3DRenderStats(C.Structure, _Dictable):
 
 
 TRACK_LEVELS = 4          # entries of I3DTrackParams::iterations
-TRACK_STATUS = {0: "tracked", 1: "too few correspondences", 2: "not positive definite", 3: "non-finite"}
+TRACK_STATUS = {0: "tracked", 1: "too few correspondences", 2: "not positive definite", 3: "non-finite", 4: "anchored"}
 
 
 class I3DTrackParams(C.Structure, _Dictable):

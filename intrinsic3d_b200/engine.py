@@ -35,7 +35,7 @@ EXPORTED_SYMBOLS = [
     "i3d_sizeof_render_params", "i3d_sizeof_render_stats", "i3d_default_render_params", "i3d_render_keyframes", "i3d_download_render",
     "i3d_debug_set_render_skip",
     "i3d_sizeof_track_params", "i3d_sizeof_track_info", "i3d_default_track_params", "i3d_track_sensor_frames", "i3d_debug_get_track_system",
-    "i3d_debug_get_track_planes",
+    "i3d_debug_get_track_planes", "i3d_fusion_track_sensor_frames", "i3d_fusion_track_and_integrate_sensor",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
     "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_pcg_vectors", "i3d_debug_get_normal_equations",
@@ -105,6 +105,9 @@ def load_library():
     L.i3d_track_sensor_frames.restype = C.c_int
     L.i3d_track_sensor_frames.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(I3DTrackParams),
                                           C.POINTER(C.c_double), C.POINTER(I3DTrackInfo)]
+    for fn in (L.i3d_fusion_track_sensor_frames, L.i3d_fusion_track_and_integrate_sensor):
+        fn.restype = C.c_int
+        fn.argtypes = L.i3d_track_sensor_frames.argtypes
     L.i3d_debug_get_track_system.restype = C.c_int
     L.i3d_debug_get_track_system.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     L.i3d_debug_get_track_planes.restype = C.c_int
@@ -467,14 +470,10 @@ class Engine:
         self._check(self.L.i3d_fusion_integrate_sensor(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(c2w, C.c_float), _p(w2c, C.c_float)))
 
     # ---- tracking stored frames against the surface (DESIGN.md §6n) --------------------------------------------------------------
-    def track_sensor_frames(self, ids, pose_w2c, source: str = "fused", **params):
-        """Point-to-plane ICP of the stored frames `ids` (distinct) against the surface of `source` ("fused": sdf0, "refined"), over the
-        depth pyramid, starting from pose_w2c float64 [len(ids), 12] (world -> camera, R row-major | t).  params: fields of
-        I3DTrackParams (num_levels, iterations (up to 4 values, level 0 first), max_distance, min_normal_cos, min_correspondences);
-        the rest keep default_track_params().  Returns (poses float64 [n, 12] world -> camera, infos: one dict per frame).
-        Device time: phase_ms("track")."""
+    @staticmethod
+    def _track_params(sdf_source, params):
         p = default_track_params()
-        p.sdf_source = self._mesh_source(source)
+        p.sdf_source = sdf_source
         for k, v in params.items():
             if k == "iterations":
                 v = list(v) + [0] * (TRACK_LEVELS - len(v))
@@ -488,15 +487,43 @@ class Engine:
                 setattr(p, k, float(v))
             else:
                 raise ValueError(f"unknown tracking parameter {k!r}")
+        return p
+
+    def _track_call(self, fn, ids, pose, name, n_pose, p):
         ids, n = self._ids(ids)
-        pose = np.ascontiguousarray(pose_w2c, np.float64)
-        if pose.shape != (n, 12):
-            raise ValueError(f"pose_w2c must be [{n}, 12], got {pose.shape}")
+        if pose is not None:
+            pose = np.ascontiguousarray(pose, np.float64)
+            if pose.shape != (n_pose(n), 12):
+                raise ValueError(f"{name} must be [{n_pose(n)}, 12], got {pose.shape}")
         out = np.empty((max(n, 1), 12), np.float64)
         infos = (I3DTrackInfo * max(n, 1))()
-        self._check(self.L.i3d_track_sensor_frames(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(pose, C.c_double), C.byref(p),
-                                                   _p(out, C.c_double), infos))
+        self._check(fn(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(pose, C.c_double), C.byref(p), _p(out, C.c_double), infos))
         return out[:n], [infos[i].as_dict() for i in range(n)]
+
+    def track_sensor_frames(self, ids, pose_w2c, source: str = "fused", **params):
+        """Point-to-plane ICP of the stored frames `ids` (distinct) against the surface of `source` ("fused": sdf0, "refined"), over the
+        depth pyramid, starting from pose_w2c float64 [len(ids), 12] (world -> camera, R row-major | t).  params: fields of
+        I3DTrackParams (num_levels, iterations (up to 4 values, level 0 first), max_distance, min_normal_cos, min_correspondences);
+        the rest keep default_track_params().  Returns (poses float64 [n, 12] world -> camera, infos: one dict per frame).
+        Device time: phase_ms("track")."""
+        p = self._track_params(self._mesh_source(source), params)
+        return self._track_call(self.L.i3d_track_sensor_frames, ids, pose_w2c, "pose_w2c", lambda n: n, p)
+
+    # ---- tracking against the fusion in progress, and RGB-D odometry (DESIGN.md §6o) ---------------------------------------------
+    def fusion_track_sensor_frames(self, ids, pose_w2c, **params):
+        """track_sensor_frames with the fusion volume in progress as the model (equal to fusion_finish with correct_sdf_iterations 0
+        followed by track_sensor_frames(..., "fused"), but the fusion goes on).  Returns (poses float64 [n, 12], infos)."""
+        p = self._track_params(0, params)
+        return self._track_call(self.L.i3d_fusion_track_sensor_frames, ids, pose_w2c, "pose_w2c", lambda n: n, p)
+
+    def fusion_track_and_integrate_sensor(self, ids, pose_first=None, **params):
+        """Dense odometry: each stored frame of `ids` (in order, repeats allowed) is tracked against the fusion in progress from a
+        constant-velocity guess and integrated at the tracked pose; pose_first (world -> camera [12]) is the guess of the first frame,
+        None continues from the previous call.  A frame that fails to track is not integrated.  Returns (poses float64 [n, 12] world ->
+        camera, infos with status "anchored" (4) for a frame integrated untracked into an empty volume).  Time: phase_ms("odometry")."""
+        p = self._track_params(0, params)
+        pose = None if pose_first is None else np.asarray(pose_first, np.float64).reshape(1, 12)
+        return self._track_call(self.L.i3d_fusion_track_and_integrate_sensor, ids, pose, "pose_first", lambda n: 1, p)
 
     def debug_track_system(self, n):
         """(sums float64 [n, 29], pose camera -> world float64 [n, 12]) of the last tracking call of n frames."""
