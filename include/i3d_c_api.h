@@ -284,6 +284,37 @@ int         i3d_fusion_track_sensor_frames(I3DEngine* e, int32_t n, const int32_
 int         i3d_fusion_track_and_integrate_sensor(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_first,
                                                   const I3DTrackParams* params, double* pose_out, I3DTrackInfo* info);
 
+/* ---- tracking with colour as well as depth: a photometric term (DESIGN.md §6p) ---- */
+uint64_t    i3d_sizeof_track_color_params(void);
+uint64_t    i3d_sizeof_track_color_info(void);
+/* weight {0.05, 0.05, 0.05, 0.05}, max_color_diff 0.1, min_color_gradient 0.01 (the best of the weights measured on C2, DESIGN.md §6p). */
+void        i3d_default_track_color_params(I3DTrackColorParams* p);
+/* The three tracking calls with a photometric term added to every system: per level the prediction pixels (2^l u, 2^l v) with a hit give
+ * a world point q and the model intensity I_m (the trilinear blend of the voxel colours' intensities at the hit), the residual is
+ * I_f(pi(R^T (q - t))) - I_m against the stored colour frame's intensity in the depth camera at level l, and the system solved is
+ * A_depth + lambda_l^2 A_colour, b likewise; the row count, sum r^2 and every status keep their depth-only meaning.  With every weight 0
+ * the results are the bytes of the depth-only call.  color_info[n] (may be NULL): the photometric rows and sum r^2 of the first and the
+ * last evaluated system.  Fail, writing nothing, for every refusal of the depth-only call, NULL color params, a weight that is negative or
+ * not finite, max_color_diff not finite and > 0, and min_color_gradient negative or not finite.  Device time as the depth-only call, plus
+ * i3d_phase_ms("track_color") (intensity pyramid and gradients); i3d_phase_count("track_photo_correspondences") = photometric rows of
+ * every evaluated system; with i3d_debug_set_kernel_timers(e, 1) also "track_photo_rows". */
+int         i3d_track_sensor_frames_rgbd(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params,
+                                         const I3DTrackColorParams* color, double* pose_out, I3DTrackInfo* info, I3DTrackColorInfo* color_info);
+int         i3d_fusion_track_sensor_frames_rgbd(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params,
+                                                const I3DTrackColorParams* color, double* pose_out, I3DTrackInfo* info,
+                                                I3DTrackColorInfo* color_info);
+int         i3d_fusion_track_and_integrate_sensor_rgbd(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_first,
+                                                       const I3DTrackParams* params, const I3DTrackColorParams* color, double* pose_out,
+                                                       I3DTrackInfo* info, I3DTrackColorInfo* color_info);
+/* Parity hook: the planes of the last pass of the last _rgbd call, for the frames of that pass: model_intensity [m][H][W] (0 without a
+ * hit), and at pyramid level `level` the frame intensity, grad_x and grad_y [m][H_l][W_l].  Any pointer may be NULL; m in *frames.  Fails
+ * when the last tracking call had no photometric term and for a level it did not build. */
+int         i3d_debug_get_track_color_planes(I3DEngine* e, int32_t level, float* model_intensity, float* intensity, float* grad_x,
+                                             float* grad_y, int32_t* frames);
+/* Parity hook: sums [n][29] = the photometric values of the last evaluated system of each frame of the last _rgbd call, in the layout of
+ * i3d_debug_get_track_system, unweighted.  Fails when the last tracking call had no photometric term. */
+int         i3d_debug_get_track_color_system(I3DEngine* e, double* sums);
+
 /* ---- keyframe selection and the RGB-D image pyramid: the inputs of fusion and refinement (DESIGN.md §6i) ---- */
 /* Frames scored per device pass by i3d_keyframe_scores: bounds its scratch memory (I3D_KEYFRAME_CHUNK * W * H * 3 bytes). */
 #define I3D_KEYFRAME_CHUNK 32

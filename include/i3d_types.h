@@ -266,6 +266,23 @@ typedef struct I3DTrackInfo
     I3DRenderStats initial;               /* the prediction render against the frame's depth, at the input pose */
 } I3DTrackInfo;
 
+/* ---- the photometric term of tracking: joint depth and colour Gauss-Newton (DESIGN.md §6p) ---- */
+typedef struct I3DTrackColorParams
+{
+    float   weight[4];                    /* lambda per pyramid level, level 0 first: A = A_depth + lambda^2 A_colour; 0 = depth only */
+    float   max_color_diff;               /* photometric gate |I_frame - I_model| (intensity in [0, 1]) */
+    float   min_color_gradient;           /* texture gate |grad I_frame| (intensity per pixel, central differences); 0 = off */
+    int32_t reserved[2];
+} I3DTrackColorParams;
+
+typedef struct I3DTrackColorInfo
+{
+    int64_t first_rows;                   /* photometric rows of the first evaluated system (at the input pose, coarsest level) */
+    double  first_residual_sq;            /* sum of their squared intensity residuals */
+    int64_t last_rows;                    /* photometric rows of the last evaluated system */
+    double  last_residual_sq;
+} I3DTrackColorInfo;
+
 #ifdef __cplusplus
 }
 #endif

@@ -1827,10 +1827,24 @@ static int check_finite_poses(I3DEngine* e, const char* who, int32_t n, const do
     return 0;
 }
 
-int i3d_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params, double* pose_out,
-                            I3DTrackInfo* info)
+// The refusals of a photometric term (DESIGN.md §6p); fills col
+static int check_track_color(I3DEngine* e, const char* who, const I3DTrackColorParams* cp, I3DTrackColorInfo* ci, TrackColor& col)
 {
-    static const char* who = "i3d_track_sensor_frames";
+    if (!cp) return fail(e, "%s: color params must not be NULL", who);
+    for (int l = 0; l < kTrackMaxLevels; ++l)
+        if (!(std::isfinite(cp->weight[l]) && cp->weight[l] >= 0.0f)) return fail(e, "%s: weight[%d] must be finite and >= 0, got %g", who, l, cp->weight[l]);
+    if (!(std::isfinite(cp->max_color_diff) && cp->max_color_diff > 0.0f))
+        return fail(e, "%s: max_color_diff must be finite and > 0, got %g", who, cp->max_color_diff);
+    if (!(std::isfinite(cp->min_color_gradient) && cp->min_color_gradient >= 0.0f))
+        return fail(e, "%s: min_color_gradient must be finite and >= 0, got %g", who, cp->min_color_gradient);
+    col = TrackColor{cp, &e->sensor, ci};
+    return 0;
+}
+
+// i3d_track_sensor_frames, with the photometric term cp when it is not nullptr (the _rgbd call)
+static int track_sensor_frames(I3DEngine* e, const char* who, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params,
+                               double* pose_out, I3DTrackInfo* info, bool rgbd, const I3DTrackColorParams* cp, I3DTrackColorInfo* ci)
+{
     if (!e) return 1;
     if (!params || !pose_in || !pose_out) return fail(e, "%s: params, pose_in and pose_out must not be NULL", who);
     if (e->world > 1) return fail(e, "%s: tracking runs on one GPU (world = %d)", who, e->world);
@@ -1842,11 +1856,25 @@ int i3d_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const d
     if (check_sdf_source(e, who, P.sdf_source)) return 1;
     int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
     if (check_track_params(e, who, P, Wl, Hl)) return 1;
+    TrackColor col{};
+    if (rgbd && check_track_color(e, who, cp, ci, col)) return 1;
     return guarded(e, [&]() {
         track::sensor_frames(e->track, e->render, e->timing, render_grid(e, P.sdf_source, false), e->sensor.dcam, e->sensor.depth.p, e->sensor.F, n, ids, pose_in, P,
-                             Wl, Hl, pose_out, info, e->stream);
+                             Wl, Hl, pose_out, info, e->stream, rgbd ? &col : nullptr);
         return 0;
     });
+}
+
+int i3d_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params, double* pose_out,
+                            I3DTrackInfo* info)
+{
+    return track_sensor_frames(e, "i3d_track_sensor_frames", n, ids, pose_in, params, pose_out, info, false, nullptr, nullptr);
+}
+
+int i3d_track_sensor_frames_rgbd(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params,
+                                 const I3DTrackColorParams* color, double* pose_out, I3DTrackInfo* info, I3DTrackColorInfo* color_info)
+{
+    return track_sensor_frames(e, "i3d_track_sensor_frames_rgbd", n, ids, pose_in, params, pose_out, info, true, color, color_info);
 }
 
 // The checks of the two calls that track against the fusion in progress, up to the poses
@@ -1858,10 +1886,10 @@ static int check_fusion_track(I3DEngine* e, const char* who, int32_t n, const in
     return check_sensor_ids(e, who, n, ids);
 }
 
-int i3d_fusion_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params, double* pose_out,
-                                   I3DTrackInfo* info)
+static int fusion_track_sensor_frames(I3DEngine* e, const char* who, int32_t n, const int32_t* ids, const double* pose_in,
+                                      const I3DTrackParams* params, double* pose_out, I3DTrackInfo* info, bool rgbd, const I3DTrackColorParams* cp,
+                                      I3DTrackColorInfo* ci)
 {
-    static const char* who = "i3d_fusion_track_sensor_frames";
     if (!e) return 1;
     if (!pose_in) return fail(e, "%s: pose_in must not be NULL", who);
     if (check_fusion_track(e, who, n, ids, params, pose_out)) return 1;
@@ -1871,17 +1899,32 @@ int i3d_fusion_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, 
     if (P.sdf_source != 0) return fail(e, "%s: sdf_source must be 0 (the fusion volume holds one sdf), got %d", who, P.sdf_source);
     int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
     if (check_track_params(e, who, P, Wl, Hl)) return 1;
+    TrackColor col{};
+    if (rgbd && check_track_color(e, who, cp, ci, col)) return 1;
     return guarded(e, [&]() {
-        if (track::fusion_frames(e->track, e->fusion, e->render.skip, e->timing, e->sensor, n, ids, pose_in, P, Wl, Hl, pose_out, info, e->stream))
+        if (track::fusion_frames(e->track, e->fusion, e->render.skip, e->timing, e->sensor, n, ids, pose_in, P, Wl, Hl, pose_out, info, e->stream,
+                                 rgbd ? &col : nullptr))
             return fail(e, "%s: the fusion volume has no voxel with weight > 0", who);
         return 0;
     });
 }
 
-int i3d_fusion_track_and_integrate_sensor(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_first, const I3DTrackParams* params,
-                                          double* pose_out, I3DTrackInfo* info)
+int i3d_fusion_track_sensor_frames(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params, double* pose_out,
+                                   I3DTrackInfo* info)
 {
-    static const char* who = "i3d_fusion_track_and_integrate_sensor";
+    return fusion_track_sensor_frames(e, "i3d_fusion_track_sensor_frames", n, ids, pose_in, params, pose_out, info, false, nullptr, nullptr);
+}
+
+int i3d_fusion_track_sensor_frames_rgbd(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params,
+                                        const I3DTrackColorParams* color, double* pose_out, I3DTrackInfo* info, I3DTrackColorInfo* color_info)
+{
+    return fusion_track_sensor_frames(e, "i3d_fusion_track_sensor_frames_rgbd", n, ids, pose_in, params, pose_out, info, true, color, color_info);
+}
+
+static int fusion_track_and_integrate_sensor(I3DEngine* e, const char* who, int32_t n, const int32_t* ids, const double* pose_first,
+                                             const I3DTrackParams* params, double* pose_out, I3DTrackInfo* info, bool rgbd,
+                                             const I3DTrackColorParams* cp, I3DTrackColorInfo* ci)
+{
     if (!e) return 1;
     if (check_fusion_track(e, who, n, ids, params, pose_out)) return 1;
     if (pose_first ? check_finite_poses(e, who, 1, pose_first, "pose_first") : 0) return 1;
@@ -1891,14 +1934,31 @@ int i3d_fusion_track_and_integrate_sensor(I3DEngine* e, int32_t n, const int32_t
     if (P.sdf_source != 0) return fail(e, "%s: sdf_source must be 0 (the fusion volume holds one sdf), got %d", who, P.sdf_source);
     int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
     if (check_track_params(e, who, P, Wl, Hl)) return 1;
+    TrackColor col{};
+    if (rgbd && check_track_color(e, who, cp, ci, col)) return 1;
     const int rc = guarded(e, [&]() {
         std::string err;
-        if (track::odometry(e->track, e->fusion, e->render.skip, e->timing, e->sensor, n, ids, pose_first, P, Wl, Hl, pose_out, info, err, e->stream))
+        if (track::odometry(e->track, e->fusion, e->render.skip, e->timing, e->sensor, n, ids, pose_first, P, Wl, Hl, pose_out, info, err, e->stream,
+                            rgbd ? &col : nullptr))
             return fail(e, "%s: %s", who, err.c_str());
         return 0;
     });
     if (rc != 0) e->fusion.active = false;
     return rc;
+}
+
+int i3d_fusion_track_and_integrate_sensor(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_first, const I3DTrackParams* params,
+                                          double* pose_out, I3DTrackInfo* info)
+{
+    return fusion_track_and_integrate_sensor(e, "i3d_fusion_track_and_integrate_sensor", n, ids, pose_first, params, pose_out, info, false, nullptr,
+                                             nullptr);
+}
+
+int i3d_fusion_track_and_integrate_sensor_rgbd(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_first, const I3DTrackParams* params,
+                                               const I3DTrackColorParams* color, double* pose_out, I3DTrackInfo* info, I3DTrackColorInfo* color_info)
+{
+    return fusion_track_and_integrate_sensor(e, "i3d_fusion_track_and_integrate_sensor_rgbd", n, ids, pose_first, params, pose_out, info, true, color,
+                                             color_info);
 }
 
 int i3d_debug_get_track_system(I3DEngine* e, double* sums, double* pose_cam_to_world)
@@ -1933,6 +1993,50 @@ int i3d_debug_get_track_planes(I3DEngine* e, int32_t level, float* depth, float*
         if (mask) CK(cudaMemcpyAsync(mask, e->track.mask.p, img, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         if (frames) *frames = static_cast<int32_t>(m);
+        return 0;
+    });
+}
+
+// ---- the photometric term of tracking (i3d_track.cuh, DESIGN.md §6p) ------------------------------
+uint64_t i3d_sizeof_track_color_params(void) { return sizeof(I3DTrackColorParams); }
+uint64_t i3d_sizeof_track_color_info(void) { return sizeof(I3DTrackColorInfo); }
+
+void i3d_default_track_color_params(I3DTrackColorParams* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    for (int l = 0; l < kTrackMaxLevels; ++l) p->weight[l] = 0.05f;      // measured on C2 (DESIGN.md §6p)
+    p->max_color_diff = 0.1f; p->min_color_gradient = 0.01f;
+}
+
+int i3d_debug_get_track_color_planes(I3DEngine* e, int32_t level, float* model_intensity, float* intensity, float* grad_x, float* grad_y,
+                                     int32_t* frames)
+{
+    static const char* who = "i3d_debug_get_track_color_planes";
+    if (!e) return 1;
+    if (e->track.n <= 0 || !e->track.color) return fail(e, "%s: the last tracking call had no photometric term", who);
+    if (level < 0 || level >= e->track.levels) return fail(e, "%s: level %d was not built (%d levels)", who, level, e->track.levels);
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t m = static_cast<size_t>(e->track.last_m);
+        const size_t lv = m * e->track.W[level] * e->track.H[level], img = m * e->track.W[0] * e->track.H[0];
+        if (model_intensity) CK(cudaMemcpyAsync(model_intensity, e->track.pint.p, img * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (intensity) CK(cudaMemcpyAsync(intensity, e->track.inten[level].p, lv * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (grad_x) CK(cudaMemcpyAsync(grad_x, e->track.gx[level].p, lv * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (grad_y) CK(cudaMemcpyAsync(grad_y, e->track.gy[level].p, lv * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (frames) *frames = static_cast<int32_t>(m);
+        return 0;
+    });
+}
+
+int i3d_debug_get_track_color_system(I3DEngine* e, double* sums)
+{
+    if (!e) return 1;
+    if (e->track.n <= 0 || !e->track.color) return fail(e, "i3d_debug_get_track_color_system: the last tracking call had no photometric term");
+    return guarded(e, [&]() {
+        if (sums)
+            CK(cudaMemcpyAsync(sums, e->track.sys_c.p, static_cast<size_t>(e->track.n) * kTrackVals * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaStreamSynchronize(e->stream));
         return 0;
     });
 }

@@ -39,6 +39,26 @@ void frames::depthdown(int n, int W, int H, const float* src, float* dst, cudaSt
     k_frames_depthdown<<<grid, dim3(32, 8), 0, st>>>(n, W, H, src, dst);
 }
 
+void frames::pyrdown(int n, int W, int H, const float* src, float* dst, cudaStream_t st)
+{
+    const int wd = W / 2, hd = H / 2;
+    k_frames_pyrdown<<<dim3((wd + 31) / 32, (hd + 7) / 8, std::min(n, 65535)), dim3(32, 8), 0, st>>>(n, W, H, src, dst);
+}
+
+void frames::sensor_intensity(const SensorStore& ss, int n, const int32_t* ids, const int32_t* iota, Dev<float>& tmp, float* dst, cudaStream_t st)
+{
+    const I3DFusionCamera &dc = ss.dcam, &cc = ss.ccam;
+    const size_t cpx = static_cast<size_t>(cc.width) * cc.height;
+    const bool same = dc.width == cc.width && dc.height == cc.height;
+    if (!same) tmp.ensure(cpx * n);
+    float* lum = same ? dst : tmp.p;
+    for (int k = 0; k < n; ++k)
+        k_frames_lum0<<<blocks_for(cpx), kThreads, 0, st>>>(cpx, ss.bgr.p + 3 * cpx * ids[k], lum + cpx * k);
+    if (same) return;
+    const ResizeCams rc{cc.width, cc.height, cc.fx, cc.fy, cc.cx, cc.cy, dc.width, dc.height, dc.fx, dc.fy, dc.cx, dc.cy};
+    k_resize_depth<<<dim3((dc.width + 31) / 32, (dc.height + 7) / 8, std::min(n, 65535)), dim3(32, 8), 0, st>>>(n, iota, rc, tmp.p, dst);
+}
+
 void frames::keyframe_scores(ScoreScratch& ks, Timing& tm, int F, int W, int H, const uint8_t* bgr, double* scores, cudaStream_t st)
 {
     const size_t img = static_cast<size_t>(W) * H * 3;
@@ -169,7 +189,7 @@ void frames::level(RgbdStore& rs, Timing& tm, int lvl, float* lum, float* depth,
             rs.tmp[k & 1].ensure(c); rs.tmp[2 + (k & 1)].ensure(c);
             dl = rs.tmp[k & 1].p; dd = rs.tmp[2 + (k & 1)].p;
         }
-        k_frames_pyrdown<<<dim3((wd + 31) / 32, (hd + 7) / 8, std::min(F, 65535)), dim3(32, 8), 0, st>>>(F, w, h, sl, dl);
+        pyrdown(F, w, h, sl, dl, st);
         depthdown(F, w, h, sd, dd, st);
         sl = dl; sd = dd; w = wd; h = hd;
     }

@@ -42,6 +42,13 @@ namespace frames
 {
 // Pyramid::downsampleDepth (k_frames_depthdown) of n W x H depth planes into n (W / 2) x (H / 2) planes
 void depthdown(int n, int W, int H, const float* src, float* dst, cudaStream_t st);
+// cv::pyrDown (k_frames_pyrdown) of n W x H planes into n (W / 2) x (H / 2) planes
+void pyrdown(int n, int W, int H, const float* src, float* dst, cudaStream_t st);
+// The level-0 intensity of the stored colour frames ids[0..n) (host list, validated by the caller) in the depth camera, into dst
+// [n][depth cam]: k_frames_lum0 of each frame's colour plane, then resizeDepth's mapping and interpolate<float> (k_resize_depth) from the
+// colour camera to the depth camera with the identity list iota [n] (device: 0, 1, ...).  With equal sizes that is a copy (Q51), so
+// lum0 writes dst directly; otherwise tmp holds the colour-size planes.
+void sensor_intensity(const SensorStore& ss, int n, const int32_t* ids, const int32_t* iota, Dev<float>& tmp, float* dst, cudaStream_t st);
 // Blur scores of F host frames of W x H (validated by the caller), uploaded in chunks of I3D_KEYFRAME_CHUNK: one "keyframe_scores" timer
 // per chunk, and a synchronisation per chunk, which frees the chunk buffer again
 void keyframe_scores(ScoreScratch& ks, Timing& tm, int F, int W, int H, const uint8_t* bgr, double* scores, cudaStream_t st);

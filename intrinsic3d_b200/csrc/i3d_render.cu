@@ -62,9 +62,18 @@ void add_voxel_box(RenderState& rs, Timing& tm, RenderGrid& rg, cudaStream_t st)
     rg.bricks = (rs.skip && rs.have_bricks) ? rs.bits.p : nullptr;
 }
 
-void march(const RenderGrid& rg, const RenderCam& cam, const RenderViews& rv, cudaStream_t st)
+// The march of the installed grid; with mi also its model intensity plane from GridView::rgb
+void march(const RenderGrid& rg, const RenderCam& cam, const RenderViews& rv, cudaStream_t st, float* mi = nullptr)
 {
-    k_render_march<<<dim3(rv.tiles_x, rv.tiles_y, rv.n), dim3(kRenderTile, kRenderTile), 0, st>>>(rg, cam, rv);
+    const dim3 grid(rv.tiles_x, rv.tiles_y, rv.n), block(kRenderTile, kRenderTile);
+    if (mi)
+    {
+        Colored<RenderGrid> cg{};
+        static_cast<RenderGrid&>(cg) = rg;
+        cg.rgb = rg.g.rgb; cg.out_mi = mi;
+        k_render_march_color<<<grid, block, 0, st>>>(cg, cam, rv);
+    }
+    else k_render_march<<<grid, block, 0, st>>>(rg, cam, rv);
 }
 
 // out[n][V] = the fixed-order sums of the n views' partials [n][tiles][V]
@@ -132,17 +141,24 @@ void render::keyframes(RenderState& rs, Timing& tm, RenderGrid rg, const RenderC
 namespace
 {
 // The phase names of one tracking pass (whole: nullptr = not timed as a whole)
-struct TrackPhases { const char* whole; const char* predict; const char* pyramid; const char* icp; const char* correspondences; };
-constexpr TrackPhases kTrackPhases{"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences"};
-constexpr TrackPhases kOdometryPhases{nullptr, "odometry_predict", "odometry_icp", "odometry_icp", "odometry_correspondences"};
+struct TrackPhases
+{
+    const char* whole; const char* predict; const char* pyramid; const char* icp; const char* correspondences;
+    const char* color; const char* photo_correspondences;
+};
+constexpr TrackPhases kTrackPhases{"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences", "track_color",
+                                   "track_photo_correspondences"};
+constexpr TrackPhases kOdometryPhases{nullptr, "odometry_predict", "odometry_icp", "odometry_icp", "odometry_correspondences", "odometry_icp",
+                                      "odometry_photo_correspondences"};
 
 // The tracker's passes over ids[0..n), shared by the grid and the fusion volume: prepare() (false: stop, nothing tracked) runs once
-// after the uploads, predict(cam, rv) marches a chunk's prediction into rv.  pose_cw_out [n][12] (may be nullptr): the tracked
-// camera -> world poses.  Returns false when prepare() stopped the call.
+// after the uploads, predict(cam, rv, mi) marches a chunk's prediction into rv, and with mi != nullptr the model intensity plane into mi.
+// pose_cw_out [n][12] (may be nullptr): the tracked camera -> world poses.  col: the photometric term (nullptr: depth only).  Returns
+// false when prepare() stopped the call.
 template <class Prepare, class Predict>
 bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&& prepare, Predict&& predict, const I3DFusionCamera& dc,
                   const float* store_depth, int store_F, int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl,
-                  const int* Hl, double* pose_out, double* pose_cw_out, I3DTrackInfo* info, cudaStream_t st)
+                  const int* Hl, double* pose_out, double* pose_cw_out, I3DTrackInfo* info, cudaStream_t st, const TrackColor* col)
 {
     const int L = P.num_levels, W = dc.width, H = dc.height, C = std::min<int>(n, I3D_TRACK_CHUNK);
     const size_t img = static_cast<size_t>(W) * H;
@@ -151,7 +167,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
     ts.n = 0;
     ts.ids.ensure(n); ts.pose_in.ensure(12 * static_cast<size_t>(n)); ts.state.ensure(n);
     ts.sys.ensure(static_cast<size_t>(n) * kTrackVals); ts.rd_sums.ensure(static_cast<size_t>(n) * kRenderStats);
-    ts.rt.ensure(12 * static_cast<size_t>(store_F)); ts.counters.ensure(2);
+    ts.rt.ensure(12 * static_cast<size_t>(store_F)); ts.counters.ensure(3);
     ts.rd_partials.ensure(static_cast<size_t>(C) * tiles_x * tiles_y * kRenderStats);
     ts.partials.ensure(static_cast<size_t>(C) * tiles_x * tiles_y * kTrackVals); ts.sums.ensure(static_cast<size_t>(C) * kTrackVals);
     ts.pdepth.ensure(C * img); ts.pnrm.ensure(3 * C * img); ts.mask.ensure(C * img);
@@ -159,6 +175,18 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
     {
         const size_t c = static_cast<size_t>(C) * Wl[l] * Hl[l];
         ts.depth[l].ensure(c); ts.nrm[l].ensure(3 * c);
+        if (col) { ts.inten[l].ensure(c); ts.gx[l].ensure(c); ts.gy[l].ensure(c); }
+    }
+    if (col)
+    {
+        ts.pint.ensure(C * img); ts.iota.ensure(C);
+        ts.partials_c.ensure(static_cast<size_t>(C) * tiles_x * tiles_y * kTrackVals);
+        ts.sums_c.ensure(static_cast<size_t>(C) * kTrackVals); ts.sums_comb.ensure(static_cast<size_t>(C) * kTrackVals);
+        ts.sys_c.ensure(static_cast<size_t>(n) * kTrackVals); ts.cstate.ensure(n);
+        std::vector<int32_t> iota(C);
+        for (int k = 0; k < C; ++k) iota[k] = k;
+        CK(cudaMemcpyAsync(ts.iota.p, iota.data(), C * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(ts.cstate.p, 0, n * sizeof(TrackColorState), st));
     }
     // the input poses in float, scattered by sensor id: the march reads Rt + 12 * id
     std::vector<float> hrt(12 * static_cast<size_t>(store_F), 0.0f);
@@ -167,7 +195,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
     CK(cudaMemcpyAsync(ts.ids.p, ids, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ts.pose_in.p, pose_in, 12 * static_cast<size_t>(n) * sizeof(double), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ts.rt.p, hrt.data(), hrt.size() * sizeof(float), cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(ts.counters.p, 0, 2 * sizeof(unsigned long long), st));
+    CK(cudaMemsetAsync(ts.counters.p, 0, 3 * sizeof(unsigned long long), st));
     int total_iters = 0;
     for (int l = 0; l < L; ++l) total_iters += P.iterations[l];
     TrackCam cam[kTrackMaxLevels];
@@ -196,7 +224,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
             rv.ids = ids_d; rv.Rt = ts.rt.p; rv.depth = store_depth; rv.lum = nullptr;
             rv.out_depth = ts.pdepth.p; rv.out_normal = ts.pnrm.p;
             rv.partials = ts.rd_partials.p; rv.samples = ts.counters.p + 1; rv.photometric = 0;
-            predict(rcam, rv);
+            predict(rcam, rv, col ? ts.pint.p : nullptr);
             tile_sums<kRenderStats>(m, tiles_x * tiles_y, ts.rd_partials.p, ts.rd_sums.p + static_cast<size_t>(c0) * kRenderStats, st);
         }
         {
@@ -206,6 +234,15 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
             for (int l = 0; l < L; ++l)
                 k_track_normals<<<dim3(blocks_for(static_cast<size_t>(Wl[l]) * Hl[l]), m), kThreads, 0, st>>>(cam[l], ts.depth[l].p, ts.nrm[l].p);
         }
+        if (col)
+        {
+            // the frame intensity pyramid in the depth camera and its gradients
+            Timer t(tm, st, ph.color);
+            frames::sensor_intensity(*col->ss, m, ids + c0, ts.iota.p, ts.lum_c, ts.inten[0].p, st);
+            for (int l = 1; l < L; ++l) frames::pyrdown(m, Wl[l - 1], Hl[l - 1], ts.inten[l - 1].p, ts.inten[l].p, st);
+            for (int l = 0; l < L; ++l)
+                k_track_grad<<<dim3(blocks_for(static_cast<size_t>(Wl[l]) * Hl[l]), m), kThreads, 0, st>>>(cam[l], ts.inten[l].p, ts.gx[l].p, ts.gy[l].p);
+        }
         {
             Timer t(tm, st, ph.icp);
             CK(cudaMemsetAsync(ts.mask.p, 0, m * img, st));
@@ -213,6 +250,13 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
             tr.pcam = cam[0]; tr.pdepth = ts.pdepth.p; tr.pnrm = ts.pnrm.p; tr.ids = ids_d; tr.rt_in = ts.rt.p;
             tr.state = ts.state.p + c0; tr.max_dist_sq = max_dist_sq; tr.min_cos = P.min_normal_cos;
             tr.use_cos = P.min_normal_cos > -1.0f ? 1 : 0; tr.partials = ts.partials.p;
+            TrackPhoto tp{};
+            if (col)
+            {
+                tp.pcam = cam[0]; tp.pdepth = ts.pdepth.p; tp.pint = ts.pint.p; tp.ids = ids_d; tp.rt_in = ts.rt.p; tp.state = ts.state.p + c0;
+                tp.max_distance = P.max_distance; tp.max_diff = col->P->max_color_diff;
+                tp.min_grad_sq = col->P->min_color_gradient * col->P->min_color_gradient; tp.partials = ts.partials_c.p;
+            }
             auto system = [&](int l, int solve) {
                 tr.cam = cam[l]; tr.depth = ts.depth[l].p; tr.nrm = ts.nrm[l].p; tr.mask = l == 0 ? ts.mask.p : nullptr;
                 tr.tiles_x = (Wl[l] + kTrackTile - 1) / kTrackTile; tr.tiles_y = (Hl[l] + kTrackTile - 1) / kTrackTile;
@@ -221,7 +265,22 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
                     k_track_rows<<<dim3(tr.tiles_x, tr.tiles_y, m), dim3(kTrackTile, kTrackTile), 0, st>>>(tr);
                 }
                 tile_sums<kTrackVals>(m, tr.tiles_x * tr.tiles_y, ts.partials.p, ts.sums.p, st);
-                k_track_solve<<<blocks_for(m, 64), 64, 0, st>>>(m, ts.sums.p, ts.state.p + c0, ts.sys.p + static_cast<size_t>(c0) * kTrackVals,
+                const double* S = ts.sums.p;
+                if (col)
+                {
+                    tp.cam = cam[l]; tp.step = 1 << l; tp.inten = ts.inten[l].p; tp.gx = ts.gx[l].p; tp.gy = ts.gy[l].p; tp.depth = ts.depth[l].p;
+                    tp.tiles_x = tr.tiles_x; tp.tiles_y = tr.tiles_y;
+                    {
+                        Timer tk(tm, st, "track_photo_rows", 1);
+                        k_track_photo_rows<<<dim3(tp.tiles_x, tp.tiles_y, m), dim3(kTrackTile, kTrackTile), 0, st>>>(tp);
+                    }
+                    tile_sums<kTrackVals>(m, tp.tiles_x * tp.tiles_y, ts.partials_c.p, ts.sums_c.p, st);
+                    const double w = static_cast<double>(col->P->weight[l]);
+                    k_track_combine<<<blocks_for(m, 64), 64, 0, st>>>(m, w * w, ts.sums.p, ts.sums_c.p, ts.state.p + c0, ts.cstate.p + c0, ts.sums_comb.p,
+                                                                      ts.sys_c.p + static_cast<size_t>(c0) * kTrackVals, ts.counters.p + 2);
+                    S = ts.sums_comb.p;
+                }
+                k_track_solve<<<blocks_for(m, 64), 64, 0, st>>>(m, S, ts.state.p + c0, ts.sys.p + static_cast<size_t>(c0) * kTrackVals,
                                                                 P.min_correspondences, solve, ts.counters.p);
             };
             for (int l = L - 1; l >= 0; --l)
@@ -231,18 +290,22 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
     }
     std::vector<TrackState> hs(n);
     std::vector<double> rs_sums(static_cast<size_t>(n) * kRenderStats);
-    unsigned long long counters[2] = {0, 0};
+    std::vector<TrackColorState> hc(col ? n : 0);
+    unsigned long long counters[3] = {0, 0, 0};
     CK(cudaMemcpyAsync(hs.data(), ts.state.p, n * sizeof(TrackState), cudaMemcpyDeviceToHost, st));
+    if (col) CK(cudaMemcpyAsync(hc.data(), ts.cstate.p, n * sizeof(TrackColorState), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(rs_sums.data(), ts.rd_sums.p, rs_sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(counters, ts.counters.p, sizeof(counters), cudaMemcpyDeviceToHost, st));
     if (whole) whole->stop();
     collect_kernel_times(tm, st);
     CK(cudaGetLastError());
     tm.phases[ph.correspondences].count += static_cast<int64_t>(counters[0]);
+    if (col) tm.phases[ph.photo_correspondences].count += static_cast<int64_t>(counters[2]);
     for (int k = 0; k < n; ++k)
     {
         std::memcpy(pose_out + 12 * static_cast<size_t>(k), hs[k].w2c, 12 * sizeof(double));
         if (pose_cw_out) std::memcpy(pose_cw_out + 12 * static_cast<size_t>(k), hs[k].T, 12 * sizeof(double));
+        if (col && col->info) col->info[k] = I3DTrackColorInfo{hc[k].first_rows, hc[k].first_sq, hc[k].last_rows, hc[k].last_sq};
         if (!info) continue;
         I3DTrackInfo r{};
         r.status = hs[k].status; r.iterations = hs[k].iterations; r.correspondences = hs[k].correspondences;
@@ -250,7 +313,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
         r.initial = render_stats(rs_sums.data() + static_cast<size_t>(k) * kRenderStats);
         info[k] = r;
     }
-    ts.n = n; ts.levels = L; ts.last_m = m;
+    ts.n = n; ts.levels = L; ts.last_m = m; ts.color = col != nullptr;
     for (int l = 0; l < L; ++l) { ts.W[l] = Wl[l]; ts.H[l] = Hl[l]; }
     return true;
 }
@@ -290,9 +353,18 @@ bool live_box(TrackScratch& ts, Timing& tm, const char* phase, const FuseView& f
     return true;
 }
 
-void march_live(const LiveGrid& lg, const RenderCam& cam, const RenderViews& rv, cudaStream_t st)
+// The march of the volume in progress; with mi also its model intensity plane from the voxel colours rgb
+void march_live(const LiveGrid& lg, const RenderCam& cam, const RenderViews& rv, const uchar4* rgb, float* mi, cudaStream_t st)
 {
-    k_render_march_live<<<dim3(rv.tiles_x, rv.tiles_y, rv.n), dim3(kRenderTile, kRenderTile), 0, st>>>(lg, cam, rv);
+    const dim3 grid(rv.tiles_x, rv.tiles_y, rv.n), block(kRenderTile, kRenderTile);
+    if (mi)
+    {
+        Colored<LiveGrid> cg{};
+        static_cast<LiveGrid&>(cg) = lg;
+        cg.rgb = rgb; cg.out_mi = mi;
+        k_render_march_live_color<<<grid, block, 0, st>>>(cg, cam, rv);
+    }
+    else k_render_march_live<<<grid, block, 0, st>>>(lg, cam, rv);
 }
 
 // Poses R row-major | t in double, every sum left to right as tests/test_odometry.py restates them.  The inverse is tr_inverse's.
@@ -318,33 +390,38 @@ void pose_compose(const double* A, const double* B, double* out)
 
 void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderGrid rg, const I3DFusionCamera& dc, const float* store_depth,
                           int store_F, int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl,
-                          double* pose_out, I3DTrackInfo* info, cudaStream_t st)
+                          double* pose_out, I3DTrackInfo* info, cudaStream_t st, const TrackColor* col)
 {
-    begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences"});
+    begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences", "track_color", "track_photo_rows",
+                      "track_photo_correspondences"});
     track_passes(
         ts, tm, kTrackPhases, [&]() { add_voxel_box(rs, tm, rg, st); return true; },
-        [&](const RenderCam& cam, const RenderViews& rv) { march(rg, cam, rv, st); }, dc, store_depth, store_F, n, ids, pose_in, P, Wl, Hl,
-        pose_out, nullptr, info, st);
+        [&](const RenderCam& cam, const RenderViews& rv, float* mi) { march(rg, cam, rv, st, mi); }, dc, store_depth, store_F, n, ids, pose_in, P,
+        Wl, Hl, pose_out, nullptr, info, st, col);
 }
 
 int track::fusion_frames(TrackScratch& ts, const FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids,
-                         const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, cudaStream_t st)
+                         const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, cudaStream_t st,
+                         const TrackColor* col)
 {
-    begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences", "track_bricks"});
+    begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences", "track_bricks", "track_color",
+                      "track_photo_rows", "track_photo_correspondences"});
     LiveGrid lg{};
     const bool ok = track_passes(
         ts, tm, kTrackPhases, [&]() { return live_box(ts, tm, "track_bricks", fusion::view(fs), fs.p.voxel_size, skip, lg, st); },
-        [&](const RenderCam& cam, const RenderViews& rv) { march_live(lg, cam, rv, st); }, ss.dcam, ss.depth.p, ss.F, n, ids, pose_in, P, Wl, Hl,
-        pose_out, nullptr, info, st);
+        [&](const RenderCam& cam, const RenderViews& rv, float* mi) { march_live(lg, cam, rv, fs.rgb.p, mi, st); }, ss.dcam, ss.depth.p, ss.F, n,
+        ids, pose_in, P, Wl, Hl, pose_out, nullptr, info, st, col);
     if (!ok) collect_kernel_times(tm, st);
     return ok ? 0 : 1;
 }
 
 int track::odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids, const double* pose_first,
-                    const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, std::string& error, cudaStream_t st)
+                    const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, std::string& error, cudaStream_t st,
+                    const TrackColor* col)
 {
     const auto t0 = std::chrono::steady_clock::now();
-    for (const char* nm : {"odometry", "odometry_predict", "odometry_icp", "odometry_correspondences"}) tm.phases.erase(nm);
+    for (const char* nm : {"odometry", "odometry_predict", "odometry_icp", "odometry_correspondences", "odometry_photo_correspondences", "track_photo_rows"})
+        tm.phases.erase(nm);
     // the motion state, kept here while fusion::integrate (which clears fs's) runs
     int motion = pose_first ? 0 : fs.motion;
     double prev[12], last[12];
@@ -372,6 +449,7 @@ int track::odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, co
         }
         begin_timing(tm, {});
         I3DTrackInfo r{};
+        I3DTrackColorInfo rc{};
         double Tt[12], Wt[12];
         const double* Ti = nullptr;
         const double* Wi = nullptr;
@@ -384,9 +462,12 @@ int track::odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, co
         }
         else
         {
+            TrackColor c1{};
+            if (col) c1 = TrackColor{col->P, col->ss, &rc};
             track_passes(
-                ts, tm, kOdometryPhases, []() { return true; }, [&](const RenderCam& cam, const RenderViews& rv) { march_live(lg, cam, rv, st); },
-                ss.dcam, ss.depth.p, ss.F, 1, ids + k, W, P, Wl, Hl, Wt, Tt, &r, st);
+                ts, tm, kOdometryPhases, []() { return true; },
+                [&](const RenderCam& cam, const RenderViews& rv, float* mi) { march_live(lg, cam, rv, fs.rgb.p, mi, st); }, ss.dcam, ss.depth.p, ss.F,
+                1, ids + k, W, P, Wl, Hl, Wt, Tt, &r, st, col ? &c1 : nullptr);
             if (r.status == I3D_TRACK_OK) { Ti = Tt; Wi = Wt; }
         }
         if (Ti)
@@ -407,6 +488,7 @@ int track::odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, co
         std::memcpy(fs.motion_T[0], prev, sizeof(prev)); std::memcpy(fs.motion_T[1], last, sizeof(last));
         std::memcpy(pose_out + 12 * static_cast<size_t>(k), Wi ? Wi : W, 12 * sizeof(double));
         if (info) info[k] = r;
+        if (col && col->info) col->info[k] = rc;
     }
     tm.phases["odometry"].ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     tm.phases["odometry"].count += 1;

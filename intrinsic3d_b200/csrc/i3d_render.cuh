@@ -8,6 +8,8 @@
  *   k_render_march    one thread per pixel, 16 x 16 tiles, views in gridDim.z: planes + per-tile statistic partials
  *   k_live_bounds / k_live_bricks / k_render_march_live   the same three over the fusion volume in progress (DESIGN.md §6o): the voxels
  *                     with weight > 0, and the cube rule by one fusion-hash probe per corner (the volume has no neighbour table)
+ *   k_render_march_color / k_render_march_live_color   the two marches with the model intensity plane of the tracker's photometric term
+ *                     (DESIGN.md §6p): the voxel colours' intensities blended at the hit
  *   k_tile_sums       the fixed-order sum of a view's partials (also the tracker's)
  *
  * Compiled with the tracker in i3d_render.cu, which launches them (render::keyframes, i3d_render.h).  Every float
@@ -109,6 +111,14 @@ __device__ __forceinline__ int rd_cube(const LiveGrid& lg, const float p[3], RdC
 
 __device__ __forceinline__ float rd_float(double a) { return __double2float_rn(a); }
 __device__ __forceinline__ float rd_float(float a) { return a; }
+// A voxel colour (R, G, B) as the frame store's level-0 intensity rule reads a pixel (k_frames_lum0): c = float(u8) * float(1/255) per
+// channel, then (B 0.114 + G 0.587) + R 0.299 (DESIGN.md §6p)
+__device__ __forceinline__ float rd_float(uchar4 c)
+{
+    const float inv = static_cast<float>(1.0 / 255.0);
+    const float b = FM(static_cast<float>(c.z), inv), g = FM(static_cast<float>(c.y), inv), r = FM(static_cast<float>(c.x), inv);
+    return FA(FA(FM(b, 0.114f), FM(g, 0.587f)), FM(r, 0.299f));
+}
 
 // Trilinear blend of float(a[c]) over the cube: along x, then y, then z.  s_out (optional) gets the 8 corner values.
 template <class T>
@@ -177,6 +187,26 @@ __device__ __forceinline__ float rd_albedo(const RenderGrid& rg, const RdCube& q
 __device__ __forceinline__ float rd_albedo(const LiveGrid&, const RdCube&) { return 0.0f; }
 __device__ __forceinline__ bool rd_sh(const LiveGrid&, const RdCube&, float*) { return false; }
 
+// A grid G with the model intensity plane of the tracker's photometric term (DESIGN.md §6p): the voxel colours rgb (GridView::rgb of the
+// installed grid, the Voxel colour array of the volume in progress, held here so that LiveGrid and FuseView keep their layout) and the
+// output plane out_mi [n][H][W]
+template <class G>
+struct Colored : G
+{
+    const uchar4* rgb;
+    float* out_mi;
+};
+
+// The march's model intensity output: nothing for a plain grid; for Colored<G> the trilinear blend of the corners' intensities
+// (rd_float of the voxel colours) at the hit, 0 without one
+template <class G>
+__device__ __forceinline__ void rd_model_intensity(const G&, const RdCube&, bool, int64_t) {}
+template <class G>
+__device__ __forceinline__ void rd_model_intensity(const Colored<G>& cg, const RdCube& q, bool hit, int64_t pix)
+{
+    cg.out_mi[pix] = hit ? rd_trilinear(cg.rgb, q) : 0.0f;
+}
+
 // The point at ray parameter s
 __device__ __forceinline__ void rd_point(const float o[3], const float dn[3], float s, float p[3])
 {
@@ -187,7 +217,8 @@ __device__ __forceinline__ void rd_point(const float o[3], const float dn[3], fl
 // One thread per pixel (u, v) of view blockIdx.z.  Ray: the pixel centre through the inverse of observation_weight's projection, in
 // world coordinates; samples s_k = s0 + k * voxel_size / 2 from where the ray enters the voxel box (clipped to s >= 0) to where it
 // leaves it; the hit is the first pair of consecutive valid samples going from > 0 to <= 0 whose linearly interpolated crossing lies in a
-// valid cube.  G: the installed grid (RenderGrid) or the fusion volume in progress (LiveGrid).
+// valid cube.  G: the installed grid (RenderGrid), the fusion volume in progress (LiveGrid), or either with the model intensity plane
+// (Colored<G>, rd_model_intensity).
 template <class G>
 __device__ __forceinline__ void rd_march(G rg, RenderCam cam, RenderViews rv)
 {
@@ -328,6 +359,7 @@ __device__ __forceinline__ void rd_march(G rg, RenderCam cam, RenderViews rv)
         if (rv.out_albedo) rv.out_albedo[pix] = alb;
         if (rv.out_shading) rv.out_shading[pix] = shade;
         if (rv.out_intensity) rv.out_intensity[pix] = inten;
+        rd_model_intensity(rg, q, hit, pix);
         // statistics against the keyframe
         const int64_t fp = (static_cast<int64_t>(f) * rv.H + v) * rv.W + u;
         const float zo = rv.depth[fp];
@@ -370,6 +402,16 @@ __global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march(Rend
 
 // The march of the fusion volume in progress (geometry only: albedo 0, no shading), for the tracker's prediction
 __global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march_live(LiveGrid lg, RenderCam cam, RenderViews rv) { rd_march(lg, cam, rv); }
+
+// The tracker's prediction with the model intensity plane (DESIGN.md §6p), from the installed grid and from the volume in progress
+__global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march_color(Colored<RenderGrid> cg, RenderCam cam, RenderViews rv)
+{
+    rd_march(cg, cam, rv);
+}
+__global__ void __launch_bounds__(kRenderTile * kRenderTile) k_render_march_live_color(Colored<LiveGrid> cg, RenderCam cam, RenderViews rv)
+{
+    rd_march(cg, cam, rv);
+}
 
 // One thread per (view, value) of V per-tile values: the view's tiles summed in order.  V = kRenderStats (k_render_march's statistics),
 // kTrackVals (k_track_rows' systems).

@@ -10,6 +10,12 @@
  *   k_tile_sums<kTrackVals> (i3d_render.cuh)  per (frame, value) the frame's tiles summed in order
  *   k_track_solve    one thread per frame: Cholesky of the 6 x 6 system in a fixed order, xi = -A^-1 b, T_cw <- [Rodrigues(w) | v] T_cw
  *
+ * The photometric term of the _rgbd calls (DESIGN.md §6p):
+ *   k_track_grad        central differences of the frame intensity pyramid, frames in gridDim.y
+ *   k_track_photo_rows  one thread per pixel of a level: the model sample at prediction pixel (2^l u, 2^l v), the intensity residual at its
+ *                       projection, the gates and the row [g_w x q, -g_w], reduced as k_track_rows reduces
+ *   k_track_combine     one thread per frame: A_g + lam^2 A_c, b_g + lam^2 b_c, the geometric r^2 and rows, for the unchanged k_track_solve
+ *
  * Compiled with the renderer in i3d_render.cu, which launches them (track::sensor_frames, i3d_track.h).  Every float
  * operation is explicitly rounded and every double operation is an explicit __d*_rn (no FMA contraction), so tests/track_ref.py restates
  * the planes, masks and sums exactly.  A frame's bytes depend only on that frame.
@@ -192,6 +198,175 @@ __global__ void __launch_bounds__(kTrackTile * kTrackTile) k_track_rows(TrackRow
         const int64_t tile = (static_cast<int64_t>(z) * tr.tiles_y + blockIdx.y) * tr.tiles_x + blockIdx.x;
         tr.partials[tile * kTrackVals + tid] = t;
     }
+}
+
+// ---- the photometric term (DESIGN.md §6p) ----------------------------------------------------------------------------------------
+
+// The 29 products of one pixel's row (J, r, cnt), each summed over the warp by a fixed shuffle tree as it is formed (lane 0 keeps the
+// warp's sums), then the 8 warps in order into the partials of tile (blockIdx.x, blockIdx.y) of frame z: k_track_rows' reduction, written
+// out there again because sharing it changes that kernel's instructions
+__device__ __forceinline__ void tr_tile_partials(double (&warp_sums)[kTrackTile * kTrackTile / 32][kTrackVals], const double (&J)[6], double r, double cnt, int tid, int z,
+                                                 int tiles_x, int tiles_y, double* partials)
+{
+    const int lane = tid & 31, warp = tid >> 5;
+    int j = 0;
+#pragma unroll
+    for (int a = 0; a < 6; ++a)
+    {
+#pragma unroll
+        for (int b = a; b < 6; ++b, ++j)
+        {
+            double x = DM(J[a], J[b]);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) x = DA(x, __shfl_down_sync(0xffffffffu, x, o));
+            if (lane == 0) warp_sums[warp][j] = x;
+        }
+    }
+#pragma unroll
+    for (int a = 0; a < 8; ++a, ++j)
+    {
+        double x = a < 6 ? DM(J[a], r) : (a == 6 ? DM(r, r) : cnt);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) x = DA(x, __shfl_down_sync(0xffffffffu, x, o));
+        if (lane == 0) warp_sums[warp][j] = x;
+    }
+    __syncthreads();
+    if (tid < kTrackVals)
+    {
+        double t = warp_sums[0][tid];
+#pragma unroll
+        for (int w = 1; w < kTrackTile * kTrackTile / 32; ++w) t = DA(t, warp_sums[w][tid]);
+        const int64_t tile = (static_cast<int64_t>(z) * tiles_y + blockIdx.y) * tiles_x + blockIdx.x;
+        partials[tile * kTrackVals + tid] = t;
+    }
+}
+
+// Central differences FM(0.5, I[+1] - I[-1]) of frame blockIdx.y's intensity plane on 1..W-2 x 1..H-2, 0 on the border
+__global__ void k_track_grad(TrackCam cam, const float* __restrict__ inten_all, float* __restrict__ gx_all, float* __restrict__ gy_all)
+{
+    const int64_t img = static_cast<int64_t>(cam.W) * cam.H;
+    const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    if (i >= img) return;
+    const float* I = inten_all + blockIdx.y * img;
+    const int y = static_cast<int>(i / cam.W), x = static_cast<int>(i - static_cast<int64_t>(y) * cam.W);
+    float gx = 0.0f, gy = 0.0f;
+    if (x >= 1 && y >= 1 && x < cam.W - 1 && y < cam.H - 1)
+    {
+        gx = FM(0.5f, FS(I[i + 1], I[i - 1]));
+        gy = FM(0.5f, FS(I[i + cam.W], I[i - cam.W]));
+    }
+    gx_all[blockIdx.y * img + i] = gx;
+    gy_all[blockIdx.y * img + i] = gy;
+}
+
+// Bilinear sample of plane P (row stride W) at x0 + fx, y0 + fy: along x, then y
+__device__ __forceinline__ float tr_bilinear(const float* __restrict__ P, int W, int x0, int y0, float fx, float fy)
+{
+    const float* a = P + static_cast<int64_t>(y0) * W + x0;
+    const float r0 = FA(a[0], FM(fx, FS(a[1], a[0]))), r1 = FA(a[W], FM(fx, FS(a[W + 1], a[W])));
+    return FA(r0, FM(fy, FS(r1, r0)));
+}
+
+// One thread per pixel (u, v) of level l of frame blockIdx.z: the model sample at prediction pixel (2^l u, 2^l v), the intensity residual
+// at its projection with the current pose, the gates and the photometric row, reduced as k_track_rows reduces (DESIGN.md §6p)
+__global__ void __launch_bounds__(kTrackTile * kTrackTile) k_track_photo_rows(TrackPhoto tp)
+{
+    __shared__ double warp_sums[kTrackTile * kTrackTile / 32][kTrackVals];
+    const int u = blockIdx.x * kTrackTile + threadIdx.x, v = blockIdx.y * kTrackTile + threadIdx.y, z = blockIdx.z;
+    const int tid = threadIdx.y * kTrackTile + threadIdx.x;
+    const TrackState& s = tp.state[z];
+    double J[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, r = 0.0, cnt = 0.0;
+    if (u < tp.cam.W && v < tp.cam.H && s.frozen == 0)
+    {
+        const TrackCam& c0 = tp.pcam;
+        const int iu = u * tp.step, iv = v * tp.step;
+        const int64_t pp = (static_cast<int64_t>(z) * c0.H + iv) * c0.W + iu;
+        const float zm = tp.pdepth[pp];
+        if (zm > 0.0f)
+        {
+            // q = o0 + z_m R0^T (x', y', 1), as tr_associate builds it
+            const float* R0 = tp.rt_in + 12 * static_cast<int64_t>(tp.ids[z]);
+            const float xn = FD(FS(__int2float_rn(iu), c0.cx), c0.fx), yn = FD(FS(__int2float_rn(iv), c0.cy), c0.fy);
+            float q[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k)
+            {
+                const float o = -FA(FA(FM(R0[k], R0[9]), FM(R0[3 + k], R0[10])), FM(R0[6 + k], R0[11]));
+                const float dir = FA(FA(FM(R0[k], xn), FM(R0[3 + k], yn)), R0[6 + k]);
+                q[k] = FA(o, FM(zm, dir));
+            }
+            // x_c = R^T (q - t) with the float camera -> world pose
+            float Tf[12];
+#pragma unroll
+            for (int i = 0; i < 12; ++i) Tf[i] = s.Tf[i];
+            const float e[3] = {FS(q[0], Tf[9]), FS(q[1], Tf[10]), FS(q[2], Tf[11])};
+            float xc[3];
+#pragma unroll
+            for (int d = 0; d < 3; ++d) xc[d] = FA(FA(FM(Tf[d], e[0]), FM(Tf[3 + d], e[1])), FM(Tf[6 + d], e[2]));
+            const TrackCam& c = tp.cam;
+            if (xc[2] > 0.0f)
+            {
+                const float x = FA(FM(c.fx, FD(xc[0], xc[2])), c.cx), y = FA(FM(c.fy, FD(xc[1], xc[2])), c.cy);
+                // all four taps in [1, W - 2] x [1, H - 2] (tested on the float: a NaN fails)
+                if (x >= 1.0f && x < static_cast<float>(c.W - 2) && y >= 1.0f && y < static_cast<float>(c.H - 2))
+                {
+                    const int64_t img = static_cast<int64_t>(c.W) * c.H;
+                    const float d = tp.depth[z * img + static_cast<int64_t>(__float2int_rz(FA(y, 0.5f))) * c.W + __float2int_rz(FA(x, 0.5f))];
+                    if (d > 0.0f && fabsf(FS(d, xc[2])) <= tp.max_distance)
+                    {
+                        const float xf = floorf(x), yf = floorf(y);
+                        const int x0 = __float2int_rz(xf), y0 = __float2int_rz(yf);
+                        const float fx = FS(x, xf), fy = FS(y, yf);
+                        const float If = tr_bilinear(tp.inten + z * img, c.W, x0, y0, fx, fy);
+                        const float gx = tr_bilinear(tp.gx + z * img, c.W, x0, y0, fx, fy);
+                        const float gy = tr_bilinear(tp.gy + z * img, c.W, x0, y0, fx, fy);
+                        const float rc = FS(If, tp.pint[pp]);
+                        if (fabsf(rc) <= tp.max_diff && FA(FM(gx, gx), FM(gy, gy)) >= tp.min_grad_sq)
+                        {
+                            // d r / d x_c, then world: g_w = R g_c; xi perturbs on the left, so J = [g_w x q, -g_w]
+                            const float gfx = FM(gx, c.fx), gfy = FM(gy, c.fy);
+                            const float gc[3] = {FD(gfx, xc[2]), FD(gfy, xc[2]), -FD(FA(FM(gfx, xc[0]), FM(gfy, xc[1])), FM(xc[2], xc[2]))};
+                            float gw[3];
+                            tr_xform(Tf, nullptr, gc, gw);
+                            double g[3], qd[3];
+#pragma unroll
+                            for (int k = 0; k < 3; ++k) { g[k] = static_cast<double>(gw[k]); qd[k] = static_cast<double>(q[k]); }
+                            J[0] = DS(DM(g[1], qd[2]), DM(g[2], qd[1]));
+                            J[1] = DS(DM(g[2], qd[0]), DM(g[0], qd[2]));
+                            J[2] = DS(DM(g[0], qd[1]), DM(g[1], qd[0]));
+                            J[3] = -g[0]; J[4] = -g[1]; J[5] = -g[2];
+                            r = static_cast<double>(rc);
+                            cnt = 1.0;
+                        }
+                    }
+                }
+            }
+        }
+    }
+    tr_tile_partials(warp_sums, J, r, cnt, tid, z, tp.tiles_x, tp.tiles_y, tp.partials);
+}
+
+// One thread per frame that is not frozen: the system k_track_solve reads, A = A_g + lam2 A_c and b = b_g + lam2 b_c (entries 0..26;
+// exactly the geometric entries for lam2 = 0), with the geometric sum r^2 and row count (27, 28); records the photometric system and
+// its rows and sum r^2 (the first and the last evaluated), and adds its rows to *rows.
+__global__ void k_track_combine(int n, double lam2, const double* __restrict__ sums_g, const double* __restrict__ sums_c,
+                                const TrackState* __restrict__ state, TrackColorState* __restrict__ cstate, double* __restrict__ out,
+                                double* __restrict__ sys_c, unsigned long long* rows)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n || state[k].frozen) return;
+    const double* G = sums_g + static_cast<int64_t>(k) * kTrackVals;
+    const double* P = sums_c + static_cast<int64_t>(k) * kTrackVals;
+    double* o = out + static_cast<int64_t>(k) * kTrackVals;
+    double* sc = sys_c + static_cast<int64_t>(k) * kTrackVals;
+    for (int j = 0; j < 27; ++j) o[j] = lam2 == 0.0 ? G[j] : DA(G[j], DM(lam2, P[j]));
+    o[27] = G[27]; o[28] = G[28];
+    for (int j = 0; j < kTrackVals; ++j) sc[j] = P[j];
+    TrackColorState& cs = cstate[k];
+    const long long nr = static_cast<long long>(P[28]);
+    if (!cs.have_first) { cs.first_rows = nr; cs.first_sq = P[27]; cs.have_first = 1; }
+    cs.last_rows = nr; cs.last_sq = P[27];
+    atomicAdd(rows, static_cast<unsigned long long>(nr));
 }
 
 // One thread per frame.  Records the system; with solve = 1: freezes on too few rows or a non-finite system, factors A = L L^T

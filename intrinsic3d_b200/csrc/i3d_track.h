@@ -52,15 +52,52 @@ struct TrackRows
     int tiles_x, tiles_y;
 };
 
+// One photometric rows launch (DESIGN.md §6p): level `cam` of the chunk's frames [gridDim.z]; pixel (u, v) samples the prediction pixel
+// (step u, step v), step = 2^l, of the level-0 prediction depth / model intensity, and frame z reads the level's intensity, gradient and
+// depth planes + z * W * H.
+struct TrackPhoto
+{
+    TrackCam cam, pcam;
+    int step;
+    const float* inten; const float* gx; const float* gy; const float* depth;   // level planes [n][H][W]
+    const float* pdepth; const float* pint;                                     // prediction [n][H0][W0]
+    const int32_t* ids; const float* rt_in;
+    const TrackState* state;
+    float max_distance, max_diff, min_grad_sq;
+    double* partials;                                     // [n][tiles][kTrackVals]
+    int tiles_x, tiles_y;
+};
+
+// Per-frame photometric outcome of a call (k_track_combine): rows and sum r^2 of the first and the last evaluated system
+struct TrackColorState
+{
+    long long first_rows, last_rows;
+    double first_sq, last_sq;
+    int have_first, pad;
+};
+
 // Tracker scratch of an engine (grows only): the per-call state of n frames, and the chunk's prediction, pyramid, normal and mask planes.
-// The planes of the last chunk stay for i3d_debug_get_track_planes.
+// The planes of the last chunk stay for i3d_debug_get_track_planes.  With a photometric term also the model intensity, the frame
+// intensity pyramid with its gradients (i3d_debug_get_track_color_planes), the photometric systems and the combined ones.
 struct TrackScratch
 {
     Dev<float> rt; Dev<int32_t> ids; Dev<double> pose_in; Dev<TrackState> state;
     Dev<double> sys, sums, partials, rd_partials, rd_sums; Dev<unsigned long long> counters;
     Dev<float> pdepth, pnrm, depth[kTrackMaxLevels], nrm[kTrackMaxLevels]; Dev<uint8_t> mask;
     Dev<int> live_box; Dev<uint32_t> live_bits;           // box and brick bitmap of the fusion volume in progress, rebuilt per use
+    Dev<float> pint, lum_c, inten[kTrackMaxLevels], gx[kTrackMaxLevels], gy[kTrackMaxLevels];
+    Dev<double> sys_c, sums_c, sums_comb, partials_c; Dev<TrackColorState> cstate; Dev<int32_t> iota;
     int n = 0, levels = 0, last_m = 0, W[kTrackMaxLevels] = {}, H[kTrackMaxLevels] = {};
+    bool color = false;                                   // the last call had a photometric term
+};
+
+// The photometric term of a call: its parameters (validated by the caller), the store whose colour frames it reads, and the per-frame
+// outcome (may be nullptr)
+struct TrackColor
+{
+    const I3DTrackColorParams* P;
+    const SensorStore* ss;
+    I3DTrackColorInfo* info;
 };
 
 namespace track
@@ -70,21 +107,25 @@ namespace track
 // geometry only; rg is the grid without its voxel box, built in rs when the voxel set changed), the depth pyramid (frames::depthdown on
 // the gathered store depth) with its normals, then every Gauss-Newton iteration of every level, coarsest first, with no host
 // synchronisation; one read-back at the end.  Writes only ts, rs's voxel box, pose_out [n][12] and info [n].
+// col (nullptr: depth only) adds the photometric term of DESIGN.md §6p: the colour march (model intensity), the frame intensity pyramid
+// with its gradients timed as "track_color", and per system k_track_photo_rows and k_track_combine before the unchanged solve.
 void sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderGrid rg, const I3DFusionCamera& dc, const float* store_depth, int store_F,
                    int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out,
-                   I3DTrackInfo* info, cudaStream_t st);
+                   I3DTrackInfo* info, cudaStream_t st, const TrackColor* col = nullptr);
 // sensor_frames with the prediction marched from the fusion volume in progress (k_render_march_live; fs unchanged) instead of a grid.  The
 // box and bitmap of the volume's voxels with weight > 0 are built first, timed as "track_bricks"; skip: march with the bitmap
 // (i3d_debug_set_render_skip).  Returns non-zero, having tracked nothing, when no voxel has weight > 0.
 int fusion_frames(TrackScratch& ts, const FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids,
-                  const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, cudaStream_t st);
+                  const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, cudaStream_t st,
+                  const TrackColor* col = nullptr);
 // Dense frame-to-model odometry over the stored frames ids[0..n) (validated by the caller; repeats allowed), in list order.  Per frame:
 // the guess (pose_first for ids[0] when given, which resets fs's motion state; else constant velocity from it), then with no voxel of
 // weight > 0 the frame is integrated at the guess (I3D_TRACK_ANCHORED), otherwise fusion_frames' tracking of that one frame (m = 1) and,
 // at status 0 only, fusion::integrate at the tracked pose.  Timed as "odometry" (host wall time of the call), "odometry_predict",
 // "odometry_icp" and the fusion phases.  Returns non-zero with the message in `error` when fusion::integrate fails.
 int odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids, const double* pose_first,
-             const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, std::string& error, cudaStream_t st);
+             const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, std::string& error, cudaStream_t st,
+             const TrackColor* col = nullptr);
 } // namespace track
 
 } // namespace i3d

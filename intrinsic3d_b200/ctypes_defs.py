@@ -265,3 +265,21 @@ class I3DTrackInfo(C.Structure, _Dictable):
         out = _Dictable.as_dict(self)
         out["initial"] = self.initial.as_dict()
         return out
+
+
+class I3DTrackColorParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("weight", C.c_float * TRACK_LEVELS),
+        ("max_color_diff", C.c_float),
+        ("min_color_gradient", C.c_float),
+        ("reserved", C.c_int32 * 2),
+    ]
+
+
+class I3DTrackColorInfo(C.Structure, _Dictable):
+    _fields_ = [
+        ("first_rows", C.c_int64),
+        ("first_residual_sq", C.c_double),
+        ("last_rows", C.c_int64),
+        ("last_residual_sq", C.c_double),
+    ]

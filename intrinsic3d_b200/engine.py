@@ -12,7 +12,8 @@ import os
 import numpy as np
 
 from .ctypes_defs import (RENDER_PLANES, I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo,
-                          I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats, I3DTrackInfo, I3DTrackParams, TRACK_LEVELS)
+                          I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats, I3DTrackColorInfo, I3DTrackColorParams, I3DTrackInfo,
+                          I3DTrackParams, TRACK_LEVELS)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("I3D_LIB", os.path.join(_HERE, "libi3d_b200.so"))   # I3D_LIB: A/B builds of the same library
@@ -36,6 +37,9 @@ EXPORTED_SYMBOLS = [
     "i3d_debug_set_render_skip",
     "i3d_sizeof_track_params", "i3d_sizeof_track_info", "i3d_default_track_params", "i3d_track_sensor_frames", "i3d_debug_get_track_system",
     "i3d_debug_get_track_planes", "i3d_fusion_track_sensor_frames", "i3d_fusion_track_and_integrate_sensor",
+    "i3d_sizeof_track_color_params", "i3d_sizeof_track_color_info", "i3d_default_track_color_params", "i3d_track_sensor_frames_rgbd",
+    "i3d_fusion_track_sensor_frames_rgbd", "i3d_fusion_track_and_integrate_sensor_rgbd", "i3d_debug_get_track_color_planes",
+    "i3d_debug_get_track_color_system",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
     "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_pcg_vectors", "i3d_debug_get_normal_equations",
@@ -112,6 +116,18 @@ def load_library():
     L.i3d_debug_get_track_system.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     L.i3d_debug_get_track_planes.restype = C.c_int
     L.i3d_debug_get_track_planes.argtypes = [C.c_void_p, C.c_int32] + [C.POINTER(C.c_float)] * 4 + [C.POINTER(C.c_uint8), C.POINTER(C.c_int32)]
+    L.i3d_sizeof_track_color_params.restype = C.c_uint64
+    L.i3d_sizeof_track_color_info.restype = C.c_uint64
+    if L.i3d_sizeof_track_color_params() != C.sizeof(I3DTrackColorParams) or L.i3d_sizeof_track_color_info() != C.sizeof(I3DTrackColorInfo):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (track colour structs)")
+    for fn in (L.i3d_track_sensor_frames_rgbd, L.i3d_fusion_track_sensor_frames_rgbd, L.i3d_fusion_track_and_integrate_sensor_rgbd):
+        fn.restype = C.c_int
+        fn.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(I3DTrackParams),
+                       C.POINTER(I3DTrackColorParams), C.POINTER(C.c_double), C.POINTER(I3DTrackInfo), C.POINTER(I3DTrackColorInfo)]
+    L.i3d_debug_get_track_color_planes.restype = C.c_int
+    L.i3d_debug_get_track_color_planes.argtypes = [C.c_void_p, C.c_int32] + [C.POINTER(C.c_float)] * 4 + [C.POINTER(C.c_int32)]
+    L.i3d_debug_get_track_color_system.restype = C.c_int
+    L.i3d_debug_get_track_color_system.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
     _LIB = L
     return L
 
@@ -141,6 +157,12 @@ def default_fusion_params() -> I3DFusionParams:
 def default_track_params() -> I3DTrackParams:
     p = I3DTrackParams()
     load_library().i3d_default_track_params(C.byref(p))
+    return p
+
+
+def default_track_color_params() -> I3DTrackColorParams:
+    p = I3DTrackColorParams()
+    load_library().i3d_default_track_color_params(C.byref(p))
     return p
 
 
@@ -489,7 +511,25 @@ class Engine:
                 raise ValueError(f"unknown tracking parameter {k!r}")
         return p
 
-    def _track_call(self, fn, ids, pose, name, n_pose, p):
+    @staticmethod
+    def _track_color_params(color):
+        """I3DTrackColorParams from a dict: weight (one value for every level, or up to 4 values, level 0 first), max_color_diff,
+        min_color_gradient; the rest keep default_track_color_params()."""
+        p = default_track_color_params()
+        for k, v in (color or {}).items():
+            if k == "weight":
+                v = [float(v)] * TRACK_LEVELS if np.ndim(v) == 0 else list(v) + [0.0] * (TRACK_LEVELS - len(v))
+                if len(v) != TRACK_LEVELS:
+                    raise ValueError(f"weight takes at most {TRACK_LEVELS} values")
+                for i, x in enumerate(v):
+                    p.weight[i] = float(x)
+            elif k in ("max_color_diff", "min_color_gradient"):
+                setattr(p, k, float(v))
+            else:
+                raise ValueError(f"unknown colour tracking parameter {k!r}")
+        return p
+
+    def _track_call(self, fn, ids, pose, name, n_pose, p, color=None):
         ids, n = self._ids(ids)
         if pose is not None:
             pose = np.ascontiguousarray(pose, np.float64)
@@ -497,8 +537,13 @@ class Engine:
                 raise ValueError(f"{name} must be [{n_pose(n)}, 12], got {pose.shape}")
         out = np.empty((max(n, 1), 12), np.float64)
         infos = (I3DTrackInfo * max(n, 1))()
-        self._check(fn(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(pose, C.c_double), C.byref(p), _p(out, C.c_double), infos))
-        return out[:n], [infos[i].as_dict() for i in range(n)]
+        if color is None:
+            self._check(fn(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(pose, C.c_double), C.byref(p), _p(out, C.c_double), infos))
+            return out[:n], [infos[i].as_dict() for i in range(n)]
+        cinfos = (I3DTrackColorInfo * max(n, 1))()
+        self._check(fn(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(pose, C.c_double), C.byref(p), C.byref(color), _p(out, C.c_double), infos,
+                       cinfos))
+        return out[:n], [dict(infos[i].as_dict(), color=cinfos[i].as_dict()) for i in range(n)]
 
     def track_sensor_frames(self, ids, pose_w2c, source: str = "fused", **params):
         """Point-to-plane ICP of the stored frames `ids` (distinct) against the surface of `source` ("fused": sdf0, "refined"), over the
@@ -524,6 +569,50 @@ class Engine:
         p = self._track_params(0, params)
         pose = None if pose_first is None else np.asarray(pose_first, np.float64).reshape(1, 12)
         return self._track_call(self.L.i3d_fusion_track_and_integrate_sensor, ids, pose, "pose_first", lambda n: 1, p)
+
+    # ---- tracking with colour as well as depth (DESIGN.md §6p) ------------------------------------------------------------------
+    def track_sensor_frames_rgbd(self, ids, pose_w2c, source: str = "fused", color=None, **params):
+        """track_sensor_frames with the photometric term: color = dict of I3DTrackColorParams fields (weight: lambda for every level
+        or up to 4 values, level 0 first; max_color_diff; min_color_gradient), the rest default_track_color_params().  Returns
+        (poses, infos); each info also has "color": the photometric rows and sum r^2 of the first and the last evaluated system."""
+        p = self._track_params(self._mesh_source(source), params)
+        return self._track_call(self.L.i3d_track_sensor_frames_rgbd, ids, pose_w2c, "pose_w2c", lambda n: n, p, self._track_color_params(color))
+
+    def fusion_track_sensor_frames_rgbd(self, ids, pose_w2c, color=None, **params):
+        """fusion_track_sensor_frames with the photometric term (see track_sensor_frames_rgbd)."""
+        p = self._track_params(0, params)
+        return self._track_call(self.L.i3d_fusion_track_sensor_frames_rgbd, ids, pose_w2c, "pose_w2c", lambda n: n, p,
+                                self._track_color_params(color))
+
+    def fusion_track_and_integrate_sensor_rgbd(self, ids, pose_first=None, color=None, **params):
+        """fusion_track_and_integrate_sensor (dense odometry) with the photometric term (see track_sensor_frames_rgbd)."""
+        p = self._track_params(0, params)
+        pose = None if pose_first is None else np.asarray(pose_first, np.float64).reshape(1, 12)
+        return self._track_call(self.L.i3d_fusion_track_and_integrate_sensor_rgbd, ids, pose, "pose_first", lambda n: 1, p,
+                                self._track_color_params(color))
+
+    def debug_track_color_system(self, n):
+        """the unweighted photometric sums float64 [n, 29] of the last evaluated system of each frame of the last _rgbd call of n frames"""
+        sums = np.empty((n, 29), np.float64)
+        self._check(self.L.i3d_debug_get_track_color_system(self.h, _p(sums, C.c_double)))
+        return sums
+
+    def debug_track_color_planes(self, level, frames):
+        """The last pass's colour planes of the last _rgbd call (`frames` = its frame count): model_intensity [frames, H, W] and the
+        frame intensity / grad_x / grad_y at pyramid `level`."""
+        dc = self._sensor_cams[0]
+        W, H = dc.width, dc.height
+        Wl, Hl = W, H
+        for _ in range(level):
+            Wl, Hl = Wl // 2, Hl // 2
+        out = dict(model_intensity=np.empty((frames, H, W), np.float32), intensity=np.empty((frames, Hl, Wl), np.float32),
+                   grad_x=np.empty((frames, Hl, Wl), np.float32), grad_y=np.empty((frames, Hl, Wl), np.float32))
+        m = C.c_int32(0)
+        self._check(self.L.i3d_debug_get_track_color_planes(self.h, C.c_int32(int(level)), _p(out["model_intensity"], C.c_float),
+                                                            _p(out["intensity"], C.c_float), _p(out["grad_x"], C.c_float),
+                                                            _p(out["grad_y"], C.c_float), C.byref(m)))
+        assert m.value == frames, (m.value, frames)
+        return out
 
     def debug_track_system(self, n):
         """(sums float64 [n, 29], pose camera -> world float64 [n, 12]) of the last tracking call of n frames."""
