@@ -2,7 +2,7 @@
 """bench_rgbd_odometry.py — dense RGB-D odometry depth-only (i3d_fusion_track_and_integrate_sensor) and with the photometric term
 (i3d_fusion_track_and_integrate_sensor_rgbd) side by side over every frame of a workload, one JSON line.
 
-    python bench_rgbd_odometry.py [--workload c2|c3|small|tiny] [--frames 200] [--weights 0.1] [--reps 1]
+    python bench_rgbd_odometry.py [--workload c2|c3|small|tiny] [--frames 200] [--weights 0.1] [--ref-weights 0.01,0.05] [--reps 1]
 
 The workload's frames go into the sensor store; each run begins a fusion and runs the loop over all frames from the true pose of frame 0
 (anchored) with the default tracking parameters, once depth-only and once per colour weight in --weights (lambda for every level, the
@@ -10,7 +10,9 @@ other colour parameters at their defaults).  Reported per mode, the median over 
 pose errors against the true poses (median and max), the first frame that breaks the 0.2 deg / 2 mm gates, the wall time (phase "odometry",
 host clock, ends in a synchronise) in total and per frame, and the device phases.  For each colour mode one more run with the per-kernel
 timers gives the time of k_track_photo_rows ("track_photo_rows") and its byte-model share of 3350 GB/s.  The GPU name and power limit are
-read in the same run.  Writes nothing.
+read in the same run.  --ref-weights adds, in the same format, one mode per weight of the loop with the reference model
+(i3d_fusion_track_and_integrate_sensor_rgbd_ref, DESIGN.md §6q), whose timed run gives k_track_ref_model ("track_ref_model") and its
+byte-model share.  Writes nothing.
 """
 import argparse
 import json
@@ -30,6 +32,9 @@ HBM_GBS = 3350.0
 # k_track_photo_rows' byte model per pixel of a level and per system, an upper bound as if every pixel passed every gate: prediction
 # depth and model intensity (8 B), the occlusion depth tap (4 B), four bilinear taps of intensity, grad_x and grad_y (48 B)
 PHOTO_BYTES_PER_PIXEL = 60
+# k_track_ref_model's byte model per pixel of a level and per frame, an upper bound as if every pixel passed every test: prediction depth
+# (4 B), the reference depth tap (4 B), four intensity taps (16 B) and the model write (4 B)
+REF_BYTES_PER_PIXEL = 28
 
 
 def main():
@@ -37,6 +42,7 @@ def main():
     ap.add_argument("--workload", default="c2", choices=("c3", "c2", "small", "tiny"))
     ap.add_argument("--frames", type=int, default=200)
     ap.add_argument("--weights", default="0.1")
+    ap.add_argument("--ref-weights", default="")
     ap.add_argument("--reps", type=int, default=1)
     args = ap.parse_args()
 
@@ -60,24 +66,30 @@ def main():
     true = tr.aa_to_rt(s["poses_true"])
     tp = engine.default_track_params()
     pixels_per_frame = sum(tp.iterations[l] * (W >> l) * (H >> l) for l in range(tp.num_levels))
+    level_pixels = sum((W >> l) * (H >> l) for l in range(tp.num_levels))
 
-    def run(weight, timers=False):
+    def run(mode, timers=False):
         e.set_kernel_timers(1 if timers else 0)
         e.fusion_begin(p)
+        ref, weight = mode
         if weight is None:
             out, infos = e.fusion_track_and_integrate_sensor(ids, true[0])
+        elif ref:
+            out, infos = e.fusion_track_and_integrate_sensor_rgbd_ref(ids, true[0], color=dict(weight=weight))
         else:
             out, infos = e.fusion_track_and_integrate_sensor_rgbd(ids, true[0], color=dict(weight=weight))
         e.set_kernel_timers(0)
         return out, infos
 
-    modes = [None] + [float(w) for w in args.weights.split(",")]
+    modes = [(False, None)] + [(False, float(w)) for w in args.weights.split(",")]
+    modes += [(True, float(w)) for w in args.ref_weights.split(",") if w]
     run(modes[0])                                                       # warm-up
     results = {}
-    for w in modes:
+    for mode in modes:
+        ref, w = mode
         wall, dev = [], {k: [] for k in PHASES}
         for _ in range(max(1, args.reps)):
-            out, infos = run(w)
+            out, infos = run(mode)
             wall.append(e.phase_ms("odometry"))
             for k in PHASES:
                 dev[k].append(e.phase_ms(k))
@@ -94,14 +106,20 @@ def main():
                "correspondences": int(e.phase_count("odometry_correspondences"))}
         if w is not None:
             res["photo_correspondences"] = int(e.phase_count("odometry_photo_correspondences"))
-            run(w, timers=True)
+            run(mode, timers=True)
             ms = e.phase_ms("track_photo_rows")
             gb = F * pixels_per_frame * PHOTO_BYTES_PER_PIXEL / 1e9
             res["k_track_photo_rows"] = {"ms": ms, "launches": int(e.phase_count("track_photo_rows")), "model_gb": gb,
                                          "gbs": gb / (ms / 1e3) if ms > 0 else None,
                                          "share_of_hbm": gb / (ms / 1e3) / HBM_GBS if ms > 0 else None}
-        results["depth_only" if w is None else f"color_w{w:g}"] = res
-    line = {"metric": "rgbd_odometry_all_frames_ms", "value": results[f"color_w{modes[1]:g}"]["wall_ms"], "unit": "ms",
+            if ref:
+                ms = e.phase_ms("track_ref_model")
+                n = int(e.phase_count("track_ref_model"))
+                gb = n // tp.num_levels * level_pixels * REF_BYTES_PER_PIXEL / 1e9
+                res["k_track_ref_model"] = {"ms": ms, "launches": n, "model_gb": gb, "gbs": gb / (ms / 1e3) if ms > 0 else None,
+                                            "share_of_hbm": gb / (ms / 1e3) / HBM_GBS if ms > 0 else None}
+        results["depth_only" if w is None else (f"ref_w{w:g}" if ref else f"color_w{w:g}")] = res
+    line = {"metric": "rgbd_odometry_all_frames_ms", "value": results[f"color_w{modes[1][1]:g}"]["wall_ms"], "unit": "ms",
             "higher_is_better": False, "workload": args.workload, "gpu": gpu, "reps": max(1, args.reps), "frames": int(F),
             "size": [int(W), int(H)], "modes": results}
     print(json.dumps(line))

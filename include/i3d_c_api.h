@@ -315,6 +315,39 @@ int         i3d_debug_get_track_color_planes(I3DEngine* e, int32_t level, float*
  * i3d_debug_get_track_system, unweighted.  Fails when the last tracking call had no photometric term. */
 int         i3d_debug_get_track_color_system(I3DEngine* e, double* sums);
 
+/* ---- the photometric term against a reference frame's image (DESIGN.md §6q) ---- */
+/* i3d_default_track_color_params with weight {0.01, 0.01, 0.01, 0.01}: the best of the weights measured with the reference model on C2
+ * (DESIGN.md §6q). */
+void        i3d_default_track_color_ref_params(I3DTrackColorParams* p);
+/* The _rgbd calls with the model intensity taken from a reference frame instead of the voxel colours: the prediction is marched without
+ * colour, and at level l the model value of prediction pixel (2^l u, 2^l v) with a hit is the stored frame ref_ids[k]'s level-l intensity
+ * (the frame's own rules: intensity in the depth camera, then pyrDown), bilinear at the projection of the model point q with ref_pose[k]
+ * (world -> camera [12], R row-major | t, used in float), when the projection lies in [1, W_l - 2) x [1, H_l - 2) and the reference's
+ * level-l depth at the rounded pixel is > 0 and within max_distance of q's depth there; else no photometric row.  A frame may be its own
+ * reference.  Fail, writing nothing, for every refusal of the matching _rgbd call, NULL ref_ids or ref_pose, a reference id out of range
+ * and a non-finite reference pose.  Device time as the _rgbd call, plus i3d_phase_ms("track_reference") (the references' pyramids and
+ * model planes); with i3d_debug_set_kernel_timers(e, 1) also "track_ref_model". */
+int         i3d_track_sensor_frames_rgbd_ref(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const int32_t* ref_ids,
+                                             const double* ref_pose, const I3DTrackParams* params, const I3DTrackColorParams* color,
+                                             double* pose_out, I3DTrackInfo* info, I3DTrackColorInfo* color_info);
+int         i3d_fusion_track_sensor_frames_rgbd_ref(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const int32_t* ref_ids,
+                                                    const double* ref_pose, const I3DTrackParams* params, const I3DTrackColorParams* color,
+                                                    double* pose_out, I3DTrackInfo* info, I3DTrackColorInfo* color_info);
+/* Dense odometry with the reference model: each frame's reference is the last frame this loop integrated (anchored or tracked), at the
+ * camera -> world pose it was integrated with.  The reference lives in the fusion beside the motion state and is cleared where that is
+ * (i3d_fusion_begin, every i3d_fusion_integrate* call, a pose_first) and by i3d_sensor_frames_begin, whose new store no longer holds it;
+ * a frame without one is tracked on depth alone, with zero color_info.
+ * Timed as the _rgbd loop; the reference work counts as "odometry_icp". */
+int         i3d_fusion_track_and_integrate_sensor_rgbd_ref(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_first,
+                                                           const I3DTrackParams* params, const I3DTrackColorParams* color, double* pose_out,
+                                                           I3DTrackInfo* info, I3DTrackColorInfo* color_info);
+/* Parity hook: the planes of the last pass of the last _ref call at pyramid `level`, compact [m][H_l][W_l] each: the model value (the quiet
+ * NaN where there is none), and the references' intensity and depth.  Any pointer may be NULL; m in *frames.  Fails when the last
+ * tracking call was not a _ref call with a reference and for a level it did not build.  After a _ref call
+ * i3d_debug_get_track_color_planes refuses a non-NULL model_intensity. */
+int         i3d_debug_get_track_reference_planes(I3DEngine* e, int32_t level, float* model, float* ref_intensity, float* ref_depth,
+                                                 int32_t* frames);
+
 /* ---- keyframe selection and the RGB-D image pyramid: the inputs of fusion and refinement (DESIGN.md §6i) ---- */
 /* Frames scored per device pass by i3d_keyframe_scores: bounds its scratch memory (I3D_KEYFRAME_CHUNK * W * H * 3 bytes). */
 #define I3D_KEYFRAME_CHUNK 32
@@ -338,7 +371,8 @@ int         i3d_use_rgbd_level(I3DEngine* e, int32_t lvl, int32_t* W_out, int32_
 /* Starts an empty store of `capacity` frames (Sensor::depth(i) / Sensor::color(i)) and allocates its device memory for all of them:
  * depth float metres [depth_cam.height][depth_cam.width], already range-thresholded as i3d_fusion_integrate takes it, and colour uint8
  * [color_cam.height][color_cam.width][3] interleaved B,G,R.  Replaces any previous store; the frame store of i3d_upload_rgbd_frames is a
- * separate one and is left alone.  Fails for a camera without a positive size, finite intrinsics and fx, fy > 0, and for capacity <= 0. */
+ * separate one and is left alone.  Clears the reference of the _ref odometry (a frame of the replaced store); the next frame of that loop
+ * is tracked on depth alone.  Fails for a camera without a positive size, finite intrinsics and fx, fy > 0, and for capacity <= 0. */
 int         i3d_sensor_frames_begin(I3DEngine* e, const I3DFusionCamera* depth_cam, const I3DFusionCamera* color_cam, int32_t capacity);
 /* Appends F frames (ids i3d_sensor_num_frames(), +1, ...): depth [F][...] and bgr [F][...] in the layouts above.  Fails without a store,
  * for F <= 0 and beyond the capacity. */

@@ -1565,6 +1565,7 @@ int i3d_sensor_frames_begin(I3DEngine* e, const I3DFusionCamera* depth_cam, cons
         return fail(e, "i3d_sensor_frames_begin: bad camera (a positive size, finite intrinsics and fx, fy > 0 are needed)");
     if (capacity <= 0) return fail(e, "i3d_sensor_frames_begin: capacity must be > 0 (got %d)", capacity);
     e->sensor.F = 0; e->sensor.cap = 0;
+    e->fusion.ref_id = -1;             // the _ref odometry's reference is a frame of the store being replaced (DESIGN.md §6q)
     return guarded(e, [&]() { frames::sensor_begin(e->sensor, *depth_cam, *color_cam, capacity); return 0; });
 }
 
@@ -1841,9 +1842,24 @@ static int check_track_color(I3DEngine* e, const char* who, const I3DTrackColorP
     return 0;
 }
 
-// i3d_track_sensor_frames, with the photometric term cp when it is not nullptr (the _rgbd call)
+// The references of a _ref call (DESIGN.md §6q), n frames; completes col
+struct TrackReference { bool on; const int32_t* ids; const double* pose; };
+static int check_track_reference(I3DEngine* e, const char* who, int32_t n, const TrackReference& ref, TrackColor& col)
+{
+    if (!ref.ids || !ref.pose) return fail(e, "%s: ref_ids and ref_pose must not be NULL", who);
+    for (int32_t k = 0; k < n; ++k)
+        if (ref.ids[k] < 0 || ref.ids[k] >= e->sensor.F)
+            return fail(e, "%s: reference id %d (entry %d) is out of range (%d stored frames)", who, ref.ids[k], k, e->sensor.F);
+    if (check_finite_poses(e, who, n, ref.pose, "the reference pose")) return 1;
+    col.ref_ids = ref.ids; col.ref_pose = ref.pose;
+    return 0;
+}
+static constexpr TrackReference kNoReference{false, nullptr, nullptr};
+
+// i3d_track_sensor_frames, with the photometric term cp when it is not nullptr (the _rgbd call) and its reference model (the _ref call)
 static int track_sensor_frames(I3DEngine* e, const char* who, int32_t n, const int32_t* ids, const double* pose_in, const I3DTrackParams* params,
-                               double* pose_out, I3DTrackInfo* info, bool rgbd, const I3DTrackColorParams* cp, I3DTrackColorInfo* ci)
+                               double* pose_out, I3DTrackInfo* info, bool rgbd, const I3DTrackColorParams* cp, I3DTrackColorInfo* ci,
+                               const TrackReference& ref = kNoReference)
 {
     if (!e) return 1;
     if (!params || !pose_in || !pose_out) return fail(e, "%s: params, pose_in and pose_out must not be NULL", who);
@@ -1858,6 +1874,7 @@ static int track_sensor_frames(I3DEngine* e, const char* who, int32_t n, const i
     if (check_track_params(e, who, P, Wl, Hl)) return 1;
     TrackColor col{};
     if (rgbd && check_track_color(e, who, cp, ci, col)) return 1;
+    if (ref.on && check_track_reference(e, who, n, ref, col)) return 1;
     return guarded(e, [&]() {
         track::sensor_frames(e->track, e->render, e->timing, render_grid(e, P.sdf_source, false), e->sensor.dcam, e->sensor.depth.p, e->sensor.F, n, ids, pose_in, P,
                              Wl, Hl, pose_out, info, e->stream, rgbd ? &col : nullptr);
@@ -1877,6 +1894,14 @@ int i3d_track_sensor_frames_rgbd(I3DEngine* e, int32_t n, const int32_t* ids, co
     return track_sensor_frames(e, "i3d_track_sensor_frames_rgbd", n, ids, pose_in, params, pose_out, info, true, color, color_info);
 }
 
+int i3d_track_sensor_frames_rgbd_ref(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const int32_t* ref_ids, const double* ref_pose,
+                                     const I3DTrackParams* params, const I3DTrackColorParams* color, double* pose_out, I3DTrackInfo* info,
+                                     I3DTrackColorInfo* color_info)
+{
+    return track_sensor_frames(e, "i3d_track_sensor_frames_rgbd_ref", n, ids, pose_in, params, pose_out, info, true, color, color_info,
+                               TrackReference{true, ref_ids, ref_pose});
+}
+
 // The checks of the two calls that track against the fusion in progress, up to the poses
 static int check_fusion_track(I3DEngine* e, const char* who, int32_t n, const int32_t* ids, const I3DTrackParams* params, double* pose_out)
 {
@@ -1888,7 +1913,7 @@ static int check_fusion_track(I3DEngine* e, const char* who, int32_t n, const in
 
 static int fusion_track_sensor_frames(I3DEngine* e, const char* who, int32_t n, const int32_t* ids, const double* pose_in,
                                       const I3DTrackParams* params, double* pose_out, I3DTrackInfo* info, bool rgbd, const I3DTrackColorParams* cp,
-                                      I3DTrackColorInfo* ci)
+                                      I3DTrackColorInfo* ci, const TrackReference& ref = kNoReference)
 {
     if (!e) return 1;
     if (!pose_in) return fail(e, "%s: pose_in must not be NULL", who);
@@ -1901,6 +1926,7 @@ static int fusion_track_sensor_frames(I3DEngine* e, const char* who, int32_t n, 
     if (check_track_params(e, who, P, Wl, Hl)) return 1;
     TrackColor col{};
     if (rgbd && check_track_color(e, who, cp, ci, col)) return 1;
+    if (ref.on && check_track_reference(e, who, n, ref, col)) return 1;
     return guarded(e, [&]() {
         if (track::fusion_frames(e->track, e->fusion, e->render.skip, e->timing, e->sensor, n, ids, pose_in, P, Wl, Hl, pose_out, info, e->stream,
                                  rgbd ? &col : nullptr))
@@ -1921,9 +1947,18 @@ int i3d_fusion_track_sensor_frames_rgbd(I3DEngine* e, int32_t n, const int32_t* 
     return fusion_track_sensor_frames(e, "i3d_fusion_track_sensor_frames_rgbd", n, ids, pose_in, params, pose_out, info, true, color, color_info);
 }
 
+int i3d_fusion_track_sensor_frames_rgbd_ref(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_in, const int32_t* ref_ids,
+                                            const double* ref_pose, const I3DTrackParams* params, const I3DTrackColorParams* color, double* pose_out,
+                                            I3DTrackInfo* info, I3DTrackColorInfo* color_info)
+{
+    return fusion_track_sensor_frames(e, "i3d_fusion_track_sensor_frames_rgbd_ref", n, ids, pose_in, params, pose_out, info, true, color, color_info,
+                                      TrackReference{true, ref_ids, ref_pose});
+}
+
+// reference: the loop's own reference model (DESIGN.md §6q)
 static int fusion_track_and_integrate_sensor(I3DEngine* e, const char* who, int32_t n, const int32_t* ids, const double* pose_first,
                                              const I3DTrackParams* params, double* pose_out, I3DTrackInfo* info, bool rgbd,
-                                             const I3DTrackColorParams* cp, I3DTrackColorInfo* ci)
+                                             const I3DTrackColorParams* cp, I3DTrackColorInfo* ci, bool reference = false)
 {
     if (!e) return 1;
     if (check_fusion_track(e, who, n, ids, params, pose_out)) return 1;
@@ -1939,7 +1974,7 @@ static int fusion_track_and_integrate_sensor(I3DEngine* e, const char* who, int3
     const int rc = guarded(e, [&]() {
         std::string err;
         if (track::odometry(e->track, e->fusion, e->render.skip, e->timing, e->sensor, n, ids, pose_first, P, Wl, Hl, pose_out, info, err, e->stream,
-                            rgbd ? &col : nullptr))
+                            rgbd ? &col : nullptr, reference))
             return fail(e, "%s: %s", who, err.c_str());
         return 0;
     });
@@ -1959,6 +1994,13 @@ int i3d_fusion_track_and_integrate_sensor_rgbd(I3DEngine* e, int32_t n, const in
 {
     return fusion_track_and_integrate_sensor(e, "i3d_fusion_track_and_integrate_sensor_rgbd", n, ids, pose_first, params, pose_out, info, true, color,
                                              color_info);
+}
+
+int i3d_fusion_track_and_integrate_sensor_rgbd_ref(I3DEngine* e, int32_t n, const int32_t* ids, const double* pose_first, const I3DTrackParams* params,
+                                                   const I3DTrackColorParams* color, double* pose_out, I3DTrackInfo* info, I3DTrackColorInfo* color_info)
+{
+    return fusion_track_and_integrate_sensor(e, "i3d_fusion_track_and_integrate_sensor_rgbd_ref", n, ids, pose_first, params, pose_out, info, true,
+                                             color, color_info, true);
 }
 
 int i3d_debug_get_track_system(I3DEngine* e, double* sums, double* pose_cam_to_world)
@@ -2015,6 +2057,8 @@ int i3d_debug_get_track_color_planes(I3DEngine* e, int32_t level, float* model_i
     if (!e) return 1;
     if (e->track.n <= 0 || !e->track.color) return fail(e, "%s: the last tracking call had no photometric term", who);
     if (level < 0 || level >= e->track.levels) return fail(e, "%s: level %d was not built (%d levels)", who, level, e->track.levels);
+    if (model_intensity && e->track.reference)
+        return fail(e, "%s: the last call took its model from reference frames (i3d_debug_get_track_reference_planes)", who);
     return guarded(e, [&]() {
         cudaStream_t st = e->stream;
         const size_t m = static_cast<size_t>(e->track.last_m);
@@ -2037,6 +2081,40 @@ int i3d_debug_get_track_color_system(I3DEngine* e, double* sums)
         if (sums)
             CK(cudaMemcpyAsync(sums, e->track.sys_c.p, static_cast<size_t>(e->track.n) * kTrackVals * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
         CK(cudaStreamSynchronize(e->stream));
+        return 0;
+    });
+}
+
+// ---- the reference model of the photometric term (i3d_track.cuh, DESIGN.md §6q) --------------------
+void i3d_default_track_color_ref_params(I3DTrackColorParams* p)
+{
+    i3d_default_track_color_params(p);
+    for (int l = 0; l < kTrackMaxLevels; ++l) p->weight[l] = 0.01f;      // measured on C2 (DESIGN.md §6q)
+}
+
+int i3d_debug_get_track_reference_planes(I3DEngine* e, int32_t level, float* model, float* ref_intensity, float* ref_depth, int32_t* frames)
+{
+    static const char* who = "i3d_debug_get_track_reference_planes";
+    if (!e) return 1;
+    if (e->track.n <= 0 || !e->track.reference) return fail(e, "%s: the last tracking call had no reference model", who);
+    if (level < 0 || level >= e->track.levels) return fail(e, "%s: level %d was not built (%d levels)", who, level, e->track.levels);
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const int m = e->track.last_m, W0 = e->track.W[0], H0 = e->track.H[0], Wl = e->track.W[level], Hl = e->track.H[level];
+        const size_t lv = static_cast<size_t>(m) * Wl * Hl;
+        if (ref_intensity) CK(cudaMemcpyAsync(ref_intensity, e->track.ref_inten[level].p, lv * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (ref_depth) CK(cudaMemcpyAsync(ref_depth, e->track.ref_depth[level].p, lv * sizeof(float), cudaMemcpyDeviceToHost, st));
+        // the model plane is in the level-0 layout: pixel (u, v) of level l at (2^l v) W0 + 2^l u
+        std::vector<float> full(model ? static_cast<size_t>(m) * W0 * H0 : 0);
+        if (model)
+            CK(cudaMemcpyAsync(full.data(), (level == 0 ? e->track.pint : e->track.ref_model[level]).p, full.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        const size_t s = size_t{1} << level;
+        for (size_t z = 0; model && z < static_cast<size_t>(m); ++z)
+            for (size_t v = 0; v < static_cast<size_t>(Hl); ++v)
+                for (size_t u = 0; u < static_cast<size_t>(Wl); ++u)
+                    model[(z * Hl + v) * Wl + u] = full[(z * H0 + s * v) * W0 + s * u];
+        if (frames) *frames = m;
         return 0;
     });
 }

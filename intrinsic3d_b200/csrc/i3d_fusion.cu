@@ -124,6 +124,7 @@ void fusion::begin(FusionState& fs, Timing& tm, const I3DFusionParams& P, cudaSt
     fuse_reset_table(fs, cap, st);
     fs.n = 0;
     fs.motion = 0;
+    fs.ref_id = -1;
     begin_timing(tm, {"fusion_prep", "fusion_alloc", "fusion_integrate", "fusion_correct", "fusion_finish", "fusion_growths", "fusion_sweeps"});
 }
 
@@ -152,6 +153,7 @@ int fusion::integrate(FusionState& fs, Timing& tm, int n, const I3DFusionCamera&
     const FuseCam cc{color_cam.width, color_cam.height, color_cam.fx, color_cam.fy, color_cam.cx, color_cam.cy};
     const FuseConst c = fuse_const(P);
     fs.motion = 0;
+    fs.ref_id = -1;
     begin_timing(tm, {});                        // the fusion phases were reset by begin
     for (int f = 0; f < n; ++f)
     {

@@ -33,6 +33,10 @@ struct FusionState
     // double, newest in motion_T[1]; begin and every integrate clear it
     int motion = 0;
     double motion_T[2][12] = {};
+    // the reference of the _ref odometry (DESIGN.md §6q): the last frame the loop integrated (-1: none) and its camera -> world pose;
+    // kept and cleared with the motion state, and cleared by i3d_sensor_frames_begin, since it indexes the sensor store
+    int32_t ref_id = -1;
+    double ref_T[12] = {};
 };
 
 namespace fusion

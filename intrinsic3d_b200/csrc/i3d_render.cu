@@ -144,16 +144,17 @@ namespace
 struct TrackPhases
 {
     const char* whole; const char* predict; const char* pyramid; const char* icp; const char* correspondences;
-    const char* color; const char* photo_correspondences;
+    const char* color; const char* photo_correspondences; const char* reference;
 };
 constexpr TrackPhases kTrackPhases{"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences", "track_color",
-                                   "track_photo_correspondences"};
+                                   "track_photo_correspondences", "track_reference"};
 constexpr TrackPhases kOdometryPhases{nullptr, "odometry_predict", "odometry_icp", "odometry_icp", "odometry_correspondences", "odometry_icp",
-                                      "odometry_photo_correspondences"};
+                                      "odometry_photo_correspondences", "odometry_icp"};
 
 // The tracker's passes over ids[0..n), shared by the grid and the fusion volume: prepare() (false: stop, nothing tracked) runs once
 // after the uploads, predict(cam, rv, mi) marches a chunk's prediction into rv, and with mi != nullptr the model intensity plane into mi.
-// pose_cw_out [n][12] (may be nullptr): the tracked camera -> world poses.  col: the photometric term (nullptr: depth only).  Returns
+// pose_cw_out [n][12] (may be nullptr): the tracked camera -> world poses.  col: the photometric term (nullptr: depth only); with its
+// reference the plain march, then per pass the references' pyramids and k_track_ref_model per level, timed as ph.reference.  Returns
 // false when prepare() stopped the call.
 template <class Prepare, class Predict>
 bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&& prepare, Predict&& predict, const I3DFusionCamera& dc,
@@ -162,6 +163,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
 {
     const int L = P.num_levels, W = dc.width, H = dc.height, C = std::min<int>(n, I3D_TRACK_CHUNK);
     const size_t img = static_cast<size_t>(W) * H;
+    const bool ref = col && col->ref_ids;
     const int tiles_x = (W + kRenderTile - 1) / kRenderTile, tiles_y = (H + kRenderTile - 1) / kRenderTile;
     static_assert(kRenderTile == kTrackTile, "the prediction and the rows share the level-0 tile grid");
     ts.n = 0;
@@ -176,6 +178,16 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
         const size_t c = static_cast<size_t>(C) * Wl[l] * Hl[l];
         ts.depth[l].ensure(c); ts.nrm[l].ensure(3 * c);
         if (col) { ts.inten[l].ensure(c); ts.gx[l].ensure(c); ts.gy[l].ensure(c); }
+        if (ref) { ts.ref_inten[l].ensure(c); ts.ref_depth[l].ensure(c); }
+        if (ref && l > 0) ts.ref_model[l].ensure(C * img);
+    }
+    std::vector<float> hr(ref ? 12 * static_cast<size_t>(n) : 0);      // the reference poses in float, by call order
+    if (ref)
+    {
+        for (size_t i = 0; i < hr.size(); ++i) hr[i] = static_cast<float>(col->ref_pose[i]);
+        ts.ref_ids.ensure(n); ts.ref_rt.ensure(hr.size());
+        CK(cudaMemcpyAsync(ts.ref_ids.p, col->ref_ids, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ts.ref_rt.p, hr.data(), hr.size() * sizeof(float), cudaMemcpyHostToDevice, st));
     }
     if (col)
     {
@@ -224,7 +236,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
             rv.ids = ids_d; rv.Rt = ts.rt.p; rv.depth = store_depth; rv.lum = nullptr;
             rv.out_depth = ts.pdepth.p; rv.out_normal = ts.pnrm.p;
             rv.partials = ts.rd_partials.p; rv.samples = ts.counters.p + 1; rv.photometric = 0;
-            predict(rcam, rv, col ? ts.pint.p : nullptr);
+            predict(rcam, rv, col && !ref ? ts.pint.p : nullptr);
             tile_sums<kRenderStats>(m, tiles_x * tiles_y, ts.rd_partials.p, ts.rd_sums.p + static_cast<size_t>(c0) * kRenderStats, st);
         }
         {
@@ -242,6 +254,29 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
             for (int l = 1; l < L; ++l) frames::pyrdown(m, Wl[l - 1], Hl[l - 1], ts.inten[l - 1].p, ts.inten[l].p, st);
             for (int l = 0; l < L; ++l)
                 k_track_grad<<<dim3(blocks_for(static_cast<size_t>(Wl[l]) * Hl[l]), m), kThreads, 0, st>>>(cam[l], ts.inten[l].p, ts.gx[l].p, ts.gy[l].p);
+        }
+        if (ref)
+        {
+            // the references' intensity and depth pyramids by the frame's own rules, then each level's model plane
+            Timer t(tm, st, ph.reference);
+            const int32_t* rids_d = ts.ref_ids.p + c0;
+            frames::sensor_intensity(*col->ss, m, col->ref_ids + c0, ts.iota.p, ts.lum_c, ts.ref_inten[0].p, st);
+            k_track_gather<<<dim3(blocks_for(img), m), kThreads, 0, st>>>(m, W, H, rids_d, store_depth, ts.ref_depth[0].p);
+            for (int l = 1; l < L; ++l)
+            {
+                frames::pyrdown(m, Wl[l - 1], Hl[l - 1], ts.ref_inten[l - 1].p, ts.ref_inten[l].p, st);
+                frames::depthdown(m, Wl[l - 1], Hl[l - 1], ts.ref_depth[l - 1].p, ts.ref_depth[l].p, st);
+            }
+            TrackRef tf{};
+            tf.pcam = cam[0]; tf.pdepth = ts.pdepth.p; tf.ids = ids_d; tf.rt_in = ts.rt.p; tf.ref_rt = ts.ref_rt.p + 12 * static_cast<size_t>(c0);
+            tf.max_distance = P.max_distance;
+            for (int l = 0; l < L; ++l)
+            {
+                tf.cam = cam[l]; tf.step = 1 << l; tf.inten = ts.ref_inten[l].p; tf.depth = ts.ref_depth[l].p;
+                tf.model = l == 0 ? ts.pint.p : ts.ref_model[l].p;
+                Timer tk(tm, st, "track_ref_model", 1);
+                k_track_ref_model<<<dim3(blocks_for(static_cast<size_t>(Wl[l]) * Hl[l]), m), kThreads, 0, st>>>(tf);
+            }
         }
         {
             Timer t(tm, st, ph.icp);
@@ -269,6 +304,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
                 if (col)
                 {
                     tp.cam = cam[l]; tp.step = 1 << l; tp.inten = ts.inten[l].p; tp.gx = ts.gx[l].p; tp.gy = ts.gy[l].p; tp.depth = ts.depth[l].p;
+                    if (ref) tp.pint = l == 0 ? ts.pint.p : ts.ref_model[l].p;
                     tp.tiles_x = tr.tiles_x; tp.tiles_y = tr.tiles_y;
                     {
                         Timer tk(tm, st, "track_photo_rows", 1);
@@ -313,7 +349,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
         r.initial = render_stats(rs_sums.data() + static_cast<size_t>(k) * kRenderStats);
         info[k] = r;
     }
-    ts.n = n; ts.levels = L; ts.last_m = m; ts.color = col != nullptr;
+    ts.n = n; ts.levels = L; ts.last_m = m; ts.color = col != nullptr; ts.reference = ref;
     for (int l = 0; l < L; ++l) { ts.W[l] = Wl[l]; ts.H[l] = Hl[l]; }
     return true;
 }
@@ -393,7 +429,7 @@ void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderG
                           double* pose_out, I3DTrackInfo* info, cudaStream_t st, const TrackColor* col)
 {
     begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences", "track_color", "track_photo_rows",
-                      "track_photo_correspondences"});
+                      "track_photo_correspondences", "track_reference", "track_ref_model"});
     track_passes(
         ts, tm, kTrackPhases, [&]() { add_voxel_box(rs, tm, rg, st); return true; },
         [&](const RenderCam& cam, const RenderViews& rv, float* mi) { march(rg, cam, rv, st, mi); }, dc, store_depth, store_F, n, ids, pose_in, P,
@@ -405,7 +441,7 @@ int track::fusion_frames(TrackScratch& ts, const FusionState& fs, bool skip, Tim
                          const TrackColor* col)
 {
     begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences", "track_bricks", "track_color",
-                      "track_photo_rows", "track_photo_correspondences"});
+                      "track_photo_rows", "track_photo_correspondences", "track_reference", "track_ref_model"});
     LiveGrid lg{};
     const bool ok = track_passes(
         ts, tm, kTrackPhases, [&]() { return live_box(ts, tm, "track_bricks", fusion::view(fs), fs.p.voxel_size, skip, lg, st); },
@@ -417,15 +453,19 @@ int track::fusion_frames(TrackScratch& ts, const FusionState& fs, bool skip, Tim
 
 int track::odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids, const double* pose_first,
                     const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, std::string& error, cudaStream_t st,
-                    const TrackColor* col)
+                    const TrackColor* col, bool reference)
 {
     const auto t0 = std::chrono::steady_clock::now();
-    for (const char* nm : {"odometry", "odometry_predict", "odometry_icp", "odometry_correspondences", "odometry_photo_correspondences", "track_photo_rows"})
+    for (const char* nm : {"odometry", "odometry_predict", "odometry_icp", "odometry_correspondences", "odometry_photo_correspondences", "track_photo_rows",
+                           "track_ref_model"})
         tm.phases.erase(nm);
-    // the motion state, kept here while fusion::integrate (which clears fs's) runs
+    // the motion state and the reference, kept here while fusion::integrate (which clears fs's) runs
     int motion = pose_first ? 0 : fs.motion;
     double prev[12], last[12];
     std::memcpy(prev, fs.motion_T[0], sizeof(prev)); std::memcpy(last, fs.motion_T[1], sizeof(last));
+    int32_t ref_id = pose_first ? -1 : fs.ref_id;
+    double ref_T[12];
+    std::memcpy(ref_T, fs.ref_T, sizeof(ref_T));
     for (int k = 0; k < n; ++k)
     {
         // the guess: T_cw(k) = T_cw(k-1) . (T_cw(k-2)^-1 . T_cw(k-1)), or T_cw(k-1) with one previous pose
@@ -463,11 +503,18 @@ int track::odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, co
         else
         {
             TrackColor c1{};
+            double ref_W[12];
             if (col) c1 = TrackColor{col->P, col->ss, &rc};
+            if (reference && ref_id >= 0)
+            {
+                pose_inverse(ref_T, ref_W);
+                c1.ref_ids = &ref_id; c1.ref_pose = ref_W;
+            }
+            const bool with_color = col && (!reference || ref_id >= 0);          // no reference yet: depth alone
             track_passes(
                 ts, tm, kOdometryPhases, []() { return true; },
                 [&](const RenderCam& cam, const RenderViews& rv, float* mi) { march_live(lg, cam, rv, fs.rgb.p, mi, st); }, ss.dcam, ss.depth.p, ss.F,
-                1, ids + k, W, P, Wl, Hl, Wt, Tt, &r, st, col ? &c1 : nullptr);
+                1, ids + k, W, P, Wl, Hl, Wt, Tt, &r, st, with_color ? &c1 : nullptr);
             if (r.status == I3D_TRACK_OK) { Ti = Tt; Wi = Wt; }
         }
         if (Ti)
@@ -477,6 +524,8 @@ int track::odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, co
             if (fusion::integrate(fs, tm, 1, ss.dcam, ss.depth.p, ss.ccam, ss.bgr.p, ids + k, c2w, w2c, error, st)) return 1;
             std::memcpy(prev, last, sizeof(prev)); std::memcpy(last, Ti, sizeof(last));
             motion = std::min(motion + 1, 2);
+            ref_id = ids[k];
+            std::memcpy(ref_T, Ti, sizeof(ref_T));
         }
         else
         {
@@ -486,6 +535,8 @@ int track::odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, co
         }
         fs.motion = motion;
         std::memcpy(fs.motion_T[0], prev, sizeof(prev)); std::memcpy(fs.motion_T[1], last, sizeof(last));
+        fs.ref_id = ref_id;
+        std::memcpy(fs.ref_T, ref_T, sizeof(ref_T));
         std::memcpy(pose_out + 12 * static_cast<size_t>(k), Wi ? Wi : W, 12 * sizeof(double));
         if (info) info[k] = r;
         if (col && col->info) col->info[k] = rc;

@@ -16,6 +16,10 @@
  *                       projection, the gates and the row [g_w x q, -g_w], reduced as k_track_rows reduces
  *   k_track_combine     one thread per frame: A_g + lam^2 A_c, b_g + lam^2 b_c, the geometric r^2 and rows, for the unchanged k_track_solve
  *
+ * The reference model of the _ref calls (DESIGN.md §6q), which replaces the voxel colours as k_track_photo_rows' model intensity:
+ *   k_track_ref_model   one thread per pixel of a level: the model point of prediction pixel (2^l u, 2^l v) sampled from the frame's
+ *                       reference image at the reference's pose, or the quiet NaN
+ *
  * Compiled with the renderer in i3d_render.cu, which launches them (track::sensor_frames, i3d_track.h).  Every float
  * operation is explicitly rounded and every double operation is an explicit __d*_rn (no FMA contraction), so tests/track_ref.py restates
  * the planes, masks and sums exactly.  A frame's bytes depend only on that frame.
@@ -344,6 +348,58 @@ __global__ void __launch_bounds__(kTrackTile * kTrackTile) k_track_photo_rows(Tr
         }
     }
     tr_tile_partials(warp_sums, J, r, cnt, tid, z, tp.tiles_x, tp.tiles_y, tp.partials);
+}
+
+// ---- the reference model (DESIGN.md §6q) ---------------------------------------------------------------------------------------------
+
+// One thread per pixel (u, v) of level l of frame blockIdx.y: the model point q of prediction pixel (2^l u, 2^l v), projected into the
+// frame's reference and sampled from the reference's level-l intensity, with k_track_photo_rows' bounds and occlusion tests
+__global__ void k_track_ref_model(TrackRef tf)
+{
+    const TrackCam& c = tf.cam;
+    const int64_t img = static_cast<int64_t>(c.W) * c.H;
+    const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    if (i >= img) return;
+    const int z = blockIdx.y;
+    const int v = static_cast<int>(i / c.W), u = static_cast<int>(i - static_cast<int64_t>(v) * c.W);
+    const TrackCam& c0 = tf.pcam;
+    const int iu = u * tf.step, iv = v * tf.step;
+    const int64_t pp = (static_cast<int64_t>(z) * c0.H + iv) * c0.W + iu;
+    // the quiet NaN where any test fails: k_track_photo_rows then forms rc = I_f - NaN = NaN, and its gate fabsf(rc) <= max_diff (an
+    // ordered compare, FSETP.LE) is false, so the pixel gives no row
+    float val = __int_as_float(0x7FC00000);
+    const float zm = tf.pdepth[pp];
+    if (zm > 0.0f)
+    {
+        // q = o0 + z_m R0^T (x', y', 1), as tr_associate builds it
+        const float* R0 = tf.rt_in + 12 * static_cast<int64_t>(tf.ids[z]);
+        const float xn = FD(FS(__int2float_rn(iu), c0.cx), c0.fx), yn = FD(FS(__int2float_rn(iv), c0.cy), c0.fy);
+        float q[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+        {
+            const float o = -FA(FA(FM(R0[k], R0[9]), FM(R0[3 + k], R0[10])), FM(R0[6 + k], R0[11]));
+            const float dir = FA(FA(FM(R0[k], xn), FM(R0[3 + k], yn)), R0[6 + k]);
+            q[k] = FA(o, FM(zm, dir));
+        }
+        const float* Rr = tf.ref_rt + 12 * static_cast<int64_t>(z);
+        float xr[3];
+        tr_xform(Rr, Rr + 9, q, xr);
+        if (xr[2] > 0.0f)
+        {
+            const float x = FA(FM(c.fx, FD(xr[0], xr[2])), c.cx), y = FA(FM(c.fy, FD(xr[1], xr[2])), c.cy);
+            if (x >= 1.0f && x < static_cast<float>(c.W - 2) && y >= 1.0f && y < static_cast<float>(c.H - 2))
+            {
+                const float d = tf.depth[z * img + static_cast<int64_t>(__float2int_rz(FA(y, 0.5f))) * c.W + __float2int_rz(FA(x, 0.5f))];
+                if (d > 0.0f && fabsf(FS(d, xr[2])) <= tf.max_distance)
+                {
+                    const float xf = floorf(x), yf = floorf(y);
+                    val = tr_bilinear(tf.inten + z * img, c.W, __float2int_rz(xf), __float2int_rz(yf), FS(x, xf), FS(y, yf));
+                }
+            }
+        }
+    }
+    tf.model[pp] = val;
 }
 
 // One thread per frame that is not frozen: the system k_track_solve reads, A = A_g + lam2 A_c and b = b_g + lam2 b_c (entries 0..26;

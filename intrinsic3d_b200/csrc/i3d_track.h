@@ -68,6 +68,21 @@ struct TrackPhoto
     int tiles_x, tiles_y;
 };
 
+// One reference-model launch (DESIGN.md §6q): level `cam` of the chunk's frames [gridDim.y]; pixel (u, v) of frame z projects the model
+// point of prediction pixel (step u, step v) into its reference (float world -> camera ref_rt + 12 z) and samples the reference's level
+// planes + z * W * H there; the value (or the quiet NaN) goes to model at the level-0 index of that prediction pixel.
+struct TrackRef
+{
+    TrackCam cam, pcam;
+    int step;
+    const float* pdepth;                                  // prediction [n][H0][W0]
+    const int32_t* ids; const float* rt_in;               // as TrackRows
+    const float* ref_rt;                                  // [n][12]
+    const float* inten; const float* depth;               // the references' level planes [n][H][W]
+    float max_distance;
+    float* model;                                         // [n][H0][W0]
+};
+
 // Per-frame photometric outcome of a call (k_track_combine): rows and sum r^2 of the first and the last evaluated system
 struct TrackColorState
 {
@@ -87,17 +102,24 @@ struct TrackScratch
     Dev<int> live_box; Dev<uint32_t> live_bits;           // box and brick bitmap of the fusion volume in progress, rebuilt per use
     Dev<float> pint, lum_c, inten[kTrackMaxLevels], gx[kTrackMaxLevels], gy[kTrackMaxLevels];
     Dev<double> sys_c, sums_c, sums_comb, partials_c; Dev<TrackColorState> cstate; Dev<int32_t> iota;
+    // with a reference model (DESIGN.md §6q): the references' ids and float poses, their intensity and depth pyramids, and the model
+    // planes of levels 1.. (level 0 is pint), each in the level-0 layout (i3d_debug_get_track_reference_planes)
+    Dev<int32_t> ref_ids; Dev<float> ref_rt, ref_inten[kTrackMaxLevels], ref_depth[kTrackMaxLevels], ref_model[kTrackMaxLevels];
     int n = 0, levels = 0, last_m = 0, W[kTrackMaxLevels] = {}, H[kTrackMaxLevels] = {};
     bool color = false;                                   // the last call had a photometric term
+    bool reference = false;                               // ... taken from reference frames
 };
 
 // The photometric term of a call: its parameters (validated by the caller), the store whose colour frames it reads, and the per-frame
-// outcome (may be nullptr)
+// outcome (may be nullptr).  With ref_ids (host, validated; nullptr: the voxel model of DESIGN.md §6p) the model intensity of frame k is
+// sampled from the stored frame ref_ids[k] at its world -> camera pose ref_pose + 12 k (DESIGN.md §6q).
 struct TrackColor
 {
     const I3DTrackColorParams* P;
     const SensorStore* ss;
     I3DTrackColorInfo* info;
+    const int32_t* ref_ids = nullptr;
+    const double* ref_pose = nullptr;
 };
 
 namespace track
@@ -123,9 +145,11 @@ int fusion_frames(TrackScratch& ts, const FusionState& fs, bool skip, Timing& tm
 // weight > 0 the frame is integrated at the guess (I3D_TRACK_ANCHORED), otherwise fusion_frames' tracking of that one frame (m = 1) and,
 // at status 0 only, fusion::integrate at the tracked pose.  Timed as "odometry" (host wall time of the call), "odometry_predict",
 // "odometry_icp" and the fusion phases.  Returns non-zero with the message in `error` when fusion::integrate fails.
+// reference (col must be set, its ref_ids nullptr): each frame's model intensity comes from the last frame the loop integrated, at the
+// pose it was integrated with (fs.ref_id / fs.ref_T, kept like the motion state); a frame with no such reference is tracked on depth alone.
 int odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids, const double* pose_first,
              const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, std::string& error, cudaStream_t st,
-             const TrackColor* col = nullptr);
+             const TrackColor* col = nullptr, bool reference = false);
 } // namespace track
 
 } // namespace i3d

@@ -39,7 +39,8 @@ EXPORTED_SYMBOLS = [
     "i3d_debug_get_track_planes", "i3d_fusion_track_sensor_frames", "i3d_fusion_track_and_integrate_sensor",
     "i3d_sizeof_track_color_params", "i3d_sizeof_track_color_info", "i3d_default_track_color_params", "i3d_track_sensor_frames_rgbd",
     "i3d_fusion_track_sensor_frames_rgbd", "i3d_fusion_track_and_integrate_sensor_rgbd", "i3d_debug_get_track_color_planes",
-    "i3d_debug_get_track_color_system",
+    "i3d_debug_get_track_color_system", "i3d_track_sensor_frames_rgbd_ref", "i3d_fusion_track_sensor_frames_rgbd_ref",
+    "i3d_fusion_track_and_integrate_sensor_rgbd_ref", "i3d_debug_get_track_reference_planes", "i3d_default_track_color_ref_params",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
     "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_pcg_vectors", "i3d_debug_get_normal_equations",
@@ -128,6 +129,15 @@ def load_library():
     L.i3d_debug_get_track_color_planes.argtypes = [C.c_void_p, C.c_int32] + [C.POINTER(C.c_float)] * 4 + [C.POINTER(C.c_int32)]
     L.i3d_debug_get_track_color_system.restype = C.c_int
     L.i3d_debug_get_track_color_system.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+    for fn in (L.i3d_track_sensor_frames_rgbd_ref, L.i3d_fusion_track_sensor_frames_rgbd_ref):
+        fn.restype = C.c_int
+        fn.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(C.c_int32), C.POINTER(C.c_double),
+                       C.POINTER(I3DTrackParams), C.POINTER(I3DTrackColorParams), C.POINTER(C.c_double), C.POINTER(I3DTrackInfo),
+                       C.POINTER(I3DTrackColorInfo)]
+    L.i3d_fusion_track_and_integrate_sensor_rgbd_ref.restype = C.c_int
+    L.i3d_fusion_track_and_integrate_sensor_rgbd_ref.argtypes = L.i3d_fusion_track_and_integrate_sensor_rgbd.argtypes
+    L.i3d_debug_get_track_reference_planes.restype = C.c_int
+    L.i3d_debug_get_track_reference_planes.argtypes = [C.c_void_p, C.c_int32] + [C.POINTER(C.c_float)] * 3 + [C.POINTER(C.c_int32)]
     _LIB = L
     return L
 
@@ -163,6 +173,12 @@ def default_track_params() -> I3DTrackParams:
 def default_track_color_params() -> I3DTrackColorParams:
     p = I3DTrackColorParams()
     load_library().i3d_default_track_color_params(C.byref(p))
+    return p
+
+
+def default_track_color_ref_params() -> I3DTrackColorParams:
+    p = I3DTrackColorParams()
+    load_library().i3d_default_track_color_ref_params(C.byref(p))
     return p
 
 
@@ -512,10 +528,10 @@ class Engine:
         return p
 
     @staticmethod
-    def _track_color_params(color):
+    def _track_color_params(color, ref=False):
         """I3DTrackColorParams from a dict: weight (one value for every level, or up to 4 values, level 0 first), max_color_diff,
-        min_color_gradient; the rest keep default_track_color_params()."""
-        p = default_track_color_params()
+        min_color_gradient; the rest keep default_track_color_params() (ref: default_track_color_ref_params())."""
+        p = default_track_color_ref_params() if ref else default_track_color_params()
         for k, v in (color or {}).items():
             if k == "weight":
                 v = [float(v)] * TRACK_LEVELS if np.ndim(v) == 0 else list(v) + [0.0] * (TRACK_LEVELS - len(v))
@@ -529,20 +545,28 @@ class Engine:
                 raise ValueError(f"unknown colour tracking parameter {k!r}")
         return p
 
-    def _track_call(self, fn, ids, pose, name, n_pose, p, color=None):
+    def _track_call(self, fn, ids, pose, name, n_pose, p, color=None, ref=None):
+        """ref: (ref_ids, ref_pose) of a _ref call, passed after the pose"""
         ids, n = self._ids(ids)
         if pose is not None:
             pose = np.ascontiguousarray(pose, np.float64)
             if pose.shape != (n_pose(n), 12):
                 raise ValueError(f"{name} must be [{n_pose(n)}, 12], got {pose.shape}")
+        refs = ()
+        if ref is not None:
+            rid = np.ascontiguousarray(ref[0], np.int32).reshape(-1)
+            rpose = np.ascontiguousarray(ref[1], np.float64)
+            if rid.shape != (n,) or rpose.shape != (n, 12):
+                raise ValueError(f"ref_ids and ref_pose_w2c must be [{n}] and [{n}, 12], got {rid.shape} and {rpose.shape}")
+            refs = (_p(rid, C.c_int32), _p(rpose, C.c_double))
         out = np.empty((max(n, 1), 12), np.float64)
         infos = (I3DTrackInfo * max(n, 1))()
         if color is None:
             self._check(fn(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(pose, C.c_double), C.byref(p), _p(out, C.c_double), infos))
             return out[:n], [infos[i].as_dict() for i in range(n)]
         cinfos = (I3DTrackColorInfo * max(n, 1))()
-        self._check(fn(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(pose, C.c_double), C.byref(p), C.byref(color), _p(out, C.c_double), infos,
-                       cinfos))
+        self._check(fn(self.h, C.c_int32(n), _p(ids, C.c_int32), _p(pose, C.c_double), *refs, C.byref(p), C.byref(color), _p(out, C.c_double),
+                       infos, cinfos))
         return out[:n], [dict(infos[i].as_dict(), color=cinfos[i].as_dict()) for i in range(n)]
 
     def track_sensor_frames(self, ids, pose_w2c, source: str = "fused", **params):
@@ -591,21 +615,59 @@ class Engine:
         return self._track_call(self.L.i3d_fusion_track_and_integrate_sensor_rgbd, ids, pose, "pose_first", lambda n: 1, p,
                                 self._track_color_params(color))
 
+    # ---- the photometric term against a reference frame's image (DESIGN.md §6q) ----------------------------------------------------
+    def track_sensor_frames_rgbd_ref(self, ids, pose_w2c, ref_ids, ref_pose_w2c, source: str = "fused", color=None, **params):
+        """track_sensor_frames_rgbd with the model intensity of frame k sampled from the stored frame ref_ids[k] (may be ids[k] itself) at
+        its world -> camera pose ref_pose_w2c[k] float64 [12] instead of from the voxel colours.  Returns (poses, infos) as the _rgbd call."""
+        p = self._track_params(self._mesh_source(source), params)
+        return self._track_call(self.L.i3d_track_sensor_frames_rgbd_ref, ids, pose_w2c, "pose_w2c", lambda n: n, p,
+                                self._track_color_params(color, True), ref=(ref_ids, ref_pose_w2c))
+
+    def fusion_track_sensor_frames_rgbd_ref(self, ids, pose_w2c, ref_ids, ref_pose_w2c, color=None, **params):
+        """fusion_track_sensor_frames_rgbd with the reference model (see track_sensor_frames_rgbd_ref)."""
+        p = self._track_params(0, params)
+        return self._track_call(self.L.i3d_fusion_track_sensor_frames_rgbd_ref, ids, pose_w2c, "pose_w2c", lambda n: n, p,
+                                self._track_color_params(color, True), ref=(ref_ids, ref_pose_w2c))
+
+    def fusion_track_and_integrate_sensor_rgbd_ref(self, ids, pose_first=None, color=None, **params):
+        """Dense odometry with the reference model: each frame's reference is the last frame the loop integrated, at the pose it was
+        integrated with; a frame without one (the first after pose_first, a fusion_begin or an integrate) is tracked on depth alone."""
+        p = self._track_params(0, params)
+        pose = None if pose_first is None else np.asarray(pose_first, np.float64).reshape(1, 12)
+        return self._track_call(self.L.i3d_fusion_track_and_integrate_sensor_rgbd_ref, ids, pose, "pose_first", lambda n: 1, p,
+                                self._track_color_params(color, True))
+
+    def debug_track_reference_planes(self, level, n):
+        """The last pass's planes of the last _ref call (`n` = its frame count) at pyramid `level`, each [n, H_l, W_l]: model (NaN where
+        there is no model value), ref_intensity and ref_depth."""
+        dc = self._sensor_cams[0]
+        Wl, Hl = dc.width, dc.height
+        for _ in range(level):
+            Wl, Hl = Wl // 2, Hl // 2
+        out = {k: np.empty((n, Hl, Wl), np.float32) for k in ("model", "ref_intensity", "ref_depth")}
+        m = C.c_int32(0)
+        self._check(self.L.i3d_debug_get_track_reference_planes(self.h, C.c_int32(int(level)), _p(out["model"], C.c_float),
+                                                                _p(out["ref_intensity"], C.c_float), _p(out["ref_depth"], C.c_float), C.byref(m)))
+        assert m.value == n, (m.value, n)
+        return out
+
     def debug_track_color_system(self, n):
         """the unweighted photometric sums float64 [n, 29] of the last evaluated system of each frame of the last _rgbd call of n frames"""
         sums = np.empty((n, 29), np.float64)
         self._check(self.L.i3d_debug_get_track_color_system(self.h, _p(sums, C.c_double)))
         return sums
 
-    def debug_track_color_planes(self, level, frames):
+    def debug_track_color_planes(self, level, frames, model_intensity=True):
         """The last pass's colour planes of the last _rgbd call (`frames` = its frame count): model_intensity [frames, H, W] and the
-        frame intensity / grad_x / grad_y at pyramid `level`."""
+        frame intensity / grad_x / grad_y at pyramid `level`.  model_intensity=False leaves the model plane out (None), as after a _ref
+        call, whose model planes debug_track_reference_planes returns."""
         dc = self._sensor_cams[0]
         W, H = dc.width, dc.height
         Wl, Hl = W, H
         for _ in range(level):
             Wl, Hl = Wl // 2, Hl // 2
-        out = dict(model_intensity=np.empty((frames, H, W), np.float32), intensity=np.empty((frames, Hl, Wl), np.float32),
+        out = dict(model_intensity=np.empty((frames, H, W), np.float32) if model_intensity else None,
+                   intensity=np.empty((frames, Hl, Wl), np.float32),
                    grad_x=np.empty((frames, Hl, Wl), np.float32), grad_y=np.empty((frames, Hl, Wl), np.float32))
         m = C.c_int32(0)
         self._check(self.L.i3d_debug_get_track_color_planes(self.h, C.c_int32(int(level)), _p(out["model_intensity"], C.c_float),
