@@ -225,6 +225,15 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
     k_track_init<<<blocks_for(n, 64), 64, 0, st>>>(n, ts.pose_in.p, ts.state.p);
     const float max_dist_sq = P.max_distance * P.max_distance;
     int m = 0;
+    // a chunk's pyramid lv: the stored depth of device ids then frames::depthdown, or frames::sensor_intensity of host ids then pyrdown
+    auto depth_pyramid = [&](const int32_t* ids_dev, Dev<float>* lv) {
+        k_track_gather<<<dim3(blocks_for(img), m), kThreads, 0, st>>>(m, W, H, ids_dev, store_depth, lv[0].p);
+        for (int l = 1; l < L; ++l) frames::depthdown(m, Wl[l - 1], Hl[l - 1], lv[l - 1].p, lv[l].p, st);
+    };
+    auto intensity_pyramid = [&](const int32_t* ids_host, Dev<float>* lv) {
+        frames::sensor_intensity(*col->ss, m, ids_host, ts.iota.p, ts.lum_c, lv[0].p, st);
+        for (int l = 1; l < L; ++l) frames::pyrdown(m, Wl[l - 1], Hl[l - 1], lv[l - 1].p, lv[l].p, st);
+    };
     for (int c0 = 0; c0 < n; c0 += C)
     {
         m = std::min(C, n - c0);
@@ -241,8 +250,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
         }
         {
             Timer t(tm, st, ph.pyramid);
-            k_track_gather<<<dim3(blocks_for(img), m), kThreads, 0, st>>>(m, W, H, ids_d, store_depth, ts.depth[0].p);
-            for (int l = 1; l < L; ++l) frames::depthdown(m, Wl[l - 1], Hl[l - 1], ts.depth[l - 1].p, ts.depth[l].p, st);
+            depth_pyramid(ids_d, ts.depth);
             for (int l = 0; l < L; ++l)
                 k_track_normals<<<dim3(blocks_for(static_cast<size_t>(Wl[l]) * Hl[l]), m), kThreads, 0, st>>>(cam[l], ts.depth[l].p, ts.nrm[l].p);
         }
@@ -250,8 +258,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
         {
             // the frame intensity pyramid in the depth camera and its gradients
             Timer t(tm, st, ph.color);
-            frames::sensor_intensity(*col->ss, m, ids + c0, ts.iota.p, ts.lum_c, ts.inten[0].p, st);
-            for (int l = 1; l < L; ++l) frames::pyrdown(m, Wl[l - 1], Hl[l - 1], ts.inten[l - 1].p, ts.inten[l].p, st);
+            intensity_pyramid(ids + c0, ts.inten);
             for (int l = 0; l < L; ++l)
                 k_track_grad<<<dim3(blocks_for(static_cast<size_t>(Wl[l]) * Hl[l]), m), kThreads, 0, st>>>(cam[l], ts.inten[l].p, ts.gx[l].p, ts.gy[l].p);
         }
@@ -259,14 +266,8 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
         {
             // the references' intensity and depth pyramids by the frame's own rules, then each level's model plane
             Timer t(tm, st, ph.reference);
-            const int32_t* rids_d = ts.ref_ids.p + c0;
-            frames::sensor_intensity(*col->ss, m, col->ref_ids + c0, ts.iota.p, ts.lum_c, ts.ref_inten[0].p, st);
-            k_track_gather<<<dim3(blocks_for(img), m), kThreads, 0, st>>>(m, W, H, rids_d, store_depth, ts.ref_depth[0].p);
-            for (int l = 1; l < L; ++l)
-            {
-                frames::pyrdown(m, Wl[l - 1], Hl[l - 1], ts.ref_inten[l - 1].p, ts.ref_inten[l].p, st);
-                frames::depthdown(m, Wl[l - 1], Hl[l - 1], ts.ref_depth[l - 1].p, ts.ref_depth[l].p, st);
-            }
+            intensity_pyramid(col->ref_ids + c0, ts.ref_inten);
+            depth_pyramid(ts.ref_ids.p + c0, ts.ref_depth);
             TrackRef tf{};
             tf.pcam = cam[0]; tf.pdepth = ts.pdepth.p; tf.ids = ids_d; tf.rt_in = ts.rt.p; tf.ref_rt = ts.ref_rt.p + 12 * static_cast<size_t>(c0);
             tf.max_distance = P.max_distance;

@@ -73,7 +73,9 @@ __device__ __forceinline__ int rd_cube(const RenderGrid& rg, const float p[3], R
 }
 
 // The same rule on the fusion volume in progress, which has no neighbour table: one probe of its hash per corner.  The base and brick
-// steps are rd_cube's above, written out again: sharing them changes that function's register allocation in k_render_march.
+// steps are rd_cube's above, written out again because one shared helper for them adds 16 instructions to each of the four marches and
+// slows k_render_march: i3d_render_keyframes (C3, statistics of all 200 keyframes, skipping on) took 106.3-106.9 ms as written here and
+// 107.9-108.4 ms shared, and the C3 track_predict 112.6-113.1 ms against 114.4-114.9 ms (three alternating runs each, H100 80GB HBM3, 700 W).
 __device__ __forceinline__ int rd_cube(const LiveGrid& lg, const float p[3], RdCube& q)
 {
     const float vs = lg.voxel_size;

@@ -92,6 +92,20 @@ __global__ void k_track_normals(TrackCam cam, const float* __restrict__ depth_al
     nrm[3 * i] = n.x; nrm[3 * i + 1] = n.y; nrm[3 * i + 2] = n.z;
 }
 
+// The model point of prediction pixel (iu, iv) at depth zm, as the march built the ray of that pixel (camera c0, input pose R0 | t0):
+// q = o0 + z_m R0^T (x', y', 1), o0 = -R0^T t0
+__device__ __forceinline__ void tr_model_point(const float* R0, const TrackCam& c0, int iu, int iv, float zm, float q[3])
+{
+    const float xn = FD(FS(__int2float_rn(iu), c0.cx), c0.fx), yn = FD(FS(__int2float_rn(iv), c0.cy), c0.fy);
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+    {
+        const float o = -FA(FA(FM(R0[k], R0[9]), FM(R0[3 + k], R0[10])), FM(R0[6 + k], R0[11]));
+        const float dir = FA(FA(FM(R0[k], xn), FM(R0[3 + k], yn)), R0[6 + k]);
+        q[k] = FA(o, FM(zm, dir));
+    }
+}
+
 // The correspondence of pixel (u, v) of frame z at the current pose (DESIGN.md §6n): p (world), q (model point), n_m (model normal)
 __device__ __forceinline__ bool tr_associate(const TrackRows& tr, int z, int u, int v, const float* Tf, float p[3], float q[3], float nm[3])
 {
@@ -114,15 +128,11 @@ __device__ __forceinline__ bool tr_associate(const TrackRows& tr, int z, int u, 
     if (!(zm > 0.0f)) return false;
     nm[0] = tr.pnrm[3 * pp]; nm[1] = tr.pnrm[3 * pp + 1]; nm[2] = tr.pnrm[3 * pp + 2];
     if (nm[0] == 0.0f && nm[1] == 0.0f && nm[2] == 0.0f) return false;
-    // q = o0 + z_m R0^T (x', y', 1), o0 = -R0^T t0, as the march built the ray of that pixel
-    const float xn = FD(FS(__int2float_rn(iu), c0.cx), c0.fx), yn = FD(FS(__int2float_rn(iv), c0.cy), c0.fy);
+    tr_model_point(R0, c0, iu, iv, zm, q);
     float dsq = 0.0f;
 #pragma unroll
     for (int k = 0; k < 3; ++k)
     {
-        const float o = -FA(FA(FM(R0[k], R0[9]), FM(R0[3 + k], R0[10])), FM(R0[6 + k], R0[11]));
-        const float dir = FA(FA(FM(R0[k], xn), FM(R0[3 + k], yn)), R0[6 + k]);
-        q[k] = FA(o, FM(zm, dir));
         const float e = FS(p[k], q[k]);
         dsq = FA(dsq, FM(e, e));
     }
@@ -138,77 +148,8 @@ __device__ __forceinline__ bool tr_associate(const TrackRows& tr, int z, int u, 
     return true;
 }
 
-// One thread per pixel of frame blockIdx.z at the rows launch's level
-__global__ void __launch_bounds__(kTrackTile * kTrackTile) k_track_rows(TrackRows tr)
-{
-    __shared__ double warp_sums[kTrackTile * kTrackTile / 32][kTrackVals];
-    const int u = blockIdx.x * kTrackTile + threadIdx.x, v = blockIdx.y * kTrackTile + threadIdx.y, z = blockIdx.z;
-    const int tid = threadIdx.y * kTrackTile + threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const TrackState& s = tr.state[z];
-    const bool frozen = s.frozen != 0;
-    double J[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, r = 0.0, cnt = 0.0;
-    if (u < tr.cam.W && v < tr.cam.H && !frozen)
-    {
-        float Tf[12];
-#pragma unroll
-        for (int i = 0; i < 12; ++i) Tf[i] = s.Tf[i];
-        float p[3], q[3], nm[3];
-        const bool ok = tr_associate(tr, z, u, v, Tf, p, q, nm);
-        if (tr.mask) tr.mask[(static_cast<int64_t>(z) * tr.cam.H + v) * tr.cam.W + u] = ok ? 1 : 0;
-        if (ok)
-        {
-            double pd[3], nd[3];
-#pragma unroll
-            for (int k = 0; k < 3; ++k) { pd[k] = static_cast<double>(p[k]); nd[k] = static_cast<double>(nm[k]); }
-            r = DA(DA(DM(nd[0], DS(pd[0], static_cast<double>(q[0]))), DM(nd[1], DS(pd[1], static_cast<double>(q[1])))),
-                   DM(nd[2], DS(pd[2], static_cast<double>(q[2]))));
-            J[0] = DS(DM(pd[1], nd[2]), DM(pd[2], nd[1]));
-            J[1] = DS(DM(pd[2], nd[0]), DM(pd[0], nd[2]));
-            J[2] = DS(DM(pd[0], nd[1]), DM(pd[1], nd[0]));
-            J[3] = nd[0]; J[4] = nd[1]; J[5] = nd[2];
-            cnt = 1.0;
-        }
-    }
-    else if (u < tr.cam.W && v < tr.cam.H && tr.mask)
-        tr.mask[(static_cast<int64_t>(z) * tr.cam.H + v) * tr.cam.W + u] = 0;
-    // the 29 products, each summed over the warp by a fixed shuffle tree as it is formed; lane 0 keeps the warp's sums
-    int j = 0;
-#pragma unroll
-    for (int a = 0; a < 6; ++a)
-    {
-#pragma unroll
-        for (int b = a; b < 6; ++b, ++j)
-        {
-            double x = DM(J[a], J[b]);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) x = DA(x, __shfl_down_sync(0xffffffffu, x, o));
-            if (lane == 0) warp_sums[warp][j] = x;
-        }
-    }
-#pragma unroll
-    for (int a = 0; a < 8; ++a, ++j)
-    {
-        double x = a < 6 ? DM(J[a], r) : (a == 6 ? DM(r, r) : cnt);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) x = DA(x, __shfl_down_sync(0xffffffffu, x, o));
-        if (lane == 0) warp_sums[warp][j] = x;
-    }
-    __syncthreads();
-    if (tid < kTrackVals)
-    {
-        double t = warp_sums[0][tid];
-#pragma unroll
-        for (int w = 1; w < kTrackTile * kTrackTile / 32; ++w) t = DA(t, warp_sums[w][tid]);
-        const int64_t tile = (static_cast<int64_t>(z) * tr.tiles_y + blockIdx.y) * tr.tiles_x + blockIdx.x;
-        tr.partials[tile * kTrackVals + tid] = t;
-    }
-}
-
-// ---- the photometric term (DESIGN.md §6p) ----------------------------------------------------------------------------------------
-
 // The 29 products of one pixel's row (J, r, cnt), each summed over the warp by a fixed shuffle tree as it is formed (lane 0 keeps the
-// warp's sums), then the 8 warps in order into the partials of tile (blockIdx.x, blockIdx.y) of frame z: k_track_rows' reduction, written
-// out there again because sharing it changes that kernel's instructions
+// warp's sums), then the 8 warps in order into the partials of tile (blockIdx.x, blockIdx.y) of frame z
 __device__ __forceinline__ void tr_tile_partials(double (&warp_sums)[kTrackTile * kTrackTile / 32][kTrackVals], const double (&J)[6], double r, double cnt, int tid, int z,
                                                  int tiles_x, int tiles_y, double* partials)
 {
@@ -245,6 +186,44 @@ __device__ __forceinline__ void tr_tile_partials(double (&warp_sums)[kTrackTile 
     }
 }
 
+// One thread per pixel of frame blockIdx.z at the rows launch's level
+__global__ void __launch_bounds__(kTrackTile * kTrackTile) k_track_rows(TrackRows tr)
+{
+    __shared__ double warp_sums[kTrackTile * kTrackTile / 32][kTrackVals];
+    const int u = blockIdx.x * kTrackTile + threadIdx.x, v = blockIdx.y * kTrackTile + threadIdx.y, z = blockIdx.z;
+    const int tid = threadIdx.y * kTrackTile + threadIdx.x;
+    const TrackState& s = tr.state[z];
+    const bool frozen = s.frozen != 0;
+    double J[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, r = 0.0, cnt = 0.0;
+    if (u < tr.cam.W && v < tr.cam.H && !frozen)
+    {
+        float Tf[12];
+#pragma unroll
+        for (int i = 0; i < 12; ++i) Tf[i] = s.Tf[i];
+        float p[3], q[3], nm[3];
+        const bool ok = tr_associate(tr, z, u, v, Tf, p, q, nm);
+        if (tr.mask) tr.mask[(static_cast<int64_t>(z) * tr.cam.H + v) * tr.cam.W + u] = ok ? 1 : 0;
+        if (ok)
+        {
+            double pd[3], nd[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) { pd[k] = static_cast<double>(p[k]); nd[k] = static_cast<double>(nm[k]); }
+            r = DA(DA(DM(nd[0], DS(pd[0], static_cast<double>(q[0]))), DM(nd[1], DS(pd[1], static_cast<double>(q[1])))),
+                   DM(nd[2], DS(pd[2], static_cast<double>(q[2]))));
+            J[0] = DS(DM(pd[1], nd[2]), DM(pd[2], nd[1]));
+            J[1] = DS(DM(pd[2], nd[0]), DM(pd[0], nd[2]));
+            J[2] = DS(DM(pd[0], nd[1]), DM(pd[1], nd[0]));
+            J[3] = nd[0]; J[4] = nd[1]; J[5] = nd[2];
+            cnt = 1.0;
+        }
+    }
+    else if (u < tr.cam.W && v < tr.cam.H && tr.mask)
+        tr.mask[(static_cast<int64_t>(z) * tr.cam.H + v) * tr.cam.W + u] = 0;
+    tr_tile_partials(warp_sums, J, r, cnt, tid, z, tr.tiles_x, tr.tiles_y, tr.partials);
+}
+
+// ---- the photometric term (DESIGN.md §6p) ----------------------------------------------------------------------------------------
+
 // Central differences FM(0.5, I[+1] - I[-1]) of frame blockIdx.y's intensity plane on 1..W-2 x 1..H-2, 0 on the border
 __global__ void k_track_grad(TrackCam cam, const float* __restrict__ inten_all, float* __restrict__ gx_all, float* __restrict__ gy_all)
 {
@@ -271,6 +250,23 @@ __device__ __forceinline__ float tr_bilinear(const float* __restrict__ P, int W,
     return FA(r0, FM(fy, FS(r1, r0)));
 }
 
+// The projection of the camera-frame point xc into level camera c, for a bilinear sample there: false unless xc is in front (z > 0),
+// all four taps lie in [1, W - 2] x [1, H - 2] (tested on the float: a NaN fails) and the level depth plane's nearest pixel d is not
+// occluding (d > 0, |d - z| <= max_distance).  Otherwise the corner (x0, y0) and the fractions (fx, fy) of tr_bilinear.
+__device__ __forceinline__ bool tr_project(const TrackCam& c, const float* __restrict__ depth, float max_distance, const float xc[3], int& x0, int& y0,
+                                           float& fx, float& fy)
+{
+    if (!(xc[2] > 0.0f)) return false;
+    const float x = FA(FM(c.fx, FD(xc[0], xc[2])), c.cx), y = FA(FM(c.fy, FD(xc[1], xc[2])), c.cy);
+    if (!(x >= 1.0f && x < static_cast<float>(c.W - 2) && y >= 1.0f && y < static_cast<float>(c.H - 2))) return false;
+    const float d = depth[static_cast<int64_t>(__float2int_rz(FA(y, 0.5f))) * c.W + __float2int_rz(FA(x, 0.5f))];
+    if (!(d > 0.0f && fabsf(FS(d, xc[2])) <= max_distance)) return false;
+    const float xf = floorf(x), yf = floorf(y);
+    x0 = __float2int_rz(xf); y0 = __float2int_rz(yf);
+    fx = FS(x, xf); fy = FS(y, yf);
+    return true;
+}
+
 // One thread per pixel (u, v) of level l of frame blockIdx.z: the model sample at prediction pixel (2^l u, 2^l v), the intensity residual
 // at its projection with the current pose, the gates and the photometric row, reduced as k_track_rows reduces (DESIGN.md §6p)
 __global__ void __launch_bounds__(kTrackTile * kTrackTile) k_track_photo_rows(TrackPhoto tp)
@@ -288,17 +284,8 @@ __global__ void __launch_bounds__(kTrackTile * kTrackTile) k_track_photo_rows(Tr
         const float zm = tp.pdepth[pp];
         if (zm > 0.0f)
         {
-            // q = o0 + z_m R0^T (x', y', 1), as tr_associate builds it
-            const float* R0 = tp.rt_in + 12 * static_cast<int64_t>(tp.ids[z]);
-            const float xn = FD(FS(__int2float_rn(iu), c0.cx), c0.fx), yn = FD(FS(__int2float_rn(iv), c0.cy), c0.fy);
             float q[3];
-#pragma unroll
-            for (int k = 0; k < 3; ++k)
-            {
-                const float o = -FA(FA(FM(R0[k], R0[9]), FM(R0[3 + k], R0[10])), FM(R0[6 + k], R0[11]));
-                const float dir = FA(FA(FM(R0[k], xn), FM(R0[3 + k], yn)), R0[6 + k]);
-                q[k] = FA(o, FM(zm, dir));
-            }
+            tr_model_point(tp.rt_in + 12 * static_cast<int64_t>(tp.ids[z]), c0, iu, iv, zm, q);
             // x_c = R^T (q - t) with the float camera -> world pose
             float Tf[12];
 #pragma unroll
@@ -308,41 +295,31 @@ __global__ void __launch_bounds__(kTrackTile * kTrackTile) k_track_photo_rows(Tr
 #pragma unroll
             for (int d = 0; d < 3; ++d) xc[d] = FA(FA(FM(Tf[d], e[0]), FM(Tf[3 + d], e[1])), FM(Tf[6 + d], e[2]));
             const TrackCam& c = tp.cam;
-            if (xc[2] > 0.0f)
+            const int64_t img = static_cast<int64_t>(c.W) * c.H;
+            int x0, y0;
+            float fx, fy;
+            if (tr_project(c, tp.depth + z * img, tp.max_distance, xc, x0, y0, fx, fy))
             {
-                const float x = FA(FM(c.fx, FD(xc[0], xc[2])), c.cx), y = FA(FM(c.fy, FD(xc[1], xc[2])), c.cy);
-                // all four taps in [1, W - 2] x [1, H - 2] (tested on the float: a NaN fails)
-                if (x >= 1.0f && x < static_cast<float>(c.W - 2) && y >= 1.0f && y < static_cast<float>(c.H - 2))
+                const float If = tr_bilinear(tp.inten + z * img, c.W, x0, y0, fx, fy);
+                const float gx = tr_bilinear(tp.gx + z * img, c.W, x0, y0, fx, fy);
+                const float gy = tr_bilinear(tp.gy + z * img, c.W, x0, y0, fx, fy);
+                const float rc = FS(If, tp.pint[pp]);
+                if (fabsf(rc) <= tp.max_diff && FA(FM(gx, gx), FM(gy, gy)) >= tp.min_grad_sq)
                 {
-                    const int64_t img = static_cast<int64_t>(c.W) * c.H;
-                    const float d = tp.depth[z * img + static_cast<int64_t>(__float2int_rz(FA(y, 0.5f))) * c.W + __float2int_rz(FA(x, 0.5f))];
-                    if (d > 0.0f && fabsf(FS(d, xc[2])) <= tp.max_distance)
-                    {
-                        const float xf = floorf(x), yf = floorf(y);
-                        const int x0 = __float2int_rz(xf), y0 = __float2int_rz(yf);
-                        const float fx = FS(x, xf), fy = FS(y, yf);
-                        const float If = tr_bilinear(tp.inten + z * img, c.W, x0, y0, fx, fy);
-                        const float gx = tr_bilinear(tp.gx + z * img, c.W, x0, y0, fx, fy);
-                        const float gy = tr_bilinear(tp.gy + z * img, c.W, x0, y0, fx, fy);
-                        const float rc = FS(If, tp.pint[pp]);
-                        if (fabsf(rc) <= tp.max_diff && FA(FM(gx, gx), FM(gy, gy)) >= tp.min_grad_sq)
-                        {
-                            // d r / d x_c, then world: g_w = R g_c; xi perturbs on the left, so J = [g_w x q, -g_w]
-                            const float gfx = FM(gx, c.fx), gfy = FM(gy, c.fy);
-                            const float gc[3] = {FD(gfx, xc[2]), FD(gfy, xc[2]), -FD(FA(FM(gfx, xc[0]), FM(gfy, xc[1])), FM(xc[2], xc[2]))};
-                            float gw[3];
-                            tr_xform(Tf, nullptr, gc, gw);
-                            double g[3], qd[3];
+                    // d r / d x_c, then world: g_w = R g_c; xi perturbs on the left, so J = [g_w x q, -g_w]
+                    const float gfx = FM(gx, c.fx), gfy = FM(gy, c.fy);
+                    const float gc[3] = {FD(gfx, xc[2]), FD(gfy, xc[2]), -FD(FA(FM(gfx, xc[0]), FM(gfy, xc[1])), FM(xc[2], xc[2]))};
+                    float gw[3];
+                    tr_xform(Tf, nullptr, gc, gw);
+                    double g[3], qd[3];
 #pragma unroll
-                            for (int k = 0; k < 3; ++k) { g[k] = static_cast<double>(gw[k]); qd[k] = static_cast<double>(q[k]); }
-                            J[0] = DS(DM(g[1], qd[2]), DM(g[2], qd[1]));
-                            J[1] = DS(DM(g[2], qd[0]), DM(g[0], qd[2]));
-                            J[2] = DS(DM(g[0], qd[1]), DM(g[1], qd[0]));
-                            J[3] = -g[0]; J[4] = -g[1]; J[5] = -g[2];
-                            r = static_cast<double>(rc);
-                            cnt = 1.0;
-                        }
-                    }
+                    for (int k = 0; k < 3; ++k) { g[k] = static_cast<double>(gw[k]); qd[k] = static_cast<double>(q[k]); }
+                    J[0] = DS(DM(g[1], qd[2]), DM(g[2], qd[1]));
+                    J[1] = DS(DM(g[2], qd[0]), DM(g[0], qd[2]));
+                    J[2] = DS(DM(g[0], qd[1]), DM(g[1], qd[0]));
+                    J[3] = -g[0]; J[4] = -g[1]; J[5] = -g[2];
+                    r = static_cast<double>(rc);
+                    cnt = 1.0;
                 }
             }
         }
@@ -353,7 +330,7 @@ __global__ void __launch_bounds__(kTrackTile * kTrackTile) k_track_photo_rows(Tr
 // ---- the reference model (DESIGN.md §6q) ---------------------------------------------------------------------------------------------
 
 // One thread per pixel (u, v) of level l of frame blockIdx.y: the model point q of prediction pixel (2^l u, 2^l v), projected into the
-// frame's reference and sampled from the reference's level-l intensity, with k_track_photo_rows' bounds and occlusion tests
+// frame's reference and sampled from the reference's level-l intensity, with k_track_photo_rows' bounds and occlusion tests (tr_project)
 __global__ void k_track_ref_model(TrackRef tf)
 {
     const TrackCam& c = tf.cam;
@@ -371,33 +348,14 @@ __global__ void k_track_ref_model(TrackRef tf)
     const float zm = tf.pdepth[pp];
     if (zm > 0.0f)
     {
-        // q = o0 + z_m R0^T (x', y', 1), as tr_associate builds it
-        const float* R0 = tf.rt_in + 12 * static_cast<int64_t>(tf.ids[z]);
-        const float xn = FD(FS(__int2float_rn(iu), c0.cx), c0.fx), yn = FD(FS(__int2float_rn(iv), c0.cy), c0.fy);
         float q[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k)
-        {
-            const float o = -FA(FA(FM(R0[k], R0[9]), FM(R0[3 + k], R0[10])), FM(R0[6 + k], R0[11]));
-            const float dir = FA(FA(FM(R0[k], xn), FM(R0[3 + k], yn)), R0[6 + k]);
-            q[k] = FA(o, FM(zm, dir));
-        }
+        tr_model_point(tf.rt_in + 12 * static_cast<int64_t>(tf.ids[z]), c0, iu, iv, zm, q);
         const float* Rr = tf.ref_rt + 12 * static_cast<int64_t>(z);
         float xr[3];
         tr_xform(Rr, Rr + 9, q, xr);
-        if (xr[2] > 0.0f)
-        {
-            const float x = FA(FM(c.fx, FD(xr[0], xr[2])), c.cx), y = FA(FM(c.fy, FD(xr[1], xr[2])), c.cy);
-            if (x >= 1.0f && x < static_cast<float>(c.W - 2) && y >= 1.0f && y < static_cast<float>(c.H - 2))
-            {
-                const float d = tf.depth[z * img + static_cast<int64_t>(__float2int_rz(FA(y, 0.5f))) * c.W + __float2int_rz(FA(x, 0.5f))];
-                if (d > 0.0f && fabsf(FS(d, xr[2])) <= tf.max_distance)
-                {
-                    const float xf = floorf(x), yf = floorf(y);
-                    val = tr_bilinear(tf.inten + z * img, c.W, __float2int_rz(xf), __float2int_rz(yf), FS(x, xf), FS(y, yf));
-                }
-            }
-        }
+        int x0, y0;
+        float fx, fy;
+        if (tr_project(c, tf.depth + z * img, tf.max_distance, xr, x0, y0, fx, fy)) val = tr_bilinear(tf.inten + z * img, c.W, x0, y0, fx, fy);
     }
     tf.model[pp] = val;
 }
