@@ -2,9 +2,9 @@
  * i3d_grid.cuh — what every device module of the engine shares about the grid: the neighbour-table slots, the block size, the device
  * hash (coordinates -> voxel index), the explicitly rounded float operations, the grid view with the per-voxel operators both modules
  * evaluate (surface normal, intensity), the voxel arrays a new voxel set is written into, the normal rule of a depth plane (fusion and
- * tracking) and the subvolume table of the lighting.  No kernels: i3d_kernels.cuh (the engine's module), i3d_fusion.cuh (the fusion's),
- * i3d_frames.cuh (the frames'), i3d_mesh.cuh / i3d_vis.cuh (the surface extraction's) and i3d_render.cuh / i3d_track.cuh (the
- * renderer's) all include it.
+ * tracking) and the subvolume table and SH blend of the lighting.  No kernels: i3d_kernels.cuh, i3d_observe.cuh, i3d_lighting.cuh and
+ * i3d_gridops.cuh (the engine's module), i3d_fusion.cuh (the fusion's), i3d_frames.cuh (the frames'), i3d_mesh.cuh / i3d_vis.cuh (the
+ * surface extraction's) and i3d_render.cuh / i3d_track.cuh (the renderer's) all include it.
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -159,5 +159,48 @@ struct SubvolGrid
         return table[(static_cast<int64_t>(z) * dim[1] + y) * dim[0] + x];
     }
 };
+
+// Subvolumes::interpolate(linear) at voxelToWorld of voxel v (subvolumes.cpp:165-205, math::interpolationWeights / average, src/math.cpp:74-128),
+// the blend of the SVSH lighting's per-voxel coefficients (k_svsh_interpolate) and of the shading colour modes (i3d_vis.cuh):
+// float trilinear weights of the 8 surrounding subvolumes at p / size - 0.5, missing cubes and zero weights skipped, the sub_sh [S][9]
+// vectors summed in double (product and sum rounded separately), times double(1.0f / sum of the weights).  avg must be zero on entry;
+// it stays zero when no weight is left.
+__device__ __forceinline__ void svsh_blend(const GridView& g, int64_t v, const SubvolGrid& sg, const double* __restrict__ sub_sh, double (&avg)[9])
+{
+    const int c[3] = {g.x[v], g.y[v], g.z[v]};
+    int v0[3]; float wg[3];
+#pragma unroll
+    for (int d = 0; d < 3; ++d)
+    {
+        const float pos = FS(FM(FM(static_cast<float>(c[d]), g.voxel_size), sg.inv_size), 0.5f);     // pointToIndexCoord
+        const float fl = floorf(pos);
+        v0[d] = static_cast<int>(fl);
+        wg[d] = FS(pos, fl);
+    }
+    // math::interpolationWeights corner order (src/math.cpp:103-128)
+    const int corner[8][3] = {{0, 0, 0}, {1, 0, 0}, {0, 1, 0}, {0, 0, 1}, {1, 1, 0}, {0, 1, 1}, {1, 0, 1}, {1, 1, 1}};
+    float sum_w = 0.0f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+    {
+        const float wx = corner[i][0] ? wg[0] : FS(1.0f, wg[0]);
+        const float wy = corner[i][1] ? wg[1] : FS(1.0f, wg[1]);
+        const float wz = corner[i][2] ? wg[2] : FS(1.0f, wg[2]);
+        const float w = FM(FM(wx, wy), wz);
+        const int id = sg.find(v0[0] + corner[i][0], v0[1] + corner[i][1], v0[2] + corner[i][2]);
+        if (id < 0 || w == 0.0f) continue;
+        const double wd = static_cast<double>(w);
+        const double* src = sub_sh + static_cast<int64_t>(id) * 9;
+#pragma unroll
+        for (int k = 0; k < 9; ++k) avg[k] = (sum_w == 0.0f) ? wd * src[k] : avg[k] + wd * src[k];
+        sum_w = FA(sum_w, w);
+    }
+    if (sum_w != 0.0f)
+    {
+        const double inv = static_cast<double>(FD(1.0f, sum_w));
+#pragma unroll
+        for (int k = 0; k < 9; ++k) avg[k] *= inv;
+    }
+}
 
 } // namespace i3d

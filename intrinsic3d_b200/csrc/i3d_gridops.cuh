@@ -13,7 +13,7 @@
  * voxel i at 8 i + (4 z + 2 y + x), the reference's loop nest (its own order is that of a fresh std::unordered_map).
  */
 #pragma once
-#include "i3d_kernels.cuh"
+#include "i3d_grid.cuh"
 
 namespace i3d
 {

@@ -23,6 +23,7 @@
 #include <limits.h>
 #include "i3d_math.cuh"
 #include "i3d_grid.cuh"
+#include "i3d_observe.cuh"
 #include "../../include/i3d_types.h"
 
 namespace i3d
@@ -81,13 +82,6 @@ __device__ __forceinline__ void pdl_prologue()
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
-
-struct FrameView
-{
-    int F, W, H;
-    const float* lum; const float* depth;
-    double pyr_scale;
-};
 
 // ----------------------------------------------------------------------------------------------
 // deterministic reductions: block partials -> last block sums them in a fixed order
@@ -416,138 +410,7 @@ __global__ void k_frame_pose(int F, const double* __restrict__ poses, FramePose*
     out[f] = fp;
 }
 
-struct SelectCam { float fx, fy, cx, cy; float d[5]; int dist_zero; float occlusion; };
-
-// SDFColorization::computeObservation -> weight (float pipeline, exact rounding; see oracle.cpp observation_weight)
-// pix (optional): Camera::project's sub-pixel position pt2f, for the colour lookup of the recolouring pass
-__device__ __forceinline__ float observation_weight(const float pt[3], const float nrm[3], const float* __restrict__ Rt, const SelectCam& cam,
-                                                    const float* __restrict__ depth, int W, int H, float* pix = nullptr)
-{
-    float q[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) q[k] = FA(FA(FA(FM(Rt[3 * k], pt[0]), FM(Rt[3 * k + 1], pt[1])), FM(Rt[3 * k + 2], pt[2])), Rt[9 + k]);
-    float x = FD(q[0], q[2]);
-    float y = FD(q[1], q[2]);
-    if (!cam.dist_zero)
-    {
-        const float r2 = FA(FM(x, x), FM(y, y));
-        const float r4 = FM(r2, r2);
-        const float r6 = FM(r4, r2);
-        const float dc = FA(FA(FA(1.0f, FM(cam.d[0], r2)), FM(cam.d[1], r4)), FM(cam.d[2], r6));
-        const float xn = FA(FA(FM(x, dc), FM(FM(FM(2.0f, cam.d[3]), x), y)), FM(cam.d[4], FA(r2, FM(FM(2.0f, x), x))));
-        const float yn = FA(FA(FM(y, dc), FM(FM(FM(2.0f, cam.d[4]), xn), y)), FM(cam.d[3], FA(r2, FM(FM(2.0f, y), y))));
-        x = xn; y = yn;
-    }
-    const float pu = FA(FM(cam.fx, x), cam.cx);
-    const float pv = FA(FM(cam.fy, y), cam.cy);
-    if (pix) { pix[0] = pu; pix[1] = pv; }
-    const float pu5 = FA(pu, 0.5f), pv5 = FA(pv, 0.5f);
-    if (!(pu5 > -2147483000.0f && pu5 < 2147483000.0f && pv5 > -2147483000.0f && pv5 < 2147483000.0f)) return 0.0f;
-    const int iu = __float2int_rz(pu5), iv = __float2int_rz(pv5);
-    if (iu < 0 || iu >= W || iv < 0 || iv >= H) return 0.0f;
-    const float d = __ldg(depth + static_cast<size_t>(iv) * W + iu);
-    if (cam.occlusion > 0.0f)
-    {
-        if (!(d > 0.0f)) return 0.0f;
-        const float sd = FS(d, q[2]);
-        if (!(fabsf(sd) <= cam.occlusion)) return 0.0f;
-    }
-    if (d <= 0.0f) return 0.0f;
-    float nc[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) nc[k] = FA(FA(FM(Rt[3 * k], nrm[0]), FM(Rt[3 * k + 1], nrm[1])), FM(Rt[3 * k + 2], nrm[2]));
-    float w_normal = 0.0f;
-    if (!(nc[0] == 0.0f && nc[1] == 0.0f && nc[2] == 0.0f))
-    {
-        const float qn2 = FA(FA(FM(q[0], q[0]), FM(q[1], q[1])), FM(q[2], q[2]));
-        float v0 = q[0], v1 = q[1], v2 = q[2];
-        if (qn2 > 0.0f) { const float ql = __fsqrt_rn(qn2); v0 = FD(q[0], ql); v1 = FD(q[1], ql); v2 = FD(q[2], ql); }
-        const float dt = FA(FA(FM(v0, nc[0]), FM(v1, nc[1])), FM(v2, nc[2]));
-        w_normal = FS(1.0f, fabsf(dt));
-        w_normal = (1.0f < w_normal) ? 1.0f : w_normal;           // std::min(w_normal, 1.0f)
-        w_normal = (w_normal < 0.0f) ? 0.0f : w_normal;           // std::max(.., 0.0f)
-        const float div = FA(1.0f, FM(2.0f, w_normal));
-        const float rk = FD(1.0f, FM(FM(div, div), div));
-        w_normal = (rk < 0.001f) ? 0.001f : rk;
-    }
-    // depth weight: the reference computes max(1 - (clamp(d) - d_min)/(d_max - d_min), 1.0f), which is exactly 1.0f for
-    // every finite d (Q1); w_normal * 1.0f == w_normal bit-for-bit, so the dead arithmetic is skipped.
-    return w_normal;
-}
-
-// observation_weight() split at its one dependent load, for software pipelining in k_select_obs: obs_probe() transforms and projects
-// the point and ISSUES the depth tap; obs_finish() consumes it.  Same operations in the same order as observation_weight()
-// (the selection stays bit-identical; tests/test_gpu_parity.py, test_golden.py).
-struct ObsProbe { float q0, q1, q2, d; int ok; };
-__device__ __forceinline__ ObsProbe obs_probe(const float pt[3], const float* __restrict__ Rt, const SelectCam& cam, const float* __restrict__ depth, int W, int H)
-{
-    ObsProbe o;
-    float q[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) q[k] = FA(FA(FA(FM(Rt[3 * k], pt[0]), FM(Rt[3 * k + 1], pt[1])), FM(Rt[3 * k + 2], pt[2])), Rt[9 + k]);
-    o.q0 = q[0]; o.q1 = q[1]; o.q2 = q[2]; o.d = 0.0f; o.ok = 0;
-    float x = FD(q[0], q[2]);
-    float y = FD(q[1], q[2]);
-    if (!cam.dist_zero)
-    {
-        const float r2 = FA(FM(x, x), FM(y, y));
-        const float r4 = FM(r2, r2);
-        const float r6 = FM(r4, r2);
-        const float dc = FA(FA(FA(1.0f, FM(cam.d[0], r2)), FM(cam.d[1], r4)), FM(cam.d[2], r6));
-        const float xn = FA(FA(FM(x, dc), FM(FM(FM(2.0f, cam.d[3]), x), y)), FM(cam.d[4], FA(r2, FM(FM(2.0f, x), x))));
-        const float yn = FA(FA(FM(y, dc), FM(FM(FM(2.0f, cam.d[4]), xn), y)), FM(cam.d[3], FA(r2, FM(FM(2.0f, y), y))));
-        x = xn; y = yn;
-    }
-    const float pu5 = FA(FA(FM(cam.fx, x), cam.cx), 0.5f), pv5 = FA(FA(FM(cam.fy, y), cam.cy), 0.5f);
-    if (!(pu5 > -2147483000.0f && pu5 < 2147483000.0f && pv5 > -2147483000.0f && pv5 < 2147483000.0f)) return o;
-    const int iu = __float2int_rz(pu5), iv = __float2int_rz(pv5);
-    if (iu < 0 || iu >= W || iv < 0 || iv >= H) return o;
-    o.d = __ldg(depth + static_cast<size_t>(iv) * W + iu);
-    o.ok = 1;
-    return o;
-}
-__device__ __forceinline__ float obs_finish(const ObsProbe& o, const float nrm[3], const float* __restrict__ Rt, const SelectCam& cam)
-{
-    if (!o.ok) return 0.0f;
-    const float d = o.d;
-    const float q[3] = {o.q0, o.q1, o.q2};
-    if (cam.occlusion > 0.0f)
-    {
-        if (!(d > 0.0f)) return 0.0f;
-        const float sd = FS(d, q[2]);
-        if (!(fabsf(sd) <= cam.occlusion)) return 0.0f;
-    }
-    if (d <= 0.0f) return 0.0f;
-    float nc[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) nc[k] = FA(FA(FM(Rt[3 * k], nrm[0]), FM(Rt[3 * k + 1], nrm[1])), FM(Rt[3 * k + 2], nrm[2]));
-    float w_normal = 0.0f;
-    if (!(nc[0] == 0.0f && nc[1] == 0.0f && nc[2] == 0.0f))
-    {
-        const float qn2 = FA(FA(FM(q[0], q[0]), FM(q[1], q[1])), FM(q[2], q[2]));
-        float v0 = q[0], v1 = q[1], v2 = q[2];
-        if (qn2 > 0.0f) { const float ql = __fsqrt_rn(qn2); v0 = FD(q[0], ql); v1 = FD(q[1], ql); v2 = FD(q[2], ql); }
-        const float dt = FA(FA(FM(v0, nc[0]), FM(v1, nc[1])), FM(v2, nc[2]));
-        w_normal = FS(1.0f, fabsf(dt));
-        w_normal = (1.0f < w_normal) ? 1.0f : w_normal;
-        w_normal = (w_normal < 0.0f) ? 0.0f : w_normal;
-        const float div = FA(1.0f, FM(2.0f, w_normal));
-        const float rk = FD(1.0f, FM(FM(div, div), div));
-        w_normal = (rk < 0.001f) ? 0.001f : rk;
-    }
-    return w_normal;
-}
-
-// ---- conservative frame culling for the observation selection ---------------------------------------------------------
-// Per frame, 32x32-pixel tiles of the depth map: minimum positive depth (+inf if none) and maximum depth.  Built once per
-// i3d_upload_frames.  A warp of k_select_obs (32 consecutive active voxels = a compact spatial cluster when the grid is in a
-// coherent order) bounds its iso-points by a sphere and asks, per frame: can ANY point of the sphere pass the reference's
-// tests (pixel inside the image, d > 0, |d - z| <= occlusion)?  If not, every voxel of the warp has weight exactly 0 for
-// that frame and the exact per-voxel computation is skipped.  The selection result is bit-identical by construction
-// (only provably-zero weights are skipped); the parity tests check it.
-constexpr int kCullTile = 32;
-constexpr int kCullMaxWords = 16;     // frames / 32 handled by the culling mask (F <= 512); beyond that no culling
-
+// per-frame 32x32 depth tiles of the frame culling (CullView, i3d_observe.cuh)
 __global__ void k_depth_tiles(int F, int W, int H, const float* __restrict__ depth, float* __restrict__ tmin, float* __restrict__ tmax)
 {
     const int TW = (W + kCullTile - 1) / kCullTile, TH = (H + kCullTile - 1) / kCullTile;
@@ -577,65 +440,10 @@ __global__ void k_depth_tiles(int F, int W, int H, const float* __restrict__ dep
     }
 }
 
-struct CullView { const float* tmin; const float* tmax; int enabled; unsigned long long* stats; /* [0] frames visited, [1] frames total (per warp), optional */ };
-
-// true = the frame may see some point of the sphere (centre c, radius rad), false = provably no voxel of the cluster is visible
-__device__ __forceinline__ bool frame_may_see(const float c[3], float rad, const float* __restrict__ Rt, const SelectCam& cam, const CullView& cv,
-                                              int f, int W, int H)
-{
-    const float qx = Rt[0] * c[0] + Rt[1] * c[1] + Rt[2] * c[2] + Rt[9];
-    const float qy = Rt[3] * c[0] + Rt[4] * c[1] + Rt[5] * c[2] + Rt[10];
-    const float qz = Rt[6] * c[0] + Rt[7] * c[1] + Rt[8] * c[2] + Rt[11];
-    const float zmin = qz - rad, zmax = qz + rad;
-    if (!(zmin > 1e-3f)) return true;                           // sphere touches the camera plane: no claim
-    const float iz = 1.0f / qz;
-    float xc = qx * iz, yc = qy * iz;
-    // |x/z - xc/zc| <= rad (1 + |xc/zc|) / zmin per axis for every point of the sphere
-    const float rnx = rad * (1.0f + fabsf(xc)) / zmin, rny = rad * (1.0f + fabsf(yc)) / zmin;
-    float lip = 1.0f;
-    if (!cam.dist_zero)
-    {
-        // lens distortion (Camera::project, y' uses the distorted x', Q2): map the centre exactly, bound the footprint growth by a
-        // Lipschitz constant of the distortion map over the disk of normalised radius R that contains the footprint
-        const float R = sqrtf(xc * xc + yc * yc) + 1.4143f * fmaxf(rnx, rny);
-        const float R2 = R * R;
-        const float grow = 3.0f * fabsf(cam.d[0]) * R2 + 5.0f * fabsf(cam.d[1]) * R2 * R2 + 7.0f * fabsf(cam.d[2]) * R2 * R2 * R2 +
-                           8.0f * (fabsf(cam.d[3]) + fabsf(cam.d[4])) * R;
-        lip = 1.0f + 2.0f * grow * (1.0f + 2.0f * fabsf(cam.d[4]) * R);      // generous: the y' term multiplies the x' growth once more
-        const float r2 = xc * xc + yc * yc;
-        const float dc = 1.0f + cam.d[0] * r2 + cam.d[1] * r2 * r2 + cam.d[2] * r2 * r2 * r2;
-        const float xd = xc * dc + 2.0f * cam.d[3] * xc * yc + cam.d[4] * (r2 + 2.0f * xc * xc);
-        const float yd = yc * dc + 2.0f * cam.d[4] * xd * yc + cam.d[3] * (r2 + 2.0f * yc * yc);
-        xc = xd; yc = yd;
-    }
-    const float uc = cam.fx * xc + cam.cx, vc = cam.fy * yc + cam.cy;
-    // + 2 px for the float pipeline's rounding and the nearest-pixel rounding
-    const float ru = cam.fx * 1.4143f * fmaxf(rnx, rny) * lip * 1.001f + 2.0f;
-    const float rv = cam.fy * 1.4143f * fmaxf(rnx, rny) * lip * 1.001f + 2.0f;
-    if (uc + ru < 0.0f || uc - ru > static_cast<float>(W) || vc + rv < 0.0f || vc - rv > static_cast<float>(H)) return false;   // entirely outside
-    const int TW = (W + kCullTile - 1) / kCullTile, TH = (H + kCullTile - 1) / kCullTile;
-    const int tx0 = max(0, static_cast<int>(floorf((uc - ru) / kCullTile))), tx1 = min(TW - 1, static_cast<int>(floorf((uc + ru) / kCullTile)));
-    const int ty0 = max(0, static_cast<int>(floorf((vc - rv) / kCullTile))), ty1 = min(TH - 1, static_cast<int>(floorf((vc + rv) / kCullTile)));
-    if (tx1 - tx0 > 3 || ty1 - ty0 > 3) return true;            // large footprint: do not bother
-    float dmin = __int_as_float(0x7f800000), dmax = 0.0f;
-    const float* mn = cv.tmin + static_cast<size_t>(f) * TW * TH;
-    const float* mx = cv.tmax + static_cast<size_t>(f) * TW * TH;
-    for (int ty = ty0; ty <= ty1; ++ty)
-        for (int tx = tx0; tx <= tx1; ++tx) { dmin = fminf(dmin, mn[ty * TW + tx]); dmax = fmaxf(dmax, mx[ty * TW + tx]); }
-    if (!(dmax > 0.0f)) return false;                           // no positive depth under the footprint: computeWeight returns 0
-    if (cam.occlusion > 0.0f)
-    {
-        const float tol = cam.occlusion * 1.001f + 1e-4f;
-        if (zmin > dmax + tol || zmax < dmin - tol) return false;   // |d - z| <= occlusion impossible
-    }
-    return true;
-}
-
 // One thread per active voxel, serial loop over the candidate frames; the best K (weight, frame) keys are kept in a small
-// sorted register list (key = weight bits << 32 | frame + 1: larger weight first, ties -> higher frame id = the
-// canonical top-K of oracle.cpp).  Neighbouring threads are neighbouring voxels, so for a given frame the 32
+// sorted register list (topk_insert).  Neighbouring threads are neighbouring voxels, so for a given frame the 32
 // depth taps of a warp fall on neighbouring pixels, and the per-frame pose (R|t) is warp-uniform (shared memory
-// broadcast).  Frames that provably see no voxel of the warp's cluster are skipped (frame_may_see).
+// broadcast).  Frames that provably see no voxel of the warp's cluster are skipped (frame_candidates).
 template <int KMAX>
 __global__ void __launch_bounds__(kThreads)
 k_select_obs(GridView g, FrameView fr, const float* __restrict__ Rt, SelectCam cam, CullView cull, int n_active, int stride,
@@ -651,61 +459,16 @@ k_select_obs(GridView g, FrameView fr, const float* __restrict__ Rt, SelectCam c
     if (__ballot_sync(0xffffffffu, in_range) == 0u) return;     // whole warp past the end
     float nrm[3] = {0.0f, 0.0f, 0.0f};
     float pt[3] = {0.0f, 0.0f, 0.0f};
-    if (in_range)
-    {
-        const int64_t v = act[a];
-        surface_normal_f(g, v, nrm);
-        const float s = static_cast<float>(g.sdf[v]);
-        pt[0] = FS(FM(static_cast<float>(g.x[v]), g.voxel_size), FM(nrm[0], s));
-        pt[1] = FS(FM(static_cast<float>(g.y[v]), g.voxel_size), FM(nrm[1], s));
-        pt[2] = FS(FM(static_cast<float>(g.z[v]), g.voxel_size), FM(nrm[2], s));
-    }
-    // ---- bounding sphere of the warp's iso-points, then the candidate-frame mask (lane l tests frames l, l+32, ...)
+    if (in_range) iso_point(g, act[a], nrm, pt);                // active voxels have a normal
     const int nwords = (fr.F + 31) / 32;
     __shared__ unsigned s_mask[kThreads / 32][kCullMaxWords];   // candidate-frame bit mask per warp (one copy of the visiting loop: no unrolling)
     unsigned* wmask = s_mask[threadIdx.x >> 5];
-    const bool culling = cull.enabled && nwords <= kCullMaxWords;
-    if (culling)
-    {
-        const float big = 3.0e38f;
-        float lo[3], hi[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) { lo[k] = in_range ? pt[k] : big; hi[k] = in_range ? pt[k] : -big; }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-            for (int k = 0; k < 3; ++k) { lo[k] = fminf(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o)); hi[k] = fmaxf(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o)); }
-        const float c[3] = {0.5f * (lo[0] + hi[0]), 0.5f * (lo[1] + hi[1]), 0.5f * (lo[2] + hi[2])};
-        const float dx = hi[0] - lo[0], dy = hi[1] - lo[1], dz = hi[2] - lo[2];
-        const float rad = 0.5f * sqrtf(dx * dx + dy * dy + dz * dz) * 1.001f + 1e-4f;
-#pragma unroll 1
-        for (int j = 0; j < nwords; ++j)
-        {
-            const int f = 32 * j + lane;
-            const bool may = (f < fr.F) && frame_may_see(c, rad, s_rt + 12 * f, cam, cull, f, fr.W, fr.H);
-            const unsigned m = __ballot_sync(0xffffffffu, may);
-            if (lane == 0) wmask[j] = m;
-        }
-        __syncwarp();
-    }
+    const bool culling = frame_candidates(pt, in_range, s_rt, fr, cam, cull, wmask);
     const size_t img = static_cast<size_t>(fr.W) * fr.H;
     unsigned long long best[KMAX];
 #pragma unroll
     for (int k = 0; k < KMAX; ++k) best[k] = 0ull;
-    auto insert = [&](float wf, int f) {
-        if (wf > 0.0f && in_range)
-        {
-            unsigned long long key = (static_cast<unsigned long long>(__float_as_uint(wf)) << 32) | static_cast<unsigned>(f + 1);
-            // sorted insertion (descending); slots >= K are never read
-#pragma unroll
-            for (int k = 0; k < KMAX; ++k)
-            {
-                const unsigned long long hi2 = key > best[k] ? key : best[k];
-                const unsigned long long lo2 = key > best[k] ? best[k] : key;
-                best[k] = hi2; key = lo2;
-            }
-        }
-    };
+    auto insert = [&](float wf, int f) { if (wf > 0.0f && in_range) topk_insert(best, wf, f); };     // slots >= K are never read
     if (cull.stats && lane == 0)
     {
         unsigned long long vis = 0;
@@ -716,7 +479,7 @@ k_select_obs(GridView g, FrameView fr, const float* __restrict__ Rt, SelectCam c
     // of the grid per GPU the whole launch is a single wave and its duration is the longest such chain (0.29 ms for 1/8 of the C3 grid
     // against 1.0 ms for all of it, profiles/r02s_bench_c3_8gpu_p2p.json).  Software pipelining, depth 2: the depth tap of frame i+1
     // is issued (obs_probe) before the weight of frame i is finished (obs_finish), so the tap's latency overlaps a visit's arithmetic.
-    ObsProbe pend; pend.ok = 0; pend.q0 = pend.q1 = pend.q2 = pend.d = 0.0f;
+    ObsProbe pend{};
     int pend_f = -1;
 #pragma unroll 1
     for (int j = 0; j < nwords; ++j)
@@ -738,22 +501,7 @@ k_select_obs(GridView g, FrameView fr, const float* __restrict__ Rt, SelectCam c
     // Slot order carries no meaning for the solve; order the K selected observations by ascending frame id so that
     // neighbouring voxels (which mostly select the same frames, in varying rank order) agree slot by slot: the
     // per-frame warp reductions of k_eg_accum / k_eg_apply then see ~1 distinct frame per warp and slot.
-    // Re-key as (frame+1) << 32 | weight bits; empty entries (0) sort last.
-#pragma unroll
-    for (int k = 0; k < KMAX; ++k)
-    {
-        if (k >= K || best[k] == 0ull) best[k] = ~0ull;
-        else best[k] = ((best[k] & 0xffffffffull) << 32) | (best[k] >> 32);
-    }
-#pragma unroll
-    for (int i = 0; i < KMAX; ++i)
-#pragma unroll
-        for (int j = 0; j + 1 < KMAX - i; ++j)
-        {
-            const unsigned long long lo = best[j] < best[j + 1] ? best[j] : best[j + 1];
-            const unsigned long long hi = best[j] < best[j + 1] ? best[j + 1] : best[j];
-            best[j] = lo; best[j + 1] = hi;
-        }
+    topk_frame_order(best, K);
 #pragma unroll
     for (int k = 0; k < KMAX; ++k)
     {

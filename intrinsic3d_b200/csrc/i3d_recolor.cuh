@@ -5,8 +5,8 @@
  * SDFColorization::add for every frame + SDFColorization::compute (src/sdf/colorization.cpp:113-189), with
  * computeObservation / computeWeight / filter / computeColor (:215-370) and interpolateRGB (src/rgbd/processing.cpp:236-302).
  *
- * One thread per voxel that has a forward-difference normal.  The frame scan is the one of k_select_obs (same float pipeline,
- * same conservative per-warp frame culling); the best K (weight, frame) keys stay in registers.  The reference keeps a
+ * One thread per voxel that has a forward-difference normal.  The frame scan is the one of k_select_obs (the observation weight,
+ * the conservative per-warp frame culling and the top-K of i3d_observe.cuh); the best K (weight, frame) keys stay in registers.  The reference keeps a
  * std::vector of observations per voxel (N x F VertexObservation objects across the F add() calls); here nothing is stored:
  * the <= K winning frames are re-projected at the end and their colours fetched bilinearly.
  *
@@ -15,7 +15,7 @@
  * oracle.cpp), otherwise (K == 0 or at most K observations) in frame order.
  */
 #pragma once
-#include "i3d_kernels.cuh"
+#include "i3d_observe.cuh"
 
 namespace i3d
 {
@@ -56,44 +56,12 @@ k_recolor(GridView g, FrameView fr, const uint8_t* __restrict__ bgr /* [F][H][W]
     const int64_t v = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
     float nrm[3] = {0.0f, 0.0f, 0.0f};
     float pt[3] = {0.0f, 0.0f, 0.0f};
-    bool in_range = false;
-    if (v < g.n && surface_normal_f(g, v, nrm))             // add(): voxels without a normal collect nothing
-    {
-        in_range = true;
-        const float s = static_cast<float>(g.sdf[v]);
-        pt[0] = FS(FM(static_cast<float>(g.x[v]), g.voxel_size), FM(nrm[0], s));
-        pt[1] = FS(FM(static_cast<float>(g.y[v]), g.voxel_size), FM(nrm[1], s));
-        pt[2] = FS(FM(static_cast<float>(g.z[v]), g.voxel_size), FM(nrm[2], s));
-    }
+    const bool in_range = v < g.n && iso_point(g, v, nrm, pt);     // add(): voxels without a normal collect nothing
     if (__ballot_sync(0xffffffffu, in_range) == 0u) return;
-    // ---- candidate-frame mask of the warp's cluster (see k_select_obs / frame_may_see)
     const int nwords = (fr.F + 31) / 32;
     __shared__ unsigned s_mask[kThreads / 32][kCullMaxWords];
     unsigned* wmask = s_mask[threadIdx.x >> 5];
-    const bool culling = cull.enabled && nwords <= kCullMaxWords;
-    if (culling)
-    {
-        const float big = 3.0e38f;
-        float lo[3], hi[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) { lo[k] = in_range ? pt[k] : big; hi[k] = in_range ? pt[k] : -big; }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-            for (int k = 0; k < 3; ++k) { lo[k] = fminf(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o)); hi[k] = fmaxf(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o)); }
-        const float c[3] = {0.5f * (lo[0] + hi[0]), 0.5f * (lo[1] + hi[1]), 0.5f * (lo[2] + hi[2])};
-        const float dx = hi[0] - lo[0], dy = hi[1] - lo[1], dz = hi[2] - lo[2];
-        const float rad = 0.5f * sqrtf(dx * dx + dy * dy + dz * dz) * 1.001f + 1e-4f;
-#pragma unroll 1
-        for (int j = 0; j < nwords; ++j)
-        {
-            const int f = 32 * j + lane;
-            const bool may = (f < fr.F) && frame_may_see(c, rad, s_rt + 12 * f, cam, cull, f, fr.W, fr.H);
-            const unsigned m = __ballot_sync(0xffffffffu, may);
-            if (lane == 0) wmask[j] = m;
-        }
-        __syncwarp();
-    }
+    const bool culling = frame_candidates(pt, in_range, s_rt, fr, cam, cull, wmask);
     const size_t img = static_cast<size_t>(fr.W) * fr.H;
     const float scale_color = FD(1.0f, 255.0f);
     unsigned long long best[KMAX];
@@ -101,14 +69,12 @@ k_recolor(GridView g, FrameView fr, const uint8_t* __restrict__ bgr /* [F][H][W]
     for (int k = 0; k < KMAX; ++k) best[k] = 0ull;
     int n_obs = 0;
     float c3[3] = {0.0f, 0.0f, 0.0f}, wsum = 0.0f;
-    auto add_color = [&](int f, float wf) {
-        float pix[2];
-        observation_weight(pt, nrm, s_rt + 12 * f, cam, fr.depth + img * f, fr.W, fr.H, pix);     // same arithmetic => same sub-pixel position
+    auto add_color = [&](int f, float wf, const ObsProbe& p) {     // p: the frame's probe, for the sub-pixel position
         const uint8_t* cimg = bgr + img * f * 3;
         const float ws = FM(wf, scale_color);
-        c3[0] = FA(c3[0], FM(static_cast<float>(interp_u8(cimg, fr.W, fr.H, pix[0], pix[1], 2)), ws));
-        c3[1] = FA(c3[1], FM(static_cast<float>(interp_u8(cimg, fr.W, fr.H, pix[0], pix[1], 1)), ws));
-        c3[2] = FA(c3[2], FM(static_cast<float>(interp_u8(cimg, fr.W, fr.H, pix[0], pix[1], 0)), ws));
+        c3[0] = FA(c3[0], FM(static_cast<float>(interp_u8(cimg, fr.W, fr.H, p.pu, p.pv, 2)), ws));
+        c3[1] = FA(c3[1], FM(static_cast<float>(interp_u8(cimg, fr.W, fr.H, p.pu, p.pv, 1)), ws));
+        c3[2] = FA(c3[2], FM(static_cast<float>(interp_u8(cimg, fr.W, fr.H, p.pu, p.pv, 0)), ws));
         wsum = FA(wsum, wf);
     };
 #pragma unroll 1
@@ -121,19 +87,13 @@ k_recolor(GridView g, FrameView fr, const uint8_t* __restrict__ bgr /* [F][H][W]
             const int f = 32 * j + __ffs(m) - 1;
             m &= m - 1;
             if (f >= fr.F) continue;
-            const float wf = observation_weight(pt, nrm, s_rt + 12 * f, cam, fr.depth + img * f, fr.W, fr.H);
+            const ObsProbe p = obs_probe(pt, s_rt + 12 * f, cam, fr.depth + img * f, fr.W, fr.H);
+            const float wf = obs_finish(p, nrm, s_rt + 12 * f, cam);
             if (wf > 0.0f && in_range)
             {
                 ++n_obs;
-                if (K == 0) { add_color(f, wf); continue; }
-                unsigned long long key = (static_cast<unsigned long long>(__float_as_uint(wf)) << 32) | static_cast<unsigned>(f + 1);
-#pragma unroll
-                for (int k = 0; k < KMAX; ++k)
-                {
-                    const unsigned long long hi2 = key > best[k] ? key : best[k];
-                    const unsigned long long lo2 = key > best[k] ? best[k] : key;
-                    best[k] = hi2; key = lo2;
-                }
+                if (K == 0) add_color(f, wf, p);
+                else topk_insert(best, wf, f);
             }
         }
     }
@@ -164,18 +124,8 @@ k_recolor(GridView g, FrameView fr, const uint8_t* __restrict__ bgr /* [F][H][W]
         }
         else
         {
-            // the filter returned early: frame order
-#pragma unroll
-            for (int k = 0; k < KMAX; ++k) best[k] = (best[k] == 0ull) ? ~0ull : (((best[k] & 0xffffffffull) << 32) | (best[k] >> 32));
-#pragma unroll
-            for (int i = 0; i < KMAX; ++i)
-#pragma unroll
-                for (int j = 0; j + 1 < KMAX - i; ++j)
-                {
-                    const unsigned long long lo = best[j] < best[j + 1] ? best[j] : best[j + 1];
-                    const unsigned long long hi = best[j] < best[j + 1] ? best[j + 1] : best[j];
-                    best[j] = lo; best[j + 1] = hi;
-                }
+            // the filter returned early: frame order.  At most K keys were inserted, so the slots from K upwards are empty already.
+            topk_frame_order(best, K);
         }
         // best[] now holds (frame + 1) << 32 | weight bits in summation order, ~0 = empty
         int sel_f[KMAX]; float sel_w[KMAX];
@@ -187,7 +137,7 @@ k_recolor(GridView g, FrameView fr, const uint8_t* __restrict__ bgr /* [F][H][W]
         }
 #pragma unroll 1
         for (int k = 0; k < KMAX; ++k)
-            if (sel_f[k] >= 0) add_color(sel_f[k], sel_w[k]);
+            if (sel_f[k] >= 0) add_color(sel_f[k], sel_w[k], obs_probe(pt, s_rt + 12 * sel_f[k], cam, fr.depth + img * sel_f[k], fr.W, fr.H));
     }
     // computeColor (colorization.cpp:318-354): mean colour, cast<unsigned char> truncates
     if (wsum > 0.0f) { const float s = FD(255.0f, wsum); c3[0] = FM(c3[0], s); c3[1] = FM(c3[1], s); c3[2] = FM(c3[2], s); }

@@ -216,7 +216,7 @@ __device__ __forceinline__ void rd_point(const float o[3], const float dn[3], fl
     for (int d = 0; d < 3; ++d) p[d] = FA(o[d], FM(s, dn[d]));
 }
 
-// One thread per pixel (u, v) of view blockIdx.z.  Ray: the pixel centre through the inverse of observation_weight's projection, in
+// One thread per pixel (u, v) of view blockIdx.z.  Ray: the pixel centre through the inverse of obs_probe's projection (i3d_observe.cuh), in
 // world coordinates; samples s_k = s0 + k * voxel_size / 2 from where the ray enters the voxel box (clipped to s >= 0) to where it
 // leaves it; the hit is the first pair of consecutive valid samples going from > 0 to <= 0 whose linearly interpolated crossing lies in a
 // valid cube.  G: the installed grid (RenderGrid), the fusion volume in progress (LiveGrid), or either with the model intensity plane
