@@ -410,7 +410,8 @@ __global__ void k_frame_pose(int F, const double* __restrict__ poses, FramePose*
     out[f] = fp;
 }
 
-// per-frame 32x32 depth tiles of the frame culling (CullView, i3d_observe.cuh)
+// per-frame 32x32 depth tiles of the frame culling (CullView, i3d_observe.cuh).  A NaN pixel makes the tile's maximum +inf: with the
+// occlusion test off the reference observes a NaN depth (only d <= 0 is rejected), so such a tile must not look empty.
 __global__ void k_depth_tiles(int F, int W, int H, const float* __restrict__ depth, float* __restrict__ tmin, float* __restrict__ tmax)
 {
     const int TW = (W + kCullTile - 1) / kCullTile, TH = (H + kCullTile - 1) / kCullTile;
@@ -426,6 +427,7 @@ __global__ void k_depth_tiles(int F, int W, int H, const float* __restrict__ dep
         {
             const float d = img[static_cast<size_t>(py) * W + px];
             if (d > 0.0f) { mn = fminf(mn, d); mx = fmaxf(mx, d); }
+            else if (d != d) mx = __int_as_float(0x7f800000);
         }
     }
 #pragma unroll

@@ -99,11 +99,14 @@ __device__ __forceinline__ bool iso_point(const GridView& g, int64_t v, float nr
 }
 
 // ---- conservative frame culling of the frame scans ----------------------------------------------------------------------
-// Per frame, 32x32-pixel tiles of the depth map: minimum positive depth (+inf if none) and maximum depth (k_depth_tiles).  Built once per
+// Per frame, 32x32-pixel tiles of the depth map: minimum positive depth (+inf if none) and maximum depth, +inf if the tile holds a NaN
+// (k_depth_tiles): with the occlusion test off the reference rejects d <= 0 only, so it observes NaN depths.  Built once per
 // i3d_upload_frames.  A warp of a frame scan (32 consecutive voxels = a compact spatial cluster when the grid is in a coherent order)
 // bounds its iso-points by a sphere and asks, per frame: can ANY point of the sphere pass the reference's tests (pixel inside the image,
-// d > 0, |d - z| <= occlusion)?  If not, every voxel of the warp has weight exactly 0 for that frame and the exact per-voxel computation
-// is skipped.  The result is bit-identical by construction (only provably-zero weights are skipped); the parity tests check it.
+// depth not rejected, |d - z| <= occlusion)?  If not, every voxel of the warp has weight exactly 0 for that frame and the exact per-voxel
+// computation is skipped.  The result is bit-identical by construction (only provably-zero weights are skipped):
+// tests/test_gpu_zz_cull_bound.py fuzzes frame_may_see against the exact weight on the device, and tests/test_gpu_zz_frame_scan.py holds
+// both frame scans bit-equal to the oracle and byte-equal to I3D_NO_CULL where the bounds are tight.
 constexpr int kCullTile = 32;
 constexpr int kCullMaxWords = 16;     // frames / 32 handled by the culling mask (F <= 512); beyond that no culling
 
