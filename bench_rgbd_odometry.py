@@ -2,7 +2,8 @@
 """bench_rgbd_odometry.py — dense RGB-D odometry depth-only (i3d_fusion_track_and_integrate_sensor) and with the photometric term
 (i3d_fusion_track_and_integrate_sensor_rgbd) side by side over every frame of a workload, one JSON line.
 
-    python bench_rgbd_odometry.py [--workload c2|c3|small|tiny] [--frames 200] [--weights 0.1] [--ref-weights 0.01,0.05] [--reps 1]
+    python bench_rgbd_odometry.py [--workload c2|c3|small|tiny] [--frames 200] [--weights 0.1] [--ref-weights 0.01,0.05]
+                                  [--lni-weights 0.002] [--lni-radius 5] [--lni-eps 0.01] [--clean-color] [--reps 1]
 
 The workload's frames go into the sensor store; each run begins a fusion and runs the loop over all frames from the true pose of frame 0
 (anchored) with the default tracking parameters, once depth-only and once per colour weight in --weights (lambda for every level, the
@@ -12,7 +13,10 @@ host clock, ends in a synchronise) in total and per frame, and the device phases
 timers gives the time of k_track_photo_rows ("track_photo_rows") and its byte-model share of 3350 GB/s.  The GPU name and power limit are
 read in the same run.  --ref-weights adds, in the same format, one mode per weight of the loop with the reference model
 (i3d_fusion_track_and_integrate_sensor_rgbd_ref, DESIGN.md §6q), whose timed run gives k_track_ref_model ("track_ref_model") and its
-byte-model share.  Writes nothing.
+byte-model share.  --lni-weights adds one mode per weight of the reference loop with locally normalised intensity (norm_radius
+--lni-radius, norm_eps --lni-eps, the other colour parameters at i3d_default_track_color_lni_params, DESIGN.md §6r), whose timed run also
+gives k_track_local_norm ("track_local_norm") and its byte-model share.  --clean-color stores colour frames with B = G = R =
+rint(255 lum) and no per-frame modulation: the bound any appearance compensation can reach with the photometric term.  Writes nothing.
 """
 import argparse
 import json
@@ -35,6 +39,9 @@ PHOTO_BYTES_PER_PIXEL = 60
 # k_track_ref_model's byte model per pixel of a level and per frame, an upper bound as if every pixel passed every test: prediction depth
 # (4 B), the reference depth tap (4 B), four intensity taps (16 B) and the model write (4 B)
 REF_BYTES_PER_PIXEL = 28
+# k_track_local_norm's byte model per pixel of a level: one read of the raw plane and one write of the normalised plane (8 B); the halo
+# rows and the (2r+1) taps along the row and down the column come from L1 / shared memory
+LNI_BYTES_PER_PIXEL = 8
 
 
 def main():
@@ -43,6 +50,10 @@ def main():
     ap.add_argument("--frames", type=int, default=200)
     ap.add_argument("--weights", default="0.1")
     ap.add_argument("--ref-weights", default="")
+    ap.add_argument("--lni-weights", default="")
+    ap.add_argument("--lni-radius", type=int, default=5)
+    ap.add_argument("--lni-eps", type=float, default=0.01)
+    ap.add_argument("--clean-color", action="store_true")
     ap.add_argument("--reps", type=int, default=1)
     args = ap.parse_args()
 
@@ -56,6 +67,8 @@ def main():
     s = config_scene(args.workload, device="cuda:0" if torch.cuda.is_available() else "cpu", frames=args.frames)
     dcam, depth, ccam, bgr, c2w, w2c = scene_inputs(s)
     F, H, W = depth.shape
+    if args.clean_color:
+        bgr = np.repeat(np.clip(np.rint(np.asarray(s["lum"], np.float32) * np.float32(255.0)), 0, 255).astype(np.uint8)[..., None], 3, axis=-1)
     e = engine.Engine(0)
     e.sensor_frames_begin(dcam, ccam, F)
     e.sensor_frames_add(depth, bgr)
@@ -74,6 +87,9 @@ def main():
         ref, weight = mode
         if weight is None:
             out, infos = e.fusion_track_and_integrate_sensor(ids, true[0])
+        elif ref == "lni":
+            out, infos = e.fusion_track_and_integrate_sensor_rgbd_ref(ids, true[0], color=dict(weight=weight, norm_radius=args.lni_radius,
+                                                                                                norm_eps=args.lni_eps))
         elif ref:
             out, infos = e.fusion_track_and_integrate_sensor_rgbd_ref(ids, true[0], color=dict(weight=weight))
         else:
@@ -83,6 +99,7 @@ def main():
 
     modes = [(False, None)] + [(False, float(w)) for w in args.weights.split(",")]
     modes += [(True, float(w)) for w in args.ref_weights.split(",") if w]
+    modes += [("lni", float(w)) for w in args.lni_weights.split(",") if w]
     run(modes[0])                                                       # warm-up
     results = {}
     for mode in modes:
@@ -118,10 +135,23 @@ def main():
                 gb = n // tp.num_levels * level_pixels * REF_BYTES_PER_PIXEL / 1e9
                 res["k_track_ref_model"] = {"ms": ms, "launches": n, "model_gb": gb, "gbs": gb / (ms / 1e3) if ms > 0 else None,
                                             "share_of_hbm": gb / (ms / 1e3) / HBM_GBS if ms > 0 else None}
-        results["depth_only" if w is None else (f"ref_w{w:g}" if ref else f"color_w{w:g}")] = res
+            if ref == "lni":
+                ms = e.phase_ms("track_local_norm")
+                n = int(e.phase_count("track_local_norm"))
+                gb = n // tp.num_levels * level_pixels * LNI_BYTES_PER_PIXEL / 1e9
+                res["k_track_local_norm"] = {"ms": ms, "launches": n, "ms_per_frame": ms / F, "model_gb": gb,
+                                             "gbs": gb / (ms / 1e3) if ms > 0 else None,
+                                             "share_of_hbm": gb / (ms / 1e3) / HBM_GBS if ms > 0 else None}
+        if w is None:
+            key = "depth_only"
+        elif ref == "lni":
+            key = f"lni_r{args.lni_radius}_eps{args.lni_eps:g}_w{w:g}"
+        else:
+            key = f"ref_w{w:g}" if ref else f"color_w{w:g}"
+        results[key] = res
     line = {"metric": "rgbd_odometry_all_frames_ms", "value": results[f"color_w{modes[1][1]:g}"]["wall_ms"], "unit": "ms",
             "higher_is_better": False, "workload": args.workload, "gpu": gpu, "reps": max(1, args.reps), "frames": int(F),
-            "size": [int(W), int(H)], "modes": results}
+            "size": [int(W), int(H)], "clean_color": bool(args.clean_color), "modes": results}
     print(json.dumps(line))
 
 

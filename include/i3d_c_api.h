@@ -348,6 +348,21 @@ int         i3d_fusion_track_and_integrate_sensor_rgbd_ref(I3DEngine* e, int32_t
 int         i3d_debug_get_track_reference_planes(I3DEngine* e, int32_t level, float* model, float* ref_intensity, float* ref_depth,
                                                  int32_t* frames);
 
+/* ---- locally normalised intensity for the reference model (DESIGN.md §6r) ---- */
+/* The largest norm_radius of I3DTrackColorParams. */
+#define I3D_TRACK_MAX_NORM_RADIUS 8
+/* With color->norm_radius = r > 0 the three _ref calls compare locally normalised intensity: every level of the frame's and of the
+ * reference's intensity pyramid (each level still the pyrDown of the raw level above) becomes (I - mu) / sqrt(max(m2 - mu^2, 0) +
+ * norm_eps^2), mu and m2 the float32 mean of I and I^2 over the (2r+1)^2 window clipped to the image, and exactly 0 where that window is
+ * constant.  A gain and offset constant over the window cancel, so per-frame exposure and white-balance changes that vary slowly across
+ * the image no longer bias the residual.  Everything after the planes is unchanged; max_color_diff, min_color_gradient and the residuals
+ * of color_info are in normalised units, and i3d_debug_get_track_color_planes / i3d_debug_get_track_reference_planes return the
+ * normalised planes the rows read.  norm_radius 0 gives the bytes of today's _ref calls.  The _ref calls fail, writing nothing, for
+ * norm_radius < 0 or > I3D_TRACK_MAX_NORM_RADIUS and, with norm_radius > 0, norm_eps not finite or <= 0; the _rgbd calls (voxel model,
+ * whose model plane has holes) fail for norm_radius != 0.  With i3d_debug_set_kernel_timers(e, 1) also "track_local_norm". */
+/* i3d_default_track_color_ref_params with the LNI parameters measured on C2 (DESIGN.md §6r). */
+void        i3d_default_track_color_lni_params(I3DTrackColorParams* p);
+
 /* ---- keyframe selection and the RGB-D image pyramid: the inputs of fusion and refinement (DESIGN.md §6i) ---- */
 /* Frames scored per device pass by i3d_keyframe_scores: bounds its scratch memory (I3D_KEYFRAME_CHUNK * W * H * 3 bytes). */
 #define I3D_KEYFRAME_CHUNK 32

@@ -272,7 +272,9 @@ typedef struct I3DTrackColorParams
     float   weight[4];                    /* lambda per pyramid level, level 0 first: A = A_depth + lambda^2 A_colour; 0 = depth only */
     float   max_color_diff;               /* photometric gate |I_frame - I_model| (intensity in [0, 1]) */
     float   min_color_gradient;           /* texture gate |grad I_frame| (intensity per pixel, central differences); 0 = off */
-    int32_t reserved[2];
+    int32_t norm_radius;                  /* _ref calls only: > 0 compares locally normalised intensity over (2r+1)^2 windows (DESIGN.md
+                                             section 6r), and max_color_diff and min_color_gradient are then in its units; 0 = raw intensity */
+    float   norm_eps;                     /* with norm_radius > 0: the normalisation's floor, (I - mu) / sqrt(var + norm_eps^2); > 0 */
 } I3DTrackColorParams;
 
 typedef struct I3DTrackColorInfo

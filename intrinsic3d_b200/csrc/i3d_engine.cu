@@ -1828,8 +1828,8 @@ static int check_finite_poses(I3DEngine* e, const char* who, int32_t n, const do
     return 0;
 }
 
-// The refusals of a photometric term (DESIGN.md §6p); fills col
-static int check_track_color(I3DEngine* e, const char* who, const I3DTrackColorParams* cp, I3DTrackColorInfo* ci, TrackColor& col)
+// The refusals of a photometric term (DESIGN.md §6p) and of its local normalisation (§6r, reference: a _ref call); fills col
+static int check_track_color(I3DEngine* e, const char* who, const I3DTrackColorParams* cp, I3DTrackColorInfo* ci, bool reference, TrackColor& col)
 {
     if (!cp) return fail(e, "%s: color params must not be NULL", who);
     for (int l = 0; l < kTrackMaxLevels; ++l)
@@ -1838,6 +1838,13 @@ static int check_track_color(I3DEngine* e, const char* who, const I3DTrackColorP
         return fail(e, "%s: max_color_diff must be finite and > 0, got %g", who, cp->max_color_diff);
     if (!(std::isfinite(cp->min_color_gradient) && cp->min_color_gradient >= 0.0f))
         return fail(e, "%s: min_color_gradient must be finite and >= 0, got %g", who, cp->min_color_gradient);
+    if (cp->norm_radius != 0 && !reference)
+        return fail(e, "%s: norm_radius must be 0 with the voxel model, whose model plane is not an image (the _ref calls take it), got %d", who,
+                    cp->norm_radius);
+    if (cp->norm_radius < 0 || cp->norm_radius > I3D_TRACK_MAX_NORM_RADIUS)
+        return fail(e, "%s: norm_radius must be in 0..%d, got %d", who, I3D_TRACK_MAX_NORM_RADIUS, cp->norm_radius);
+    if (cp->norm_radius > 0 && !(std::isfinite(cp->norm_eps) && cp->norm_eps > 0.0f))
+        return fail(e, "%s: norm_eps must be finite and > 0 with norm_radius > 0, got %g", who, cp->norm_eps);
     col = TrackColor{cp, &e->sensor, ci};
     return 0;
 }
@@ -1873,7 +1880,7 @@ static int track_sensor_frames(I3DEngine* e, const char* who, int32_t n, const i
     int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
     if (check_track_params(e, who, P, Wl, Hl)) return 1;
     TrackColor col{};
-    if (rgbd && check_track_color(e, who, cp, ci, col)) return 1;
+    if (rgbd && check_track_color(e, who, cp, ci, ref.on, col)) return 1;
     if (ref.on && check_track_reference(e, who, n, ref, col)) return 1;
     return guarded(e, [&]() {
         track::sensor_frames(e->track, e->render, e->timing, render_grid(e, P.sdf_source, false), e->sensor.dcam, e->sensor.depth.p, e->sensor.F, n, ids, pose_in, P,
@@ -1925,7 +1932,7 @@ static int fusion_track_sensor_frames(I3DEngine* e, const char* who, int32_t n, 
     int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
     if (check_track_params(e, who, P, Wl, Hl)) return 1;
     TrackColor col{};
-    if (rgbd && check_track_color(e, who, cp, ci, col)) return 1;
+    if (rgbd && check_track_color(e, who, cp, ci, ref.on, col)) return 1;
     if (ref.on && check_track_reference(e, who, n, ref, col)) return 1;
     return guarded(e, [&]() {
         if (track::fusion_frames(e->track, e->fusion, e->render.skip, e->timing, e->sensor, n, ids, pose_in, P, Wl, Hl, pose_out, info, e->stream,
@@ -1970,7 +1977,7 @@ static int fusion_track_and_integrate_sensor(I3DEngine* e, const char* who, int3
     int Wl[kTrackMaxLevels], Hl[kTrackMaxLevels];
     if (check_track_params(e, who, P, Wl, Hl)) return 1;
     TrackColor col{};
-    if (rgbd && check_track_color(e, who, cp, ci, col)) return 1;
+    if (rgbd && check_track_color(e, who, cp, ci, reference, col)) return 1;
     const int rc = guarded(e, [&]() {
         std::string err;
         if (track::odometry(e->track, e->fusion, e->render.skip, e->timing, e->sensor, n, ids, pose_first, P, Wl, Hl, pose_out, info, err, e->stream,
@@ -2090,6 +2097,14 @@ void i3d_default_track_color_ref_params(I3DTrackColorParams* p)
 {
     i3d_default_track_color_params(p);
     for (int l = 0; l < kTrackMaxLevels; ++l) p->weight[l] = 0.01f;      // measured on C2 (DESIGN.md §6q)
+}
+
+void i3d_default_track_color_lni_params(I3DTrackColorParams* p)
+{
+    i3d_default_track_color_ref_params(p);
+    for (int l = 0; l < kTrackMaxLevels; ++l) p->weight[l] = 0.005f;      // measured on C2 (DESIGN.md §6r)
+    p->max_color_diff = 1.0f; p->min_color_gradient = 0.05f;
+    p->norm_radius = 3; p->norm_eps = 0.01f;
 }
 
 int i3d_debug_get_track_reference_planes(I3DEngine* e, int32_t level, float* model, float* ref_intensity, float* ref_depth, int32_t* frames)

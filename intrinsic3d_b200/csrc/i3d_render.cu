@@ -154,8 +154,8 @@ constexpr TrackPhases kOdometryPhases{nullptr, "odometry_predict", "odometry_icp
 // The tracker's passes over ids[0..n), shared by the grid and the fusion volume: prepare() (false: stop, nothing tracked) runs once
 // after the uploads, predict(cam, rv, mi) marches a chunk's prediction into rv, and with mi != nullptr the model intensity plane into mi.
 // pose_cw_out [n][12] (may be nullptr): the tracked camera -> world poses.  col: the photometric term (nullptr: depth only); with its
-// reference the plain march, then per pass the references' pyramids and k_track_ref_model per level, timed as ph.reference.  Returns
-// false when prepare() stopped the call.
+// reference the plain march, then per pass the references' pyramids and k_track_ref_model per level, timed as ph.reference; with its
+// norm_radius > 0 also both intensity pyramids through k_track_local_norm (DESIGN.md §6r).  Returns false when prepare() stopped the call.
 template <class Prepare, class Predict>
 bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&& prepare, Predict&& predict, const I3DFusionCamera& dc,
                   const float* store_depth, int store_F, int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl,
@@ -164,6 +164,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
     const int L = P.num_levels, W = dc.width, H = dc.height, C = std::min<int>(n, I3D_TRACK_CHUNK);
     const size_t img = static_cast<size_t>(W) * H;
     const bool ref = col && col->ref_ids;
+    const int norm_r = ref ? col->P->norm_radius : 0;       // DESIGN.md §6r: > 0 normalises both intensity pyramids
     const int tiles_x = (W + kRenderTile - 1) / kRenderTile, tiles_y = (H + kRenderTile - 1) / kRenderTile;
     static_assert(kRenderTile == kTrackTile, "the prediction and the rows share the level-0 tile grid");
     ts.n = 0;
@@ -179,6 +180,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
         ts.depth[l].ensure(c); ts.nrm[l].ensure(3 * c);
         if (col) { ts.inten[l].ensure(c); ts.gx[l].ensure(c); ts.gy[l].ensure(c); }
         if (ref) { ts.ref_inten[l].ensure(c); ts.ref_depth[l].ensure(c); }
+        if (norm_r > 0) { ts.raw_inten[l].ensure(c); ts.raw_ref_inten[l].ensure(c); }
         if (ref && l > 0) ts.ref_model[l].ensure(C * img);
     }
     std::vector<float> hr(ref ? 12 * static_cast<size_t>(n) : 0);      // the reference poses in float, by call order
@@ -230,9 +232,18 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
         k_track_gather<<<dim3(blocks_for(img), m), kThreads, 0, st>>>(m, W, H, ids_dev, store_depth, lv[0].p);
         for (int l = 1; l < L; ++l) frames::depthdown(m, Wl[l - 1], Hl[l - 1], lv[l - 1].p, lv[l].p, st);
     };
-    auto intensity_pyramid = [&](const int32_t* ids_host, Dev<float>* lv) {
-        frames::sensor_intensity(*col->ss, m, ids_host, ts.iota.p, ts.lum_c, lv[0].p, st);
-        for (int l = 1; l < L; ++l) frames::pyrdown(m, Wl[l - 1], Hl[l - 1], lv[l - 1].p, lv[l].p, st);
+    // with norm_r > 0 the raw pyramid goes to raw (each level the pyrdown of the raw level above) and k_track_local_norm writes lv
+    auto intensity_pyramid = [&](const int32_t* ids_host, Dev<float>* lv, Dev<float>* raw) {
+        Dev<float>* py = norm_r > 0 ? raw : lv;
+        frames::sensor_intensity(*col->ss, m, ids_host, ts.iota.p, ts.lum_c, py[0].p, st);
+        for (int l = 1; l < L; ++l) frames::pyrdown(m, Wl[l - 1], Hl[l - 1], py[l - 1].p, py[l].p, st);
+        for (int l = 0; l < L && norm_r > 0; ++l)
+        {
+            const int blocks = ((Wl[l] + kTrackLniTileW - 1) / kTrackLniTileW) * ((Hl[l] + kTrackLniTileH - 1) / kTrackLniTileH);
+            Timer tk(tm, st, "track_local_norm", 1);
+            k_track_local_norm<<<dim3(blocks, m), dim3(kTrackLniTileW, kTrackLniTileH), 0, st>>>(Wl[l], Hl[l], norm_r, col->P->norm_eps, raw[l].p,
+                                                                                                 lv[l].p);
+        }
     };
     for (int c0 = 0; c0 < n; c0 += C)
     {
@@ -258,7 +269,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
         {
             // the frame intensity pyramid in the depth camera and its gradients
             Timer t(tm, st, ph.color);
-            intensity_pyramid(ids + c0, ts.inten);
+            intensity_pyramid(ids + c0, ts.inten, ts.raw_inten);
             for (int l = 0; l < L; ++l)
                 k_track_grad<<<dim3(blocks_for(static_cast<size_t>(Wl[l]) * Hl[l]), m), kThreads, 0, st>>>(cam[l], ts.inten[l].p, ts.gx[l].p, ts.gy[l].p);
         }
@@ -266,7 +277,7 @@ bool track_passes(TrackScratch& ts, Timing& tm, const TrackPhases& ph, Prepare&&
         {
             // the references' intensity and depth pyramids by the frame's own rules, then each level's model plane
             Timer t(tm, st, ph.reference);
-            intensity_pyramid(col->ref_ids + c0, ts.ref_inten);
+            intensity_pyramid(col->ref_ids + c0, ts.ref_inten, ts.raw_ref_inten);
             depth_pyramid(ts.ref_ids.p + c0, ts.ref_depth);
             TrackRef tf{};
             tf.pcam = cam[0]; tf.pdepth = ts.pdepth.p; tf.ids = ids_d; tf.rt_in = ts.rt.p; tf.ref_rt = ts.ref_rt.p + 12 * static_cast<size_t>(c0);
@@ -430,7 +441,7 @@ void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderG
                           double* pose_out, I3DTrackInfo* info, cudaStream_t st, const TrackColor* col)
 {
     begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences", "track_color", "track_photo_rows",
-                      "track_photo_correspondences", "track_reference", "track_ref_model"});
+                      "track_photo_correspondences", "track_reference", "track_ref_model", "track_local_norm"});
     track_passes(
         ts, tm, kTrackPhases, [&]() { add_voxel_box(rs, tm, rg, st); return true; },
         [&](const RenderCam& cam, const RenderViews& rv, float* mi) { march(rg, cam, rv, st, mi); }, dc, store_depth, store_F, n, ids, pose_in, P,
@@ -442,7 +453,7 @@ int track::fusion_frames(TrackScratch& ts, const FusionState& fs, bool skip, Tim
                          const TrackColor* col)
 {
     begin_timing(tm, {"track", "track_predict", "track_pyramid", "track_icp", "track_correspondences", "track_bricks", "track_color",
-                      "track_photo_rows", "track_photo_correspondences", "track_reference", "track_ref_model"});
+                      "track_photo_rows", "track_photo_correspondences", "track_reference", "track_ref_model", "track_local_norm"});
     LiveGrid lg{};
     const bool ok = track_passes(
         ts, tm, kTrackPhases, [&]() { return live_box(ts, tm, "track_bricks", fusion::view(fs), fs.p.voxel_size, skip, lg, st); },
@@ -458,7 +469,7 @@ int track::odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, co
 {
     const auto t0 = std::chrono::steady_clock::now();
     for (const char* nm : {"odometry", "odometry_predict", "odometry_icp", "odometry_correspondences", "odometry_photo_correspondences", "track_photo_rows",
-                           "track_ref_model"})
+                           "track_ref_model", "track_local_norm"})
         tm.phases.erase(nm);
     // the motion state and the reference, kept here while fusion::integrate (which clears fs's) runs
     int motion = pose_first ? 0 : fs.motion;

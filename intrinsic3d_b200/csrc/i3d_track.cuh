@@ -20,6 +20,10 @@
  *   k_track_ref_model   one thread per pixel of a level: the model point of prediction pixel (2^l u, 2^l v) sampled from the frame's
  *                       reference image at the reference's pose, or the quiet NaN
  *
+ * The locally normalised intensity of the _ref calls with norm_radius > 0 (DESIGN.md §6r), applied per level to the frame's and the
+ * reference's raw intensity pyramids before k_track_grad and k_track_ref_model read them:
+ *   k_track_local_norm  one thread per pixel of a level, frames in gridDim.y: (I - mu) / sqrt(var + eps^2) over the clipped window
+ *
  * Compiled with the renderer in i3d_render.cu, which launches them (track::sensor_frames, i3d_track.h).  Every float
  * operation is explicitly rounded and every double operation is an explicit __d*_rn (no FMA contraction), so tests/track_ref.py restates
  * the planes, masks and sums exactly.  A frame's bytes depend only on that frame.
@@ -358,6 +362,57 @@ __global__ void k_track_ref_model(TrackRef tf)
         if (tr_project(c, tf.depth + z * img, tf.max_distance, xr, x0, y0, fx, fy)) val = tr_bilinear(tf.inten + z * img, c.W, x0, y0, fx, fy);
     }
     tf.model[pp] = val;
+}
+
+// ---- locally normalised intensity (DESIGN.md §6r) ------------------------------------------------------------------------------------
+
+// One thread per pixel of a kTrackLniTileW x kTrackLniTileH tile (blockIdx.x, row-major over the tiles) of frame blockIdx.y's plane src
+// [W x H]: dst = (I - mu) / sqrt(max(m2 - mu^2, 0) + eps^2) over the (2r+1)^2 window clipped to the image, mu = S1 / n, m2 = S2 / n, n the
+// float count of its pixels; exactly 0 where the window is constant (its min equals its max).  Separable: the tile's rows with their r
+// halo rows are summed along the row (taps in ascending x) into shared memory, then each pixel sums its column of those (ascending y).
+__global__ void __launch_bounds__(kTrackLniTileW * kTrackLniTileH) k_track_local_norm(int W, int H, int r, float eps,
+                                                                                        const float* __restrict__ src_all, float* __restrict__ dst_all)
+{
+    constexpr int kRows = kTrackLniTileH + 2 * kTrackLniMaxRadius;
+    __shared__ float s1[kRows][kTrackLniTileW], s2[kRows][kTrackLniTileW], mn[kRows][kTrackLniTileW], mx[kRows][kTrackLniTileW];
+    const int64_t img = static_cast<int64_t>(W) * H;
+    const float* src = src_all + blockIdx.y * img;
+    const int tiles_x = (W + kTrackLniTileW - 1) / kTrackLniTileW;
+    const int tx = static_cast<int>(blockIdx.x % tiles_x), ty = static_cast<int>(blockIdx.x / tiles_x);
+    const int x = tx * kTrackLniTileW + threadIdx.x, y0 = ty * kTrackLniTileH - r, y = y0 + r + threadIdx.y;
+    const int xa = max(x - r, 0), xb = min(x + r, W - 1);
+    for (int j = threadIdx.y; j < kTrackLniTileH + 2 * r; j += kTrackLniTileH)
+    {
+        const int yy = y0 + j;
+        if (yy < 0 || yy >= H || x >= W) continue;
+        const float* row = src + static_cast<int64_t>(yy) * W;
+        float a = 0.0f, b = 0.0f, lo = INFINITY, hi = -INFINITY;
+        for (int xx = xa; xx <= xb; ++xx)
+        {
+            const float t = row[xx];
+            a = FA(a, t); b = FA(b, FM(t, t)); lo = fminf(lo, t); hi = fmaxf(hi, t);
+        }
+        s1[j][threadIdx.x] = a; s2[j][threadIdx.x] = b; mn[j][threadIdx.x] = lo; mx[j][threadIdx.x] = hi;
+    }
+    __syncthreads();
+    if (x >= W || y >= H) return;
+    const int ya = max(y - r, 0), yb = min(y + r, H - 1);
+    float a = 0.0f, b = 0.0f, lo = INFINITY, hi = -INFINITY;
+    for (int yy = ya; yy <= yb; ++yy)
+    {
+        const int j = yy - y0;
+        a = FA(a, s1[j][threadIdx.x]); b = FA(b, s2[j][threadIdx.x]); lo = fminf(lo, mn[j][threadIdx.x]); hi = fmaxf(hi, mx[j][threadIdx.x]);
+    }
+    const int64_t i = static_cast<int64_t>(y) * W + x;
+    float out = 0.0f;
+    if (lo != hi)
+    {
+        const float n = __int2float_rn((xb - xa + 1) * (yb - ya + 1));
+        const float mu = FD(a, n), m2 = FD(b, n);
+        const float var = fmaxf(FS(m2, FM(mu, mu)), 0.0f);
+        out = FD(FS(src[i], mu), __fsqrt_rn(FA(var, FM(eps, eps))));
+    }
+    dst_all[blockIdx.y * img + i] = out;
 }
 
 // One thread per frame that is not frozen: the system k_track_solve reads, A = A_g + lam2 A_c and b = b_g + lam2 b_c (entries 0..26;

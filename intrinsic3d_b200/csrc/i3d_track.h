@@ -20,6 +20,9 @@ namespace i3d
 constexpr int kTrackVals = 29;
 constexpr int kTrackTile = 16;                  // 16 x 16 pixels per block of k_track_rows
 constexpr int kTrackMaxLevels = 4;
+// k_track_local_norm (DESIGN.md §6r): 32 x 8 pixels per block; the radius is at most I3D_TRACK_MAX_NORM_RADIUS (its shared rows)
+constexpr int kTrackLniTileW = 32, kTrackLniTileH = 8;
+constexpr int kTrackLniMaxRadius = I3D_TRACK_MAX_NORM_RADIUS;
 
 // Per-frame state of a call, device-resident: the pose T_cw (camera -> world, double R row-major | t), its float copy for the rows, the
 // world -> camera pose returned to the caller, and the outcome.  Written only by k_track_init and k_track_solve.
@@ -105,6 +108,9 @@ struct TrackScratch
     // with a reference model (DESIGN.md §6q): the references' ids and float poses, their intensity and depth pyramids, and the model
     // planes of levels 1.. (level 0 is pint), each in the level-0 layout (i3d_debug_get_track_reference_planes)
     Dev<int32_t> ref_ids; Dev<float> ref_rt, ref_inten[kTrackMaxLevels], ref_depth[kTrackMaxLevels], ref_model[kTrackMaxLevels];
+    // with norm_radius > 0 (DESIGN.md §6r): the raw intensity pyramids of the frames and of the references, which k_track_local_norm
+    // normalises into inten / ref_inten; at I3D_TRACK_CHUNK frames of 640 x 480 over 3 levels 51.6 MB each
+    Dev<float> raw_inten[kTrackMaxLevels], raw_ref_inten[kTrackMaxLevels];
     int n = 0, levels = 0, last_m = 0, W[kTrackMaxLevels] = {}, H[kTrackMaxLevels] = {};
     bool color = false;                                   // the last call had a photometric term
     bool reference = false;                               // ... taken from reference frames

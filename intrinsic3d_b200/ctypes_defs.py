@@ -272,7 +272,8 @@ class I3DTrackColorParams(C.Structure, _Dictable):
         ("weight", C.c_float * TRACK_LEVELS),
         ("max_color_diff", C.c_float),
         ("min_color_gradient", C.c_float),
-        ("reserved", C.c_int32 * 2),
+        ("norm_radius", C.c_int32),
+        ("norm_eps", C.c_float),
     ]
 
 

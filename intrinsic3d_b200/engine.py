@@ -41,6 +41,7 @@ EXPORTED_SYMBOLS = [
     "i3d_fusion_track_sensor_frames_rgbd", "i3d_fusion_track_and_integrate_sensor_rgbd", "i3d_debug_get_track_color_planes",
     "i3d_debug_get_track_color_system", "i3d_track_sensor_frames_rgbd_ref", "i3d_fusion_track_sensor_frames_rgbd_ref",
     "i3d_fusion_track_and_integrate_sensor_rgbd_ref", "i3d_debug_get_track_reference_planes", "i3d_default_track_color_ref_params",
+    "i3d_default_track_color_lni_params",
     "i3d_comm_unique_id", "i3d_comm_init", "i3d_comm_p2p_export", "i3d_comm_p2p_connect", "i3d_set_shard",
     "i3d_phase_ms", "i3d_phase_count", "i3d_debug_set_kernel_timers", "i3d_debug_num_slots", "i3d_debug_set_keep_raw_jacobian",
     "i3d_debug_get_rows", "i3d_debug_get_observations", "i3d_debug_get_step", "i3d_debug_get_pcg_vectors", "i3d_debug_get_normal_equations",
@@ -179,6 +180,13 @@ def default_track_color_params() -> I3DTrackColorParams:
 def default_track_color_ref_params() -> I3DTrackColorParams:
     p = I3DTrackColorParams()
     load_library().i3d_default_track_color_ref_params(C.byref(p))
+    return p
+
+
+def default_track_color_lni_params() -> I3DTrackColorParams:
+    """the _ref calls' parameters with locally normalised intensity (norm_radius > 0, DESIGN.md §6r)"""
+    p = I3DTrackColorParams()
+    load_library().i3d_default_track_color_lni_params(C.byref(p))
     return p
 
 
@@ -530,17 +538,24 @@ class Engine:
     @staticmethod
     def _track_color_params(color, ref=False):
         """I3DTrackColorParams from a dict: weight (one value for every level, or up to 4 values, level 0 first), max_color_diff,
-        min_color_gradient; the rest keep default_track_color_params() (ref: default_track_color_ref_params())."""
-        p = default_track_color_ref_params() if ref else default_track_color_params()
-        for k, v in (color or {}).items():
+        min_color_gradient, norm_radius, norm_eps; the rest keep default_track_color_params() (ref: default_track_color_ref_params(), or
+        default_track_color_lni_params() when norm_radius > 0)."""
+        color = color or {}
+        if ref:
+            p = default_track_color_lni_params() if int(color.get("norm_radius", 0)) > 0 else default_track_color_ref_params()
+        else:
+            p = default_track_color_params()
+        for k, v in color.items():
             if k == "weight":
                 v = [float(v)] * TRACK_LEVELS if np.ndim(v) == 0 else list(v) + [0.0] * (TRACK_LEVELS - len(v))
                 if len(v) != TRACK_LEVELS:
                     raise ValueError(f"weight takes at most {TRACK_LEVELS} values")
                 for i, x in enumerate(v):
                     p.weight[i] = float(x)
-            elif k in ("max_color_diff", "min_color_gradient"):
+            elif k in ("max_color_diff", "min_color_gradient", "norm_eps"):
                 setattr(p, k, float(v))
+            elif k == "norm_radius":
+                p.norm_radius = int(v)
             else:
                 raise ValueError(f"unknown colour tracking parameter {k!r}")
         return p
@@ -618,7 +633,9 @@ class Engine:
     # ---- the photometric term against a reference frame's image (DESIGN.md §6q) ----------------------------------------------------
     def track_sensor_frames_rgbd_ref(self, ids, pose_w2c, ref_ids, ref_pose_w2c, source: str = "fused", color=None, **params):
         """track_sensor_frames_rgbd with the model intensity of frame k sampled from the stored frame ref_ids[k] (may be ids[k] itself) at
-        its world -> camera pose ref_pose_w2c[k] float64 [12] instead of from the voxel colours.  Returns (poses, infos) as the _rgbd call."""
+        its world -> camera pose ref_pose_w2c[k] float64 [12] instead of from the voxel colours.  Returns (poses, infos) as the _rgbd call.
+        color=dict(norm_radius=r, norm_eps=eps) with r > 0 compares locally normalised intensity (DESIGN.md §6r); the colour parameters
+        not given then keep default_track_color_lni_params(), in normalised units."""
         p = self._track_params(self._mesh_source(source), params)
         return self._track_call(self.L.i3d_track_sensor_frames_rgbd_ref, ids, pose_w2c, "pose_w2c", lambda n: n, p,
                                 self._track_color_params(color, True), ref=(ref_ids, ref_pose_w2c))
@@ -639,7 +656,8 @@ class Engine:
 
     def debug_track_reference_planes(self, level, n):
         """The last pass's planes of the last _ref call (`n` = its frame count) at pyramid `level`, each [n, H_l, W_l]: model (NaN where
-        there is no model value), ref_intensity and ref_depth."""
+        there is no model value), ref_intensity and ref_depth.  With norm_radius > 0 the model and ref_intensity are the normalised
+        values the rows read (DESIGN.md §6r)."""
         dc = self._sensor_cams[0]
         Wl, Hl = dc.width, dc.height
         for _ in range(level):
@@ -660,7 +678,8 @@ class Engine:
     def debug_track_color_planes(self, level, frames, model_intensity=True):
         """The last pass's colour planes of the last _rgbd call (`frames` = its frame count): model_intensity [frames, H, W] and the
         frame intensity / grad_x / grad_y at pyramid `level`.  model_intensity=False leaves the model plane out (None), as after a _ref
-        call, whose model planes debug_track_reference_planes returns."""
+        call, whose model planes debug_track_reference_planes returns.  After a _ref call with norm_radius > 0 the intensity (and the
+        gradients of it) is the normalised plane the rows read (DESIGN.md §6r)."""
         dc = self._sensor_cams[0]
         W, H = dc.width, dc.height
         Wl, Hl = W, H
