@@ -205,6 +205,19 @@ int         i3d_mode_colors(I3DEngine* e, int32_t sdf_source, int32_t color_mode
  * pointer may be NULL.  Fails when no mesh of the current grid has been extracted. */
 int         i3d_download_mesh(I3DEngine* e, float* xyz, uint8_t* rgb, int32_t* faces);
 
+/* ---- simplifying the resident mesh by quadric-error vertex clustering (DESIGN.md §6s) ---- */
+uint64_t    i3d_sizeof_simplify_params(void);
+uint64_t    i3d_sizeof_simplify_info(void);
+/* Lindstrom's vertex clustering of the resident mesh: the vertices of each world-aligned cell of edge params->cell_size become one vertex
+ * at the minimiser of the cell's summed, area-weighted face-plane quadrics (truncated pseudo-inverse around the members' mean; a
+ * single-vertex cell keeps its vertex), faces that collapse or repeat an earlier face up to rotation are dropped, then the extraction's
+ * degenerate faces and the vertices no face uses.  Deterministic: byte-equal to tests/mesh_simplify_ref.py.  The result replaces the
+ * resident mesh that i3d_download_mesh reads (a further call simplifies it again); *info (may be NULL) gets the counts and the device time
+ * per stage.  Fails, leaving the resident mesh and every other state as they were, without a resident mesh of the current grid, for a
+ * cell_size that is not finite and > 0, and when a vertex's cell coordinate x / cell_size is not finite or outside int32.  A result
+ * without faces is an empty resident mesh. */
+int         i3d_simplify_mesh(I3DEngine* e, const I3DSimplifyParams* params, I3DSimplifyInfo* info);
+
 /* ---- rendering the surface into the keyframes (DESIGN.md §6m) ---- */
 uint64_t    i3d_sizeof_render_params(void);
 uint64_t    i3d_sizeof_render_stats(void);

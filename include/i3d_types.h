@@ -186,6 +186,24 @@ typedef struct I3DMeshInfo
                                                                            segments, the host read-backs of counts excluded */
 } I3DMeshInfo;
 
+/* ---- simplifying the resident mesh: quadric-error vertex clustering (Lindstrom 2000; DESIGN.md §6s) ---- */
+typedef struct I3DSimplifyParams
+{
+    float   cell_size;                    /* edge of the world-aligned cubic cells, metres (> 0, finite) */
+    int32_t reserved;
+} I3DSimplifyParams;
+
+typedef struct I3DSimplifyInfo
+{
+    int64_t num_clusters;                 /* occupied cells = vertices before the unused ones are removed */
+    int64_t num_faces_collapsed;          /* faces whose three corners fall into fewer than three clusters */
+    int64_t num_faces_duplicate;          /* faces that repeat an earlier face up to rotation */
+    int64_t num_faces_degenerate;         /* faces left that the extraction's degenerate-face rule drops at the representatives */
+    int64_t num_faces, num_vertices;      /* the new resident mesh */
+    double  ms_cluster, ms_quadrics, ms_representatives, ms_faces, ms_compact;   /* device time per stage: CUDA events around its
+                                                                                     device-only segments, as in I3DMeshInfo */
+} I3DSimplifyInfo;
+
 /* Colour modes of a mesh (SDFVisualization::colorize, src/sdf/visualization.cpp:101-416; mode strings "", "normals", "lap", "lum",
  * "lum_grad", "albedo", "shading_sv", "shading_sv_const", "chroma").  VOXEL is the voxel colours; the others are computed per voxel from
  * the voxel and its ±1 ring (DESIGN.md §6k).  The reference's subvolume modes ("subvol", "subvol_interp") have no number. */

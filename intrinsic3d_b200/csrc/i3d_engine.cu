@@ -1715,6 +1715,24 @@ int i3d_download_mesh(I3DEngine* e, float* xyz, uint8_t* rgb, int32_t* faces)
     });
 }
 
+// ---- simplifying the resident mesh (i3d_mesh.cuh, DESIGN.md §6s) ------------------------------------
+uint64_t i3d_sizeof_simplify_params(void) { return sizeof(I3DSimplifyParams); }
+uint64_t i3d_sizeof_simplify_info(void) { return sizeof(I3DSimplifyInfo); }
+
+int i3d_simplify_mesh(I3DEngine* e, const I3DSimplifyParams* params, I3DSimplifyInfo* info)
+{
+    if (!e) return 1;
+    if (!params) return fail(e, "i3d_simplify_mesh: params is NULL");
+    if (!e->mesh.have_mesh) return fail(e, "i3d_simplify_mesh: no mesh (call i3d_extract_mesh after the last change of the voxel set)");
+    const float cell = params->cell_size;
+    if (!std::isfinite(cell) || !(cell > 0.0f)) return fail(e, "i3d_simplify_mesh: cell_size must be finite and > 0, got %g", static_cast<double>(cell));
+    return guarded(e, [&]() {
+        std::string err;
+        if (mesh::simplify(e->mesh, cell, info, err, e->stream)) return fail(e, "%s", err.c_str());
+        return 0;
+    });
+}
+
 // ---- rendering the surface into the keyframes (i3d_render.cuh, DESIGN.md §6m) ----------------------
 uint64_t i3d_sizeof_render_params(void) { return sizeof(I3DRenderParams); }
 uint64_t i3d_sizeof_render_stats(void) { return sizeof(I3DRenderStats); }

@@ -51,6 +51,12 @@ struct MeshState
     int64_t mesh_V = 0, mesh_F = 0;
     float* mesh_vpos = nullptr; uint8_t* mesh_vcol = nullptr; int3* mesh_faces = nullptr;
     Dev<uchar4> vis_rgb;
+    // simplification (mesh::simplify): per vertex its cluster, per cluster its sorted runs of vertices and corners, the corners sorted
+    // by cluster, per face its quadric [9][F] and its cluster ids, the cluster representatives, and two output slots, so that the result
+    // never overwrites the resident mesh it is computed from.  The cell and face sorts use the welding's sort scratch above.
+    Dev<int32_t> s_bad, s_cid, s_run, s_corner, s_corner2, s_cstart, s_cend; Dev<uint32_t> s_ckey, s_ckey2;
+    Dev<double> s_quad; Dev<int3> s_cfaces; Dev<float> s_rpos; Dev<uint8_t> s_rcol; Dev<unsigned long long> s_counts;
+    Dev<float> s_vpos[2]; Dev<uint8_t> s_vcol[2]; Dev<int3> s_faces[2];
 };
 
 namespace mesh
@@ -63,6 +69,11 @@ void colorize(MeshState& ms, Timing& tm, const GridView& g, const SubvolGrid& sg
 // count is read back before the buffers of the next stage are sized; info (may be nullptr) gets the counts and stage times.  Returns
 // non-zero with the message in `error`, writing no info and leaving no mesh resident, when the triangles exceed the int32 corner indices.
 int extract(MeshState& ms, const MeshGrid& g, bool largest_component_only, I3DMeshInfo* info, std::string& error, cudaStream_t st);
+// Quadric-error vertex clustering of the resident mesh of ms (which the caller checked exists) with cells of edge cell_size (finite,
+// > 0, checked by the caller); the result becomes the resident mesh.  info (may be nullptr) gets the counts and stage times.  Returns
+// non-zero with the message in `error`, leaving the resident mesh as it was and writing no info, when a cell coordinate is not finite
+// or outside int32.
+int simplify(MeshState& ms, float cell_size, I3DSimplifyInfo* info, std::string& error, cudaStream_t st);
 } // namespace mesh
 
 } // namespace i3d

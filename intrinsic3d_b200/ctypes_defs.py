@@ -209,6 +209,29 @@ class I3DMeshInfo(C.Structure, _Dictable):
     ]
 
 
+class I3DSimplifyParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("cell_size", C.c_float),
+        ("reserved", C.c_int32),
+    ]
+
+
+class I3DSimplifyInfo(C.Structure, _Dictable):
+    _fields_ = [
+        ("num_clusters", C.c_int64),
+        ("num_faces_collapsed", C.c_int64),
+        ("num_faces_duplicate", C.c_int64),
+        ("num_faces_degenerate", C.c_int64),
+        ("num_faces", C.c_int64),
+        ("num_vertices", C.c_int64),
+        ("ms_cluster", C.c_double),
+        ("ms_quadrics", C.c_double),
+        ("ms_representatives", C.c_double),
+        ("ms_faces", C.c_double),
+        ("ms_compact", C.c_double),
+    ]
+
+
 # I3D_RENDER_* plane bits of include/i3d_types.h
 RENDER_PLANES = {"depth": 1, "normal": 2, "albedo": 4, "shading": 8, "intensity": 16}
 

@@ -12,8 +12,8 @@ import os
 import numpy as np
 
 from .ctypes_defs import (RENDER_PLANES, I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo,
-                          I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats, I3DTrackColorInfo, I3DTrackColorParams, I3DTrackInfo,
-                          I3DTrackParams, TRACK_LEVELS)
+                          I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats, I3DSimplifyInfo, I3DSimplifyParams, I3DTrackColorInfo,
+                          I3DTrackColorParams, I3DTrackInfo, I3DTrackParams, TRACK_LEVELS)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("I3D_LIB", os.path.join(_HERE, "libi3d_b200.so"))   # I3D_LIB: A/B builds of the same library
@@ -33,6 +33,7 @@ EXPORTED_SYMBOLS = [
     "i3d_sensor_frames_begin", "i3d_sensor_frames_add", "i3d_sensor_num_frames", "i3d_sensor_keyframe_scores", "i3d_fusion_integrate_sensor",
     "i3d_select_rgbd_frames",
     "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh", "i3d_extract_mesh_colored", "i3d_mode_colors",
+    "i3d_sizeof_simplify_params", "i3d_sizeof_simplify_info", "i3d_simplify_mesh",
     "i3d_sizeof_render_params", "i3d_sizeof_render_stats", "i3d_default_render_params", "i3d_render_keyframes", "i3d_download_render",
     "i3d_debug_set_render_skip",
     "i3d_sizeof_track_params", "i3d_sizeof_track_info", "i3d_default_track_params", "i3d_track_sensor_frames", "i3d_debug_get_track_system",
@@ -92,6 +93,12 @@ def load_library():
         raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (mesh info)")
     L.i3d_extract_mesh_colored.restype = C.c_int
     L.i3d_extract_mesh_colored.argtypes = [C.c_void_p, C.POINTER(I3DMeshParams), C.c_int32, C.POINTER(I3DMeshInfo)]
+    L.i3d_sizeof_simplify_params.restype = C.c_uint64
+    L.i3d_sizeof_simplify_info.restype = C.c_uint64
+    if L.i3d_sizeof_simplify_params() != C.sizeof(I3DSimplifyParams) or L.i3d_sizeof_simplify_info() != C.sizeof(I3DSimplifyInfo):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (simplify structs)")
+    L.i3d_simplify_mesh.restype = C.c_int
+    L.i3d_simplify_mesh.argtypes = [C.c_void_p, C.POINTER(I3DSimplifyParams), C.POINTER(I3DSimplifyInfo)]
     L.i3d_mode_colors.restype = C.c_int
     L.i3d_mode_colors.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_uint8)]
     L.i3d_sensor_num_frames.restype = C.c_int32
@@ -398,10 +405,23 @@ class Engine:
             self._check(self.L.i3d_extract_mesh(self.h, C.byref(prm), C.byref(info)))
         else:
             self._check(self.L.i3d_extract_mesh_colored(self.h, C.byref(prm), mode, C.byref(info)))
+        return self._download_mesh(info)
+
+    def _download_mesh(self, info):
         V, F = int(info.num_vertices), int(info.num_faces)
         out = dict(vertices=np.empty((V, 3), np.float32), colors=np.empty((V, 3), np.uint8), faces=np.empty((F, 3), np.int32), info=info)
         self._check(self.L.i3d_download_mesh(self.h, _p(out["vertices"], C.c_float), _p(out["colors"], C.c_uint8), _p(out["faces"], C.c_int32)))
         return out
+
+    def simplify_mesh(self, cell_size: float):
+        """Simplifies the resident mesh (the last extract_mesh or simplify_mesh of the current grid) on the device by quadric-error vertex
+        clustering (DESIGN.md §6s): the vertices in each world-aligned cube of edge cell_size (metres) become one vertex placed by the
+        summed face-plane quadrics, and the faces that collapse, repeat or degenerate go.  The result replaces the resident mesh, so a
+        second call gives a coarser mesh.  Returns the dict extract_mesh returns, with info an I3DSimplifyInfo (clusters, dropped faces
+        by reason, counts of the result, device ms per stage)."""
+        info = I3DSimplifyInfo()
+        self._check(self.L.i3d_simplify_mesh(self.h, C.byref(I3DSimplifyParams(float(cell_size), 0)), C.byref(info)))
+        return self._download_mesh(info)
 
     def mode_colors(self, mode: str, source: str = "refined"):
         """Every voxel's colour in colour mode `mode` (a mode string of extract_mesh), uint8 [n, 3] in the grid's order: the colours a

@@ -77,10 +77,11 @@ def mesh_file(prefix: str, mode: str) -> str:
     return prefix + ("_" + mode if mode else "") + ".ply"
 
 
-def export_meshes(engine, prefix: str, modes, largest_component_only: bool = False, source: str = "refined"):
+def export_meshes(engine, prefix: str, modes, largest_component_only: bool = False, source: str = "refined", cell_size=None):
     """SDFVisualization::colorize + exportMesh for every mode in `modes`: extracts the mesh of the engine's grid coloured in that mode on
     the device and writes it to mesh_file(prefix, mode).  Returns the paths written.  Every mode is checked before anything is extracted:
-    the subvolume modes are refused (the reference colours subvolumes with random colours, so there is nothing reproducible to write)."""
+    the subvolume modes are refused (the reference colours subvolumes with random colours, so there is nothing reproducible to write).
+    With a cell_size (metres), each mesh is simplified on the device (Engine.simplify_mesh) before it is written."""
     from .engine import COLOR_MODES
     bad = [m for m in modes if m not in COLOR_MODES]
     if bad:
@@ -88,6 +89,9 @@ def export_meshes(engine, prefix: str, modes, largest_component_only: bool = Fal
     paths = []
     for mode in modes:
         path = mesh_file(prefix, mode)
-        save_ply(path, engine.extract_mesh(source, largest_component_only, mode))
+        m = engine.extract_mesh(source, largest_component_only, mode)
+        if cell_size is not None:
+            m = engine.simplify_mesh(cell_size)
+        save_ply(path, m)
         paths.append(path)
     return paths
