@@ -218,6 +218,29 @@ uint64_t    i3d_sizeof_simplify_info(void);
  * without faces is an empty resident mesh. */
 int         i3d_simplify_mesh(I3DEngine* e, const I3DSimplifyParams* params, I3DSimplifyInfo* info);
 
+/* ---- baking the keyframes' colour into a texture atlas of the resident mesh (DESIGN.md §6t) ---- */
+uint64_t    i3d_sizeof_texture_params(void);
+uint64_t    i3d_sizeof_texture_info(void);
+/* texels_per_face 12, max_occlusion_distance 0.02, max_num_observations 5. */
+void        i3d_default_texture_params(I3DTextureParams* p);
+/* A texture atlas of the resident mesh, coloured from the keyframes.  Faces 2c and 2c+1 share square cell c of S x S texels (S =
+ * params->texels_per_face), laid out row-major in the smallest square number of columns; every texel a face owns is coloured by
+ * i3d_recompute_colors' rule at the 3-D point it maps to (observation weight at the face normal, top-K, weighted mean of the bilinear
+ * colours), and a texel no frame observes gets the barycentric blend of the face's vertex colours.  The layout, the rounding of every
+ * operation and the property that a bilinear lookup inside a face's UV triangle reads only texels of that face are in
+ * i3d_texture.cuh.  pose_world_to_cam: float [F][12] (R row-major | t), or NULL for the engine's camera, as in i3d_recompute_colors.
+ * The atlas and the per-corner UVs stay on the device until i3d_download_texture; *info (may be NULL) gets the counts and device time.
+ * The texture belongs to the resident mesh: an extraction, a successful simplification or a change of the voxel set drops it; a later
+ * change of the camera or the frames does not update it.  Reads the mesh, frames, colour frames and camera only.  Fails, writing
+ * nothing and leaving the previous texture, when world > 1, without a resident mesh with faces, without frames, camera or colour frames
+ * of the current frame size, for texels_per_face outside [I3D_TEXTURE_MIN_TEXELS_PER_FACE, I3D_TEXTURE_MAX_TEXELS_PER_FACE],
+ * max_num_observations outside [0, I3D_MAX_OBS], a max_occlusion_distance that is not finite, and an atlas side above
+ * I3D_TEXTURE_MAX_SIDE. */
+int         i3d_bake_texture(I3DEngine* e, const I3DTextureParams* params, const float* pose_world_to_cam, I3DTextureInfo* info);
+/* The baked texture: rgb uint8 [H][W][3] in R, G, B order (W, H: info->atlas_width / atlas_height), uv float [F][3][2], per face corner
+ * (u, v) as an OBJ reads them (v up).  Either pointer may be NULL.  Fails without a texture of the resident mesh. */
+int         i3d_download_texture(I3DEngine* e, uint8_t* rgb, float* uv);
+
 /* ---- rendering the surface into the keyframes (DESIGN.md §6m) ---- */
 uint64_t    i3d_sizeof_render_params(void);
 uint64_t    i3d_sizeof_render_stats(void);

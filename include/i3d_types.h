@@ -204,6 +204,33 @@ typedef struct I3DSimplifyInfo
                                                                                      device-only segments, as in I3DMeshInfo */
 } I3DSimplifyInfo;
 
+/* ---- baking the keyframes' colour into a texture atlas of the resident mesh (DESIGN.md §6t) ---- */
+#define I3D_TEXTURE_MIN_TEXELS_PER_FACE 6
+#define I3D_TEXTURE_MAX_TEXELS_PER_FACE 256
+#define I3D_TEXTURE_MAX_SIDE 16384      /* largest atlas width or height, texels */
+
+typedef struct I3DTextureParams
+{
+    int32_t texels_per_face;              /* S: faces 2c and 2c+1 share cell c of S x S texels; in [6, 256] */
+    float   max_occlusion_distance;       /* as i3d_recompute_colors: |depth - z| bound of an observation, metres; <= 0 turns the test off */
+    int32_t max_num_observations;         /* K in [0, I3D_MAX_OBS]: the best K frames per texel; 0 = every observation */
+    int32_t reserved;
+} I3DTextureParams;
+
+typedef struct I3DTextureInfo
+{
+    int32_t atlas_width, atlas_height;    /* texels */
+    int64_t num_faces;                    /* faces of the resident mesh = UV triangles */
+    int64_t num_texels_owned;             /* texels some face owns: num_faces * S (S - 1) / 2 */
+    int64_t num_texels_observed;          /* owned texels with at least one observation: coloured from the keyframes */
+    int64_t num_texels_fallback;          /* owned texels without one: the barycentric blend of the face's vertex colours */
+    int64_t num_observations;             /* (texel, frame) pairs with weight > 0 */
+    int64_t num_observations_kept;        /* observations summed into a colour: min(observations, K) per texel (all of them for K = 0) */
+    int64_t num_texel_frames_visited;     /* (owned texel, frame) pairs whose weight was computed: the ones the frame culling kept */
+    int64_t num_texel_frames_total;       /* owned texels x frames */
+    double  ms_bake;                      /* device time of the bake and the UVs (CUDA events) */
+} I3DTextureInfo;
+
 /* Colour modes of a mesh (SDFVisualization::colorize, src/sdf/visualization.cpp:101-416; mode strings "", "normals", "lap", "lum",
  * "lum_grad", "albedo", "shading_sv", "shading_sv_const", "chroma").  VOXEL is the voxel colours; the others are computed per voxel from
  * the voxel and its ±1 ring (DESIGN.md §6k).  The reference's subvolume modes ("subvol", "subvol_interp") have no number. */

@@ -34,6 +34,7 @@
 #include "i3d_fusion.h"
 #include "i3d_mesh.h"
 #include "i3d_render.h"
+#include "i3d_texture.h"
 #include "i3d_track.h"
 
 using namespace i3d;
@@ -166,6 +167,7 @@ struct I3DEngine
     RgbdStore rgbd;                    // RGB-D frame store (i3d_frames.cu)
     SensorStore sensor;                // sensor store (i3d_frames.cu)
     MeshState mesh;                    // surface extraction (i3d_mesh.cu)
+    TextureState tex;                  // texture of the resident mesh (i3d_texture.cu)
     RenderState render;                // keyframe renderer (i3d_render.cu)
     TrackScratch track;                // frame-to-model tracker (i3d_render.cu)
     // shard (multi-GPU)
@@ -269,10 +271,10 @@ int rebuild_topology(I3DEngine* e)
 }
 
 // Forgets everything derived from the voxel set: the per-voxel SH and the lighting estimate, the last iteration, the shard state and
-// range, the resident mesh, and the renderer's voxel box, brick bitmap and planes.  Every change of the voxel set calls it.
+// range, the resident mesh and its texture, and the renderer's voxel box, brick bitmap and planes.  Every change of the voxel set calls it.
 void forget_voxel_set(I3DEngine* e)
 {
-    e->have_sh = false; e->sv_S = 0; e->sv_x = nullptr; e->have_iter = false; e->mesh.have_mesh = false;
+    e->have_sh = false; e->sv_S = 0; e->sv_x = nullptr; e->have_iter = false; e->mesh.have_mesh = false; e->tex.have = false;
     e->render.box_ready = false; e->render.have_bricks = false; e->render.have_render = false;
     e->shard_ready = false; e->shard_begin = 0; e->shard_end = -1;
 }
@@ -977,6 +979,7 @@ int extract_mesh(I3DEngine* e, const I3DMeshParams& prm, int32_t color_mode, I3D
     g.rgb = color_mode == I3D_MESH_COLOR_VOXEL ? e->rgb.p : e->mesh.vis_rgb.p;
     g.nbr = e->nbr.p; g.keys = e->up_keys.p; g.vals = e->up_vals.p; g.mask = e->hash_cap - 1; g.voxel_size = e->voxel_size;
     std::string err;
+    e->tex.have = false;
     if (mesh::extract(e->mesh, g, prm.largest_component_only != 0, info, err, e->stream)) return fail(e, "%s", err.c_str());
     return 0;
 }
@@ -1078,6 +1081,7 @@ void i3d_engine_destroy(I3DEngine* e)
     if (e->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
     for (auto& ev : e->timing.pool) cudaEventDestroy(ev);
     if (e->mesh.ev_ready) for (auto& ev : e->mesh.ev) cudaEventDestroy(ev);
+    if (e->tex.ev_ready) for (auto& ev : e->tex.ev) cudaEventDestroy(ev);
     cudaStreamDestroy(e->stream);
     delete e;
 }
@@ -1729,6 +1733,64 @@ int i3d_simplify_mesh(I3DEngine* e, const I3DSimplifyParams* params, I3DSimplify
     return guarded(e, [&]() {
         std::string err;
         if (mesh::simplify(e->mesh, cell, info, err, e->stream)) return fail(e, "%s", err.c_str());
+        e->tex.have = false;
+        return 0;
+    });
+}
+
+// ---- baking the keyframes' colour into a texture atlas of the resident mesh (i3d_texture.cuh, DESIGN.md §6t) ------------
+uint64_t i3d_sizeof_texture_params(void) { return sizeof(I3DTextureParams); }
+uint64_t i3d_sizeof_texture_info(void) { return sizeof(I3DTextureInfo); }
+
+void i3d_default_texture_params(I3DTextureParams* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    p->texels_per_face = 12; p->max_occlusion_distance = 0.02f; p->max_num_observations = 5;
+}
+
+int i3d_bake_texture(I3DEngine* e, const I3DTextureParams* params, const float* pose_world_to_cam, I3DTextureInfo* info)
+{
+    static const char* who = "i3d_bake_texture";
+    if (!e) return 1;
+    if (!params) return fail(e, "%s: params is NULL", who);
+    if (e->world > 1) return fail(e, "%s: the bake runs on one GPU (world = %d)", who, e->world);
+    if (!e->mesh.have_mesh) return fail(e, "%s: no mesh (call i3d_extract_mesh after the last change of the voxel set)", who);
+    if (e->mesh.mesh_F <= 0) return fail(e, "%s: the resident mesh has no faces", who);
+    if (e->F <= 0 || !e->have_cam) return fail(e, "%s: frames and camera must be uploaded first", who);
+    if (!e->have_color) return fail(e, "%s: no colour frames of the current frame size (i3d_upload_color_frames)", who);
+    const int S = params->texels_per_face, K = params->max_num_observations;
+    if (S < I3D_TEXTURE_MIN_TEXELS_PER_FACE || S > I3D_TEXTURE_MAX_TEXELS_PER_FACE)
+        return fail(e, "%s: texels_per_face must be in [%d, %d], got %d", who, I3D_TEXTURE_MIN_TEXELS_PER_FACE, I3D_TEXTURE_MAX_TEXELS_PER_FACE, S);
+    if (K < 0 || K > I3D_MAX_OBS) return fail(e, "%s: max_num_observations must be in [0, %d], got %d", who, I3D_MAX_OBS, K);
+    if (!std::isfinite(params->max_occlusion_distance)) return fail(e, "%s: max_occlusion_distance must be finite", who);
+    TexLayout L;
+    if (!texture::layout(e->mesh.mesh_F, S, L))
+        return fail(e, "%s: %lld faces at %d texels per face need an atlas side above I3D_TEXTURE_MAX_SIDE (%d)", who,
+                    static_cast<long long>(e->mesh.mesh_F), S, I3D_TEXTURE_MAX_SIDE);
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const int F = e->F;
+        double hc9[9];
+        CK(cudaMemcpyAsync(hc9, e->cam + 6 * static_cast<size_t>(F), 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        e->tex.rt.ensure(12 * static_cast<size_t>(F));
+        if (pose_world_to_cam) CK(cudaMemcpyAsync(e->tex.rt.p, pose_world_to_cam, 12 * static_cast<size_t>(F) * sizeof(float), cudaMemcpyHostToDevice, st));
+        else k_pose_mats<<<blocks_for(F, 64), 64, 0, st>>>(F, e->cam, e->tex.rt.p);
+        const TexMesh m{static_cast<int32_t>(e->mesh.mesh_F), e->mesh.mesh_vpos, e->mesh.mesh_vcol, e->mesh.mesh_faces};
+        texture::bake(e->tex, m, L, e->frame_view(), e->color.p, select_cam(e, hc9, params->max_occlusion_distance), cull_view(e, nullptr), K, info, st);
+        return 0;
+    });
+}
+
+int i3d_download_texture(I3DEngine* e, uint8_t* rgb, float* uv)
+{
+    if (!e) return 1;
+    if (!e->tex.have) return fail(e, "i3d_download_texture: no texture (call i3d_bake_texture after the last extraction or simplification of the mesh)");
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        if (rgb) CK(cudaMemcpyAsync(rgb, e->tex.rgb.p, 3 * static_cast<size_t>(e->tex.W) * e->tex.H, cudaMemcpyDeviceToHost, st));
+        if (uv) CK(cudaMemcpyAsync(uv, e->tex.uv.p, 6 * static_cast<size_t>(e->tex.F) * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
         return 0;
     });
 }

@@ -1,7 +1,8 @@
 /*
  * i3d_observe.cuh — the observation rules of SDFColorization (libintrinsic3d/src/sdf/colorization.cpp:192-370) that the observation
- * selection (k_select_obs, i3d_kernels.cuh) and the recolouring (k_recolor, i3d_recolor.cuh) share: the observation weight of a frame
- * at a voxel's iso-point, the conservative per-warp frame culling, and the top-K of (weight, frame) keys.  No kernels.
+ * selection (k_select_obs, i3d_kernels.cuh), the recolouring (k_recolor, i3d_recolor.cuh) and the texture bake (k_tex_bake,
+ * i3d_texture.cuh) share: the observation weight of a frame at a point, the conservative per-warp frame culling, the top-K of (weight,
+ * frame) keys with the order computeColor sums them in, and the bilinear colour lookup.  No kernels.
  */
 #pragma once
 #include "i3d_grid.cuh"
@@ -235,6 +236,62 @@ __device__ __forceinline__ void topk_frame_order(unsigned long long (&best)[KMAX
             const unsigned long long hi = best[j] < best[j + 1] ? best[j + 1] : best[j];
             best[j] = lo; best[j + 1] = hi;
         }
+}
+
+// The kept observations of a top-K (K > 0) in the order computeColor (colorization.cpp:318-354) sums them: when the filter ran (more
+// than K observations) ascending (weight, frame) among the K kept ones, otherwise frame order.  sel_f = frame (-1 = empty slot), sel_w
+// = its weight.  Consumes `best`.
+template <int KMAX>
+__device__ __forceinline__ void topk_summation_order(unsigned long long (&best)[KMAX], int n_obs, int K, int (&sel_f)[KMAX], float (&sel_w)[KMAX])
+{
+    if (n_obs > K)
+    {
+        // the filter ran: ascending (weight, frame) among the K kept ones == `best` read backwards; re-key as (frame, weight)
+#pragma unroll
+        for (int k = 0; k < KMAX / 2; ++k) { const unsigned long long t = best[k]; best[k] = best[KMAX - 1 - k]; best[KMAX - 1 - k] = t; }
+#pragma unroll
+        for (int k = 0; k < KMAX; ++k)
+        {
+            // after the reversal, entries beyond the best K sit in front: drop them (slot index KMAX-1-k was the rank)
+            const bool keep = (KMAX - 1 - k) < K && best[k] != 0ull;
+            best[k] = keep ? (((best[k] & 0xffffffffull) << 32) | (best[k] >> 32)) : ~0ull;
+        }
+    }
+    else
+    {
+        // the filter returned early: frame order.  At most K keys were inserted, so the slots from K upwards are empty already.
+        topk_frame_order(best, K);
+    }
+    // best[] now holds (frame + 1) << 32 | weight bits in summation order, ~0 = empty
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k)
+    {
+        sel_f[k] = best[k] == ~0ull ? -1 : static_cast<int>(best[k] >> 32) - 1;
+        sel_w[k] = __uint_as_float(static_cast<unsigned>(best[k] & 0xffffffffull));
+    }
+}
+
+// interpolate<unsigned char> (src/rgbd/processing.cpp:236-291): bilinear on an interleaved B,G,R image, out-of-image taps dropped
+__device__ __forceinline__ unsigned char interp_u8(const uint8_t* __restrict__ img, int w, int h, float x, float y, int channel)
+{
+    const float fx0 = floorf(x), fy0 = floorf(y);
+    const int x0 = static_cast<int>(fx0), y0 = static_cast<int>(fy0);
+    const int x1 = x0 + 1, y1 = y0 + 1;
+    float x1w = FS(x, fx0), y1w = FS(y, fy0);
+    float x0w = FS(1.0f, x1w), y0w = FS(1.0f, y1w);
+    if (x0 < 0 || x0 >= w) x0w = 0.0f;
+    if (x1 < 0 || x1 >= w) x1w = 0.0f;
+    if (y0 < 0 || y0 >= h) y0w = 0.0f;
+    if (y1 < 0 || y1 >= h) y1w = 0.0f;
+    const float w00 = FM(x0w, y0w), w10 = FM(x1w, y0w), w01 = FM(x0w, y1w), w11 = FM(x1w, y1w);
+    const float sum_w = FA(FA(FA(w00, w10), w01), w11);
+    float sum = 0.0f;
+    if (w00 > 0.0f) sum = FA(sum, FM(static_cast<float>(img[(static_cast<size_t>(y0) * w + x0) * 3 + channel]), w00));
+    if (w01 > 0.0f) sum = FA(sum, FM(static_cast<float>(img[(static_cast<size_t>(y1) * w + x0) * 3 + channel]), w01));
+    if (w10 > 0.0f) sum = FA(sum, FM(static_cast<float>(img[(static_cast<size_t>(y0) * w + x1) * 3 + channel]), w10));
+    if (w11 > 0.0f) sum = FA(sum, FM(static_cast<float>(img[(static_cast<size_t>(y1) * w + x1) * 3 + channel]), w11));
+    if (!(sum_w > 0.0f)) return 0;
+    return static_cast<unsigned char>(__float2int_rz(FD(sum, sum_w)));
 }
 
 } // namespace i3d

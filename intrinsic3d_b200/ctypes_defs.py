@@ -232,6 +232,31 @@ class I3DSimplifyInfo(C.Structure, _Dictable):
     ]
 
 
+class I3DTextureParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("texels_per_face", C.c_int32),
+        ("max_occlusion_distance", C.c_float),
+        ("max_num_observations", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
+class I3DTextureInfo(C.Structure, _Dictable):
+    _fields_ = [
+        ("atlas_width", C.c_int32),
+        ("atlas_height", C.c_int32),
+        ("num_faces", C.c_int64),
+        ("num_texels_owned", C.c_int64),
+        ("num_texels_observed", C.c_int64),
+        ("num_texels_fallback", C.c_int64),
+        ("num_observations", C.c_int64),
+        ("num_observations_kept", C.c_int64),
+        ("num_texel_frames_visited", C.c_int64),
+        ("num_texel_frames_total", C.c_int64),
+        ("ms_bake", C.c_double),
+    ]
+
+
 # I3D_RENDER_* plane bits of include/i3d_types.h
 RENDER_PLANES = {"depth": 1, "normal": 2, "albedo": 4, "shading": 8, "intensity": 16}
 

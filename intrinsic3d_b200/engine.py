@@ -12,8 +12,8 @@ import os
 import numpy as np
 
 from .ctypes_defs import (RENDER_PLANES, I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo,
-                          I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats, I3DSimplifyInfo, I3DSimplifyParams, I3DTrackColorInfo,
-                          I3DTrackColorParams, I3DTrackInfo, I3DTrackParams, TRACK_LEVELS)
+                          I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats, I3DSimplifyInfo, I3DSimplifyParams, I3DTextureInfo,
+                          I3DTextureParams, I3DTrackColorInfo, I3DTrackColorParams, I3DTrackInfo, I3DTrackParams, TRACK_LEVELS)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("I3D_LIB", os.path.join(_HERE, "libi3d_b200.so"))   # I3D_LIB: A/B builds of the same library
@@ -34,6 +34,7 @@ EXPORTED_SYMBOLS = [
     "i3d_select_rgbd_frames",
     "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh", "i3d_extract_mesh_colored", "i3d_mode_colors",
     "i3d_sizeof_simplify_params", "i3d_sizeof_simplify_info", "i3d_simplify_mesh",
+    "i3d_sizeof_texture_params", "i3d_sizeof_texture_info", "i3d_default_texture_params", "i3d_bake_texture", "i3d_download_texture",
     "i3d_sizeof_render_params", "i3d_sizeof_render_stats", "i3d_default_render_params", "i3d_render_keyframes", "i3d_download_render",
     "i3d_debug_set_render_skip",
     "i3d_sizeof_track_params", "i3d_sizeof_track_info", "i3d_default_track_params", "i3d_track_sensor_frames", "i3d_debug_get_track_system",
@@ -99,6 +100,16 @@ def load_library():
         raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (simplify structs)")
     L.i3d_simplify_mesh.restype = C.c_int
     L.i3d_simplify_mesh.argtypes = [C.c_void_p, C.POINTER(I3DSimplifyParams), C.POINTER(I3DSimplifyInfo)]
+    L.i3d_sizeof_texture_params.restype = C.c_uint64
+    L.i3d_sizeof_texture_info.restype = C.c_uint64
+    if L.i3d_sizeof_texture_params() != C.sizeof(I3DTextureParams) or L.i3d_sizeof_texture_info() != C.sizeof(I3DTextureInfo):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (texture structs)")
+    L.i3d_default_texture_params.restype = None
+    L.i3d_default_texture_params.argtypes = [C.POINTER(I3DTextureParams)]
+    L.i3d_bake_texture.restype = C.c_int
+    L.i3d_bake_texture.argtypes = [C.c_void_p, C.POINTER(I3DTextureParams), C.POINTER(C.c_float), C.POINTER(I3DTextureInfo)]
+    L.i3d_download_texture.restype = C.c_int
+    L.i3d_download_texture.argtypes = [C.c_void_p, C.POINTER(C.c_uint8), C.POINTER(C.c_float)]
     L.i3d_mode_colors.restype = C.c_int
     L.i3d_mode_colors.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_uint8)]
     L.i3d_sensor_num_frames.restype = C.c_int32
@@ -194,6 +205,12 @@ def default_track_color_lni_params() -> I3DTrackColorParams:
     """the _ref calls' parameters with locally normalised intensity (norm_radius > 0, DESIGN.md §6r)"""
     p = I3DTrackColorParams()
     load_library().i3d_default_track_color_lni_params(C.byref(p))
+    return p
+
+
+def default_texture_params() -> I3DTextureParams:
+    p = I3DTextureParams()
+    load_library().i3d_default_texture_params(C.byref(p))
     return p
 
 
@@ -422,6 +439,23 @@ class Engine:
         info = I3DSimplifyInfo()
         self._check(self.L.i3d_simplify_mesh(self.h, C.byref(I3DSimplifyParams(float(cell_size), 0)), C.byref(info)))
         return self._download_mesh(info)
+
+    def bake_texture(self, texels_per_face: int = 12, max_occlusion_distance: float = 0.02, max_num_observations: int = 5, pose_rt=None):
+        """Bakes the keyframes' colour into a texture atlas of the resident mesh (the last extract_mesh or simplify_mesh) on the device
+        (DESIGN.md §6t): faces 2c and 2c+1 share a cell of texels_per_face x texels_per_face texels, and every texel a face owns gets
+        recompute_colors' colour at its 3-D point, or the barycentric blend of the vertex colours where no frame observes it.  pose_rt:
+        optional float32 [F, 12] (R row-major | t, world -> camera), else the engine's camera.  Returns a dict with image uint8 [H, W, 3]
+        (R, G, B), uv float32 [F, 3, 2] (per face corner, v up as an OBJ reads it) and info (I3DTextureInfo).  Write it with
+        mesh.save_textured_obj."""
+        if pose_rt is not None:
+            pose_rt = np.ascontiguousarray(pose_rt, np.float32)
+            assert pose_rt.shape == (self.F, 12)
+        prm = I3DTextureParams(int(texels_per_face), float(max_occlusion_distance), int(max_num_observations), 0)
+        info = I3DTextureInfo()
+        self._check(self.L.i3d_bake_texture(self.h, C.byref(prm), _p(pose_rt, C.c_float), C.byref(info)))
+        out = dict(image=np.empty((info.atlas_height, info.atlas_width, 3), np.uint8), uv=np.empty((int(info.num_faces), 3, 2), np.float32), info=info)
+        self._check(self.L.i3d_download_texture(self.h, _p(out["image"], C.c_uint8), _p(out["uv"], C.c_float)))
+        return out
 
     def mode_colors(self, mode: str, source: str = "refined"):
         """Every voxel's colour in colour mode `mode` (a mode string of extract_mesh), uint8 [n, 3] in the grid's order: the colours a
