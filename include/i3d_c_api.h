@@ -241,6 +241,35 @@ int         i3d_bake_texture(I3DEngine* e, const I3DTextureParams* params, const
  * (u, v) as an OBJ reads them (v up).  Either pointer may be NULL.  Fails without a texture of the resident mesh. */
 int         i3d_download_texture(I3DEngine* e, uint8_t* rgb, float* uv);
 
+/* ---- distance from the resident mesh to a reference surface (DESIGN.md §6u) ---- */
+uint64_t    i3d_sizeof_distance_params(void);
+uint64_t    i3d_sizeof_distance_info(void);
+/* samples_per_edge 2, max_distance 0.01, cell_size 0 (automatic), thresholds 0.0002, 0.0005, 0.001. */
+void        i3d_default_distance_params(I3DDistanceParams* p);
+/* Copies a reference mesh xyz float [V][3], faces int32 [F][3] to the device, replacing the previous one.  It stays through grid,
+ * frame and mesh changes.  Fails, keeping the previous reference, for V <= 0, F <= 0, NULL buffers, a vertex index outside [0, V), a
+ * coordinate that is not finite, V > INT_MAX or 3 F > INT_MAX. */
+int         i3d_upload_reference_mesh(I3DEngine* e, int64_t V, const float* xyz, int64_t F, const int32_t* faces);
+/* Distances between the resident mesh A (the last extraction or simplification) and the reference mesh B: every face of either mesh is
+ * sampled at the centroids of its L^2 congruent sub-triangles, weighted by area / L^2, and each sample gets the nearest face of the
+ * other mesh within max_distance (the lexicographic minimum of (float d^2, face id) over all faces, so equal distances go to the
+ * lowest face id); every vertex of A gets its nearest face of B.  *info gets per direction the sample counts, area-weighted mean, RMS
+ * and maximum distance, the area fraction within each threshold, the grid used and the device time per stage, and precision, recall
+ * and F-score per threshold.  The rounding of every operation is stated in i3d_distance.cuh; every result is bit-identical from run to
+ * run.  Reads the meshes only.  Fails, leaving the resident mesh, its texture and the previous results as they were, when world > 1,
+ * without a resident mesh with faces, without a reference mesh, for samples_per_edge outside [1, 16], a max_distance that is not
+ * finite and > 0, a cell_size that is negative or not finite, num_thresholds outside [0, 8], thresholds that are not finite, not
+ * ascending or above max_distance, and a search grid above I3D_DISTANCE_MAX_CELLS cells or I3D_DISTANCE_MAX_CELL_ENTRIES entries. */
+int         i3d_surface_distance(I3DEngine* e, const I3DDistanceParams* params, I3DDistanceInfo* info);
+/* The per-vertex results of the last i3d_surface_distance: vertex_distance float [V] (metres, +inf when no face of the reference is
+ * within max_distance) and vertex_face int32 [V] (-1 then), V = info->num_vertices.  Either pointer may be NULL.  Fails before the
+ * first successful call. */
+int         i3d_download_surface_distance(I3DEngine* e, float* vertex_distance, int32_t* vertex_face);
+/* Tests: keep the per-sample (d^2, face) of later i3d_surface_distance calls (on != 0), and read those of the last call: direction
+ * 0 = resident -> reference, 1 = reference -> resident; d2 float [side[direction].num_samples] (+inf when unmatched), face int32 (-1). */
+int         i3d_debug_set_keep_distance_samples(I3DEngine* e, int on);
+int         i3d_debug_get_distance_samples(I3DEngine* e, int direction, float* d2, int32_t* face);
+
 /* ---- rendering the surface into the keyframes (DESIGN.md §6m) ---- */
 uint64_t    i3d_sizeof_render_params(void);
 uint64_t    i3d_sizeof_render_stats(void);

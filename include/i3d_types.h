@@ -231,6 +231,46 @@ typedef struct I3DTextureInfo
     double  ms_bake;                      /* device time of the bake and the UVs (CUDA events) */
 } I3DTextureInfo;
 
+/* ---- distance from the resident mesh to a reference mesh (DESIGN.md §6u) ---- */
+#define I3D_DISTANCE_MAX_THRESHOLDS 8
+#define I3D_DISTANCE_MAX_SAMPLES_PER_EDGE 16
+#define I3D_DISTANCE_MAX_CELLS (1ll << 26)           /* largest search grid, cells */
+#define I3D_DISTANCE_MAX_CELL_ENTRIES (1ll << 30)    /* largest (face, cell) list of a search grid */
+
+typedef struct I3DDistanceParams
+{
+    int32_t samples_per_edge;             /* L in [1, 16]: every face is split into L^2 congruent sub-triangles, sampled at their centroids */
+    float   max_distance;                 /* metres, finite and > 0: a sample with no face within it is unmatched */
+    float   cell_size;                    /* search-grid cell edge, metres; 0 = twice the target mesh's mean edge length */
+    int32_t num_thresholds;               /* in [0, 8] */
+    float   thresholds[I3D_DISTANCE_MAX_THRESHOLDS];  /* tau: finite, ascending, <= max_distance */
+} I3DDistanceParams;
+
+/* One direction: the samples of one mesh against the faces of the other (the target) */
+typedef struct I3DDistanceSide
+{
+    int64_t num_samples, num_matched;
+    double  area;                         /* total sample weight = the sampled mesh's area, m^2 */
+    double  unmatched_area;
+    double  mean, rms, max;               /* of d over the matched samples, area-weighted (max: one-sided Hausdorff within max_distance) */
+    double  fraction[I3D_DISTANCE_MAX_THRESHOLDS];   /* area with d <= tau over the total area; unmatched samples count as beyond every tau */
+    int64_t point_triangle_tests;         /* closest-point evaluations of the query */
+    float   cell_size;                    /* the target's search grid: cell edge (metres) and cells per axis */
+    int32_t grid[3];
+    int64_t num_cells, num_cell_entries;  /* cells, (face, cell) pairs */
+    double  ms_grid, ms_query, ms_reduce; /* device time: grid build, sampling and query, statistics (CUDA events) */
+} I3DDistanceSide;
+
+typedef struct I3DDistanceInfo
+{
+    I3DDistanceSide side[2];              /* [0] resident -> reference (accuracy, precision), [1] reference -> resident (completeness, recall) */
+    int32_t num_thresholds, reserved;
+    double  precision[I3D_DISTANCE_MAX_THRESHOLDS], recall[I3D_DISTANCE_MAX_THRESHOLDS], fscore[I3D_DISTANCE_MAX_THRESHOLDS];
+    int64_t num_vertices;                 /* vertices of the resident mesh, each queried against the reference */
+    int64_t vertex_point_triangle_tests;
+    double  ms_vertices;                  /* device time of the vertex query */
+} I3DDistanceInfo;
+
 /* Colour modes of a mesh (SDFVisualization::colorize, src/sdf/visualization.cpp:101-416; mode strings "", "normals", "lap", "lum",
  * "lum_grad", "albedo", "shading_sv", "shading_sv_const", "chroma").  VOXEL is the voxel colours; the others are computed per voxel from
  * the voxel and its ±1 ring (DESIGN.md §6k).  The reference's subvolume modes ("subvol", "subvol_interp") have no number. */

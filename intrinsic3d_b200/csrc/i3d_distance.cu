@@ -1,0 +1,225 @@
+/*
+ * i3d_distance.cu — the distance between the resident mesh and a reference mesh: its kernels (i3d_distance.cuh) and the host code that
+ * sizes the search grids and launches them (i3d_distance.h).  Keeping them out of i3d_engine.cu leaves the engine's device module as it is.
+ */
+#include <climits>
+#include <cstdarg>
+#include <cmath>
+#include <cstdio>
+#include <cstring>
+
+#include "i3d_distance.cuh"
+
+#include <cub/device/device_scan.cuh>
+
+namespace i3d
+{
+namespace distance
+{
+namespace
+{
+struct AddI64 { __device__ __forceinline__ int64_t operator()(int64_t a, int64_t b) const { return a + b; } };
+
+std::string format(const char* fmt, ...)
+{
+    char buf[512];
+    va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof(buf), fmt, ap); va_end(ap);
+    return buf;
+}
+
+// The search grid of target t (F > 0): its size, cell edge, margin and entry count; false with the message when a cap is exceeded
+bool plan(DistanceState& ds, const DistMesh& t, const I3DDistanceParams& p, DistGrid& g, int64_t& entries, std::string& error, cudaStream_t st)
+{
+    const unsigned nb = blocks_for(static_cast<size_t>(t.F));
+    ds.partials.ensure(static_cast<size_t>(nb) * kDistBounds);
+    k_dist_bounds<<<nb, kThreads, 0, st>>>(t, ds.partials.p);
+    std::vector<double> h(static_cast<size_t>(nb) * kDistBounds);
+    CK(cudaMemcpyAsync(h.data(), ds.partials.p, h.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    double b[kDistBounds];
+    for (int j = 0; j < kDistBounds; ++j) b[j] = h[j];
+    for (unsigned i = 1; i < nb; ++i)
+        for (int j = 0; j < kDistBounds; ++j) b[j] = j < 6 ? std::max(b[j], h[i * kDistBounds + j]) : b[j] + h[i * kDistBounds + j];
+    const double mean_edge = b[6] / (3.0 * static_cast<double>(t.F));
+    float cell = p.cell_size > 0.0f ? p.cell_size : static_cast<float>(2.0 * mean_edge);
+    if (!(cell > 0.0f)) cell = p.max_distance;          // every face of the target is a point
+    std::memset(&g, 0, sizeof(g));
+    g.h = cell;
+    double extent = 0.0, mag = 0.0, cells = 1.0;
+    for (int k = 0; k < 3; ++k)
+    {
+        const float lo = static_cast<float>(-b[k]) - p.max_distance, hi = static_cast<float>(b[3 + k]) + p.max_distance;
+        const double n = std::floor((static_cast<double>(hi) - lo) / cell) + 1.0;
+        cells *= n;
+        g.lo[k] = lo;
+        g.n[k] = n < static_cast<double>(I3D_DISTANCE_MAX_CELLS) ? static_cast<int>(n) : static_cast<int>(I3D_DISTANCE_MAX_CELLS);
+        extent = std::max(extent, static_cast<double>(hi) - lo);
+        mag = std::max(mag, std::max(std::fabs(static_cast<double>(lo)), std::fabs(static_cast<double>(hi))));
+    }
+    if (cells > static_cast<double>(I3D_DISTANCE_MAX_CELLS))
+    {
+        error = format("a search grid of %.0f cells at cell_size %g m exceeds I3D_DISTANCE_MAX_CELLS (%lld); use a larger cell_size", cells,
+                       static_cast<double>(cell), static_cast<long long>(I3D_DISTANCE_MAX_CELLS));
+        return false;
+    }
+    g.margin = std::ldexp(mag + extent + cell, -16);
+    ds.vtests.ensure(1);
+    CK(cudaMemsetAsync(ds.vtests.p, 0, sizeof(unsigned long long), st));
+    k_dist_entries<<<nb, kThreads, 0, st>>>(t, g, ds.vtests.p);
+    unsigned long long e = 0;
+    CK(cudaMemcpyAsync(&e, ds.vtests.p, sizeof(e), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    entries = static_cast<int64_t>(e);
+    if (entries > I3D_DISTANCE_MAX_CELL_ENTRIES)
+    {
+        error = format("a search grid of %lld (face, cell) entries at cell_size %g m exceeds I3D_DISTANCE_MAX_CELL_ENTRIES (%lld); use a larger cell_size",
+                       static_cast<long long>(entries), static_cast<double>(cell), static_cast<long long>(I3D_DISTANCE_MAX_CELL_ENTRIES));
+        return false;
+    }
+    return true;
+}
+
+// Count, scan and fill the grid g of target t into ds (cell_count ends as the per-cell counts again)
+void build(DistanceState& ds, const DistMesh& t, DistGrid& g, int64_t entries, cudaStream_t st)
+{
+    const size_t cells = static_cast<size_t>(g.n[0]) * g.n[1] * g.n[2];
+    ds.cell_count.ensure(cells); ds.cell_off.ensure(cells); ds.cell_faces.ensure(static_cast<size_t>(entries));
+    const unsigned nb = blocks_for(static_cast<size_t>(t.F));
+    CK(cudaMemsetAsync(ds.cell_count.p, 0, cells * sizeof(int32_t), st));
+    k_dist_insert<<<nb, kThreads, 0, st>>>(t, g, nullptr, ds.cell_count.p, nullptr);
+    size_t bytes = 0;
+    CK(cub::DeviceScan::ExclusiveScan(nullptr, bytes, static_cast<const int32_t*>(ds.cell_count.p), ds.cell_off.p, AddI64(), static_cast<int64_t>(0),
+                                      static_cast<int64_t>(cells), st));
+    ds.cub.ensure(bytes);
+    CK(cub::DeviceScan::ExclusiveScan(static_cast<void*>(ds.cub.p), bytes, static_cast<const int32_t*>(ds.cell_count.p), ds.cell_off.p, AddI64(),
+                                      static_cast<int64_t>(0), static_cast<int64_t>(cells), st));
+    CK(cudaMemsetAsync(ds.cell_count.p, 0, cells * sizeof(int32_t), st));
+    k_dist_insert<<<nb, kThreads, 0, st>>>(t, g, ds.cell_off.p, ds.cell_count.p, ds.cell_faces.p);
+    g.off = ds.cell_off.p; g.cnt = ds.cell_count.p; g.faces = ds.cell_faces.p;
+}
+
+void side_info(const double* s, const DistGrid& g, int64_t samples, int64_t entries, int nt, I3DDistanceSide& o)
+{
+    o.num_samples = samples;
+    o.num_matched = static_cast<int64_t>(s[1]);
+    o.area = s[2]; o.unmatched_area = s[3];
+    o.mean = s[0] > 0.0 ? s[4] / s[0] : 0.0;
+    o.rms = s[0] > 0.0 ? std::sqrt(s[5] / s[0]) : 0.0;
+    o.max = s[6];
+    for (int k = 0; k < nt; ++k) o.fraction[k] = s[2] > 0.0 ? s[8 + k] / s[2] : 0.0;
+    o.point_triangle_tests = static_cast<int64_t>(s[7]);
+    o.cell_size = g.h;
+    for (int k = 0; k < 3; ++k) o.grid[k] = g.n[k];
+    o.num_cells = static_cast<int64_t>(g.n[0]) * g.n[1] * g.n[2];
+    o.num_cell_entries = entries;
+}
+} // namespace
+
+int upload_reference(DistanceState& ds, int64_t V, const float* xyz, int64_t F, const int32_t* faces, std::string& error, cudaStream_t st)
+{
+    if (V <= 0 || F <= 0) { error = format("the reference mesh needs V > 0 and F > 0, got V = %lld, F = %lld", static_cast<long long>(V), static_cast<long long>(F)); return 1; }
+    if (!xyz || !faces) { error = "xyz or faces is NULL"; return 1; }
+    if (V > INT_MAX || F > INT_MAX / 3)
+    {
+        error = format("%lld vertices and %lld faces exceed the int32 indices of a mesh", static_cast<long long>(V), static_cast<long long>(F));
+        return 1;
+    }
+    for (int64_t i = 0; i < 3 * V; ++i)
+        if (!std::isfinite(xyz[i])) { error = format("coordinate %lld of vertex %lld is not finite", static_cast<long long>(i % 3), static_cast<long long>(i / 3)); return 1; }
+    for (int64_t i = 0; i < 3 * F; ++i)
+        if (faces[i] < 0 || faces[i] >= V)
+        {
+            error = format("face %lld has vertex index %d outside [0, %lld)", static_cast<long long>(i / 3), faces[i], static_cast<long long>(V));
+            return 1;
+        }
+    ds.have_ref = false;
+    ds.ref_vpos.ensure(3 * static_cast<size_t>(V)); ds.ref_faces.ensure(static_cast<size_t>(F));
+    CK(cudaMemcpyAsync(ds.ref_vpos.p, xyz, 3 * static_cast<size_t>(V) * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ds.ref_faces.p, faces, static_cast<size_t>(F) * sizeof(int3), cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));
+    ds.ref_V = V; ds.ref_F = F; ds.have_ref = true;
+    return 0;
+}
+
+int compute(DistanceState& ds, const DistMesh& a, const I3DDistanceParams& p, I3DDistanceInfo* info, std::string& error, cudaStream_t st)
+{
+    if (!ds.ev_ready) { for (auto& ev : ds.ev) CK(cudaEventCreate(&ev)); ds.ev_ready = true; }
+    const DistMesh b{ds.ref_V, ds.ref_F, ds.ref_vpos.p, ds.ref_faces.p};
+    // both grids are sized, and refused, before anything is written
+    DistGrid gb, ga;
+    int64_t eb = 0, ea = 0;
+    if (!plan(ds, b, p, gb, eb, error, st) || !plan(ds, a, p, ga, ea, error, st)) return 1;
+    const int L = p.samples_per_edge, LL = L * L;
+    DistQuery q;
+    std::memset(&q, 0, sizeof(q));
+    q.max_distance = p.max_distance; q.L = L; q.num_thresholds = p.num_thresholds;
+    for (int k = 0; k < p.num_thresholds; ++k) q.tau[k] = p.thresholds[k];
+    const DistMesh src[2] = {a, b};
+    DistGrid* grid[2] = {&gb, &ga};
+    const DistMesh* tgt[2] = {&b, &a};
+    const int64_t ns[2] = {a.F * LL, b.F * LL};
+    const unsigned nbs[2] = {blocks_for(static_cast<size_t>(ns[0])), blocks_for(static_cast<size_t>(ns[1]))};
+    ds.partials.ensure(static_cast<size_t>(std::max(nbs[0], nbs[1])) * kDistStats);
+    ds.stats.ensure(2 * kDistStats);
+    ds.vdist.ensure(static_cast<size_t>(a.V)); ds.vface.ensure(static_cast<size_t>(a.V));
+    ds.have_keep = false;
+    for (int d = 0; d < 2; ++d)
+    {
+        if (ds.keep) { ds.keep_d2[d].ensure(static_cast<size_t>(ns[d])); ds.keep_face[d].ensure(static_cast<size_t>(ns[d])); }
+        ds.keep_n[d] = ds.keep ? ns[d] : 0;
+    }
+    CK(cudaMemsetAsync(ds.vtests.p, 0, sizeof(unsigned long long), st));
+    for (int d = 0; d < 2; ++d)
+    {
+        cudaEvent_t* ev = ds.ev + (d == 0 ? 0 : 8);
+        CK(cudaEventRecord(ev[0], st));
+        build(ds, *tgt[d], *grid[d], d == 0 ? eb : ea, st);
+        CK(cudaEventRecord(ev[1], st));
+        k_dist_samples<<<nbs[d], kThreads, 0, st>>>(src[d], *tgt[d], *grid[d], q, ds.keep ? ds.keep_d2[d].p : nullptr, ds.keep ? ds.keep_face[d].p : nullptr,
+                                                    ds.partials.p);
+        CK(cudaEventRecord(ev[2], st));
+        k_dist_finish<<<1, 32 * kDistStats, 0, st>>>(static_cast<int>(nbs[d]), ds.partials.p, ds.stats.p + d * kDistStats);
+        CK(cudaEventRecord(ev[3], st));
+        if (d == 0)
+        {
+            CK(cudaEventRecord(ds.ev[4], st));
+            k_dist_vertices<<<blocks_for(static_cast<size_t>(a.V)), kThreads, 0, st>>>(a, b, gb, p.max_distance, ds.vdist.p, ds.vface.p, ds.vtests.p);
+            CK(cudaEventRecord(ds.ev[5], st));
+        }
+    }
+    double s[2 * kDistStats];
+    unsigned long long vt = 0;
+    CK(cudaMemcpyAsync(s, ds.stats.p, sizeof(s), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&vt, ds.vtests.p, sizeof(vt), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
+    ds.result_V = a.V; ds.have_result = true; ds.have_keep = ds.keep;
+    if (info)
+    {
+        I3DDistanceInfo inf;
+        std::memset(&inf, 0, sizeof(inf));
+        auto ms = [&](int i, int j) { float m = 0.f; CK(cudaEventElapsedTime(&m, ds.ev[i], ds.ev[j])); return static_cast<double>(m); };
+        for (int d = 0; d < 2; ++d)
+        {
+            I3DDistanceSide& o = inf.side[d];
+            side_info(s + d * kDistStats, *grid[d], ns[d], d == 0 ? eb : ea, p.num_thresholds, o);
+            const int e0 = d == 0 ? 0 : 8;
+            o.ms_grid = ms(e0, e0 + 1); o.ms_query = ms(e0 + 1, e0 + 2); o.ms_reduce = ms(e0 + 2, e0 + 3);
+        }
+        inf.num_thresholds = p.num_thresholds;
+        for (int k = 0; k < p.num_thresholds; ++k)
+        {
+            const double P = inf.side[0].fraction[k], R = inf.side[1].fraction[k];
+            inf.precision[k] = P; inf.recall[k] = R;
+            inf.fscore[k] = P + R > 0.0 ? 2.0 * P * R / (P + R) : 0.0;
+        }
+        inf.num_vertices = a.V;
+        inf.vertex_point_triangle_tests = static_cast<int64_t>(vt);
+        inf.ms_vertices = ms(4, 5);
+        *info = inf;
+    }
+    return 0;
+}
+
+} // namespace distance
+} // namespace i3d

@@ -1,0 +1,51 @@
+/*
+ * i3d_distance.h — the distance between the resident mesh and a reference mesh (i3d_distance.cuh), compiled in i3d_distance.cu, a device
+ * module of its own: its state (the reference mesh, the search-grid scratch and the last results) and the calls the engine
+ * (i3d_engine.cu) makes after it has validated them.
+ */
+#pragma once
+#include <cuda_runtime.h>
+#include <stddef.h>
+#include <stdint.h>
+
+#include <string>
+
+#include "../../include/i3d_types.h"
+#include "i3d_host.h"
+
+namespace i3d
+{
+
+// A triangle mesh as the distance kernels read it
+struct DistMesh { int64_t V, F; const float* vpos; const int3* faces; };
+
+// Reference mesh, grid scratch and results of the distance calls of one engine
+struct DistanceState
+{
+    Dev<float> ref_vpos; Dev<int3> ref_faces;
+    int64_t ref_V = 0, ref_F = 0;
+    bool have_ref = false;
+    // search grid of the current target: per cell its face count and the int64 offset of its run in cell_faces
+    Dev<int32_t> cell_count, cell_faces; Dev<int64_t> cell_off; Dev<uint8_t> cub;
+    Dev<double> partials, stats;           // per-block partials and the finished statistics of both directions
+    Dev<unsigned long long> vtests;
+    // the last results: per-vertex distance and face of the resident mesh, and (when keep) the per-sample (d^2, face) of both directions
+    Dev<float> vdist; Dev<int32_t> vface; int64_t result_V = 0;
+    bool have_result = false;
+    bool keep = false;
+    Dev<float> keep_d2[2]; Dev<int32_t> keep_face[2]; int64_t keep_n[2] = {0, 0};
+    bool have_keep = false;
+    cudaEvent_t ev[14] = {};
+    bool ev_ready = false;
+};
+
+namespace distance
+{
+// Uploads the reference mesh after checking it on the host; returns non-zero with the message in `error`, keeping the previous one
+int upload_reference(DistanceState& ds, int64_t V, const float* xyz, int64_t F, const int32_t* faces, std::string& error, cudaStream_t st);
+// Both directions and the vertex query between the resident mesh a (F > 0) and the reference (present), with parameters the caller
+// validated.  Returns non-zero with the message in `error`, writing nothing, when a search grid exceeds its cell or entry cap.
+int compute(DistanceState& ds, const DistMesh& a, const I3DDistanceParams& p, I3DDistanceInfo* info, std::string& error, cudaStream_t st);
+} // namespace distance
+
+} // namespace i3d

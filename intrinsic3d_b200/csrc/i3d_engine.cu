@@ -35,6 +35,7 @@
 #include "i3d_mesh.h"
 #include "i3d_render.h"
 #include "i3d_texture.h"
+#include "i3d_distance.h"
 #include "i3d_track.h"
 
 using namespace i3d;
@@ -168,6 +169,7 @@ struct I3DEngine
     SensorStore sensor;                // sensor store (i3d_frames.cu)
     MeshState mesh;                    // surface extraction (i3d_mesh.cu)
     TextureState tex;                  // texture of the resident mesh (i3d_texture.cu)
+    DistanceState dist;                // reference mesh and distance results (i3d_distance.cu)
     RenderState render;                // keyframe renderer (i3d_render.cu)
     TrackScratch track;                // frame-to-model tracker (i3d_render.cu)
     // shard (multi-GPU)
@@ -1790,6 +1792,93 @@ int i3d_download_texture(I3DEngine* e, uint8_t* rgb, float* uv)
         cudaStream_t st = e->stream;
         if (rgb) CK(cudaMemcpyAsync(rgb, e->tex.rgb.p, 3 * static_cast<size_t>(e->tex.W) * e->tex.H, cudaMemcpyDeviceToHost, st));
         if (uv) CK(cudaMemcpyAsync(uv, e->tex.uv.p, 6 * static_cast<size_t>(e->tex.F) * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    });
+}
+
+// ---- distance from the resident mesh to a reference mesh (i3d_distance.cuh, DESIGN.md §6u) -----------
+uint64_t i3d_sizeof_distance_params(void) { return sizeof(I3DDistanceParams); }
+uint64_t i3d_sizeof_distance_info(void) { return sizeof(I3DDistanceInfo); }
+
+void i3d_default_distance_params(I3DDistanceParams* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    p->samples_per_edge = 2; p->max_distance = 0.01f; p->cell_size = 0.0f;
+    p->num_thresholds = 3; p->thresholds[0] = 0.0002f; p->thresholds[1] = 0.0005f; p->thresholds[2] = 0.001f;
+}
+
+int i3d_upload_reference_mesh(I3DEngine* e, int64_t V, const float* xyz, int64_t F, const int32_t* faces)
+{
+    if (!e) return 1;
+    return guarded(e, [&]() {
+        std::string err;
+        if (distance::upload_reference(e->dist, V, xyz, F, faces, err, e->stream)) return fail(e, "i3d_upload_reference_mesh: %s", err.c_str());
+        return 0;
+    });
+}
+
+int i3d_surface_distance(I3DEngine* e, const I3DDistanceParams* params, I3DDistanceInfo* info)
+{
+    static const char* who = "i3d_surface_distance";
+    if (!e) return 1;
+    if (!params) return fail(e, "%s: params is NULL", who);
+    if (e->world > 1) return fail(e, "%s: the distance runs on one GPU (world = %d)", who, e->world);
+    if (!e->mesh.have_mesh) return fail(e, "%s: no mesh (call i3d_extract_mesh after the last change of the voxel set)", who);
+    if (e->mesh.mesh_F <= 0) return fail(e, "%s: the resident mesh has no faces", who);
+    if (!e->dist.have_ref) return fail(e, "%s: no reference mesh (i3d_upload_reference_mesh)", who);
+    const I3DDistanceParams& p = *params;
+    if (p.samples_per_edge < 1 || p.samples_per_edge > I3D_DISTANCE_MAX_SAMPLES_PER_EDGE)
+        return fail(e, "%s: samples_per_edge must be in [1, %d], got %d", who, I3D_DISTANCE_MAX_SAMPLES_PER_EDGE, p.samples_per_edge);
+    if (!std::isfinite(p.max_distance) || !(p.max_distance > 0.0f)) return fail(e, "%s: max_distance must be finite and > 0, got %g", who, static_cast<double>(p.max_distance));
+    if (!std::isfinite(p.cell_size) || p.cell_size < 0.0f) return fail(e, "%s: cell_size must be finite and >= 0, got %g", who, static_cast<double>(p.cell_size));
+    if (p.num_thresholds < 0 || p.num_thresholds > I3D_DISTANCE_MAX_THRESHOLDS)
+        return fail(e, "%s: num_thresholds must be in [0, %d], got %d", who, I3D_DISTANCE_MAX_THRESHOLDS, p.num_thresholds);
+    for (int k = 0; k < p.num_thresholds; ++k)
+    {
+        const float t = p.thresholds[k];
+        if (!std::isfinite(t) || t < 0.0f || t > p.max_distance || (k > 0 && t < p.thresholds[k - 1]))
+            return fail(e, "%s: thresholds must be finite, ascending and in [0, max_distance]; threshold %d is %g", who, k, static_cast<double>(t));
+    }
+    return guarded(e, [&]() {
+        std::string err;
+        const DistMesh a{e->mesh.mesh_V, e->mesh.mesh_F, e->mesh.mesh_vpos, e->mesh.mesh_faces};
+        if (distance::compute(e->dist, a, p, info, err, e->stream)) return fail(e, "%s: %s", who, err.c_str());
+        return 0;
+    });
+}
+
+int i3d_download_surface_distance(I3DEngine* e, float* vertex_distance, int32_t* vertex_face)
+{
+    if (!e) return 1;
+    if (!e->dist.have_result) return fail(e, "i3d_download_surface_distance: no result (call i3d_surface_distance first)");
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t V = static_cast<size_t>(e->dist.result_V);
+        if (vertex_distance && V) CK(cudaMemcpyAsync(vertex_distance, e->dist.vdist.p, V * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (vertex_face && V) CK(cudaMemcpyAsync(vertex_face, e->dist.vface.p, V * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    });
+}
+
+int i3d_debug_set_keep_distance_samples(I3DEngine* e, int on)
+{
+    if (!e) return 1;
+    e->dist.keep = on != 0;
+    return 0;
+}
+
+int i3d_debug_get_distance_samples(I3DEngine* e, int direction, float* d2, int32_t* face)
+{
+    if (!e) return 1;
+    if (direction < 0 || direction > 1) return fail(e, "i3d_debug_get_distance_samples: direction must be 0 or 1, got %d", direction);
+    if (!e->dist.have_keep) return fail(e, "i3d_debug_get_distance_samples: the last i3d_surface_distance kept no samples");
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t n = static_cast<size_t>(e->dist.keep_n[direction]);
+        if (d2 && n) CK(cudaMemcpyAsync(d2, e->dist.keep_d2[direction].p, n * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (face && n) CK(cudaMemcpyAsync(face, e->dist.keep_face[direction].p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         return 0;
     });

@@ -257,6 +257,54 @@ class I3DTextureInfo(C.Structure, _Dictable):
     ]
 
 
+DISTANCE_MAX_THRESHOLDS = 8     # I3D_DISTANCE_MAX_THRESHOLDS of include/i3d_types.h
+
+
+class I3DDistanceParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("samples_per_edge", C.c_int32),
+        ("max_distance", C.c_float),
+        ("cell_size", C.c_float),
+        ("num_thresholds", C.c_int32),
+        ("thresholds", C.c_float * DISTANCE_MAX_THRESHOLDS),
+    ]
+
+
+class I3DDistanceSide(C.Structure, _Dictable):
+    _fields_ = [
+        ("num_samples", C.c_int64),
+        ("num_matched", C.c_int64),
+        ("area", C.c_double),
+        ("unmatched_area", C.c_double),
+        ("mean", C.c_double),
+        ("rms", C.c_double),
+        ("max", C.c_double),
+        ("fraction", C.c_double * DISTANCE_MAX_THRESHOLDS),
+        ("point_triangle_tests", C.c_int64),
+        ("cell_size", C.c_float),
+        ("grid", C.c_int32 * 3),
+        ("num_cells", C.c_int64),
+        ("num_cell_entries", C.c_int64),
+        ("ms_grid", C.c_double),
+        ("ms_query", C.c_double),
+        ("ms_reduce", C.c_double),
+    ]
+
+
+class I3DDistanceInfo(C.Structure, _Dictable):
+    _fields_ = [
+        ("side", I3DDistanceSide * 2),
+        ("num_thresholds", C.c_int32),
+        ("reserved", C.c_int32),
+        ("precision", C.c_double * DISTANCE_MAX_THRESHOLDS),
+        ("recall", C.c_double * DISTANCE_MAX_THRESHOLDS),
+        ("fscore", C.c_double * DISTANCE_MAX_THRESHOLDS),
+        ("num_vertices", C.c_int64),
+        ("vertex_point_triangle_tests", C.c_int64),
+        ("ms_vertices", C.c_double),
+    ]
+
+
 # I3D_RENDER_* plane bits of include/i3d_types.h
 RENDER_PLANES = {"depth": 1, "normal": 2, "albedo": 4, "shading": 8, "intensity": 16}
 

@@ -11,7 +11,7 @@ import os
 
 import numpy as np
 
-from .ctypes_defs import (RENDER_PLANES, I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo,
+from .ctypes_defs import (DISTANCE_MAX_THRESHOLDS, RENDER_PLANES, I3DDistanceInfo, I3DDistanceParams, I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo,
                           I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats, I3DSimplifyInfo, I3DSimplifyParams, I3DTextureInfo,
                           I3DTextureParams, I3DTrackColorInfo, I3DTrackColorParams, I3DTrackInfo, I3DTrackParams, TRACK_LEVELS)
 
@@ -35,6 +35,8 @@ EXPORTED_SYMBOLS = [
     "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh", "i3d_extract_mesh_colored", "i3d_mode_colors",
     "i3d_sizeof_simplify_params", "i3d_sizeof_simplify_info", "i3d_simplify_mesh",
     "i3d_sizeof_texture_params", "i3d_sizeof_texture_info", "i3d_default_texture_params", "i3d_bake_texture", "i3d_download_texture",
+    "i3d_sizeof_distance_params", "i3d_sizeof_distance_info", "i3d_default_distance_params", "i3d_upload_reference_mesh",
+    "i3d_surface_distance", "i3d_download_surface_distance", "i3d_debug_set_keep_distance_samples", "i3d_debug_get_distance_samples",
     "i3d_sizeof_render_params", "i3d_sizeof_render_stats", "i3d_default_render_params", "i3d_render_keyframes", "i3d_download_render",
     "i3d_debug_set_render_skip",
     "i3d_sizeof_track_params", "i3d_sizeof_track_info", "i3d_default_track_params", "i3d_track_sensor_frames", "i3d_debug_get_track_system",
@@ -110,6 +112,22 @@ def load_library():
     L.i3d_bake_texture.argtypes = [C.c_void_p, C.POINTER(I3DTextureParams), C.POINTER(C.c_float), C.POINTER(I3DTextureInfo)]
     L.i3d_download_texture.restype = C.c_int
     L.i3d_download_texture.argtypes = [C.c_void_p, C.POINTER(C.c_uint8), C.POINTER(C.c_float)]
+    L.i3d_sizeof_distance_params.restype = C.c_uint64
+    L.i3d_sizeof_distance_info.restype = C.c_uint64
+    if L.i3d_sizeof_distance_params() != C.sizeof(I3DDistanceParams) or L.i3d_sizeof_distance_info() != C.sizeof(I3DDistanceInfo):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (distance structs)")
+    L.i3d_default_distance_params.restype = None
+    L.i3d_default_distance_params.argtypes = [C.POINTER(I3DDistanceParams)]
+    L.i3d_upload_reference_mesh.restype = C.c_int
+    L.i3d_upload_reference_mesh.argtypes = [C.c_void_p, C.c_int64, C.POINTER(C.c_float), C.c_int64, C.POINTER(C.c_int32)]
+    L.i3d_surface_distance.restype = C.c_int
+    L.i3d_surface_distance.argtypes = [C.c_void_p, C.POINTER(I3DDistanceParams), C.POINTER(I3DDistanceInfo)]
+    L.i3d_download_surface_distance.restype = C.c_int
+    L.i3d_download_surface_distance.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int32)]
+    L.i3d_debug_set_keep_distance_samples.restype = C.c_int
+    L.i3d_debug_set_keep_distance_samples.argtypes = [C.c_void_p, C.c_int]
+    L.i3d_debug_get_distance_samples.restype = C.c_int
+    L.i3d_debug_get_distance_samples.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int32)]
     L.i3d_mode_colors.restype = C.c_int
     L.i3d_mode_colors.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_uint8)]
     L.i3d_sensor_num_frames.restype = C.c_int32
@@ -211,6 +229,12 @@ def default_track_color_lni_params() -> I3DTrackColorParams:
 def default_texture_params() -> I3DTextureParams:
     p = I3DTextureParams()
     load_library().i3d_default_texture_params(C.byref(p))
+    return p
+
+
+def default_distance_params() -> I3DDistanceParams:
+    p = I3DDistanceParams()
+    load_library().i3d_default_distance_params(C.byref(p))
     return p
 
 
@@ -456,6 +480,50 @@ class Engine:
         out = dict(image=np.empty((info.atlas_height, info.atlas_width, 3), np.uint8), uv=np.empty((int(info.num_faces), 3, 2), np.float32), info=info)
         self._check(self.L.i3d_download_texture(self.h, _p(out["image"], C.c_uint8), _p(out["uv"], C.c_float)))
         return out
+
+    def upload_reference_mesh(self, mesh):
+        """Uploads a reference surface for surface_distance: a dict with vertices float32 [V, 3] and faces int32 [F, 3] (an extract_mesh
+        dict; its colours are ignored).  It replaces the previous reference and stays through grid, frame and mesh changes."""
+        v = np.ascontiguousarray(mesh["vertices"], np.float32).reshape(-1, 3)
+        f = np.ascontiguousarray(mesh["faces"], np.int32).reshape(-1, 3)
+        self._check(self.L.i3d_upload_reference_mesh(self.h, len(v), _p(v, C.c_float), len(f), _p(f, C.c_int32)))
+
+    def surface_distance(self, thresholds=(0.0002, 0.0005, 0.001), max_distance: float = 0.01, samples_per_edge: int = 2, cell_size=None):
+        """Distances between the resident mesh (the last extract_mesh or simplify_mesh) and the reference mesh, on the device (DESIGN.md
+        §6u).  Every face of either mesh is sampled at samples_per_edge^2 area-uniform points, and each point gets the nearest face of the
+        other mesh within max_distance (metres).  Returns a dict with accuracy (resident -> reference) and completeness (reference ->
+        resident), each with the sample counts, area, area-weighted mean / rms / max distance over the matched samples and the area
+        fraction within each threshold; precision, recall and fscore per threshold; vertex_distance float32 [V] (inf beyond max_distance)
+        and vertex_face int32 [V] (-1 then) of the resident mesh's vertices; and info (I3DDistanceInfo, with the grids and device times).
+        cell_size None picks the search grid's cell edge automatically; the results do not depend on it."""
+        thresholds = [float(t) for t in thresholds]
+        if len(thresholds) > DISTANCE_MAX_THRESHOLDS:
+            raise ValueError(f"at most {DISTANCE_MAX_THRESHOLDS} thresholds, got {len(thresholds)}")
+        prm = I3DDistanceParams(int(samples_per_edge), float(max_distance), 0.0 if cell_size is None else float(cell_size), len(thresholds),
+                                (C.c_float * DISTANCE_MAX_THRESHOLDS)(*thresholds))
+        info = I3DDistanceInfo()
+        self._check(self.L.i3d_surface_distance(self.h, C.byref(prm), C.byref(info)))
+        V = int(info.num_vertices)
+        vd, vf = np.empty(V, np.float32), np.empty(V, np.int32)
+        self._check(self.L.i3d_download_surface_distance(self.h, _p(vd, C.c_float), _p(vf, C.c_int32)))
+        nt = len(thresholds)
+
+        def side(s):
+            d = s.as_dict()
+            d["fraction"] = d["fraction"][:nt]
+            return d
+        return dict(accuracy=side(info.side[0]), completeness=side(info.side[1]), thresholds=thresholds, precision=list(info.precision)[:nt],
+                    recall=list(info.recall)[:nt], fscore=list(info.fscore)[:nt], vertex_distance=vd, vertex_face=vf, info=info)
+
+    def debug_distance_samples(self, direction: int, n: int):
+        """(d2 float32 [n], face int32 [n]) per sample of the last surface_distance after debug_set_keep_distance_samples(True); direction
+        0 = resident -> reference, 1 = reference -> resident; n = that side's num_samples"""
+        d2, face = np.empty(n, np.float32), np.empty(n, np.int32)
+        self._check(self.L.i3d_debug_get_distance_samples(self.h, int(direction), _p(d2, C.c_float), _p(face, C.c_int32)))
+        return d2, face
+
+    def debug_set_keep_distance_samples(self, on: bool = True):
+        self._check(self.L.i3d_debug_set_keep_distance_samples(self.h, 1 if on else 0))
 
     def mode_colors(self, mode: str, source: str = "refined"):
         """Every voxel's colour in colour mode `mode` (a mode string of extract_mesh), uint8 [n, 3] in the grid's order: the colours a

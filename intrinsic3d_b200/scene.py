@@ -301,18 +301,83 @@ def make_color_frames(scene, seed: int = 7):
     return out
 
 
+def _latlong(n_theta: int):
+    """unit-sphere directions on n_theta rings of latitude (the two poles included) by 2 n_theta meridians, and the faces between them:
+    a fan at each pole, two triangles per quad elsewhere (2 n_theta (2 n_theta - 2) faces)"""
+    n_phi = 2 * n_theta
+    th = np.arange(1, n_theta) * (math.pi / n_theta)
+    ph = np.arange(n_phi) * (2.0 * math.pi / n_phi)
+    T, P = np.meshgrid(th, ph, indexing="ij")
+    ring = np.stack([np.sin(T) * np.cos(P), np.sin(T) * np.sin(P), np.cos(T)], -1).reshape(-1, 3)
+    d = np.concatenate([[[0.0, 0.0, 1.0]], ring, [[0.0, 0.0, -1.0]]])
+    south = len(d) - 1
+    j = np.arange(n_phi)
+    jn = (j + 1) % n_phi
+    idx = lambda i, jj: 1 + i * n_phi + jj          # noqa: E731  ring i (0 .. n_theta - 2), meridian jj
+    faces = [np.stack([np.zeros_like(j), idx(0, j), idx(0, jn)], 1)]
+    for i in range(n_theta - 2):
+        faces.append(np.stack([idx(i, j), idx(i + 1, j), idx(i + 1, jn)], 1))
+        faces.append(np.stack([idx(i, j), idx(i + 1, jn), idx(i, jn)], 1))
+    faces.append(np.stack([np.full_like(j, south), idx(n_theta - 2, jn), idx(n_theta - 2, j)], 1))
+    return d, np.concatenate(faces)
+
+
+def _truth_geometry(radius_vox=24.0, voxel_size=0.004, band=3.0, dense_dim=None, bump=0.03, **_):
+    """rho0, centre and bump exactly as make_scene computes them (the other make_scene arguments do not move the surface)"""
+    vs = float(np.float32(voxel_size))
+    rho0 = radius_vox * vs
+    centre_v = np.array([dense_dim // 2] * 3, np.float64) if dense_dim is not None else np.zeros(3)
+    return rho0, centre_v * vs, bump, vs
+
+
+def truth_mesh(n_theta: int | None = None, **geometry):
+    """The analytic surface of make_scene as a fine triangle mesh: every vertex of a latitude-longitude grid of directions d at
+    centre + d rho(d).  The bump's sin(6 theta) sin(5 phi) has a cone-like point at each pole; the grid puts a vertex there and a fan of
+    2 n_theta thin faces around it, which follows it closely.  geometry: make_scene's (or config_geometry's) arguments; only
+    radius_vox, voxel_size, dense_dim and bump matter.  n_theta: the rings (2 n_theta (2 n_theta - 2) faces); None picks the smallest
+    power of two >= 128 whose ring spacing is at most a voxel.  Returns a dict with vertices float32 [V, 3], faces int32 [F, 3] and colors
+    uint8 [V, 3] (zero), the shape of an extract_mesh dict.  truth_mesh_error states how far it lies from the analytic surface."""
+    rho0, centre, bump, vs = _truth_geometry(**geometry)
+    if n_theta is None:
+        n_theta = 128
+        while math.pi * rho0 * (1 + bump) / n_theta > vs:
+            n_theta *= 2
+    d, f = _latlong(n_theta)
+    v = centre[None, :] + d * _rho(torch.from_numpy(d), rho0, bump).numpy()[:, None]
+    return dict(vertices=v.astype(np.float32), faces=f.astype(np.int32), colors=np.zeros((len(v), 3), np.uint8))
+
+
+def truth_mesh_error(mesh, **geometry):
+    """The largest |implicit| of make_scene's surface (metres, float64) at the face centroids and edge midpoints of the float32 mesh:
+    a bound on how far the tessellation lies from the analytic surface where it is furthest from its vertices"""
+    rho0, centre, bump, _ = _truth_geometry(**geometry)
+    v = np.asarray(mesh["vertices"], np.float64)
+    f = np.asarray(mesh["faces"], np.int64)
+    pts = [(v[f[:, 0]] + v[f[:, 1]] + v[f[:, 2]]) / 3.0] + [(v[f[:, k]] + v[f[:, (k + 1) % 3]]) / 2.0 for k in range(3)]
+    c = torch.tensor(centre, dtype=torch.float64)
+    return max(float(_implicit(torch.from_numpy(p), c, rho0, bump).abs().max()) for p in pts)
+
+
+def config_geometry(name: str):
+    """make_scene's arguments of config_scene(name): what truth_mesh(**config_geometry(name)) takes"""
+    return dict(_PRESETS[name])
+
+
 def config_scene(name: str, device: str = "cpu", **over):
-    presets = {
-        # C1: 64^3 dense, 8 frames
-        "c1": dict(dense_dim=64, radius_vox=24.0, frames=8, voxel_size=0.004),
-        # small hashed case for fast CPU tests
-        "tiny": dict(radius_vox=10.0, frames=6, width=160, height=120, voxel_size=0.004),
-        "small": dict(radius_vox=20.0, frames=8, width=320, height=240, voxel_size=0.004),
-        # C2: ~500 K voxels, 50 frames      (N = 4*pi*R^2*2*band => R ~ 81.5 at band 3)
-        "c2": dict(radius_vox=81.4, frames=50, voxel_size=0.002),
-        # C3: ~2 M voxels, 200 frames, spatially varying SH
-        "c3": dict(radius_vox=162.9, frames=200, voxel_size=0.002, sh_mode="varying"),
-    }
-    kw = dict(presets[name])
+    kw = dict(_PRESETS[name])
     kw.update(over)
     return make_scene(device=device, **kw)
+
+
+# config name -> make_scene arguments (N is the number of hash entries)
+_PRESETS = {
+    # C1: 64^3 dense, 8 frames
+    "c1": dict(dense_dim=64, radius_vox=24.0, frames=8, voxel_size=0.004),
+    # small hashed case for fast CPU tests
+    "tiny": dict(radius_vox=10.0, frames=6, width=160, height=120, voxel_size=0.004),
+    "small": dict(radius_vox=20.0, frames=8, width=320, height=240, voxel_size=0.004),
+    # C2: ~500 K voxels, 50 frames      (N = 4*pi*R^2*2*band => R ~ 81.5 at band 3)
+    "c2": dict(radius_vox=81.4, frames=50, voxel_size=0.002),
+    # C3: ~2 M voxels, 200 frames, spatially varying SH
+    "c3": dict(radius_vox=162.9, frames=200, voxel_size=0.002, sh_mode="varying"),
+}
