@@ -270,6 +270,29 @@ int         i3d_download_surface_distance(I3DEngine* e, float* vertex_distance, 
 int         i3d_debug_set_keep_distance_samples(I3DEngine* e, int on);
 int         i3d_debug_get_distance_samples(I3DEngine* e, int direction, float* d2, int32_t* face);
 
+/* ---- the voxel grid from a triangle mesh: narrow-band signed distance (DESIGN.md §6v) ---- */
+uint64_t    i3d_sizeof_grid_from_mesh_params(void);
+uint64_t    i3d_sizeof_grid_from_mesh_info(void);
+/* source I3D_GRID_FROM_MESH_REFERENCE, voxel_size 0.002, band 3, cell_size 0 (automatic). */
+void        i3d_default_grid_from_mesh_params(I3DGridFromMeshParams* p);
+/* Replaces the voxel set by the narrow-band signed distance field of a triangle mesh on the lattice c * voxel_size: every voxel with a
+ * face within b = band * voxel_size gets the nearest face (the lexicographic minimum of (float d^2, face id), as i3d_surface_distance
+ * finds it), |sdf| = sqrt(d^2) and the sign of dot(p - q, N), N the angle-weighted pseudonormal of the feature of the face the closest
+ * point q lies on, over vertices welded by exact position.  A voxel is dropped when N = 0, when dot = 0 at d > 0, and when the feature
+ * lies on the mesh's boundary and |cos(p - q, N)| < I3D_GRID_FROM_MESH_RIM_COS.  Voxels come in canonical 8^3-brick-major order with
+ * sdf0 = sdf, albedo 0.6, weight 1 and colour 0 (i3d_recompute_colors colours them); voxel_size and truncation (5 voxels) are set as
+ * i3d_fusion_finish sets them.  The rounding of every operation is stated in i3d_grid_from_mesh.cuh; the result does not depend on
+ * cell_size and is bit-identical from run to run.  On success everything derived from the voxel set is forgotten (as after a pruning),
+ * and the frames, camera, sensor store, reference mesh and any fusion in progress stay.  *info (may be NULL) gets the counts and the
+ * device time per stage.  Fails, changing nothing, when world > 1, without the source mesh or with one without faces, for a bad
+ * source, a voxel_size that is not finite and > 0, a band outside (0, 16], a cell_size that is negative or not finite, a lattice
+ * coordinate outside +-(2^20 - 8), a search grid above the caps of i3d_surface_distance, more than I3D_GRID_FROM_MESH_MAX_PAIRS
+ * (face, brick) pairs or I3D_GRID_FROM_MESH_MAX_VOXELS candidate voxels, and when no voxel is emitted. */
+int         i3d_grid_from_mesh(I3DEngine* e, const I3DGridFromMeshParams* params, I3DGridFromMeshInfo* info);
+/* Tests: per voxel of the last successful i3d_grid_from_mesh (in its order), the nearest face int32 and the I3D_FEATURE_* of the
+ * closest point int8.  Either pointer may be NULL.  Fails before the first successful call. */
+int         i3d_debug_get_grid_from_mesh_voxels(I3DEngine* e, int32_t* face, int8_t* feature);
+
 /* ---- rendering the surface into the keyframes (DESIGN.md §6m) ---- */
 uint64_t    i3d_sizeof_render_params(void);
 uint64_t    i3d_sizeof_render_stats(void);

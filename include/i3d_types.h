@@ -271,6 +271,46 @@ typedef struct I3DDistanceInfo
     double  ms_vertices;                  /* device time of the vertex query */
 } I3DDistanceInfo;
 
+/* ---- the voxel grid from a triangle mesh: narrow-band signed distance (DESIGN.md §6v) ---- */
+#define I3D_GRID_FROM_MESH_REFERENCE 0      /* source: the mesh of i3d_upload_reference_mesh */
+#define I3D_GRID_FROM_MESH_RESIDENT 1       /* source: the resident mesh (the last extraction or simplification) */
+#define I3D_GRID_FROM_MESH_MAX_BAND 16.0f   /* largest band, voxels */
+#define I3D_GRID_FROM_MESH_MAX_PAIRS (1ll << 28)     /* largest sum over faces of the 8^3 bricks their band-grown AABB covers */
+#define I3D_GRID_FROM_MESH_MAX_VOXELS (1ll << 30)    /* largest number of candidate voxels (512 per candidate brick) */
+/* A voxel whose closest feature is a boundary edge or vertex is kept only when |cos| of the angle between p - q and the feature's
+ * pseudonormal is >= this: an open mesh grows no skirt past its rim */
+#define I3D_GRID_FROM_MESH_RIM_COS 0.5
+
+typedef struct I3DGridFromMeshParams
+{
+    int32_t source;                       /* I3D_GRID_FROM_MESH_REFERENCE or I3D_GRID_FROM_MESH_RESIDENT */
+    float   voxel_size;                   /* metres, finite and > 0: voxel c sits at c * voxel_size */
+    float   band;                         /* voxels, in (0, 16]: voxels with a face within band * voxel_size are emitted */
+    float   cell_size;                    /* search-grid cell edge, metres; 0 = twice the mesh's mean edge length.  Never changes the result */
+} I3DGridFromMeshParams;
+
+typedef struct I3DGridFromMeshInfo
+{
+    int64_t num_faces;                    /* faces of the source mesh */
+    int64_t num_vertices_welded;          /* distinct vertex positions */
+    int64_t num_boundary_edges;           /* welded edges used by exactly one non-degenerate face */
+    int64_t num_brick_pairs;              /* (face, brick) pairs of the band-grown face AABBs, before the distance test */
+    int64_t num_candidate_bricks, num_candidate_voxels;
+    int64_t num_voxels, num_negative;     /* emitted voxels, and those with sdf < 0 */
+    int64_t num_beyond_band;              /* candidate voxels with no face within the band */
+    int64_t num_dropped_rim;              /* closest feature on the boundary and |cos| < I3D_GRID_FROM_MESH_RIM_COS */
+    int64_t num_dropped_zero_normal;      /* closest feature with a zero pseudonormal */
+    int64_t num_dropped_zero_dot;         /* d > 0 and p - q orthogonal to the pseudonormal: no sign */
+    int64_t point_triangle_tests;         /* closest-point evaluations of the query */
+    float   cell_size;                    /* the search grid used: cell edge (metres) and cells per axis */
+    int32_t grid[3];
+    double  ms_topology, ms_grid, ms_bricks, ms_query, ms_install;   /* device time per stage (CUDA events) */
+} I3DGridFromMeshInfo;
+
+/* Features of the closest point on a face (i3d_debug_get_grid_from_mesh_voxels): vertex a, b, c, edge ab, ac, bc, interior */
+enum { I3D_FEATURE_VERTEX_A = 0, I3D_FEATURE_VERTEX_B, I3D_FEATURE_VERTEX_C, I3D_FEATURE_EDGE_AB, I3D_FEATURE_EDGE_AC, I3D_FEATURE_EDGE_BC,
+       I3D_FEATURE_INTERIOR };
+
 /* Colour modes of a mesh (SDFVisualization::colorize, src/sdf/visualization.cpp:101-416; mode strings "", "normals", "lap", "lum",
  * "lum_grad", "albedo", "shading_sv", "shading_sv_const", "chroma").  VOXEL is the voxel colours; the others are computed per voxel from
  * the voxel and its ±1 ring (DESIGN.md §6k).  The reference's subvolume modes ("subvol", "subvol_interp") have no number. */

@@ -27,8 +27,25 @@ std::string format(const char* fmt, ...)
     return buf;
 }
 
-// The search grid of target t (F > 0): its size, cell edge, margin and entry count; false with the message when a cap is exceeded
-bool plan(DistanceState& ds, const DistMesh& t, const I3DDistanceParams& p, DistGrid& g, int64_t& entries, std::string& error, cudaStream_t st)
+void side_info(const double* s, const DistGrid& g, int64_t samples, int64_t entries, int nt, I3DDistanceSide& o)
+{
+    o.num_samples = samples;
+    o.num_matched = static_cast<int64_t>(s[1]);
+    o.area = s[2]; o.unmatched_area = s[3];
+    o.mean = s[0] > 0.0 ? s[4] / s[0] : 0.0;
+    o.rms = s[0] > 0.0 ? std::sqrt(s[5] / s[0]) : 0.0;
+    o.max = s[6];
+    for (int k = 0; k < nt; ++k) o.fraction[k] = s[2] > 0.0 ? s[8 + k] / s[2] : 0.0;
+    o.point_triangle_tests = static_cast<int64_t>(s[7]);
+    o.cell_size = g.h;
+    for (int k = 0; k < 3; ++k) o.grid[k] = g.n[k];
+    o.num_cells = static_cast<int64_t>(g.n[0]) * g.n[1] * g.n[2];
+    o.num_cell_entries = entries;
+}
+} // namespace
+
+bool plan(DistGridScratch& ds, const DistMesh& t, float cell_size, float max_distance, DistGrid& g, int64_t& entries, double* bounds, std::string& error,
+          cudaStream_t st)
 {
     const unsigned nb = blocks_for(static_cast<size_t>(t.F));
     ds.partials.ensure(static_cast<size_t>(nb) * kDistBounds);
@@ -40,15 +57,17 @@ bool plan(DistanceState& ds, const DistMesh& t, const I3DDistanceParams& p, Dist
     for (int j = 0; j < kDistBounds; ++j) b[j] = h[j];
     for (unsigned i = 1; i < nb; ++i)
         for (int j = 0; j < kDistBounds; ++j) b[j] = j < 6 ? std::max(b[j], h[i * kDistBounds + j]) : b[j] + h[i * kDistBounds + j];
+    if (bounds)
+        for (int k = 0; k < 3; ++k) { bounds[k] = -b[k]; bounds[3 + k] = b[3 + k]; }
     const double mean_edge = b[6] / (3.0 * static_cast<double>(t.F));
-    float cell = p.cell_size > 0.0f ? p.cell_size : static_cast<float>(2.0 * mean_edge);
-    if (!(cell > 0.0f)) cell = p.max_distance;          // every face of the target is a point
+    float cell = cell_size > 0.0f ? cell_size : static_cast<float>(2.0 * mean_edge);
+    if (!(cell > 0.0f)) cell = max_distance;          // every face of the target is a point
     std::memset(&g, 0, sizeof(g));
     g.h = cell;
     double extent = 0.0, mag = 0.0, cells = 1.0;
     for (int k = 0; k < 3; ++k)
     {
-        const float lo = static_cast<float>(-b[k]) - p.max_distance, hi = static_cast<float>(b[3 + k]) + p.max_distance;
+        const float lo = static_cast<float>(-b[k]) - max_distance, hi = static_cast<float>(b[3 + k]) + max_distance;
         const double n = std::floor((static_cast<double>(hi) - lo) / cell) + 1.0;
         cells *= n;
         g.lo[k] = lo;
@@ -63,11 +82,11 @@ bool plan(DistanceState& ds, const DistMesh& t, const I3DDistanceParams& p, Dist
         return false;
     }
     g.margin = std::ldexp(mag + extent + cell, -16);
-    ds.vtests.ensure(1);
-    CK(cudaMemsetAsync(ds.vtests.p, 0, sizeof(unsigned long long), st));
-    k_dist_entries<<<nb, kThreads, 0, st>>>(t, g, ds.vtests.p);
+    ds.counter.ensure(1);
+    CK(cudaMemsetAsync(ds.counter.p, 0, sizeof(unsigned long long), st));
+    k_dist_entries<<<nb, kThreads, 0, st>>>(t, g, ds.counter.p);
     unsigned long long e = 0;
-    CK(cudaMemcpyAsync(&e, ds.vtests.p, sizeof(e), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&e, ds.counter.p, sizeof(e), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     entries = static_cast<int64_t>(e);
     if (entries > I3D_DISTANCE_MAX_CELL_ENTRIES)
@@ -79,8 +98,8 @@ bool plan(DistanceState& ds, const DistMesh& t, const I3DDistanceParams& p, Dist
     return true;
 }
 
-// Count, scan and fill the grid g of target t into ds (cell_count ends as the per-cell counts again)
-void build(DistanceState& ds, const DistMesh& t, DistGrid& g, int64_t entries, cudaStream_t st)
+// cell_count ends as the per-cell counts again
+void build(DistGridScratch& ds, const DistMesh& t, DistGrid& g, int64_t entries, cudaStream_t st)
 {
     const size_t cells = static_cast<size_t>(g.n[0]) * g.n[1] * g.n[2];
     ds.cell_count.ensure(cells); ds.cell_off.ensure(cells); ds.cell_faces.ensure(static_cast<size_t>(entries));
@@ -98,22 +117,6 @@ void build(DistanceState& ds, const DistMesh& t, DistGrid& g, int64_t entries, c
     g.off = ds.cell_off.p; g.cnt = ds.cell_count.p; g.faces = ds.cell_faces.p;
 }
 
-void side_info(const double* s, const DistGrid& g, int64_t samples, int64_t entries, int nt, I3DDistanceSide& o)
-{
-    o.num_samples = samples;
-    o.num_matched = static_cast<int64_t>(s[1]);
-    o.area = s[2]; o.unmatched_area = s[3];
-    o.mean = s[0] > 0.0 ? s[4] / s[0] : 0.0;
-    o.rms = s[0] > 0.0 ? std::sqrt(s[5] / s[0]) : 0.0;
-    o.max = s[6];
-    for (int k = 0; k < nt; ++k) o.fraction[k] = s[2] > 0.0 ? s[8 + k] / s[2] : 0.0;
-    o.point_triangle_tests = static_cast<int64_t>(s[7]);
-    o.cell_size = g.h;
-    for (int k = 0; k < 3; ++k) o.grid[k] = g.n[k];
-    o.num_cells = static_cast<int64_t>(g.n[0]) * g.n[1] * g.n[2];
-    o.num_cell_entries = entries;
-}
-} // namespace
 
 int upload_reference(DistanceState& ds, int64_t V, const float* xyz, int64_t F, const int32_t* faces, std::string& error, cudaStream_t st)
 {
@@ -148,7 +151,8 @@ int compute(DistanceState& ds, const DistMesh& a, const I3DDistanceParams& p, I3
     // both grids are sized, and refused, before anything is written
     DistGrid gb, ga;
     int64_t eb = 0, ea = 0;
-    if (!plan(ds, b, p, gb, eb, error, st) || !plan(ds, a, p, ga, ea, error, st)) return 1;
+    if (!plan(ds.grid, b, p.cell_size, p.max_distance, gb, eb, nullptr, error, st) || !plan(ds.grid, a, p.cell_size, p.max_distance, ga, ea, nullptr, error, st))
+        return 1;
     const int L = p.samples_per_edge, LL = L * L;
     DistQuery q;
     std::memset(&q, 0, sizeof(q));
@@ -168,12 +172,13 @@ int compute(DistanceState& ds, const DistMesh& a, const I3DDistanceParams& p, I3
         if (ds.keep) { ds.keep_d2[d].ensure(static_cast<size_t>(ns[d])); ds.keep_face[d].ensure(static_cast<size_t>(ns[d])); }
         ds.keep_n[d] = ds.keep ? ns[d] : 0;
     }
+    ds.vtests.ensure(1);
     CK(cudaMemsetAsync(ds.vtests.p, 0, sizeof(unsigned long long), st));
     for (int d = 0; d < 2; ++d)
     {
         cudaEvent_t* ev = ds.ev + (d == 0 ? 0 : 8);
         CK(cudaEventRecord(ev[0], st));
-        build(ds, *tgt[d], *grid[d], d == 0 ? eb : ea, st);
+        build(ds.grid, *tgt[d], *grid[d], d == 0 ? eb : ea, st);
         CK(cudaEventRecord(ev[1], st));
         k_dist_samples<<<nbs[d], kThreads, 0, st>>>(src[d], *tgt[d], *grid[d], q, ds.keep ? ds.keep_d2[d].p : nullptr, ds.keep ? ds.keep_face[d].p : nullptr,
                                                     ds.partials.p);

@@ -10,6 +10,8 @@
  *   area = FM(1/2, sqrt(FA(FA(FM(n0, n0), FM(n1, n1)), FM(n2, n2)))) (__fsqrt_rn), n = (v1 - v0) x (v2 - v0), each component
  *   FS(FM(e1[p], e2[q]), FM(e1[q], e2[p])); the sample's weight is double(area) / double(L^2).  Samples are never stored.
  *
+ * The closest point and the nearest-face query are in i3d_distance_query.cuh, which the mesh-to-grid conversion shares.
+ *
  * Closest point (dist_point_tri_d2): Ericson, Real-Time Collision Detection §5.1.5, in the order written below, then d^2 = dot(p - q,
  * p - q), dot(x, y) = FA(FA(FM(x0, y0), FM(x1, y1)), FM(x2, y2)).  A triangle with dot(n, n) = 0, one where a division of the
  * procedure would have a denominator that is not > 0 and one whose interior (v, w) fall outside v, w >= 0, FA(v, w) <= 1 is measured
@@ -30,8 +32,7 @@
  * k_dist_finish sums the blocks in order.  No atomics: every number is bit-identical from run to run.
  */
 #pragma once
-#include "i3d_distance.h"
-#include "i3d_grid.cuh"
+#include "i3d_distance_query.cuh"
 
 namespace i3d
 {
@@ -44,113 +45,11 @@ constexpr unsigned kDistStatsMax = 1u << 6;
 constexpr int kDistBounds = 7;
 constexpr unsigned kDistBoundsMax = 0x3Fu;
 
-// The search grid of a target mesh; off / cnt / faces are null while it is being counted
-struct DistGrid
-{
-    float lo[3]; float h; int n[3];
-    double margin;
-    const int64_t* off; const int32_t* cnt; const int32_t* faces;
-};
-
-// A triangle with dot(n, n) <= 2^-20 dot(ab, ab) dot(ac, ac) (an angle below about 1e-3 rad) is a sliver: the float signs of Ericson's
-// region tests cancel there, so its d^2 is also bounded by its edges'
-constexpr float kDistSliver = 9.5367431640625e-07f;
-
 struct DistQuery
 {
     float max_distance; int L; int num_thresholds;
     float tau[I3D_DISTANCE_MAX_THRESHOLDS];
 };
-
-__device__ __forceinline__ float dist_dot(const float* x, const float* y) { return FA(FA(FM(x[0], y[0]), FM(x[1], y[1])), FM(x[2], y[2])); }
-
-__device__ __forceinline__ float dist_seg_d2(const float* p, const float* s0, const float* s1)
-{
-    float e[3], sp[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) { e[k] = FS(s1[k], s0[k]); sp[k] = FS(p[k], s0[k]); }
-    const float ll = dist_dot(e, e);
-    float t = ll > 0.0f ? FD(dist_dot(sp, e), ll) : 0.0f;
-    t = t < 0.0f ? 0.0f : (t > 1.0f ? 1.0f : t);
-    float d[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) d[k] = FS(p[k], FA(s0[k], FM(t, e[k])));
-    return dist_dot(d, d);
-}
-
-// float d^2 from p to triangle (a, b, c) (the rule at the top of the file)
-__device__ __forceinline__ float dist_point_tri_d2(const float* p, const float* a, const float* b, const float* c)
-{
-    float ab[3], ac[3], ap[3], bp[3], cp[3], bc[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k)
-    {
-        ab[k] = FS(b[k], a[k]); ac[k] = FS(c[k], a[k]); ap[k] = FS(p[k], a[k]);
-        bp[k] = FS(p[k], b[k]); cp[k] = FS(p[k], c[k]); bc[k] = FS(c[k], b[k]);
-    }
-    const float n[3] = {FS(FM(ab[1], ac[2]), FM(ab[2], ac[1])), FS(FM(ab[2], ac[0]), FM(ab[0], ac[2])), FS(FM(ab[0], ac[1]), FM(ab[1], ac[0]))};
-    // the closest point: region 0, 1, 2 the vertex a, b, c; 3, 4, 5 the point at s along ab, ac, bc; 6 the interior a + v ab + w ac
-    int region = 0;
-    float s = 0.0f, vi = 0.0f, wi = 0.0f;
-    const float nn = dist_dot(n, n);
-    bool edges = !(nn > 0.0f);
-    const bool sliver = !(nn > FM(FM(kDistSliver, dist_dot(ab, ab)), dist_dot(ac, ac)));
-    if (!edges)
-    {
-        const float d1 = dist_dot(ab, ap), d2 = dist_dot(ac, ap);
-        const float d3 = dist_dot(ab, bp), d4 = dist_dot(ac, bp);
-        const float d5 = dist_dot(ab, cp), d6 = dist_dot(ac, cp);
-        const float vc = FS(FM(d1, d4), FM(d3, d2));
-        const float vb = FS(FM(d5, d2), FM(d1, d6));
-        const float va = FS(FM(d3, d6), FM(d5, d4));
-        const float e43 = FS(d4, d3), e56 = FS(d5, d6);
-        float num = 0.0f, den = 1.0f;
-        if (d1 <= 0.0f && d2 <= 0.0f) region = 0;
-        else if (d3 >= 0.0f && d4 <= d3) region = 1;
-        else if (vc <= 0.0f && d1 >= 0.0f && d3 <= 0.0f) { region = 3; num = d1; den = FS(d1, d3); }
-        else if (d6 >= 0.0f && d5 <= d6) region = 2;
-        else if (vb <= 0.0f && d2 >= 0.0f && d6 <= 0.0f) { region = 4; num = d2; den = FS(d2, d6); }
-        else if (va <= 0.0f && e43 >= 0.0f && e56 >= 0.0f) { region = 5; num = e43; den = FA(e43, e56); }
-        else { region = 6; den = FA(FA(va, vb), vc); }
-        if (!(den > 0.0f)) edges = true;
-        else if (region == 6)
-        {
-            const float r = FD(1.0f, den);
-            vi = FM(vb, r); wi = FM(vc, r);
-            if (!(vi >= 0.0f && wi >= 0.0f && FA(vi, wi) <= 1.0f)) edges = true;
-        }
-        else if (region >= 3) s = FD(num, den);
-    }
-    float de = 0.0f;
-    if (edges || sliver) de = fminf(fminf(dist_seg_d2(p, a, b), dist_seg_d2(p, b, c)), dist_seg_d2(p, c, a));
-    if (edges) return de;
-    float d[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k)
-    {
-        float q;
-        switch (region)
-        {
-        case 0: q = a[k]; break;
-        case 1: q = b[k]; break;
-        case 2: q = c[k]; break;
-        case 3: q = FA(a[k], FM(s, ab[k])); break;
-        case 4: q = FA(a[k], FM(s, ac[k])); break;
-        case 5: q = FA(b[k], FM(s, bc[k])); break;
-        default: q = FA(FA(a[k], FM(ab[k], vi)), FM(ac[k], wi)); break;
-        }
-        d[k] = FS(p[k], q);
-    }
-    const float dq = dist_dot(d, d);
-    return sliver ? fminf(dq, de) : dq;
-}
-
-__device__ __forceinline__ int dist_cell(float x, float lo, float h, int n)
-{
-    float v = FD(FS(x, lo), h);
-    v = fminf(fmaxf(v, 0.0f), static_cast<float>(n - 1));
-    return static_cast<int>(floorf(v));
-}
 
 // Sample s of face f of m: the point P and the face's float area
 __device__ __forceinline__ void dist_sample(const DistMesh& m, int64_t f, int s, int L, float* P, float& area)
@@ -177,58 +76,6 @@ __device__ __forceinline__ void dist_sample(const DistMesh& m, int64_t f, int s,
     const float n1 = FS(FM(e1[2], e2[0]), FM(e1[0], e2[2]));
     const float n2 = FS(FM(e1[0], e2[1]), FM(e1[1], e2[0]));
     area = FM(0.5f, __fsqrt_rn(FA(FA(FM(n0, n0), FM(n1, n1)), FM(n2, n2))));
-}
-
-// The nearest face of m to p within lim2 = max_distance^2: (bd2, bf), or (+inf, -1); tests counts the point-triangle evaluations
-__device__ __forceinline__ void dist_nearest(const float* p, const DistMesh& m, const DistGrid& g, float lim2, float& bd2, int& bf, long long& tests)
-{
-    int c[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) c[k] = dist_cell(p[k], g.lo[k], g.h, g.n[k]);
-    const double margin = g.margin + ldexp(static_cast<double>(fmaxf(fmaxf(fabsf(p[0]), fabsf(p[1])), fabsf(p[2]))), -16);
-    bd2 = __int_as_float(0x7f800000); bf = -1;
-#pragma unroll 1
-    for (int r = 0;; ++r)
-    {
-        const int z0 = max(c[2] - r, 0), z1 = min(c[2] + r, g.n[2] - 1), y0 = max(c[1] - r, 0), y1 = min(c[1] + r, g.n[1] - 1);
-#pragma unroll 1
-        for (int z = z0; z <= z1; ++z)
-#pragma unroll 1
-            for (int y = y0; y <= y1; ++y)
-            {
-                const bool full = r == 0 || z == c[2] - r || z == c[2] + r || y == c[1] - r || y == c[1] + r;
-                const int step = full ? 1 : 2 * r;
-#pragma unroll 1
-                for (int x = c[0] - r; x <= c[0] + r; x += step)
-                {
-                    if (x < 0 || x >= g.n[0]) continue;
-                    const int64_t cell = (static_cast<int64_t>(z) * g.n[1] + y) * g.n[0] + x;
-                    const int64_t e0 = g.off[cell], e1 = e0 + g.cnt[cell];
-#pragma unroll 1
-                    for (int64_t e = e0; e < e1; ++e)
-                    {
-                        const int f = g.faces[e];
-                        const int3 fv = m.faces[f];
-                        ++tests;
-                        const float d2 = dist_point_tri_d2(p, m.vpos + 3 * static_cast<size_t>(fv.x), m.vpos + 3 * static_cast<size_t>(fv.y),
-                                                           m.vpos + 3 * static_cast<size_t>(fv.z));
-                        if (d2 <= lim2 && (d2 < bd2 || (d2 == bd2 && f < bf))) { bd2 = d2; bf = f; }
-                    }
-                }
-            }
-        double lb = 1e300;
-        bool more = false;
-#pragma unroll
-        for (int k = 0; k < 3; ++k)
-        {
-            if (c[k] - r > 0) { more = true; lb = fmin(lb, static_cast<double>(p[k]) - (static_cast<double>(g.lo[k]) + static_cast<double>(c[k] - r) * g.h)); }
-            if (c[k] + r < g.n[k] - 1) { more = true; lb = fmin(lb, (static_cast<double>(g.lo[k]) + static_cast<double>(c[k] + r + 1) * g.h) - static_cast<double>(p[k])); }
-        }
-        if (!more) break;
-        lb -= margin;
-        const double lim = static_cast<double>(bf >= 0 ? bd2 : lim2);
-        if (lb > 0.0 && lb * lb > lim) break;
-    }
 }
 
 // Block reduction of NS slots into out[blockIdx.x][NS]: per warp a shuffle-down tree, then the warps in order; slot j is a maximum when

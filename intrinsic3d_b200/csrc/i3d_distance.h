@@ -19,14 +19,30 @@ namespace i3d
 // A triangle mesh as the distance kernels read it
 struct DistMesh { int64_t V, F; const float* vpos; const int3* faces; };
 
+// The search grid of a target mesh (i3d_distance.cuh); off / cnt / faces are null while it is being counted
+struct DistGrid
+{
+    float lo[3]; float h; int n[3];
+    double margin;
+    const int64_t* off; const int32_t* cnt; const int32_t* faces;
+};
+
+// What sizing and filling one search grid needs: per cell its face count and the int64 offset of its run in cell_faces, the bounds
+// partials and the entry counter
+struct DistGridScratch
+{
+    Dev<int32_t> cell_count, cell_faces; Dev<int64_t> cell_off; Dev<uint8_t> cub;
+    Dev<double> partials;
+    Dev<unsigned long long> counter;
+};
+
 // Reference mesh, grid scratch and results of the distance calls of one engine
 struct DistanceState
 {
     Dev<float> ref_vpos; Dev<int3> ref_faces;
     int64_t ref_V = 0, ref_F = 0;
     bool have_ref = false;
-    // search grid of the current target: per cell its face count and the int64 offset of its run in cell_faces
-    Dev<int32_t> cell_count, cell_faces; Dev<int64_t> cell_off; Dev<uint8_t> cub;
+    DistGridScratch grid;                  // search grid of the current target
     Dev<double> partials, stats;           // per-block partials and the finished statistics of both directions
     Dev<unsigned long long> vtests;
     // the last results: per-vertex distance and face of the resident mesh, and (when keep) the per-sample (d^2, face) of both directions
@@ -41,6 +57,13 @@ struct DistanceState
 
 namespace distance
 {
+// The search grid of target t (F > 0) for queries within max_distance: its size, cell edge (cell_size, or twice the mean edge length
+// when 0), margin and entry count, and when bounds is set the faces' AABB (min x, y, z, max x, y, z).  Returns false with the message
+// when a cap is exceeded.
+bool plan(DistGridScratch& s, const DistMesh& t, float cell_size, float max_distance, DistGrid& g, int64_t& entries, double* bounds, std::string& error,
+          cudaStream_t st);
+// Counts, scans and fills the planned grid g of target t into s, and points g at it
+void build(DistGridScratch& s, const DistMesh& t, DistGrid& g, int64_t entries, cudaStream_t st);
 // Uploads the reference mesh after checking it on the host; returns non-zero with the message in `error`, keeping the previous one
 int upload_reference(DistanceState& ds, int64_t V, const float* xyz, int64_t F, const int32_t* faces, std::string& error, cudaStream_t st);
 // Both directions and the vertex query between the resident mesh a (F > 0) and the reference (present), with parameters the caller

@@ -36,6 +36,7 @@
 #include "i3d_render.h"
 #include "i3d_texture.h"
 #include "i3d_distance.h"
+#include "i3d_grid_from_mesh.h"
 #include "i3d_track.h"
 
 using namespace i3d;
@@ -170,6 +171,7 @@ struct I3DEngine
     MeshState mesh;                    // surface extraction (i3d_mesh.cu)
     TextureState tex;                  // texture of the resident mesh (i3d_texture.cu)
     DistanceState dist;                // reference mesh and distance results (i3d_distance.cu)
+    GridFromMeshState gfm;             // the voxel grid from a mesh (i3d_grid_from_mesh.cu)
     RenderState render;                // keyframe renderer (i3d_render.cu)
     TrackScratch track;                // frame-to-model tracker (i3d_render.cu)
     // shard (multi-GPU)
@@ -1879,6 +1881,90 @@ int i3d_debug_get_distance_samples(I3DEngine* e, int direction, float* d2, int32
         const size_t n = static_cast<size_t>(e->dist.keep_n[direction]);
         if (d2 && n) CK(cudaMemcpyAsync(d2, e->dist.keep_d2[direction].p, n * sizeof(float), cudaMemcpyDeviceToHost, st));
         if (face && n) CK(cudaMemcpyAsync(face, e->dist.keep_face[direction].p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    });
+}
+
+// ---- the voxel grid from a triangle mesh (i3d_grid_from_mesh.cuh, DESIGN.md §6v) -----------------------
+uint64_t i3d_sizeof_grid_from_mesh_params(void) { return sizeof(I3DGridFromMeshParams); }
+uint64_t i3d_sizeof_grid_from_mesh_info(void) { return sizeof(I3DGridFromMeshInfo); }
+
+void i3d_default_grid_from_mesh_params(I3DGridFromMeshParams* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    p->source = I3D_GRID_FROM_MESH_REFERENCE; p->voxel_size = 0.002f; p->band = 3.0f; p->cell_size = 0.0f;
+}
+
+int i3d_grid_from_mesh(I3DEngine* e, const I3DGridFromMeshParams* params, I3DGridFromMeshInfo* info)
+{
+    static const char* who = "i3d_grid_from_mesh";
+    if (!e) return 1;
+    if (!params) return fail(e, "%s: params is NULL", who);
+    if (e->world > 1) return fail(e, "%s: the conversion runs on one GPU (world = %d)", who, e->world);
+    const I3DGridFromMeshParams& p = *params;
+    DistMesh m{};
+    if (p.source == I3D_GRID_FROM_MESH_REFERENCE)
+    {
+        if (!e->dist.have_ref) return fail(e, "%s: no reference mesh (i3d_upload_reference_mesh)", who);
+        m = DistMesh{e->dist.ref_V, e->dist.ref_F, e->dist.ref_vpos.p, e->dist.ref_faces.p};
+    }
+    else if (p.source == I3D_GRID_FROM_MESH_RESIDENT)
+    {
+        if (!e->mesh.have_mesh) return fail(e, "%s: no resident mesh (call i3d_extract_mesh after the last change of the voxel set)", who);
+        m = DistMesh{e->mesh.mesh_V, e->mesh.mesh_F, e->mesh.mesh_vpos, e->mesh.mesh_faces};
+    }
+    else return fail(e, "%s: source must be %d (reference) or %d (resident), got %d", who, I3D_GRID_FROM_MESH_REFERENCE, I3D_GRID_FROM_MESH_RESIDENT, p.source);
+    if (m.F <= 0) return fail(e, "%s: the source mesh has no faces", who);
+    if (!std::isfinite(p.voxel_size) || !(p.voxel_size > 0.0f)) return fail(e, "%s: voxel_size must be finite and > 0, got %g", who, static_cast<double>(p.voxel_size));
+    if (!(p.band > 0.0f && p.band <= I3D_GRID_FROM_MESH_MAX_BAND))
+        return fail(e, "%s: band must be in (0, %g] voxels, got %g", who, static_cast<double>(I3D_GRID_FROM_MESH_MAX_BAND), static_cast<double>(p.band));
+    if (!std::isfinite(p.cell_size) || p.cell_size < 0.0f) return fail(e, "%s: cell_size must be finite and >= 0, got %g", who, static_cast<double>(p.cell_size));
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        I3DGridFromMeshInfo inf;
+        std::string err;
+        if (gfm::query(e->gfm, m, p, inf, err, st)) return fail(e, "%s: %s", who, err.c_str());
+        const int64_t nc = inf.num_candidate_voxels;
+        int mk = 0;
+        if (nc > 0)
+        {
+            const int nscan = static_cast<int>((nc + kScanChunk - 1) / kScanChunk);
+            e->scan_counts.ensure(static_cast<size_t>(nscan) + 1); e->scan_total.ensure(1); e->act.ensure(static_cast<size_t>(nc));
+            k_scan_count<<<nscan, kThreads, 0, st>>>(nc, e->gfm.keep.p, 1, e->scan_counts.p);
+            k_scan_blocks<<<1, 1024, 0, st>>>(nscan, e->scan_counts.p, e->scan_total.p);
+            k_scan_scatter<<<nscan, kThreads, 0, st>>>(nc, e->gfm.keep.p, 1, e->scan_counts.p, e->act.p);
+            CK(cudaMemcpyAsync(&mk, e->scan_total.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            CK(cudaGetLastError());
+        }
+        if (mk <= 0) return fail(e, "%s: no voxel lies within the band of a face (%lld candidates)", who, static_cast<long long>(nc));
+        cudaEvent_t ev[2];
+        CK(cudaEventCreate(&ev[0])); CK(cudaEventCreate(&ev[1]));
+        CK(cudaEventRecord(ev[0], st));
+        const int hdup = install_grid(e, mk, [&](const VoxelArrays& out) { gfm::gather(e->gfm, e->act.p, mk, out, st); });
+        CK(cudaEventRecord(ev[1], st));
+        CK(cudaEventSynchronize(ev[1]));
+        float ms = 0.f;
+        CK(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+        CK(cudaEventDestroy(ev[0])); CK(cudaEventDestroy(ev[1]));
+        if (hdup) return fail(e, "%s: internal error (duplicate voxels)", who);
+        e->voxel_size = p.voxel_size; e->truncation = p.voxel_size * 5.0f;
+        inf.ms_install = ms;
+        if (info) *info = inf;
+        return 0;
+    });
+}
+
+int i3d_debug_get_grid_from_mesh_voxels(I3DEngine* e, int32_t* face, int8_t* feature)
+{
+    if (!e) return 1;
+    if (!e->gfm.have_last) return fail(e, "i3d_debug_get_grid_from_mesh_voxels: no conversion (call i3d_grid_from_mesh first)");
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t n = static_cast<size_t>(e->gfm.last_n);
+        if (face) CK(cudaMemcpyAsync(face, e->gfm.last_face.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        if (feature) CK(cudaMemcpyAsync(feature, e->gfm.last_feat.p, n, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         return 0;
     });

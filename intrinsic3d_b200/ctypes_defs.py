@@ -305,6 +305,44 @@ class I3DDistanceInfo(C.Structure, _Dictable):
     ]
 
 
+# I3D_GRID_FROM_MESH_* sources of include/i3d_types.h
+GRID_FROM_MESH_SOURCES = {"reference": 0, "resident": 1}
+
+
+class I3DGridFromMeshParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("source", C.c_int32),
+        ("voxel_size", C.c_float),
+        ("band", C.c_float),
+        ("cell_size", C.c_float),
+    ]
+
+
+class I3DGridFromMeshInfo(C.Structure, _Dictable):
+    _fields_ = [
+        ("num_faces", C.c_int64),
+        ("num_vertices_welded", C.c_int64),
+        ("num_boundary_edges", C.c_int64),
+        ("num_brick_pairs", C.c_int64),
+        ("num_candidate_bricks", C.c_int64),
+        ("num_candidate_voxels", C.c_int64),
+        ("num_voxels", C.c_int64),
+        ("num_negative", C.c_int64),
+        ("num_beyond_band", C.c_int64),
+        ("num_dropped_rim", C.c_int64),
+        ("num_dropped_zero_normal", C.c_int64),
+        ("num_dropped_zero_dot", C.c_int64),
+        ("point_triangle_tests", C.c_int64),
+        ("cell_size", C.c_float),
+        ("grid", C.c_int32 * 3),
+        ("ms_topology", C.c_double),
+        ("ms_grid", C.c_double),
+        ("ms_bricks", C.c_double),
+        ("ms_query", C.c_double),
+        ("ms_install", C.c_double),
+    ]
+
+
 # I3D_RENDER_* plane bits of include/i3d_types.h
 RENDER_PLANES = {"depth": 1, "normal": 2, "albedo": 4, "shading": 8, "intensity": 16}
 

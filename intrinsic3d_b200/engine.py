@@ -11,7 +11,8 @@ import os
 
 import numpy as np
 
-from .ctypes_defs import (DISTANCE_MAX_THRESHOLDS, RENDER_PLANES, I3DDistanceInfo, I3DDistanceParams, I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo,
+from .ctypes_defs import (DISTANCE_MAX_THRESHOLDS, GRID_FROM_MESH_SOURCES, RENDER_PLANES, I3DDistanceInfo, I3DDistanceParams, I3DGridFromMeshInfo,
+                          I3DGridFromMeshParams, I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo,
                           I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats, I3DSimplifyInfo, I3DSimplifyParams, I3DTextureInfo,
                           I3DTextureParams, I3DTrackColorInfo, I3DTrackColorParams, I3DTrackInfo, I3DTrackParams, TRACK_LEVELS)
 
@@ -37,6 +38,8 @@ EXPORTED_SYMBOLS = [
     "i3d_sizeof_texture_params", "i3d_sizeof_texture_info", "i3d_default_texture_params", "i3d_bake_texture", "i3d_download_texture",
     "i3d_sizeof_distance_params", "i3d_sizeof_distance_info", "i3d_default_distance_params", "i3d_upload_reference_mesh",
     "i3d_surface_distance", "i3d_download_surface_distance", "i3d_debug_set_keep_distance_samples", "i3d_debug_get_distance_samples",
+    "i3d_sizeof_grid_from_mesh_params", "i3d_sizeof_grid_from_mesh_info", "i3d_default_grid_from_mesh_params", "i3d_grid_from_mesh",
+    "i3d_debug_get_grid_from_mesh_voxels",
     "i3d_sizeof_render_params", "i3d_sizeof_render_stats", "i3d_default_render_params", "i3d_render_keyframes", "i3d_download_render",
     "i3d_debug_set_render_skip",
     "i3d_sizeof_track_params", "i3d_sizeof_track_info", "i3d_default_track_params", "i3d_track_sensor_frames", "i3d_debug_get_track_system",
@@ -128,6 +131,16 @@ def load_library():
     L.i3d_debug_set_keep_distance_samples.argtypes = [C.c_void_p, C.c_int]
     L.i3d_debug_get_distance_samples.restype = C.c_int
     L.i3d_debug_get_distance_samples.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int32)]
+    L.i3d_sizeof_grid_from_mesh_params.restype = C.c_uint64
+    L.i3d_sizeof_grid_from_mesh_info.restype = C.c_uint64
+    if L.i3d_sizeof_grid_from_mesh_params() != C.sizeof(I3DGridFromMeshParams) or L.i3d_sizeof_grid_from_mesh_info() != C.sizeof(I3DGridFromMeshInfo):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (grid-from-mesh structs)")
+    L.i3d_default_grid_from_mesh_params.restype = None
+    L.i3d_default_grid_from_mesh_params.argtypes = [C.POINTER(I3DGridFromMeshParams)]
+    L.i3d_grid_from_mesh.restype = C.c_int
+    L.i3d_grid_from_mesh.argtypes = [C.c_void_p, C.POINTER(I3DGridFromMeshParams), C.POINTER(I3DGridFromMeshInfo)]
+    L.i3d_debug_get_grid_from_mesh_voxels.restype = C.c_int
+    L.i3d_debug_get_grid_from_mesh_voxels.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int8)]
     L.i3d_mode_colors.restype = C.c_int
     L.i3d_mode_colors.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_uint8)]
     L.i3d_sensor_num_frames.restype = C.c_int32
@@ -524,6 +537,30 @@ class Engine:
 
     def debug_set_keep_distance_samples(self, on: bool = True):
         self._check(self.L.i3d_debug_set_keep_distance_samples(self.h, 1 if on else 0))
+
+    def grid_from_mesh(self, source: str = "reference", voxel_size: float = 0.002, band: float = 3.0, cell_size=None):
+        """Replaces the voxel set by the narrow-band signed distance field of a triangle mesh, built on the device (DESIGN.md §6v): every
+        voxel c (at c * voxel_size metres) with a face within band voxels gets sdf0 = sdf = the signed distance to the nearest face, signed
+        by the angle-weighted pseudonormal of the closest feature, albedo 0.6, weight 1 and colour 0 (recompute_colors colours it).
+        source "reference" converts the mesh of upload_reference_mesh (for example one read with mesh.load_ply), "resident" the last
+        extract_mesh or simplify_mesh.  An open mesh gets no voxels past its rim.  cell_size None picks the search grid's cell edge
+        automatically; the result does not depend on it.  The frames, camera and reference mesh stay; everything derived from the old
+        voxel set (SH, lighting, mesh, texture, render) is dropped.  Returns (voxels, info), info an I3DGridFromMeshInfo with the counts
+        and the device ms per stage."""
+        if source not in GRID_FROM_MESH_SOURCES:
+            raise ValueError(f"source must be one of {sorted(GRID_FROM_MESH_SOURCES)}, got {source!r}")
+        prm = I3DGridFromMeshParams(GRID_FROM_MESH_SOURCES[source], float(voxel_size), float(band), 0.0 if cell_size is None else float(cell_size))
+        info = I3DGridFromMeshInfo()
+        self._check(self.L.i3d_grid_from_mesh(self.h, C.byref(prm), C.byref(info)))
+        self.n = int(info.num_voxels)
+        return self.n, info
+
+    def debug_grid_from_mesh_voxels(self, n: int):
+        """(face int32 [n], feature int8 [n]) per voxel of the last grid_from_mesh: the nearest face and the I3D_FEATURE_* of the closest
+        point (0, 1, 2 vertex a, b, c; 3, 4, 5 edge ab, ac, bc; 6 interior)"""
+        face, feat = np.empty(n, np.int32), np.empty(n, np.int8)
+        self._check(self.L.i3d_debug_get_grid_from_mesh_voxels(self.h, _p(face, C.c_int32), _p(feat, C.c_int8)))
+        return face, feat
 
     def mode_colors(self, mode: str, source: str = "refined"):
         """Every voxel's colour in colour mode `mode` (a mode string of extract_mesh), uint8 [n, 3] in the grid's order: the colours a

@@ -43,6 +43,110 @@ def save_ply(path, mesh) -> None:
         fh.write(data)
 
 
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2", "uint16": "u2",
+              "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4", "float": "f4", "float32": "f4", "double": "f8", "float64": "f8"}
+
+
+def _ply_header(data: bytes):
+    """(format, elements, body offset) of a PLY file; elements: [(name, count, [(name, type) or (name, (count type, item type))])]"""
+    end = data.find(b"end_header")
+    if not data.startswith(b"ply") or end < 0:
+        raise ValueError("load_ply: not a PLY file (no 'ply' magic or no end_header)")
+    nl = data.find(b"\n", end)
+    body = len(data) if nl < 0 else nl + 1
+    fmt, elements = None, []
+    for line in data[:end].decode("ascii", "replace").splitlines()[1:]:
+        t = line.split()
+        if not t or t[0] in ("comment", "obj_info"):
+            continue
+        if t[0] == "format":
+            fmt = t[1]
+        elif t[0] == "element":
+            elements.append((t[1], int(t[2]), []))
+        elif t[0] == "property" and elements:
+            if t[1] == "list":
+                if t[2] not in _PLY_TYPES or t[3] not in _PLY_TYPES:
+                    raise ValueError(f"load_ply: unknown list types in {line!r}")
+                elements[-1][2].append((t[4], (_PLY_TYPES[t[2]], _PLY_TYPES[t[3]])))
+            elif t[1] in _PLY_TYPES:
+                elements[-1][2].append((t[2], _PLY_TYPES[t[1]]))
+            else:
+                raise ValueError(f"load_ply: unknown property type in {line!r}")
+    if fmt not in ("ascii", "binary_little_endian"):
+        raise ValueError(f"load_ply: format {fmt!r} is not supported (ascii or binary_little_endian)")
+    return fmt, elements, body
+
+
+def load_ply(path):
+    """Reads a triangle mesh from a PLY file: what save_ply writes, and ASCII or binary little-endian PLY with float or double x, y, z
+    and a vertex_indices (or vertex_index) list per face; other properties and elements are skipped, and red, green, blue become the
+    colours when present.  Raises ValueError for a face that is not a triangle, a missing vertex position or face list, and an index
+    outside the vertices.  Returns the dict extract_mesh returns: vertices float32 [V, 3], colors uint8 [V, 3], faces int32 [F, 3], so
+    load_ply -> Engine.upload_reference_mesh -> Engine.grid_from_mesh brings a mesh file in."""
+    with open(path, "rb") as fh:
+        data = fh.read()
+    fmt, elements, pos = _ply_header(data)
+    out = {}
+    tokens = data[pos:].split() if fmt == "ascii" else None
+    ti = 0
+    for name, count, props in elements:
+        is_list = [isinstance(t, tuple) for _, t in props]
+        if fmt == "ascii":
+            if not any(is_list):
+                n = len(props) * count
+                vals = np.array(tokens[ti:ti + n], np.float64).reshape(count, len(props))
+                ti += n
+                rec = {p: vals[:, k] for k, (p, _) in enumerate(props)}
+            else:
+                rec = {p: [] for p, _ in props}
+                for _ in range(count):
+                    for p, t in props:
+                        if isinstance(t, tuple):
+                            k = int(tokens[ti])
+                            rec[p].append([int(x) for x in tokens[ti + 1:ti + 1 + k]])
+                            ti += 1 + k
+                        else:
+                            rec[p].append(float(tokens[ti]))
+                            ti += 1
+        else:
+            if sum(is_list) > 1 or (any(is_list) and name != "face"):
+                raise ValueError(f"load_ply: element {name!r} with list properties is not supported in binary files")
+            # every list is read as a triangle (count 3); the counts are checked below, and the first count that is not 3 is read where
+            # it lies, because the records before it have the triangle size
+            dt = []
+            for p, t in props:
+                dt += [(p + "#n", "<" + t[0]), (p, "<" + t[1], 3)] if isinstance(t, tuple) else [(p, "<" + t)]
+            dt = np.dtype(dt)
+            if len(data) - pos < dt.itemsize * count:
+                raise ValueError(f"load_ply: element {name!r} is truncated or has faces that are not triangles")
+            arr = np.frombuffer(data, dt, count, pos)
+            pos += dt.itemsize * count
+            rec = {p: arr[p] for p, _ in props}
+            for p, t in props:
+                if isinstance(t, tuple) and count and (arr[p + "#n"] != 3).any():
+                    raise ValueError(f"load_ply: {name} {int(np.argmax(arr[p + '#n'] != 3))} is not a triangle")
+        out[name] = (count, rec)
+    if "vertex" not in out or not all(k in out["vertex"][1] for k in "xyz"):
+        raise ValueError("load_ply: no vertex element with x, y, z")
+    V, vr = out["vertex"]
+    verts = np.stack([np.asarray(vr[k], np.float64) for k in "xyz"], 1).astype(np.float32).reshape(V, 3)
+    cols = (np.stack([np.asarray(vr[k]) for k in ("red", "green", "blue")], 1).astype(np.uint8) if all(k in vr for k in ("red", "green", "blue"))
+            else np.zeros((V, 3), np.uint8))
+    F, fr = out.get("face", (0, {}))
+    key = "vertex_indices" if "vertex_indices" in fr else ("vertex_index" if "vertex_index" in fr else None)
+    if key is None:
+        raise ValueError("load_ply: no face element with a vertex_indices or vertex_index list")
+    lists = fr[key]
+    if fmt == "ascii":
+        bad = [i for i, lst in enumerate(lists) if len(lst) != 3]
+        if bad:
+            raise ValueError(f"load_ply: face {bad[0]} is not a triangle ({len(lists[bad[0]])} vertices)")
+    faces = np.asarray(lists, np.int64).reshape(F, 3)
+    if F and (faces.min() < 0 or faces.max() >= V):
+        raise ValueError("load_ply: a face index lies outside the vertices")
+    return dict(vertices=verts, colors=cols, faces=faces.astype(np.int32))
+
+
 # SDFVisualization::getOutputModes (src/sdf/visualization.cpp:72-89): settings key -> colour mode, in this order
 OUTPUT_MODE_KEYS = (
     ("output_mesh_normals", "normals"),
