@@ -293,6 +293,45 @@ int         i3d_grid_from_mesh(I3DEngine* e, const I3DGridFromMeshParams* params
  * closest point int8.  Either pointer may be NULL.  Fails before the first successful call. */
 int         i3d_debug_get_grid_from_mesh_voxels(I3DEngine* e, int32_t* face, int8_t* feature);
 
+/* ---- rasterizing the resident mesh into the keyframes and into new views (DESIGN.md §6w) ---- */
+uint64_t    i3d_sizeof_raster_params(void);
+uint64_t    i3d_sizeof_raster_camera(void);
+uint64_t    i3d_sizeof_raster_stats(void);
+uint64_t    i3d_sizeof_raster_info(void);
+/* every plane, vertex colours. */
+void        i3d_default_raster_params(I3DRasterParams* p);
+/* Rasterizes the resident mesh (the last extraction or simplification) into the frames ids[0..n) with the camera of the frame scans at
+ * the current pyramid level: W x H of the installed frames, the float R | t of i3d_render_keyframes and its intrinsics * pyr_scale with
+ * the five distortion coefficients.  Per pixel the nearest face of either orientation along the pixel's undistorted ray (a watertight
+ * ray-triangle test; equal depths go to the lowest face id), with the requested planes (I3D_RASTER_*) and the colour of
+ * params->color_source: the vertex colours, or the texture of i3d_bake_texture.  stats[n] (may be NULL) compares each view with its
+ * frame's depth and, with a colour source, its colour frame; *info (may be NULL) gets the counts and the device time per stage.  The
+ * rounding of every operation is stated in i3d_raster.cuh; the planes and statistics are bit-identical from run to run and do not depend
+ * on the batch.  The planes belong to the resident mesh and stay for i3d_download_raster: an extraction, a successful simplification, a
+ * change of the voxel set or of the frames drops them; a later camera change does not update them.  Reads the mesh, texture, frames and
+ * camera only.  Fails, writing nothing and leaving the previous planes, when world > 1, without a resident mesh with faces, for n <= 0,
+ * n > 65535, a NULL ids or an id out of [0, F), without frames or camera, for intrinsics (after pyr_scale) that are not finite with fx,
+ * fy > 0, distortion that is not finite, a bad plane mask or colour source, the texture source without a texture of the resident mesh,
+ * and a colour source without colour frames of the current frame size.  Device time: i3d_phase_ms("raster"), of which "raster_bin" (ray
+ * table and tile boxes), "raster_faces" (binning and triangle tests) and "raster_shade"; i3d_phase_count("raster_tests") = the
+ * ray-triangle tests. */
+int         i3d_rasterize_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DRasterParams* params, I3DRasterStats* stats,
+                                    I3DRasterInfo* info);
+/* The same into n new views of *camera (width x height, its own intrinsics and distortion) at pose_world_to_cam float [n][12] (R
+ * row-major | t, world -> camera); no statistics.  Fails as i3d_rasterize_keyframes where it applies, and for a NULL camera or pose, a
+ * pose entry that is not finite, and a width or height outside [1, I3D_RASTER_MAX_SIDE]. */
+int         i3d_rasterize_views(I3DEngine* e, int32_t n, const I3DRasterCamera* camera, const float* pose_world_to_cam,
+                                const I3DRasterParams* params, I3DRasterInfo* info);
+/* The planes of the last rasterization, [n][H][W]: depth float, face int32, bary float [2], normal float [3], rgb uint8 [3].  Any pointer
+ * may be NULL.  Fails for a plane that was not rendered and when no rasterization of the resident mesh exists. */
+int         i3d_download_raster(I3DEngine* e, float* depth, int32_t* face, float* bary, float* normal, uint8_t* rgb);
+/* on = 1 (default): faces are binned to 8 x 8 pixel tiles by their padded projected box; 0: every face goes to every tile and every
+ * pixel is tested.  The results are the same. */
+int         i3d_debug_set_raster_binning(I3DEngine* e, int on);
+/* views > 0: a rasterization runs in passes of at most that many views (the passes a large call splits into); 0 (default): as many
+ * as 2^27 (view, pixel) keys allow.  The results are the same.  Fails for views < 0. */
+int         i3d_debug_set_raster_batch(I3DEngine* e, int views);
+
 /* ---- rendering the surface into the keyframes (DESIGN.md §6m) ---- */
 uint64_t    i3d_sizeof_render_params(void);
 uint64_t    i3d_sizeof_render_stats(void);

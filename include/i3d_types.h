@@ -359,6 +359,59 @@ typedef struct I3DRenderStats
     double  photo_abs, photo_sq;          /* sum |I_r - I_obs|, sum (I_r - I_obs)^2 over the photometric pairs (I_obs: the frame's luminance) */
 } I3DRenderStats;
 
+/* ---- rasterizing the resident mesh into the keyframes and into new views (DESIGN.md §6w) ---- */
+/* Planes of a rasterization (bit mask of I3DRasterParams::planes). */
+enum
+{
+    I3D_RASTER_DEPTH = 1,                 /* float camera z of the nearest face, 0 = no hit */
+    I3D_RASTER_FACE = 2,                  /* int32 face id, -1 = no hit */
+    I3D_RASTER_BARY = 4,                  /* float [2]: barycentric weights (a, b) of v1, v2; w0 = (1 - a) - b; 0 = no hit */
+    I3D_RASTER_NORMAL = 8,                /* float [3]: unit face normal, world frame; (0,0,0) = no hit or zero area */
+    I3D_RASTER_RGB = 16,                  /* uint8 [3]: R, G, B of the colour source; 0 = no hit or no source */
+    I3D_RASTER_ALL = 31
+};
+/* Colour sources (I3DRasterParams::color_source) */
+enum { I3D_RASTER_COLOR_NONE = 0, I3D_RASTER_COLOR_VERTEX = 1, I3D_RASTER_COLOR_TEXTURE = 2 };
+#define I3D_RASTER_MAX_SIDE 8192          /* largest width or height of a new view */
+
+typedef struct I3DRasterParams
+{
+    int32_t planes;                       /* I3D_RASTER_* mask; 0 = statistics only (no plane buffers) */
+    int32_t color_source;                 /* I3D_RASTER_COLOR_* */
+    int32_t reserved[2];
+} I3DRasterParams;
+
+/* A camera of new views: intrinsics in pixels of a width x height image, and the five distortion coefficients (k1, k2, p1, p2, k3) */
+typedef struct I3DRasterCamera
+{
+    float   fx, fy, cx, cy;
+    float   distortion[5];
+    int32_t width, height;
+} I3DRasterCamera;
+
+/* Per-keyframe comparison of the rasterized mesh with the keyframe's depth and colour.  Depth sums are double in a fixed order, colour
+ * sums exact integers: a view's numbers depend only on that view. */
+typedef struct I3DRasterStats
+{
+    int64_t num_covered;                  /* pixels some face covers */
+    int64_t num_observed;                 /* pixels with frame depth > 0 */
+    int64_t depth_count;                  /* covered and observed */
+    int64_t color_count;                  /* covered, with a colour source (0 without one) */
+    double  depth_abs, depth_sq;          /* sum |e|, sum e^2 over the depth pairs, e = double(z_mesh) - double(z_frame), metres */
+    int64_t color_abs[3], color_sq[3];    /* per channel R, G, B: sum |e|, sum e^2 over the colour pairs, e = rendered - frame (uint8 units) */
+} I3DRasterStats;
+
+typedef struct I3DRasterInfo
+{
+    int64_t num_views, num_faces;         /* views of the call, faces of the resident mesh */
+    int64_t num_pairs;                    /* (8 x 8 tile, face) pairs the binning kept, over all views */
+    int64_t num_straddling;               /* (face, view) pairs with camera z <= 0 and > 0 among the vertices: binned to every tile */
+    int64_t num_behind;                   /* (face, view) pairs with every camera z <= 0: never hit, dropped */
+    int64_t num_tests;                    /* ray-triangle tests */
+    int64_t num_covered;                  /* covered pixels over all views */
+    double  ms_rays, ms_faces, ms_shade;  /* device time: ray table and tile boxes, face binning and tests, shading and statistics */
+} I3DRasterInfo;
+
 /* ---- tracking sensor frames against the surface: point-to-plane ICP over the depth pyramid (DESIGN.md §6n) ---- */
 /* Per-frame outcome of a tracking call (I3DTrackInfo::status). */
 enum

@@ -37,6 +37,7 @@
 #include "i3d_texture.h"
 #include "i3d_distance.h"
 #include "i3d_grid_from_mesh.h"
+#include "i3d_raster.h"
 #include "i3d_track.h"
 
 using namespace i3d;
@@ -173,6 +174,7 @@ struct I3DEngine
     DistanceState dist;                // reference mesh and distance results (i3d_distance.cu)
     GridFromMeshState gfm;             // the voxel grid from a mesh (i3d_grid_from_mesh.cu)
     RenderState render;                // keyframe renderer (i3d_render.cu)
+    RasterState raster;                // rasterizer of the resident mesh (i3d_raster.cu)
     TrackScratch track;                // frame-to-model tracker (i3d_render.cu)
     // shard (multi-GPU)
     int64_t shard_begin = 0, shard_end = -1;
@@ -275,10 +277,12 @@ int rebuild_topology(I3DEngine* e)
 }
 
 // Forgets everything derived from the voxel set: the per-voxel SH and the lighting estimate, the last iteration, the shard state and
-// range, the resident mesh and its texture, and the renderer's voxel box, brick bitmap and planes.  Every change of the voxel set calls it.
+// range, the resident mesh with its texture and raster planes, and the renderer's voxel box, brick bitmap and planes.  Every change of
+// the voxel set calls it.
 void forget_voxel_set(I3DEngine* e)
 {
     e->have_sh = false; e->sv_S = 0; e->sv_x = nullptr; e->have_iter = false; e->mesh.have_mesh = false; e->tex.have = false;
+    e->raster.have = false;
     e->render.box_ready = false; e->render.have_bricks = false; e->render.have_render = false;
     e->shard_ready = false; e->shard_begin = 0; e->shard_end = -1;
 }
@@ -308,12 +312,14 @@ int install_grid(I3DEngine* e, int64_t m, Fill&& fill)
 
 // Installs F frames of W x H as the engine's luminance / depth planes at scale pyr_scale: `fill` writes e->lum / e->depth (sized here) on
 // e->stream.  The one place that knows what a frame change invalidates: a new frame count drops the camera and the last iteration, a new
-// size drops the colour planes, the depth tiles of the frame culling are rebuilt, and the planes of the last render are dropped.
+// size drops the colour planes, the depth tiles of the frame culling are rebuilt, and the planes of the last render and of the last
+// keyframe rasterization are dropped.
 template <class Fill>
 void install_frames(I3DEngine* e, int32_t F, int32_t W, int32_t H, double pyr_scale, Fill&& fill)
 {
     const size_t cnt = static_cast<size_t>(F) * W * H;
     e->render.have_render = false;
+    if (e->raster.keyframes) e->raster.have = false;
     if (F != e->F) { e->have_cam = false; e->have_iter = false; }     // the unknown space of the last iteration no longer matches
     if (F != e->F || W != e->W || H != e->H) e->have_color = false;
     e->F = F; e->W = W; e->H = H; e->pyr_scale = pyr_scale;
@@ -983,7 +989,7 @@ int extract_mesh(I3DEngine* e, const I3DMeshParams& prm, int32_t color_mode, I3D
     g.rgb = color_mode == I3D_MESH_COLOR_VOXEL ? e->rgb.p : e->mesh.vis_rgb.p;
     g.nbr = e->nbr.p; g.keys = e->up_keys.p; g.vals = e->up_vals.p; g.mask = e->hash_cap - 1; g.voxel_size = e->voxel_size;
     std::string err;
-    e->tex.have = false;
+    e->tex.have = false; e->raster.have = false;
     if (mesh::extract(e->mesh, g, prm.largest_component_only != 0, info, err, e->stream)) return fail(e, "%s", err.c_str());
     return 0;
 }
@@ -1737,7 +1743,7 @@ int i3d_simplify_mesh(I3DEngine* e, const I3DSimplifyParams* params, I3DSimplify
     return guarded(e, [&]() {
         std::string err;
         if (mesh::simplify(e->mesh, cell, info, err, e->stream)) return fail(e, "%s", err.c_str());
-        e->tex.have = false;
+        e->tex.have = false; e->raster.have = false;
         return 0;
     });
 }
@@ -2028,6 +2034,148 @@ int i3d_debug_set_render_skip(I3DEngine* e, int on)
 {
     if (!e) return 1;
     e->render.skip = on != 0;
+    return 0;
+}
+
+// ---- rasterizing the resident mesh into the keyframes and into new views (i3d_raster.cuh, DESIGN.md §6w) ----------------
+uint64_t i3d_sizeof_raster_params(void) { return sizeof(I3DRasterParams); }
+uint64_t i3d_sizeof_raster_camera(void) { return sizeof(I3DRasterCamera); }
+uint64_t i3d_sizeof_raster_stats(void) { return sizeof(I3DRasterStats); }
+uint64_t i3d_sizeof_raster_info(void) { return sizeof(I3DRasterInfo); }
+
+void i3d_default_raster_params(I3DRasterParams* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    p->planes = I3D_RASTER_ALL; p->color_source = I3D_RASTER_COLOR_VERTEX;
+}
+
+// The refusals both raster calls share
+static int check_raster_call(I3DEngine* e, const char* who, int32_t n, const I3DRasterParams* params)
+{
+    if (!params) return fail(e, "%s: params is NULL", who);
+    if (e->world > 1) return fail(e, "%s: rasterization runs on one GPU (world = %d)", who, e->world);
+    if (!e->mesh.have_mesh) return fail(e, "%s: no mesh (call i3d_extract_mesh after the last change of the voxel set)", who);
+    if (e->mesh.mesh_F <= 0) return fail(e, "%s: the resident mesh has no faces", who);
+    if (n <= 0) return fail(e, "%s: need n > 0 views (n = %d)", who, n);
+    if (n > kRenderMaxViews) return fail(e, "%s: %d views exceed the %d of one call", who, n, kRenderMaxViews);
+    if (params->planes < 0 || params->planes > I3D_RASTER_ALL) return fail(e, "%s: planes must be a mask in [0, %d], got %d", who, I3D_RASTER_ALL, params->planes);
+    const int cs = params->color_source;
+    if (cs != I3D_RASTER_COLOR_NONE && cs != I3D_RASTER_COLOR_VERTEX && cs != I3D_RASTER_COLOR_TEXTURE)
+        return fail(e, "%s: color_source must be %d (none), %d (vertex) or %d (texture), got %d", who, I3D_RASTER_COLOR_NONE, I3D_RASTER_COLOR_VERTEX,
+                    I3D_RASTER_COLOR_TEXTURE, cs);
+    if (cs == I3D_RASTER_COLOR_TEXTURE && !e->tex.have)
+        return fail(e, "%s: the texture colour source needs a texture of the resident mesh (i3d_bake_texture after the last extraction or simplification)", who);
+    return 0;
+}
+
+// A camera the rasterizer can use: finite intrinsics with fx, fy > 0 and finite distortion
+static int check_raster_camera(I3DEngine* e, const char* who, const RenderCam& c)
+{
+    if (!(std::isfinite(c.fx) && c.fx > 0.0f && std::isfinite(c.fy) && c.fy > 0.0f && std::isfinite(c.cx) && std::isfinite(c.cy)))
+        return fail(e, "%s: the camera needs finite intrinsics with fx, fy > 0 (fx %g, fy %g, cx %g, cy %g)", who, c.fx, c.fy, c.cx, c.cy);
+    for (int k = 0; k < 5; ++k)
+        if (!std::isfinite(c.d[k])) return fail(e, "%s: distortion coefficient %d is not finite", who, k);
+    return 0;
+}
+
+static RastMesh raster_mesh(const I3DEngine* e, int color_source)
+{
+    RastMesh m{static_cast<int32_t>(e->mesh.mesh_F), e->mesh.mesh_vpos, e->mesh.mesh_vcol, e->mesh.mesh_faces, nullptr, 0, 0, 0, 0};
+    if (color_source == I3D_RASTER_COLOR_TEXTURE) { m.tex_rgb = e->tex.rgb.p; m.tex_W = e->tex.W; m.tex_H = e->tex.H; m.tex_S = e->tex.S; m.tex_cols = e->tex.cols; }
+    return m;
+}
+
+int i3d_rasterize_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DRasterParams* params, I3DRasterStats* stats, I3DRasterInfo* info)
+{
+    static const char* who = "i3d_rasterize_keyframes";
+    if (!e) return 1;
+    if (check_raster_call(e, who, n, params)) return 1;
+    if (!ids) return fail(e, "%s: ids is NULL", who);
+    if (e->F <= 0 || !e->have_cam) return fail(e, "%s: frames and camera must be uploaded first", who);
+    for (int32_t k = 0; k < n; ++k)
+        if (ids[k] < 0 || ids[k] >= e->F) return fail(e, "%s: frame id %d (entry %d) is out of range [0, %d)", who, ids[k], k, e->F);
+    if (params->color_source != I3D_RASTER_COLOR_NONE && !e->have_color)
+        return fail(e, "%s: a colour source needs colour frames of the current frame size (i3d_upload_color_frames)", who);
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const int F = e->F;
+        double hc9[9];
+        CK(cudaMemcpyAsync(hc9, e->cam + 6 * static_cast<size_t>(F), 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        const SelectCam sc = select_cam(e, hc9, 0.0f);
+        RenderCam cam;
+        cam.fx = sc.fx; cam.fy = sc.fy; cam.cx = sc.cx; cam.cy = sc.cy; cam.dist_zero = sc.dist_zero;
+        for (int k = 0; k < 5; ++k) cam.d[k] = sc.d[k];
+        if (check_raster_camera(e, who, cam)) return 1;
+        e->raster.rt.ensure(12 * static_cast<size_t>(F));
+        k_pose_mats<<<blocks_for(F, 64), 64, 0, st>>>(F, e->cam, e->raster.rt.p);
+        const RastCall c{n, e->W, e->H, ids, e->raster.rt.p, e->depth.p, params->color_source != I3D_RASTER_COLOR_NONE ? e->color.p : nullptr,
+                         params->planes, params->color_source, true};
+        raster::run(e->raster, e->timing, raster_mesh(e, params->color_source), cam, c, stats, info, st);
+        return 0;
+    });
+}
+
+int i3d_rasterize_views(I3DEngine* e, int32_t n, const I3DRasterCamera* camera, const float* pose_world_to_cam, const I3DRasterParams* params,
+                        I3DRasterInfo* info)
+{
+    static const char* who = "i3d_rasterize_views";
+    if (!e) return 1;
+    if (check_raster_call(e, who, n, params)) return 1;
+    if (!camera) return fail(e, "%s: camera is NULL", who);
+    if (!pose_world_to_cam) return fail(e, "%s: pose_world_to_cam is NULL", who);
+    if (camera->width < 1 || camera->width > I3D_RASTER_MAX_SIDE || camera->height < 1 || camera->height > I3D_RASTER_MAX_SIDE)
+        return fail(e, "%s: width and height must be in [1, %d], got %d x %d", who, I3D_RASTER_MAX_SIDE, camera->width, camera->height);
+    RenderCam cam;
+    cam.fx = camera->fx; cam.fy = camera->fy; cam.cx = camera->cx; cam.cy = camera->cy; cam.dist_zero = 1;
+    for (int k = 0; k < 5; ++k) { cam.d[k] = camera->distortion[k]; if (cam.d[k] != 0.0f) cam.dist_zero = 0; }
+    if (check_raster_camera(e, who, cam)) return 1;
+    for (int64_t k = 0; k < 12 * static_cast<int64_t>(n); ++k)
+        if (!std::isfinite(pose_world_to_cam[k])) return fail(e, "%s: pose entry %lld (view %lld) is not finite", who, static_cast<long long>(k), static_cast<long long>(k / 12));
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        e->raster.rt.ensure(12 * static_cast<size_t>(n));
+        CK(cudaMemcpyAsync(e->raster.rt.p, pose_world_to_cam, 12 * static_cast<size_t>(n) * sizeof(float), cudaMemcpyHostToDevice, st));
+        const RastCall c{n, camera->width, camera->height, nullptr, e->raster.rt.p, nullptr, nullptr, params->planes, params->color_source, false};
+        raster::run(e->raster, e->timing, raster_mesh(e, params->color_source), cam, c, nullptr, info, st);
+        return 0;
+    });
+}
+
+int i3d_download_raster(I3DEngine* e, float* depth, int32_t* face, float* bary, float* normal, uint8_t* rgb)
+{
+    static const char* who = "i3d_download_raster";
+    if (!e) return 1;
+    if (!e->raster.have) return fail(e, "%s: no rasterization of the resident mesh (call i3d_rasterize_keyframes or i3d_rasterize_views)", who);
+    const struct { const void* dst; int bit; const char* name; } want[5] = {{depth, I3D_RASTER_DEPTH, "depth"}, {face, I3D_RASTER_FACE, "face"},
+        {bary, I3D_RASTER_BARY, "bary"}, {normal, I3D_RASTER_NORMAL, "normal"}, {rgb, I3D_RASTER_RGB, "rgb"}};
+    for (const auto& w : want)
+        if (w.dst && !(e->raster.planes & w.bit)) return fail(e, "%s: the %s plane was not rendered", who, w.name);
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t img = static_cast<size_t>(e->raster.n) * e->raster.W * e->raster.H;
+        if (depth) CK(cudaMemcpyAsync(depth, e->raster.depth.p, img * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (face) CK(cudaMemcpyAsync(face, e->raster.face.p, img * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        if (bary) CK(cudaMemcpyAsync(bary, e->raster.bary.p, 2 * img * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (normal) CK(cudaMemcpyAsync(normal, e->raster.normal.p, 3 * img * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (rgb) CK(cudaMemcpyAsync(rgb, e->raster.rgb.p, 3 * img, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    });
+}
+
+int i3d_debug_set_raster_binning(I3DEngine* e, int on)
+{
+    if (!e) return 1;
+    e->raster.binning = on != 0;
+    return 0;
+}
+
+int i3d_debug_set_raster_batch(I3DEngine* e, int views)
+{
+    if (!e) return 1;
+    if (views < 0) return fail(e, "i3d_debug_set_raster_batch: views must be >= 0, got %d", views);
+    e->raster.max_batch = views;
     return 0;
 }
 

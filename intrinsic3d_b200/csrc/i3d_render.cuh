@@ -20,6 +20,7 @@
 #include <limits.h>
 
 #include "i3d_grid.cuh"
+#include "i3d_pixel_ray.cuh"
 #include "i3d_render.h"
 #include "i3d_vis.cuh"
 
@@ -235,23 +236,9 @@ __device__ __forceinline__ void rd_march(G rg, RenderCam cam, RenderViews rv)
     {
         const int f = rv.ids[view];
         const float* Rt = rv.Rt + 12 * f;
-        // pixel -> normalised camera coordinates; the lens distortion inverted by kUndistortIters fixed-point steps of the forward model
-        const float xd = FD(FS(__int2float_rn(u), cam.cx), cam.fx), yd = FD(FS(__int2float_rn(v), cam.cy), cam.fy);
-        float x = xd, y = yd;
-        if (!cam.dist_zero)
-        {
-            for (int it = 0; it < kUndistortIters; ++it)
-            {
-                const float r2 = FA(FM(x, x), FM(y, y));
-                const float r4 = FM(r2, r2);
-                const float r6 = FM(r4, r2);
-                const float dc = FA(FA(FA(1.0f, FM(cam.d[0], r2)), FM(cam.d[1], r4)), FM(cam.d[2], r6));
-                const float tx = FA(FM(FM(FM(2.0f, cam.d[3]), x), y), FM(cam.d[4], FA(r2, FM(FM(2.0f, x), x))));
-                const float ty = FA(FM(FM(FM(2.0f, cam.d[4]), xd), y), FM(cam.d[3], FA(r2, FM(FM(2.0f, y), y))));    // y' uses the distorted x'
-                x = FD(FS(xd, tx), dc);
-                y = FD(FS(yd, ty), dc);
-            }
-        }
+        // pixel -> normalised camera coordinates (i3d_pixel_ray.cuh)
+        float x, y;
+        pixel_ray(cam, u, v, x, y);
         // world ray: o = -R^T t, direction R^T (x, y, 1) normalised; camera z = s / |R^T (x, y, 1)|
         float o[3], dn[3];
 #pragma unroll

@@ -41,7 +41,7 @@ void bake(TextureState& ts, const TexMesh& m, const TexLayout& L, const FrameVie
     CK(cudaGetLastError());
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, ts.ev[0], ts.ev[1]));
-    ts.W = L.W; ts.H = L.H; ts.F = m.F;
+    ts.W = L.W; ts.H = L.H; ts.S = L.S; ts.cols = L.cols; ts.F = m.F;
     ts.have = true;
     if (info)
     {

@@ -28,7 +28,7 @@ struct TextureState
     cudaEvent_t ev[2] = {};
     bool ev_ready = false;
     bool have = false;                  // a texture of the current resident mesh
-    int32_t W = 0, H = 0; int64_t F = 0;
+    int32_t W = 0, H = 0, S = 0, cols = 0; int64_t F = 0;    // atlas size, layout and face count of the texture
 };
 
 namespace texture

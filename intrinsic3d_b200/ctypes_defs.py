@@ -369,6 +369,59 @@ class I3DRenderStats(C.Structure, _Dictable):
     ]
 
 
+# I3D_RASTER_* plane bits and colour sources of include/i3d_types.h
+RASTER_PLANES = {"depth": 1, "face": 2, "bary": 4, "normal": 8, "rgb": 16}
+RASTER_COLORS = {None: 0, "vertex": 1, "texture": 2}
+
+
+class I3DRasterParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("planes", C.c_int32),
+        ("color_source", C.c_int32),
+        ("reserved", C.c_int32 * 2),
+    ]
+
+
+class I3DRasterCamera(C.Structure, _Dictable):
+    _fields_ = [
+        ("fx", C.c_float),
+        ("fy", C.c_float),
+        ("cx", C.c_float),
+        ("cy", C.c_float),
+        ("distortion", C.c_float * 5),
+        ("width", C.c_int32),
+        ("height", C.c_int32),
+    ]
+
+
+class I3DRasterStats(C.Structure, _Dictable):
+    _fields_ = [
+        ("num_covered", C.c_int64),
+        ("num_observed", C.c_int64),
+        ("depth_count", C.c_int64),
+        ("color_count", C.c_int64),
+        ("depth_abs", C.c_double),
+        ("depth_sq", C.c_double),
+        ("color_abs", C.c_int64 * 3),
+        ("color_sq", C.c_int64 * 3),
+    ]
+
+
+class I3DRasterInfo(C.Structure, _Dictable):
+    _fields_ = [
+        ("num_views", C.c_int64),
+        ("num_faces", C.c_int64),
+        ("num_pairs", C.c_int64),
+        ("num_straddling", C.c_int64),
+        ("num_behind", C.c_int64),
+        ("num_tests", C.c_int64),
+        ("num_covered", C.c_int64),
+        ("ms_rays", C.c_double),
+        ("ms_faces", C.c_double),
+        ("ms_shade", C.c_double),
+    ]
+
+
 TRACK_LEVELS = 4          # entries of I3DTrackParams::iterations
 TRACK_STATUS = {0: "tracked", 1: "too few correspondences", 2: "not positive definite", 3: "non-finite", 4: "anchored"}
 

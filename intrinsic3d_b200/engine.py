@@ -11,9 +11,10 @@ import os
 
 import numpy as np
 
-from .ctypes_defs import (DISTANCE_MAX_THRESHOLDS, GRID_FROM_MESH_SOURCES, RENDER_PLANES, I3DDistanceInfo, I3DDistanceParams, I3DGridFromMeshInfo,
-                          I3DGridFromMeshParams, I3DFusionCamera, I3DFusionParams, I3DIterInfo, I3DLightingInfo, I3DLightingParams, I3DMeshInfo,
-                          I3DMeshParams, I3DParams, I3DRenderParams, I3DRenderStats, I3DSimplifyInfo, I3DSimplifyParams, I3DTextureInfo,
+from .ctypes_defs import (DISTANCE_MAX_THRESHOLDS, GRID_FROM_MESH_SOURCES, RASTER_COLORS, RASTER_PLANES, RENDER_PLANES, I3DDistanceInfo,
+                          I3DDistanceParams, I3DGridFromMeshInfo, I3DGridFromMeshParams, I3DFusionCamera, I3DFusionParams, I3DIterInfo,
+                          I3DLightingInfo, I3DLightingParams, I3DMeshInfo, I3DMeshParams, I3DParams, I3DRasterCamera, I3DRasterInfo,
+                          I3DRasterParams, I3DRasterStats, I3DRenderParams, I3DRenderStats, I3DSimplifyInfo, I3DSimplifyParams, I3DTextureInfo,
                           I3DTextureParams, I3DTrackColorInfo, I3DTrackColorParams, I3DTrackInfo, I3DTrackParams, TRACK_LEVELS)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -42,6 +43,9 @@ EXPORTED_SYMBOLS = [
     "i3d_debug_get_grid_from_mesh_voxels",
     "i3d_sizeof_render_params", "i3d_sizeof_render_stats", "i3d_default_render_params", "i3d_render_keyframes", "i3d_download_render",
     "i3d_debug_set_render_skip",
+    "i3d_sizeof_raster_params", "i3d_sizeof_raster_camera", "i3d_sizeof_raster_stats", "i3d_sizeof_raster_info", "i3d_default_raster_params",
+    "i3d_rasterize_keyframes", "i3d_rasterize_views", "i3d_download_raster", "i3d_debug_set_raster_binning",
+    "i3d_debug_set_raster_batch",
     "i3d_sizeof_track_params", "i3d_sizeof_track_info", "i3d_default_track_params", "i3d_track_sensor_frames", "i3d_debug_get_track_system",
     "i3d_debug_get_track_planes", "i3d_fusion_track_sensor_frames", "i3d_fusion_track_and_integrate_sensor",
     "i3d_sizeof_track_color_params", "i3d_sizeof_track_color_info", "i3d_default_track_color_params", "i3d_track_sensor_frames_rgbd",
@@ -153,6 +157,26 @@ def load_library():
     L.i3d_render_keyframes.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(I3DRenderParams), C.POINTER(I3DRenderStats)]
     L.i3d_download_render.restype = C.c_int
     L.i3d_download_render.argtypes = [C.c_void_p] + [C.POINTER(C.c_float)] * 5
+    for fn in (L.i3d_sizeof_raster_params, L.i3d_sizeof_raster_camera, L.i3d_sizeof_raster_stats, L.i3d_sizeof_raster_info):
+        fn.restype = C.c_uint64
+    if (L.i3d_sizeof_raster_params() != C.sizeof(I3DRasterParams) or L.i3d_sizeof_raster_camera() != C.sizeof(I3DRasterCamera)
+            or L.i3d_sizeof_raster_stats() != C.sizeof(I3DRasterStats) or L.i3d_sizeof_raster_info() != C.sizeof(I3DRasterInfo)):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (raster structs)")
+    L.i3d_default_raster_params.restype = None
+    L.i3d_default_raster_params.argtypes = [C.POINTER(I3DRasterParams)]
+    L.i3d_rasterize_keyframes.restype = C.c_int
+    L.i3d_rasterize_keyframes.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(I3DRasterParams), C.POINTER(I3DRasterStats),
+                                          C.POINTER(I3DRasterInfo)]
+    L.i3d_rasterize_views.restype = C.c_int
+    L.i3d_rasterize_views.argtypes = [C.c_void_p, C.c_int32, C.POINTER(I3DRasterCamera), C.POINTER(C.c_float), C.POINTER(I3DRasterParams),
+                                      C.POINTER(I3DRasterInfo)]
+    L.i3d_download_raster.restype = C.c_int
+    L.i3d_download_raster.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                      C.POINTER(C.c_uint8)]
+    L.i3d_debug_set_raster_binning.restype = C.c_int
+    L.i3d_debug_set_raster_binning.argtypes = [C.c_void_p, C.c_int]
+    L.i3d_debug_set_raster_batch.restype = C.c_int
+    L.i3d_debug_set_raster_batch.argtypes = [C.c_void_p, C.c_int]
     L.i3d_sizeof_track_params.restype = C.c_uint64
     L.i3d_sizeof_track_info.restype = C.c_uint64
     if L.i3d_sizeof_track_params() != C.sizeof(I3DTrackParams) or L.i3d_sizeof_track_info() != C.sizeof(I3DTrackInfo):
@@ -600,6 +624,69 @@ class Engine:
     def set_render_skip(self, on: bool):
         """True (default): the renderer jumps over empty 8^3 bricks; False: it evaluates every lattice sample (same results)."""
         self._check(self.L.i3d_debug_set_render_skip(self.h, C.c_int(1 if on else 0)))
+
+    # ---- rasterizing the resident mesh into the keyframes and into new views (DESIGN.md §6w) ---------------------------------
+    @staticmethod
+    def _raster_params(color, planes):
+        if color not in RASTER_COLORS:
+            raise ValueError(f"color must be one of None, 'vertex', 'texture', got {color!r}")
+        mask = 0
+        for p in planes:
+            if p not in RASTER_PLANES:
+                raise ValueError(f"plane must be one of {sorted(RASTER_PLANES)}, got {p!r}")
+            mask |= RASTER_PLANES[p]
+        return I3DRasterParams(mask, RASTER_COLORS[color])
+
+    def _download_raster(self, n, W, H, mask):
+        shapes = dict(depth=((n, H, W), np.float32), face=((n, H, W), np.int32), bary=((n, H, W, 2), np.float32),
+                      normal=((n, H, W, 3), np.float32), rgb=((n, H, W, 3), np.uint8))
+        ctype = dict(depth=C.c_float, face=C.c_int32, bary=C.c_float, normal=C.c_float, rgb=C.c_uint8)
+        out = {p: np.empty(*shapes[p]) for p in RASTER_PLANES if RASTER_PLANES[p] & mask}
+        if out:
+            self._check(self.L.i3d_download_raster(self.h, *(_p(out.get(p), ctype[p]) for p in RASTER_PLANES)))
+        return out
+
+    def rasterize_keyframes(self, ids, color="vertex", planes=("depth", "face", "bary", "normal", "rgb")):
+        """Rasterizes the resident mesh (the last extract_mesh or simplify_mesh) into the frames `ids` with the engine's current camera,
+        at the size of the installed frames (DESIGN.md §6w).  color: "vertex" (the vertex colours), "texture" (the last bake_texture of
+        the resident mesh) or None.  Returns a dict with the requested planes [n, H, W] (depth float32, 0 = no face; face int32, -1 = no
+        face; bary float32 [.., 2]; normal float32 [.., 3], world frame; rgb uint8 [.., 3]), stats: one dict per view (I3DRasterStats:
+        covered / observed pixels, depth pairs with sum |e| and e^2 in metres, colour pairs with per-channel integer sums of |e| and e^2
+        against the colour frame) and info (I3DRasterInfo).  planes=() gives the statistics only."""
+        prm = self._raster_params(color, planes)
+        ids, n = self._ids(ids)
+        stats = (I3DRasterStats * max(n, 1))()
+        info = I3DRasterInfo()
+        self._check(self.L.i3d_rasterize_keyframes(self.h, C.c_int32(n), _p(ids, C.c_int32), C.byref(prm), stats, C.byref(info)))
+        W, H = self.frame_size
+        out = self._download_raster(n, W, H, prm.planes)
+        out["stats"] = [stats[i].as_dict() for i in range(n)]
+        out["info"] = info
+        return out
+
+    def rasterize_views(self, camera: dict, poses, color="vertex", planes=("depth", "face", "bary", "normal", "rgb")):
+        """Rasterizes the resident mesh into new views: camera a dict with fx, fy, cx, cy (pixels), width, height and optionally
+        distortion (k1, k2, p1, p2, k3); poses float32 [n, 12] (R row-major | t, world -> camera).  Returns the planes of
+        rasterize_keyframes and info; no statistics."""
+        prm = self._raster_params(color, planes)
+        poses = np.ascontiguousarray(poses, np.float32).reshape(-1, 12)
+        n = int(poses.shape[0])
+        d = [float(x) for x in camera.get("distortion", (0.0,) * 5)]
+        cam = I3DRasterCamera(float(camera["fx"]), float(camera["fy"]), float(camera["cx"]), float(camera["cy"]), (C.c_float * 5)(*d),
+                              int(camera["width"]), int(camera["height"]))
+        info = I3DRasterInfo()
+        self._check(self.L.i3d_rasterize_views(self.h, C.c_int32(n), C.byref(cam), _p(poses, C.c_float), C.byref(prm), C.byref(info)))
+        out = self._download_raster(n, cam.width, cam.height, prm.planes)
+        out["info"] = info
+        return out
+
+    def set_raster_binning(self, on: bool):
+        """True (default): faces are binned to 8 x 8 pixel tiles; False: every face is tested against every pixel (same results)."""
+        self._check(self.L.i3d_debug_set_raster_binning(self.h, C.c_int(1 if on else 0)))
+
+    def set_raster_batch(self, views: int):
+        """views > 0: rasterize in passes of at most that many views; 0: as large as memory for 2^27 keys allows (same results)."""
+        self._check(self.L.i3d_debug_set_raster_batch(self.h, C.c_int(int(views))))
 
     # ---- keyframe selection and the RGB-D pyramid (KeyframeSelection::estimateBlur, Pyramid::create) ----------------------
     def keyframe_scores(self, bgr):
