@@ -230,6 +230,8 @@ void        i3d_default_texture_params(I3DTextureParams* p);
  * operation and the property that a bilinear lookup inside a face's UV triangle reads only texels of that face are in
  * i3d_texture.cuh.  pose_world_to_cam: float [F][12] (R row-major | t), or NULL for the engine's camera, as in i3d_recompute_colors.
  * The atlas and the per-corner UVs stay on the device until i3d_download_texture; *info (may be NULL) gets the counts and device time.
+ * The bake also records which texels a keyframe observed (for i3d_decompose_texture's fallback count), a frame scan that stops at the
+ * first observation; its device time is i3d_phase_ms("texture_observed"), not part of ms_bake.
  * The texture belongs to the resident mesh: an extraction, a successful simplification or a change of the voxel set drops it; a later
  * change of the camera or the frames does not update it.  Reads the mesh, frames, colour frames and camera only.  Fails, writing
  * nothing and leaving the previous texture, when world > 1, without a resident mesh with faces, without frames, camera or colour frames
@@ -240,6 +242,31 @@ int         i3d_bake_texture(I3DEngine* e, const I3DTextureParams* params, const
 /* The baked texture: rgb uint8 [H][W][3] in R, G, B order (W, H: info->atlas_width / atlas_height), uv float [F][3][2], per face corner
  * (u, v) as an OBJ reads them (v up).  Either pointer may be NULL.  Fails without a texture of the resident mesh. */
 int         i3d_download_texture(I3DEngine* e, uint8_t* rgb, float* uv);
+
+/* ---- albedo and shading of the baked texture, and relighting (DESIGN.md §6x) ---- */
+uint64_t    i3d_sizeof_sh_lighting(void);
+uint64_t    i3d_sizeof_intrinsic_texture_params(void);
+uint64_t    i3d_sizeof_intrinsic_texture_info(void);
+/* source I3D_SH_ESTIMATE, sh 0. */
+void        i3d_default_sh_lighting(I3DShLighting* p);
+/* lighting: i3d_default_sh_lighting; min_shading 0.05. */
+void        i3d_default_intrinsic_texture_params(I3DIntrinsicTextureParams* p);
+/* Splits the texture of the resident mesh (the last i3d_bake_texture) into albedo and shading under params->lighting.  Every texel a
+ * face owns is taken at the bake's point P and face normal n; s = sh . basis(n) with the lighting's SH at P; the texel is lit iff n != 0
+ * and s > min_shading, and then albedo = (c / 255) / s per channel of its baked colour c (the bake's fallback texels included), else 0.
+ * The rounding of every operation is in i3d_texture.cuh.  The albedo [H][W][3] and shading [H][W] atlases stay on the device until
+ * i3d_download_intrinsic_texture and are the source of I3D_RASTER_COLOR_RELIT; *info (may be NULL) gets the counts, the albedo range and
+ * the device time.  The decomposition belongs to the texture: a new bake, or anything that drops the texture, drops it; a later lighting
+ * estimate does not update it.  Fails, writing nothing and leaving the texture and any previous decomposition, when world > 1, without
+ * a texture of the resident mesh, for a bad source, for I3D_SH_ESTIMATE without a lighting estimate of the current voxel set, for an
+ * I3D_SH_GLOBAL sh that is not finite, and for a min_shading that is not finite or < 0. */
+int         i3d_decompose_texture(I3DEngine* e, const I3DIntrinsicTextureParams* params, I3DIntrinsicTextureInfo* info);
+/* The last decomposition: albedo float [H][W][3] (R, G, B), shading float [H][W] (0 where no face owns the texel or its normal is 0).
+ * Either pointer may be NULL.  Fails without a decomposition of the resident mesh's texture. */
+int         i3d_download_intrinsic_texture(I3DEngine* e, float* albedo, float* shading);
+/* The lighting of I3D_RASTER_COLOR_RELIT (engine state; default I3D_SH_ESTIMATE, read when a rasterization runs).  Fails, keeping the
+ * previous lighting, for a NULL lighting, a bad source and an I3D_SH_GLOBAL sh that is not finite. */
+int         i3d_set_relight(I3DEngine* e, const I3DShLighting* lighting);
 
 /* ---- distance from the resident mesh to a reference surface (DESIGN.md §6u) ---- */
 uint64_t    i3d_sizeof_distance_params(void);
@@ -304,7 +331,8 @@ void        i3d_default_raster_params(I3DRasterParams* p);
  * the current pyramid level: W x H of the installed frames, the float R | t of i3d_render_keyframes and its intrinsics * pyr_scale with
  * the five distortion coefficients.  Per pixel the nearest face of either orientation along the pixel's undistorted ray (a watertight
  * ray-triangle test; equal depths go to the lowest face id), with the requested planes (I3D_RASTER_*) and the colour of
- * params->color_source: the vertex colours, or the texture of i3d_bake_texture.  stats[n] (may be NULL) compares each view with its
+ * params->color_source: the vertex colours, the texture of i3d_bake_texture, or its decomposition relit (I3D_RASTER_COLOR_RELIT: the
+ * bilinear albedo times the shading at the face normal under the lighting of i3d_set_relight).  stats[n] (may be NULL) compares each view with its
  * frame's depth and, with a colour source, its colour frame; *info (may be NULL) gets the counts and the device time per stage.  The
  * rounding of every operation is stated in i3d_raster.cuh; the planes and statistics are bit-identical from run to run and do not depend
  * on the batch.  The planes belong to the resident mesh and stay for i3d_download_raster: an extraction, a successful simplification, a
@@ -312,7 +340,8 @@ void        i3d_default_raster_params(I3DRasterParams* p);
  * camera only.  Fails, writing nothing and leaving the previous planes, when world > 1, without a resident mesh with faces, for n <= 0,
  * n > 65535, a NULL ids or an id out of [0, F), without frames or camera, for intrinsics (after pyr_scale) that are not finite with fx,
  * fy > 0, distortion that is not finite, a bad plane mask or colour source, the texture source without a texture of the resident mesh,
- * and a colour source without colour frames of the current frame size.  Device time: i3d_phase_ms("raster"), of which "raster_bin" (ray
+ * the relit source without a decomposition of that texture or, under I3D_SH_ESTIMATE, without a lighting estimate of the current voxel
+ * set, and a colour source without colour frames of the current frame size.  Device time: i3d_phase_ms("raster"), of which "raster_bin" (ray
  * table and tile boxes), "raster_faces" (binning and triangle tests) and "raster_shade"; i3d_phase_count("raster_tests") = the
  * ray-triangle tests. */
 int         i3d_rasterize_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DRasterParams* params, I3DRasterStats* stats,

@@ -231,6 +231,37 @@ typedef struct I3DTextureInfo
     double  ms_bake;                      /* device time of the bake and the UVs (CUDA events) */
 } I3DTextureInfo;
 
+/* ---- albedo and shading of the baked texture, and relighting (DESIGN.md §6x) ---- */
+/* Lighting sources (I3DShLighting::source) */
+enum { I3D_SH_ESTIMATE = 0, I3D_SH_GLOBAL = 1 };
+
+/* A second-order SH lighting: the subvolume SH of the last i3d_estimate_lighting (blended at each point as the shading colour modes
+ * blend it), or the same nine coefficients everywhere */
+typedef struct I3DShLighting
+{
+    int32_t source;                       /* I3D_SH_* */
+    int32_t reserved;
+    float   sh[9];                        /* I3D_SH_GLOBAL: the coefficients, in the order of the lighting estimate; ignored otherwise */
+} I3DShLighting;
+
+typedef struct I3DIntrinsicTextureParams
+{
+    I3DShLighting lighting;
+    float   min_shading;                  /* a texel is lit iff its face normal is not 0 and its shading s > min_shading (finite, >= 0) */
+    int32_t reserved;
+} I3DIntrinsicTextureParams;
+
+typedef struct I3DIntrinsicTextureInfo
+{
+    int32_t atlas_width, atlas_height;    /* texels, as the texture's */
+    int64_t num_texels_owned;             /* texels some face owns */
+    int64_t num_texels_lit;               /* owned texels with a non-zero face normal and s > min_shading: albedo = colour / 255 / s */
+    int64_t num_texels_unlit;             /* the other owned texels: albedo 0 */
+    int64_t num_texels_lit_fallback;      /* lit texels the bake coloured from the vertex colours (no keyframe observed them) */
+    float   albedo_min[3], albedo_max[3]; /* per channel R, G, B over the lit texels (0 without one) */
+    double  ms_decompose;                 /* device time (CUDA events) */
+} I3DIntrinsicTextureInfo;
+
 /* ---- distance from the resident mesh to a reference mesh (DESIGN.md §6u) ---- */
 #define I3D_DISTANCE_MAX_THRESHOLDS 8
 #define I3D_DISTANCE_MAX_SAMPLES_PER_EDGE 16
@@ -371,7 +402,8 @@ enum
     I3D_RASTER_ALL = 31
 };
 /* Colour sources (I3DRasterParams::color_source) */
-enum { I3D_RASTER_COLOR_NONE = 0, I3D_RASTER_COLOR_VERTEX = 1, I3D_RASTER_COLOR_TEXTURE = 2 };
+enum { I3D_RASTER_COLOR_NONE = 0, I3D_RASTER_COLOR_VERTEX = 1, I3D_RASTER_COLOR_TEXTURE = 2,
+       I3D_RASTER_COLOR_RELIT = 3 /* albedo of i3d_decompose_texture x shading under the lighting of i3d_set_relight */ };
 #define I3D_RASTER_MAX_SIDE 8192          /* largest width or height of a new view */
 
 typedef struct I3DRasterParams

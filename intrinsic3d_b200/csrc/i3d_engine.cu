@@ -175,6 +175,7 @@ struct I3DEngine
     GridFromMeshState gfm;             // the voxel grid from a mesh (i3d_grid_from_mesh.cu)
     RenderState render;                // keyframe renderer (i3d_render.cu)
     RasterState raster;                // rasterizer of the resident mesh (i3d_raster.cu)
+    I3DShLighting relight{I3D_SH_ESTIMATE, 0, {}};     // lighting of the relit colour source (i3d_set_relight)
     TrackScratch track;                // frame-to-model tracker (i3d_render.cu)
     // shard (multi-GPU)
     int64_t shard_begin = 0, shard_end = -1;
@@ -972,6 +973,32 @@ int check_color_mode(I3DEngine* e, const char* who, int32_t mode)
     if ((mode == I3D_MESH_COLOR_SHADING_SV || mode == I3D_MESH_COLOR_SHADING_SV_CONST) && (e->sv_S <= 0 || !e->sv_x))
         return fail(e, "%s: the shading modes need a lighting estimate of the current grid (i3d_estimate_lighting)", who);
     return 0;
+}
+
+// A lighting the decomposition and the relit raster can use: a known source, finite global coefficients, and for the estimate a lighting
+// estimate of the current voxel set (the shading modes' rule)
+int check_sh_lighting(I3DEngine* e, const char* who, const I3DShLighting& l)
+{
+    if (l.source != I3D_SH_ESTIMATE && l.source != I3D_SH_GLOBAL)
+        return fail(e, "%s: the lighting source must be %d (estimate) or %d (global), got %d", who, I3D_SH_ESTIMATE, I3D_SH_GLOBAL, l.source);
+    if (l.source == I3D_SH_GLOBAL)
+    {
+        for (int k = 0; k < 9; ++k)
+            if (!std::isfinite(l.sh[k])) return fail(e, "%s: sh[%d] is not finite", who, k);
+    }
+    else if (e->sv_S <= 0 || !e->sv_x)
+        return fail(e, "%s: the estimate lighting needs a lighting estimate of the current grid (i3d_estimate_lighting)", who);
+    return 0;
+}
+
+// The device form of a lighting checked by check_sh_lighting
+ShLight sh_light(const I3DEngine* e, const I3DShLighting& l)
+{
+    ShLight L{};
+    L.global = l.source == I3D_SH_GLOBAL ? 1 : 0;
+    for (int k = 0; k < 9; ++k) L.sh[k] = l.sh[k];
+    if (!L.global) { L.sg = e->sv_grid; L.sub_sh = e->sv_x; L.S = e->sv_S; }
+    return L;
 }
 
 // The colour pass of a mode other than I3D_MESH_COLOR_VOXEL into e->mesh.vis_rgb; the geometric modes read the sdf the mesh is cut from
@@ -1787,7 +1814,7 @@ int i3d_bake_texture(I3DEngine* e, const I3DTextureParams* params, const float* 
         if (pose_world_to_cam) CK(cudaMemcpyAsync(e->tex.rt.p, pose_world_to_cam, 12 * static_cast<size_t>(F) * sizeof(float), cudaMemcpyHostToDevice, st));
         else k_pose_mats<<<blocks_for(F, 64), 64, 0, st>>>(F, e->cam, e->tex.rt.p);
         const TexMesh m{static_cast<int32_t>(e->mesh.mesh_F), e->mesh.mesh_vpos, e->mesh.mesh_vcol, e->mesh.mesh_faces};
-        texture::bake(e->tex, m, L, e->frame_view(), e->color.p, select_cam(e, hc9, params->max_occlusion_distance), cull_view(e, nullptr), K, info, st);
+        texture::bake(e->tex, e->timing, m, L, e->frame_view(), e->color.p, select_cam(e, hc9, params->max_occlusion_distance), cull_view(e, nullptr), K, info, st);
         return 0;
     });
 }
@@ -1803,6 +1830,70 @@ int i3d_download_texture(I3DEngine* e, uint8_t* rgb, float* uv)
         CK(cudaStreamSynchronize(st));
         return 0;
     });
+}
+
+// ---- albedo and shading of the baked texture, and relighting (i3d_texture.cuh, i3d_raster.cuh, DESIGN.md §6x) ----------
+uint64_t i3d_sizeof_sh_lighting(void) { return sizeof(I3DShLighting); }
+uint64_t i3d_sizeof_intrinsic_texture_params(void) { return sizeof(I3DIntrinsicTextureParams); }
+uint64_t i3d_sizeof_intrinsic_texture_info(void) { return sizeof(I3DIntrinsicTextureInfo); }
+
+void i3d_default_sh_lighting(I3DShLighting* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    p->source = I3D_SH_ESTIMATE;
+}
+
+void i3d_default_intrinsic_texture_params(I3DIntrinsicTextureParams* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    i3d_default_sh_lighting(&p->lighting);
+    p->min_shading = 0.05f;
+}
+
+int i3d_decompose_texture(I3DEngine* e, const I3DIntrinsicTextureParams* params, I3DIntrinsicTextureInfo* info)
+{
+    static const char* who = "i3d_decompose_texture";
+    if (!e) return 1;
+    if (!params) return fail(e, "%s: params is NULL", who);
+    if (e->world > 1) return fail(e, "%s: the decomposition runs on one GPU (world = %d)", who, e->world);
+    if (!e->tex.have) return fail(e, "%s: no texture of the resident mesh (call i3d_bake_texture after the last extraction or simplification)", who);
+    if (check_sh_lighting(e, who, params->lighting)) return 1;
+    if (!std::isfinite(params->min_shading) || params->min_shading < 0.0f)
+        return fail(e, "%s: min_shading must be finite and >= 0, got %g", who, static_cast<double>(params->min_shading));
+    return guarded(e, [&]() {
+        const TexMesh m{static_cast<int32_t>(e->mesh.mesh_F), e->mesh.mesh_vpos, e->mesh.mesh_vcol, e->mesh.mesh_faces};
+        texture::decompose(e->tex, m, sh_light(e, params->lighting), params->min_shading, info, e->stream);
+        return 0;
+    });
+}
+
+int i3d_download_intrinsic_texture(I3DEngine* e, float* albedo, float* shading)
+{
+    if (!e) return 1;
+    if (!(e->tex.have && e->tex.intrinsic))
+        return fail(e, "i3d_download_intrinsic_texture: no decomposition of the resident mesh's texture (call i3d_decompose_texture after the last bake)");
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const size_t texels = static_cast<size_t>(e->tex.W) * e->tex.H;
+        if (albedo) CK(cudaMemcpyAsync(albedo, e->tex.albedo.p, 3 * texels * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (shading) CK(cudaMemcpyAsync(shading, e->tex.shading.p, texels * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    });
+}
+
+int i3d_set_relight(I3DEngine* e, const I3DShLighting* lighting)
+{
+    static const char* who = "i3d_set_relight";
+    if (!e) return 1;
+    if (!lighting) return fail(e, "%s: lighting is NULL", who);
+    if (lighting->source != I3D_SH_ESTIMATE && lighting->source != I3D_SH_GLOBAL)
+        return fail(e, "%s: source must be %d (estimate) or %d (global), got %d", who, I3D_SH_ESTIMATE, I3D_SH_GLOBAL, lighting->source);
+    if (lighting->source == I3D_SH_GLOBAL)
+        for (int k = 0; k < 9; ++k)
+            if (!std::isfinite(lighting->sh[k])) return fail(e, "%s: sh[%d] is not finite", who, k);
+    e->relight = *lighting;
+    return 0;
 }
 
 // ---- distance from the resident mesh to a reference mesh (i3d_distance.cuh, DESIGN.md §6u) -----------
@@ -2060,11 +2151,14 @@ static int check_raster_call(I3DEngine* e, const char* who, int32_t n, const I3D
     if (n > kRenderMaxViews) return fail(e, "%s: %d views exceed the %d of one call", who, n, kRenderMaxViews);
     if (params->planes < 0 || params->planes > I3D_RASTER_ALL) return fail(e, "%s: planes must be a mask in [0, %d], got %d", who, I3D_RASTER_ALL, params->planes);
     const int cs = params->color_source;
-    if (cs != I3D_RASTER_COLOR_NONE && cs != I3D_RASTER_COLOR_VERTEX && cs != I3D_RASTER_COLOR_TEXTURE)
-        return fail(e, "%s: color_source must be %d (none), %d (vertex) or %d (texture), got %d", who, I3D_RASTER_COLOR_NONE, I3D_RASTER_COLOR_VERTEX,
-                    I3D_RASTER_COLOR_TEXTURE, cs);
+    if (cs != I3D_RASTER_COLOR_NONE && cs != I3D_RASTER_COLOR_VERTEX && cs != I3D_RASTER_COLOR_TEXTURE && cs != I3D_RASTER_COLOR_RELIT)
+        return fail(e, "%s: color_source must be %d (none), %d (vertex), %d (texture) or %d (relit), got %d", who, I3D_RASTER_COLOR_NONE,
+                    I3D_RASTER_COLOR_VERTEX, I3D_RASTER_COLOR_TEXTURE, I3D_RASTER_COLOR_RELIT, cs);
     if (cs == I3D_RASTER_COLOR_TEXTURE && !e->tex.have)
         return fail(e, "%s: the texture colour source needs a texture of the resident mesh (i3d_bake_texture after the last extraction or simplification)", who);
+    if (cs == I3D_RASTER_COLOR_RELIT && !(e->tex.have && e->tex.intrinsic))
+        return fail(e, "%s: the relit colour source needs a decomposition of the resident mesh's texture (i3d_decompose_texture after the last bake)", who);
+    if (cs == I3D_RASTER_COLOR_RELIT && check_sh_lighting(e, who, e->relight)) return 1;
     return 0;
 }
 
@@ -2081,8 +2175,19 @@ static int check_raster_camera(I3DEngine* e, const char* who, const RenderCam& c
 static RastMesh raster_mesh(const I3DEngine* e, int color_source)
 {
     RastMesh m{static_cast<int32_t>(e->mesh.mesh_F), e->mesh.mesh_vpos, e->mesh.mesh_vcol, e->mesh.mesh_faces, nullptr, 0, 0, 0, 0};
-    if (color_source == I3D_RASTER_COLOR_TEXTURE) { m.tex_rgb = e->tex.rgb.p; m.tex_W = e->tex.W; m.tex_H = e->tex.H; m.tex_S = e->tex.S; m.tex_cols = e->tex.cols; }
+    if (color_source == I3D_RASTER_COLOR_TEXTURE || color_source == I3D_RASTER_COLOR_RELIT)
+    {
+        m.tex_rgb = e->tex.rgb.p; m.tex_W = e->tex.W; m.tex_H = e->tex.H; m.tex_S = e->tex.S; m.tex_cols = e->tex.cols;
+    }
     return m;
+}
+
+// The relit source's inputs of a call (validated by check_raster_call)
+static void raster_relight(const I3DEngine* e, int color_source, RastCall& c)
+{
+    if (color_source != I3D_RASTER_COLOR_RELIT) return;
+    c.albedo = e->tex.albedo.p;
+    c.light = sh_light(e, e->relight);
 }
 
 int i3d_rasterize_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I3DRasterParams* params, I3DRasterStats* stats, I3DRasterInfo* info)
@@ -2109,8 +2214,9 @@ int i3d_rasterize_keyframes(I3DEngine* e, int32_t n, const int32_t* ids, const I
         if (check_raster_camera(e, who, cam)) return 1;
         e->raster.rt.ensure(12 * static_cast<size_t>(F));
         k_pose_mats<<<blocks_for(F, 64), 64, 0, st>>>(F, e->cam, e->raster.rt.p);
-        const RastCall c{n, e->W, e->H, ids, e->raster.rt.p, e->depth.p, params->color_source != I3D_RASTER_COLOR_NONE ? e->color.p : nullptr,
-                         params->planes, params->color_source, true};
+        RastCall c{n, e->W, e->H, ids, e->raster.rt.p, e->depth.p, params->color_source != I3D_RASTER_COLOR_NONE ? e->color.p : nullptr,
+                   params->planes, params->color_source, true};
+        raster_relight(e, params->color_source, c);
         raster::run(e->raster, e->timing, raster_mesh(e, params->color_source), cam, c, stats, info, st);
         return 0;
     });
@@ -2136,7 +2242,8 @@ int i3d_rasterize_views(I3DEngine* e, int32_t n, const I3DRasterCamera* camera, 
         cudaStream_t st = e->stream;
         e->raster.rt.ensure(12 * static_cast<size_t>(n));
         CK(cudaMemcpyAsync(e->raster.rt.p, pose_world_to_cam, 12 * static_cast<size_t>(n) * sizeof(float), cudaMemcpyHostToDevice, st));
-        const RastCall c{n, camera->width, camera->height, nullptr, e->raster.rt.p, nullptr, nullptr, params->planes, params->color_source, false};
+        RastCall c{n, camera->width, camera->height, nullptr, e->raster.rt.p, nullptr, nullptr, params->planes, params->color_source, false};
+        raster_relight(e, params->color_source, c);
         raster::run(e->raster, e->timing, raster_mesh(e, params->color_source), cam, c, nullptr, info, st);
         return 0;
     });

@@ -165,14 +165,15 @@ struct SubvolGrid
 // float trilinear weights of the 8 surrounding subvolumes at p / size - 0.5, missing cubes and zero weights skipped, the sub_sh [S][9]
 // vectors summed in double (product and sum rounded separately), times double(1.0f / sum of the weights).  avg must be zero on entry;
 // it stays zero when no weight is left.
-__device__ __forceinline__ void svsh_blend(const GridView& g, int64_t v, const SubvolGrid& sg, const double* __restrict__ sub_sh, double (&avg)[9])
+// The core takes the world point as coord(d), d = 0, 1, 2: svsh_blend_at the point p itself, svsh_blend voxel v's FM(float(c), voxel_size).
+template <class Coord>
+__device__ __forceinline__ void svsh_blend_core(Coord&& coord, const SubvolGrid& sg, const double* __restrict__ sub_sh, double (&avg)[9])
 {
-    const int c[3] = {g.x[v], g.y[v], g.z[v]};
     int v0[3]; float wg[3];
 #pragma unroll
     for (int d = 0; d < 3; ++d)
     {
-        const float pos = FS(FM(FM(static_cast<float>(c[d]), g.voxel_size), sg.inv_size), 0.5f);     // pointToIndexCoord
+        const float pos = FS(FM(coord(d), sg.inv_size), 0.5f);     // pointToIndexCoord
         const float fl = floorf(pos);
         v0[d] = static_cast<int>(fl);
         wg[d] = FS(pos, fl);
@@ -201,6 +202,57 @@ __device__ __forceinline__ void svsh_blend(const GridView& g, int64_t v, const S
 #pragma unroll
         for (int k = 0; k < 9; ++k) avg[k] *= inv;
     }
+}
+
+__device__ __forceinline__ void svsh_blend(const GridView& g, int64_t v, const SubvolGrid& sg, const double* __restrict__ sub_sh, double (&avg)[9])
+{
+    const int c[3] = {g.x[v], g.y[v], g.z[v]};
+    svsh_blend_core([&](int d) { return FM(static_cast<float>(c[d]), g.voxel_size); }, sg, sub_sh, avg);
+}
+
+__device__ __forceinline__ void svsh_blend_at(const float (&p)[3], const SubvolGrid& sg, const double* __restrict__ sub_sh, double (&avg)[9])
+{
+    svsh_blend_core([&](int d) { return p[d]; }, sg, sub_sh, avg);
+}
+
+// sh . basis(n) of Shading::computeShading on a unit normal: the basis in the order of Q9 computed in float, the dot product summed
+// k = 0..8 left to right (vis_shading multiplies it by the albedo)
+__device__ __forceinline__ float sh_dot(const float n[3], const float sh[9])
+{
+    const float x = n[0], y = n[1], z = n[2];
+    const float b[9] = {1.0f, y, z, x, FM(x, y), FM(y, z), FA(FS(-FM(x, x), FM(y, y)), FM(2.0f, FM(z, z))), FM(x, z), FS(FM(x, x), FM(y, y))};
+    float d = FM(sh[0], b[0]);
+#pragma unroll
+    for (int k = 1; k < 9; ++k) d = FA(d, FM(sh[k], b[k]));
+    return d;
+}
+
+// A lighting of the texture decomposition and the relit raster (I3DShLighting): global = the nine floats sh; otherwise the subvolume SH
+// sub_sh [S][9] of the last estimate on the table sg, taken as it is when S = 1 and blended at the point by svsh_blend_at otherwise, then
+// rounded to float
+struct ShLight
+{
+    int global;
+    float sh[9];
+    SubvolGrid sg;
+    const double* sub_sh;
+    int S;
+};
+
+__device__ __forceinline__ void sh_light_at(const ShLight& L, const float (&p)[3], float (&sh)[9])
+{
+    if (L.global)
+    {
+#pragma unroll
+        for (int k = 0; k < 9; ++k) sh[k] = L.sh[k];
+        return;
+    }
+    double avg[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) avg[k] = L.S == 1 ? L.sub_sh[k] : 0.0;
+    if (L.S != 1) svsh_blend_at(p, L.sg, L.sub_sh, avg);
+#pragma unroll
+    for (int k = 0; k < 9; ++k) sh[k] = __double2float_rn(avg[k]);
 }
 
 } // namespace i3d

@@ -80,7 +80,9 @@ void run(RasterState& rs, Timing& tm, const RastMesh& m, const RenderCam& cam, c
                 sh.out_normal = (c.planes & I3D_RASTER_NORMAL) ? rs.normal.p : nullptr;
                 sh.out_rgb = (c.planes & I3D_RASTER_RGB) ? rs.rgb.p : nullptr;
                 sh.partials = rs.partials.p; sh.counts = rs.counts.p;
-                k_rast_shade<<<dim3(SX, SY, nb), dim3(kRenderTile, kRenderTile), 0, st>>>(m, sh);
+                if (c.color_source == I3D_RASTER_COLOR_RELIT)
+                    k_rast_shade<true, RastRelit><<<dim3(SX, SY, nb), dim3(kRenderTile, kRenderTile), 0, st>>>(m, sh, RastRelit{c.albedo, c.light});
+                else k_rast_shade<false><<<dim3(SX, SY, nb), dim3(kRenderTile, kRenderTile), 0, st>>>(m, sh);
                 k_rast_sums<<<blocks_for(static_cast<size_t>(nb) * kRastSums), kThreads, 0, st>>>(nb, SX * SY, rs.partials.p,
                                                                                                    rs.sums.p + static_cast<size_t>(v0) * kRastSums);
             }

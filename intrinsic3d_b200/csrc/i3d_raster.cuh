@@ -25,6 +25,10 @@
  *            face's cell-local UV corners (tex_corner) blended as u = (w u0 + a u1) + b u2 (v alike), and interp_u8 of the atlas at
  *            ((col S + u) - 1/2, (row S + v) - 1/2), cell c = face / 2 at column c % cols, row c / cols.  The clamped point lies in the
  *            face's UV triangle, so by the atlas's no-bleed property (i3d_texture.cuh) the lookup reads only texels the face owns.
+ *   relit    (DESIGN.md §6x) the texture source's (a, b) clamping and (X, Y); A = interp_f32 of the decomposition's albedo atlas at (X, Y)
+ *            (the same taps and weights as interp_u8, so the no-bleed property holds); P = (w0 p0 + a p1) + b p2 at the clamped (a, b);
+ *            s' = sh_dot(normal, SH(P)) under the lighting of i3d_set_relight (sh_light_at); per channel trunc(clamp(((A s') 255) + 1/2,
+ *            0, 255)); 0 for a zero normal.
  *
  * Statistics (keyframes): per pixel covered = hit, observed = frame depth > 0; a depth pair (covered and observed) adds |e| and e^2,
  * e = double(t) - double(z_frame), summed in double by a fixed tree over the 16 x 16 block and then the blocks in order (k_rast_sums),
@@ -74,6 +78,13 @@ struct RastShade
     float* out_depth; int32_t* out_face; float* out_bary; float* out_normal; uint8_t* out_rgb;
     double* partials;                   // [batch][tiles16][kRastSums]
     unsigned long long* counts;         // [n][kRastCounts] of the call
+};
+
+// The relit colour source's inputs: the albedo atlas [tex_H][tex_W][3] of the texture's decomposition and the lighting of i3d_set_relight
+struct RastRelit
+{
+    const float* albedo;
+    ShLight light;
 };
 
 __device__ __forceinline__ float rast_sel(const float (&a)[3], int k) { return k == 0 ? a[0] : (k == 1 ? a[1] : a[2]); }
@@ -299,6 +310,24 @@ __global__ void __launch_bounds__(kThreads) k_rast_faces(RastMesh m, RastBin rb)
     }
 }
 
+// The texture lookup of a hit of face f at (a, b): (a, b) clamped as tex_bary does into (ac, bc), the face's cell-local UV corners blended
+// at w = (1 - ac) - bc, and the atlas position (X, Y) of the bilinear lookup (header)
+__device__ __forceinline__ void rast_tex_lookup(const RastMesh& m, int f, float a, float b, float& ac, float& bc, float& X, float& Y)
+{
+    ac = a < 0.0f ? 0.0f : a; bc = b < 0.0f ? 0.0f : b;
+    const float s = FA(ac, bc);
+    if (s > 1.0f) { ac = FD(ac, s); bc = FD(bc, s); }
+    const float w = FS(FS(1.0f, ac), bc);
+    const bool fb = f & 1;
+    float u0, v0, u1, v1, u2, v2;
+    tex_corner(m.tex_S, fb, 0, u0, v0); tex_corner(m.tex_S, fb, 1, u1, v1); tex_corner(m.tex_S, fb, 2, u2, v2);
+    const float u = FA(FA(FM(w, u0), FM(ac, u1)), FM(bc, u2));
+    const float v = FA(FA(FM(w, v0), FM(ac, v1)), FM(bc, v2));
+    const int cell = f >> 1;
+    X = FS(FA(static_cast<float>((cell % m.tex_cols) * m.tex_S), u), 0.5f);
+    Y = FS(FA(static_cast<float>((cell / m.tex_cols) * m.tex_S), v), 0.5f);
+}
+
 // The colour of a hit of face f at (a, b) from the colour source (header), R, G, B
 __device__ __forceinline__ void rast_color(const RastMesh& m, int source, int f, float a, float b, uint8_t (&c)[3])
 {
@@ -318,7 +347,7 @@ __device__ __forceinline__ void rast_color(const RastMesh& m, int source, int f,
         }
         return;
     }
-    // texture
+    // texture (the statements of rast_tex_lookup, kept inline: calling it renumbers this instance's registers)
     float ac = a < 0.0f ? 0.0f : a, bc = b < 0.0f ? 0.0f : b;
     const float s = FA(ac, bc);
     if (s > 1.0f) { ac = FD(ac, s); bc = FD(bc, s); }
@@ -335,8 +364,63 @@ __device__ __forceinline__ void rast_color(const RastMesh& m, int source, int f,
     for (int k = 0; k < 3; ++k) c[k] = interp_u8(m.tex_rgb, m.tex_W, m.tex_H, X, Y, k);
 }
 
-// One thread per pixel, 16 x 16 blocks, views of the batch in gridDim.z: the planes and the statistics of the winners
-__global__ void __launch_bounds__(kRenderTile * kRenderTile) k_rast_shade(RastMesh m, RastShade rs)
+// interp_u8's bilinear lookup on a float [h][w][3] image, without the truncation: taps (x0, y0), (x0, y1), (x1, y0), (x1, y1) with
+// x0 = floor(x), x1 = x0 + 1 (y alike), weights w00 = (1 - fx)(1 - fy), w01 = (1 - fx) fy, w10 = fx (1 - fy), w11 = fx fy, fx = x - x0,
+// out-of-image taps at weight 0; sum of w v over the taps with w > 0 in that order, over ((w00 + w10) + w01) + w11; 0 when that is 0
+__device__ __forceinline__ float interp_f32(const float* __restrict__ img, int w, int h, float x, float y, int channel)
+{
+    const float fx0 = floorf(x), fy0 = floorf(y);
+    const int x0 = static_cast<int>(fx0), y0 = static_cast<int>(fy0);
+    const int x1 = x0 + 1, y1 = y0 + 1;
+    float x1w = FS(x, fx0), y1w = FS(y, fy0);
+    float x0w = FS(1.0f, x1w), y0w = FS(1.0f, y1w);
+    if (x0 < 0 || x0 >= w) x0w = 0.0f;
+    if (x1 < 0 || x1 >= w) x1w = 0.0f;
+    if (y0 < 0 || y0 >= h) y0w = 0.0f;
+    if (y1 < 0 || y1 >= h) y1w = 0.0f;
+    const float w00 = FM(x0w, y0w), w10 = FM(x1w, y0w), w01 = FM(x0w, y1w), w11 = FM(x1w, y1w);
+    const float sum_w = FA(FA(FA(w00, w10), w01), w11);
+    float sum = 0.0f;
+    if (w00 > 0.0f) sum = FA(sum, FM(img[(static_cast<size_t>(y0) * w + x0) * 3 + channel], w00));
+    if (w01 > 0.0f) sum = FA(sum, FM(img[(static_cast<size_t>(y1) * w + x0) * 3 + channel], w01));
+    if (w10 > 0.0f) sum = FA(sum, FM(img[(static_cast<size_t>(y0) * w + x1) * 3 + channel], w10));
+    if (w11 > 0.0f) sum = FA(sum, FM(img[(static_cast<size_t>(y1) * w + x1) * 3 + channel], w11));
+    if (!(sum_w > 0.0f)) return 0.0f;
+    return FD(sum, sum_w);
+}
+
+// The relit colour of a hit of face f at (a, b) with unit face normal nrm (header): the albedo A at the texture source's lookup
+// position, s' = sh_dot(nrm, SH(P)) at P = (w0 p0 + a p1) + b p2 of the clamped (a, b), per channel trunc(clamp((A s') 255 + 1/2, 0, 255));
+// 0 for a zero normal
+__device__ __forceinline__ void rast_relit(const RastMesh& m, const RastRelit& rl, int f, float a, float b, const float (&nrm)[3], uint8_t (&c)[3])
+{
+    if (nrm[0] == 0.0f && nrm[1] == 0.0f && nrm[2] == 0.0f) { c[0] = 0; c[1] = 0; c[2] = 0; return; }
+    float ac, bc, X, Y;
+    rast_tex_lookup(m, f, a, b, ac, bc, X, Y);
+    const int3 fv = m.faces[f];
+    const float* p0 = m.vpos + 3 * static_cast<size_t>(fv.x);
+    const float* p1 = m.vpos + 3 * static_cast<size_t>(fv.y);
+    const float* p2 = m.vpos + 3 * static_cast<size_t>(fv.z);
+    const float w0 = FS(FS(1.0f, ac), bc);
+    float P[3], sh[9];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) P[k] = FA(FA(FM(w0, p0[k]), FM(ac, p1[k])), FM(bc, p2[k]));
+    sh_light_at(rl.light, P, sh);
+    const float s = sh_dot(nrm, sh);
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+    {
+        float x = FA(FM(FM(interp_f32(rl.albedo, m.tex_W, m.tex_H, X, Y, k), s), 255.0f), 0.5f);
+        x = x < 0.0f ? 0.0f : (x > 255.0f ? 255.0f : x);
+        c[k] = static_cast<uint8_t>(__float2int_rz(x));
+    }
+}
+
+// One thread per pixel, 16 x 16 blocks, views of the batch in gridDim.z: the planes and the statistics of the winners.  RELIT: the
+// relit colour source (rast_relit) with its inputs as one more parameter (Relit = RastRelit), in an instance of its own so that the
+// other sources' instance keeps its parameters and code.
+template <bool RELIT, class... Relit>
+__global__ void __launch_bounds__(kRenderTile * kRenderTile) k_rast_shade(RastMesh m, RastShade rs, Relit... relit)
 {
     __shared__ double red[kRastSums][kRenderTile * kRenderTile];
     __shared__ unsigned s_cnt[kRenderTile * kRenderTile / 32][kRastCounts];
@@ -376,7 +460,8 @@ __global__ void __launch_bounds__(kRenderTile * kRenderTile) k_rast_shade(RastMe
                 const float n2 = FS(FM(e1[0], e2[1]), FM(e1[1], e2[0]));
                 const float len = __fsqrt_rn(FA(FA(FM(n0, n0), FM(n1, n1)), FM(n2, n2)));
                 if (len > 0.0f) { nrm[0] = FD(n0, len); nrm[1] = FD(n1, len); nrm[2] = FD(n2, len); }
-                if (rs.color_source != I3D_RASTER_COLOR_NONE) rast_color(m, rs.color_source, face, a, b, c);
+                if constexpr (RELIT) rast_relit(m, relit..., face, a, b, nrm, c);
+                else if (rs.color_source != I3D_RASTER_COLOR_NONE) rast_color(m, rs.color_source, face, a, b, c);
             }
             else { face = -1; t = 0.0f; a = 0.0f; b = 0.0f; }
         }

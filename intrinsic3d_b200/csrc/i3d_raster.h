@@ -36,6 +36,8 @@ struct RastCall
     const float* depth; const uint8_t* bgr;
     int planes, color_source;
     bool stats;
+    const float* albedo;                // relit: the albedo atlas of the texture's decomposition (tex_W x tex_H of the mesh)
+    ShLight light;                      // relit: the lighting
 };
 
 // Rasterizer state of an engine: the planes of the last call (they belong to the resident mesh; the engine drops them), scratch that

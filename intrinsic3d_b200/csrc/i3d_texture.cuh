@@ -76,6 +76,8 @@ k_tex_bake(TexMesh m, TexLayout L, FrameView fr, const uint8_t* __restrict__ bgr
     float pt[3] = {0.0f, 0.0f, 0.0f}, nrm[3] = {0.0f, 0.0f, 0.0f};
     if (in_range)
     {
+        // tex_texel_point (i3d_texture_layout.cuh) restated inline, operation for operation: calling it renumbers this kernel's registers.
+        // An edit of either copy must be made in both (k_tex_observed and k_tex_decompose use the helper).
         const int3 fv = m.faces[face];
         float a, b;
         tex_bary(S, face & 1, static_cast<float>(i) + 0.5f, static_cast<float>(j) + 0.5f, a, b);
@@ -192,6 +194,139 @@ k_tex_bake(TexMesh m, TexLayout L, FrameView fr, const uint8_t* __restrict__ bgr
     }
     if (wsum > 0.0f) { const float s = FD(255.0f, wsum); c3[0] = FM(c3[0], s); c3[1] = FM(c3[1], s); c3[2] = FM(c3[2], s); }
     out[0] = static_cast<uint8_t>(__float2int_rz(c3[0])); out[1] = static_cast<uint8_t>(__float2int_rz(c3[1])); out[2] = static_cast<uint8_t>(__float2int_rz(c3[2]));
+}
+
+// Texel t of the bake's enumeration (cell-major, row-major inside a cell) of the atlas L of F faces: its local (i, j), the face that owns
+// it (-1: none, or t out of range) and its index in the atlas [H][W] (0 for t out of range)
+__device__ __forceinline__ int64_t tex_texel(const TexLayout& L, int32_t F, int64_t t, int& i, int& j, int& face)
+{
+    const int S = L.S;
+    const int64_t total = static_cast<int64_t>(L.cols) * L.rows * S * S;
+    int64_t c = 0;
+    i = 0; j = 0; face = -1;
+    if (t >= total) return 0;
+    c = t / (S * S);
+    const int r = static_cast<int>(t - c * S * S);
+    j = r / S; i = r - j * S;
+    if (i + j + 1 < S && 2 * c < F) face = static_cast<int>(2 * c);
+    else if (i + j + 1 > S && 2 * c + 1 < F) face = static_cast<int>(2 * c + 1);
+    return ((c / L.cols) * S + j) * L.W + (c % L.cols) * S + i;
+}
+
+// One thread per texel of the bake's enumeration: observed [H][W] = 1 where some frame observes the texel (a weight > 0 at its point and
+// normal, the test k_tex_bake counts), 0 for the fallback texels and the texels no face owns.  Same candidate frames as the bake, visited
+// in the same order; a texel stops at its first observation.
+__global__ void __launch_bounds__(kThreads) k_tex_observed(TexMesh m, TexLayout L, FrameView fr, const float* __restrict__ Rt, SelectCam cam,
+                                                           CullView cull, uint8_t* __restrict__ observed)
+{
+    extern __shared__ float s_rt[];     // [F][12]
+    for (int i = threadIdx.x; i < 12 * fr.F; i += blockDim.x) s_rt[i] = Rt[i];
+    __syncthreads();
+    const int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    const bool live = t < static_cast<int64_t>(L.W) * L.H;
+    int i, j, face;
+    const int64_t at = tex_texel(L, m.F, t, i, j, face);
+    const bool in_range = face >= 0;
+    if (__ballot_sync(0xffffffffu, in_range) == 0u)
+    {
+        if (live) observed[at] = 0;
+        return;
+    }
+    float pt[3] = {0.0f, 0.0f, 0.0f}, nrm[3] = {0.0f, 0.0f, 0.0f};
+    if (in_range) tex_texel_point(L.S, face & 1, i, j, m.vpos, m.faces[face], pt, nrm);
+    __shared__ unsigned s_mask[kThreads / 32][kCullMaxWords];
+    unsigned* wmask = s_mask[threadIdx.x >> 5];
+    const bool culling = frame_candidates(pt, in_range, s_rt, fr, cam, cull, wmask);
+    const size_t img = static_cast<size_t>(fr.W) * fr.H;
+    const int nwords = (fr.F + 31) / 32;
+    bool obs = false;
+#pragma unroll 1
+    for (int jw = 0; jw < nwords && in_range && !obs; ++jw)
+    {
+        unsigned mk = culling ? wmask[jw] : 0xffffffffu;
+#pragma unroll 1
+        while (mk && !obs)
+        {
+            const int f = 32 * jw + __ffs(mk) - 1;
+            mk &= mk - 1;
+            if (f >= fr.F) continue;
+            const ObsProbe p = obs_probe(pt, s_rt + 12 * f, cam, fr.depth + img * f, fr.W, fr.H);
+            obs = obs_finish(p, nrm, s_rt + 12 * f, cam) > 0.0f;
+        }
+    }
+    if (live) observed[at] = obs ? 1 : 0;
+}
+
+// The decomposition of one texture (texture::decompose): the atlas rgb [H][W][3] and observation flags of its bake, the lighting, the
+// threshold, the outputs albedo [H][W][3] and shading [H][W], counts [3] (owned, lit, lit fallback texels) and range [6] (float bits of
+// the per-channel minimum, then maximum, of the albedo over the lit texels)
+struct TexDecompose
+{
+    const uint8_t* rgb; const uint8_t* observed;
+    ShLight light;
+    float min_shading;
+    float* albedo; float* shading;
+    unsigned long long* counts; unsigned* range;
+};
+
+// One thread per texel (i3d_texture.cuh header, DESIGN.md §6x): at the texel's point P and face normal n of the bake, s = sh_dot(n, SH(P));
+// a texel is lit iff n != 0 and s > min_shading, and then A_k = (c_k / 255) / s of its baked colour c; unlit texels get A = 0.  shading
+// holds s for every owned texel with n != 0 and 0 elsewhere.
+__global__ void __launch_bounds__(kThreads) k_tex_decompose(TexMesh m, TexLayout L, TexDecompose d)
+{
+    const int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    const bool live = t < static_cast<int64_t>(L.W) * L.H;
+    int i, j, face;
+    const int64_t at = tex_texel(L, m.F, t, i, j, face);
+    const bool own = face >= 0;
+    float A[3] = {0.0f, 0.0f, 0.0f}, s = 0.0f;
+    bool lit = false, fallback = false;
+    if (own)
+    {
+        float pt[3], nrm[3] = {0.0f, 0.0f, 0.0f};
+        tex_texel_point(L.S, face & 1, i, j, m.vpos, m.faces[face], pt, nrm);
+        const bool nz = !(nrm[0] == 0.0f && nrm[1] == 0.0f && nrm[2] == 0.0f);
+        if (nz)
+        {
+            float sh[9];
+            sh_light_at(d.light, pt, sh);
+            s = sh_dot(nrm, sh);
+        }
+        lit = nz && s > d.min_shading;
+        if (lit)
+        {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) A[k] = FD(FD(static_cast<float>(d.rgb[3 * at + k]), 255.0f), s);
+            fallback = d.observed[at] == 0;
+        }
+    }
+    if (live)
+    {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) d.albedo[3 * at + k] = A[k];
+        d.shading[at] = s;
+    }
+    // per-warp counts and range (A >= +0, so the float bits order like the floats) -> one atomic each
+    const unsigned n_own = __popc(__ballot_sync(0xffffffffu, own)), n_lit = __popc(__ballot_sync(0xffffffffu, lit));
+    const unsigned n_fb = __popc(__ballot_sync(0xffffffffu, fallback));
+    unsigned lo[3], hi[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+    {
+        lo[k] = __reduce_min_sync(0xffffffffu, lit ? __float_as_uint(A[k]) : 0xffffffffu);
+        hi[k] = __reduce_max_sync(0xffffffffu, lit ? __float_as_uint(A[k]) : 0u);
+    }
+    if ((threadIdx.x & 31) == 0 && n_own)
+    {
+        atomicAdd(d.counts, static_cast<unsigned long long>(n_own));
+        if (n_lit)
+        {
+            atomicAdd(d.counts + 1, static_cast<unsigned long long>(n_lit));
+            if (n_fb) atomicAdd(d.counts + 2, static_cast<unsigned long long>(n_fb));
+#pragma unroll
+            for (int k = 0; k < 3; ++k) { atomicMin(d.range + k, lo[k]); atomicMax(d.range + 3 + k, hi[k]); }
+        }
+    }
 }
 
 // The per-corner OBJ UVs: uv [F][3][2]

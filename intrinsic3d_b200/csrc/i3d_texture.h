@@ -21,7 +21,9 @@ struct TexLayout { int S, cols, rows, W, H; };
 struct TexMesh { int32_t F; const float* vpos; const uint8_t* vcol; const int3* faces; };
 
 // The texture of the resident mesh: the atlas [H][W][3] and the UVs [F][3][2] of the last bake, the world -> camera poses [F][12] it
-// used (written by the engine), the device counters of k_tex_bake and the event pair of its device time
+// used (written by the engine), the device counters of k_tex_bake and the event pair of its device time and of the decomposition's
+// device time.  The texture's decomposition (texture::decompose) lives here too: the bake's per-texel observation flags, the albedo and
+// shading atlases and their counters; it is valid while `intrinsic` and `have` both hold, so whatever drops the texture drops it.
 struct TextureState
 {
     Dev<uint8_t> rgb; Dev<float> uv; Dev<float> rt; Dev<unsigned long long> counts;
@@ -29,6 +31,10 @@ struct TextureState
     bool ev_ready = false;
     bool have = false;                  // a texture of the current resident mesh
     int32_t W = 0, H = 0, S = 0, cols = 0; int64_t F = 0;    // atlas size, layout and face count of the texture
+    Dev<uint8_t> observed;              // [H][W]: 1 = the bake coloured the texel from the keyframes (k_tex_observed)
+    Dev<float> albedo, shading;         // [H][W][3], [H][W] of the last decomposition
+    Dev<unsigned long long> dcounts; Dev<unsigned> drange;
+    bool intrinsic = false;             // a decomposition of the texture
 };
 
 namespace texture
@@ -37,9 +43,13 @@ namespace texture
 bool layout(int64_t F, int S, TexLayout& L);
 // Bakes the texture of mesh m (F > 0 faces) with layout L from the frames fr, the colour frames bgr [F][H][W][3] and the poses in ts.rt
 // (the caller validated every argument and wrote ts.rt); the result becomes ts's texture.  info (may be nullptr) gets the counts and
-// device time.
-void bake(TextureState& ts, const TexMesh& m, const TexLayout& L, const FrameView& fr, const uint8_t* bgr, const SelectCam& cam, const CullView& cull,
-          int K, I3DTextureInfo* info, cudaStream_t st);
+// device time; the observation flags of the decomposition (k_tex_observed) are timed apart as phase "texture_observed".
+void bake(TextureState& ts, Timing& tm, const TexMesh& m, const TexLayout& L, const FrameView& fr, const uint8_t* bgr, const SelectCam& cam,
+          const CullView& cull, int K, I3DTextureInfo* info, cudaStream_t st);
+// Decomposes the texture of ts (the caller checked that it exists and belongs to mesh m, and validated the lighting and min_shading)
+// into albedo and shading under `light`; the result becomes ts's decomposition.  info (may be nullptr) gets the counts, the albedo
+// range and the device time.
+void decompose(TextureState& ts, const TexMesh& m, const ShLight& light, float min_shading, I3DIntrinsicTextureInfo* info, cudaStream_t st);
 } // namespace texture
 
 } // namespace i3d

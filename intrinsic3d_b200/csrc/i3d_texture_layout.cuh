@@ -1,7 +1,7 @@
 /*
- * i3d_texture_layout.cuh — the per-face UV corners and the clamped barycentric map of the texture atlas (DESIGN.md §6t; the layout and
- * its no-bleed property are stated in i3d_texture.cuh), shared by the bake (i3d_texture.cuh) and the rasterizer's texture lookup
- * (i3d_raster.cuh).  No kernels.
+ * i3d_texture_layout.cuh — the per-face UV corners, the clamped barycentric map and the texel-to-point rule of the texture atlas
+ * (DESIGN.md §6t; the layout and its no-bleed property are stated in i3d_texture.cuh), shared by the bake and the decomposition
+ * (i3d_texture.cuh) and the rasterizer's texture lookup (i3d_raster.cuh).  No kernels.
  */
 #pragma once
 #include "i3d_grid.cuh"
@@ -28,6 +28,31 @@ __device__ __forceinline__ void tex_bary(int S, bool faceB, float u, float v, fl
     b = b < 0.0f ? 0.0f : b;
     const float s = FA(a, b);
     if (s > 1.0f) { a = FD(a, s); b = FD(b, s); }
+}
+
+// The point P and unit face normal n of local texel (i, j) of face A or B (faceB) with vertex indices fv into vpos: (a, b) = tex_bary at
+// the texel centre, w0 = (1 - a) - b, P = (w0 p0 + a p1) + b p2 per coordinate; n = (v1 - v0) x (v2 - v0), each component (e1[p] e2[q]) -
+// (e1[q] e2[p]), over __fsqrt_rn((n0 n0 + n1 n1) + n2 n2).  nrm is left as it is (the callers pass 0) when that length is 0.
+__device__ __forceinline__ void tex_texel_point(int S, bool faceB, int i, int j, const float* vpos, int3 fv, float (&pt)[3], float (&nrm)[3])
+{
+    float a, b;
+    tex_bary(S, faceB, static_cast<float>(i) + 0.5f, static_cast<float>(j) + 0.5f, a, b);
+    const float w0 = FS(FS(1.0f, a), b);
+    const float* p0 = vpos + 3 * static_cast<size_t>(fv.x);
+    const float* p1 = vpos + 3 * static_cast<size_t>(fv.y);
+    const float* p2 = vpos + 3 * static_cast<size_t>(fv.z);
+    float e1[3], e2[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+    {
+        pt[k] = FA(FA(FM(w0, p0[k]), FM(a, p1[k])), FM(b, p2[k]));
+        e1[k] = FS(p1[k], p0[k]); e2[k] = FS(p2[k], p0[k]);
+    }
+    const float n0 = FS(FM(e1[1], e2[2]), FM(e1[2], e2[1]));
+    const float n1 = FS(FM(e1[2], e2[0]), FM(e1[0], e2[2]));
+    const float n2 = FS(FM(e1[0], e2[1]), FM(e1[1], e2[0]));
+    const float len = __fsqrt_rn(FA(FA(FM(n0, n0), FM(n1, n1)), FM(n2, n2)));
+    if (len > 0.0f) { nrm[0] = FD(n0, len); nrm[1] = FD(n1, len); nrm[2] = FD(n2, len); }
 }
 
 } // namespace i3d

@@ -45,17 +45,11 @@ __device__ __forceinline__ bool vis_normal(const GridView& g, int64_t v, float n
     return surface_normal_f(g, v, n) && !(isnan(n[0]) || isnan(n[1]) || isnan(n[2]));
 }
 
-// Shading::computeShading(n, sh, albedo) on a unit normal: albedo * (sh . basis(n)), basis in the order of Q9 computed in float, the dot
-// product summed k = 0..8 left to right; 0 for albedo 0 or NaN.
+// Shading::computeShading(n, sh, albedo) on a unit normal: albedo * sh_dot(n, sh) (i3d_grid.cuh); 0 for albedo 0 or NaN.
 __device__ __forceinline__ float vis_shading(const float n[3], const float sh[9], float albedo)
 {
     if (albedo == 0.0f || isnan(albedo)) return 0.0f;
-    const float x = n[0], y = n[1], z = n[2];
-    const float b[9] = {1.0f, y, z, x, FM(x, y), FM(y, z), FA(FS(-FM(x, x), FM(y, y)), FM(2.0f, FM(z, z))), FM(x, z), FS(FM(x, x), FM(y, y))};
-    float d = FM(sh[0], b[0]);
-#pragma unroll
-    for (int k = 1; k < 9; ++k) d = FA(d, FM(sh[k], b[k]));
-    return FM(albedo, d);
+    return FM(albedo, sh_dot(n, sh));
 }
 
 template <int MODE>

@@ -257,6 +257,39 @@ class I3DTextureInfo(C.Structure, _Dictable):
     ]
 
 
+SH_SOURCES = {"estimate": 0, "global": 1}     # I3D_SH_* of include/i3d_types.h
+
+
+class I3DShLighting(C.Structure, _Dictable):
+    _fields_ = [
+        ("source", C.c_int32),
+        ("reserved", C.c_int32),
+        ("sh", C.c_float * 9),
+    ]
+
+
+class I3DIntrinsicTextureParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("lighting", I3DShLighting),
+        ("min_shading", C.c_float),
+        ("reserved", C.c_int32),
+    ]
+
+
+class I3DIntrinsicTextureInfo(C.Structure, _Dictable):
+    _fields_ = [
+        ("atlas_width", C.c_int32),
+        ("atlas_height", C.c_int32),
+        ("num_texels_owned", C.c_int64),
+        ("num_texels_lit", C.c_int64),
+        ("num_texels_unlit", C.c_int64),
+        ("num_texels_lit_fallback", C.c_int64),
+        ("albedo_min", C.c_float * 3),
+        ("albedo_max", C.c_float * 3),
+        ("ms_decompose", C.c_double),
+    ]
+
+
 DISTANCE_MAX_THRESHOLDS = 8     # I3D_DISTANCE_MAX_THRESHOLDS of include/i3d_types.h
 
 
@@ -371,7 +404,7 @@ class I3DRenderStats(C.Structure, _Dictable):
 
 # I3D_RASTER_* plane bits and colour sources of include/i3d_types.h
 RASTER_PLANES = {"depth": 1, "face": 2, "bary": 4, "normal": 8, "rgb": 16}
-RASTER_COLORS = {None: 0, "vertex": 1, "texture": 2}
+RASTER_COLORS = {None: 0, "vertex": 1, "texture": 2, "relit": 3}
 
 
 class I3DRasterParams(C.Structure, _Dictable):

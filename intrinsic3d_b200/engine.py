@@ -11,8 +11,9 @@ import os
 
 import numpy as np
 
-from .ctypes_defs import (DISTANCE_MAX_THRESHOLDS, GRID_FROM_MESH_SOURCES, RASTER_COLORS, RASTER_PLANES, RENDER_PLANES, I3DDistanceInfo,
-                          I3DDistanceParams, I3DGridFromMeshInfo, I3DGridFromMeshParams, I3DFusionCamera, I3DFusionParams, I3DIterInfo,
+from .ctypes_defs import (DISTANCE_MAX_THRESHOLDS, GRID_FROM_MESH_SOURCES, RASTER_COLORS, RASTER_PLANES, RENDER_PLANES, SH_SOURCES, I3DDistanceInfo,
+                          I3DDistanceParams, I3DGridFromMeshInfo, I3DGridFromMeshParams, I3DFusionCamera, I3DFusionParams, I3DIntrinsicTextureInfo,
+                          I3DIntrinsicTextureParams, I3DIterInfo, I3DShLighting,
                           I3DLightingInfo, I3DLightingParams, I3DMeshInfo, I3DMeshParams, I3DParams, I3DRasterCamera, I3DRasterInfo,
                           I3DRasterParams, I3DRasterStats, I3DRenderParams, I3DRenderStats, I3DSimplifyInfo, I3DSimplifyParams, I3DTextureInfo,
                           I3DTextureParams, I3DTrackColorInfo, I3DTrackColorParams, I3DTrackInfo, I3DTrackParams, TRACK_LEVELS)
@@ -37,6 +38,8 @@ EXPORTED_SYMBOLS = [
     "i3d_sizeof_mesh_info", "i3d_extract_mesh", "i3d_download_mesh", "i3d_extract_mesh_colored", "i3d_mode_colors",
     "i3d_sizeof_simplify_params", "i3d_sizeof_simplify_info", "i3d_simplify_mesh",
     "i3d_sizeof_texture_params", "i3d_sizeof_texture_info", "i3d_default_texture_params", "i3d_bake_texture", "i3d_download_texture",
+    "i3d_sizeof_sh_lighting", "i3d_sizeof_intrinsic_texture_params", "i3d_sizeof_intrinsic_texture_info", "i3d_default_sh_lighting",
+    "i3d_default_intrinsic_texture_params", "i3d_decompose_texture", "i3d_download_intrinsic_texture", "i3d_set_relight",
     "i3d_sizeof_distance_params", "i3d_sizeof_distance_info", "i3d_default_distance_params", "i3d_upload_reference_mesh",
     "i3d_surface_distance", "i3d_download_surface_distance", "i3d_debug_set_keep_distance_samples", "i3d_debug_get_distance_samples",
     "i3d_sizeof_grid_from_mesh_params", "i3d_sizeof_grid_from_mesh_info", "i3d_default_grid_from_mesh_params", "i3d_grid_from_mesh",
@@ -119,6 +122,21 @@ def load_library():
     L.i3d_bake_texture.argtypes = [C.c_void_p, C.POINTER(I3DTextureParams), C.POINTER(C.c_float), C.POINTER(I3DTextureInfo)]
     L.i3d_download_texture.restype = C.c_int
     L.i3d_download_texture.argtypes = [C.c_void_p, C.POINTER(C.c_uint8), C.POINTER(C.c_float)]
+    for fn in (L.i3d_sizeof_sh_lighting, L.i3d_sizeof_intrinsic_texture_params, L.i3d_sizeof_intrinsic_texture_info):
+        fn.restype = C.c_uint64
+    if (L.i3d_sizeof_sh_lighting() != C.sizeof(I3DShLighting) or L.i3d_sizeof_intrinsic_texture_params() != C.sizeof(I3DIntrinsicTextureParams)
+            or L.i3d_sizeof_intrinsic_texture_info() != C.sizeof(I3DIntrinsicTextureInfo)):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (intrinsic texture structs)")
+    L.i3d_default_sh_lighting.restype = None
+    L.i3d_default_sh_lighting.argtypes = [C.POINTER(I3DShLighting)]
+    L.i3d_default_intrinsic_texture_params.restype = None
+    L.i3d_default_intrinsic_texture_params.argtypes = [C.POINTER(I3DIntrinsicTextureParams)]
+    L.i3d_decompose_texture.restype = C.c_int
+    L.i3d_decompose_texture.argtypes = [C.c_void_p, C.POINTER(I3DIntrinsicTextureParams), C.POINTER(I3DIntrinsicTextureInfo)]
+    L.i3d_download_intrinsic_texture.restype = C.c_int
+    L.i3d_download_intrinsic_texture.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float)]
+    L.i3d_set_relight.restype = C.c_int
+    L.i3d_set_relight.argtypes = [C.c_void_p, C.POINTER(I3DShLighting)]
     L.i3d_sizeof_distance_params.restype = C.c_uint64
     L.i3d_sizeof_distance_info.restype = C.c_uint64
     if L.i3d_sizeof_distance_params() != C.sizeof(I3DDistanceParams) or L.i3d_sizeof_distance_info() != C.sizeof(I3DDistanceInfo):
@@ -261,6 +279,17 @@ def default_track_color_lni_params() -> I3DTrackColorParams:
     p = I3DTrackColorParams()
     load_library().i3d_default_track_color_lni_params(C.byref(p))
     return p
+
+
+def sh_lighting(sh=None) -> I3DShLighting:
+    """The I3DShLighting of sh: None for the subvolume SH of the last lighting estimate, else nine coefficients (the order of the lighting
+    estimate) used everywhere."""
+    if sh is None:
+        return I3DShLighting(SH_SOURCES["estimate"], 0, (C.c_float * 9)())
+    v = np.asarray(sh, np.float32).reshape(-1)
+    if v.shape != (9,):
+        raise ValueError(f"sh must hold 9 coefficients, got {v.size}")
+    return I3DShLighting(SH_SOURCES["global"], 0, (C.c_float * 9)(*[float(x) for x in v]))
 
 
 def default_texture_params() -> I3DTextureParams:
@@ -518,6 +547,25 @@ class Engine:
         self._check(self.L.i3d_download_texture(self.h, _p(out["image"], C.c_uint8), _p(out["uv"], C.c_float)))
         return out
 
+    def decompose_texture(self, min_shading: float = 0.05, sh=None):
+        """Splits the texture of the resident mesh (the last bake_texture) into albedo and shading on the device (DESIGN.md §6x): at each
+        owned texel's point and face normal, s = sh . basis(n) under sh (None: the subvolume SH of the last estimate_lighting; else nine
+        coefficients used everywhere), and albedo = colour / 255 / s where the normal is not 0 and s > min_shading, else 0.  Returns a
+        dict with albedo float32 [H, W, 3] (R, G, B), shading float32 [H, W] and info (I3DIntrinsicTextureInfo).  The albedo is known up
+        to one global scale; mesh.albedo_image turns it into an image for mesh.save_textured_obj."""
+        prm = I3DIntrinsicTextureParams(sh_lighting(sh), float(min_shading), 0)
+        info = I3DIntrinsicTextureInfo()
+        self._check(self.L.i3d_decompose_texture(self.h, C.byref(prm), C.byref(info)))
+        H, W = info.atlas_height, info.atlas_width
+        out = dict(albedo=np.empty((H, W, 3), np.float32), shading=np.empty((H, W), np.float32), info=info)
+        self._check(self.L.i3d_download_intrinsic_texture(self.h, _p(out["albedo"], C.c_float), _p(out["shading"], C.c_float)))
+        return out
+
+    def set_relight(self, sh=None):
+        """The lighting of rasterize_keyframes / rasterize_views with color="relit": None (default) for the subvolume SH of the lighting
+        estimate at the time of the rasterization, else nine coefficients used everywhere."""
+        self._check(self.L.i3d_set_relight(self.h, C.byref(sh_lighting(sh))))
+
     def upload_reference_mesh(self, mesh):
         """Uploads a reference surface for surface_distance: a dict with vertices float32 [V, 3] and faces int32 [F, 3] (an extract_mesh
         dict; its colours are ignored).  It replaces the previous reference and stays through grid, frame and mesh changes."""
@@ -629,7 +677,7 @@ class Engine:
     @staticmethod
     def _raster_params(color, planes):
         if color not in RASTER_COLORS:
-            raise ValueError(f"color must be one of None, 'vertex', 'texture', got {color!r}")
+            raise ValueError(f"color must be one of None, 'vertex', 'texture', 'relit', got {color!r}")
         mask = 0
         for p in planes:
             if p not in RASTER_PLANES:
@@ -649,7 +697,8 @@ class Engine:
     def rasterize_keyframes(self, ids, color="vertex", planes=("depth", "face", "bary", "normal", "rgb")):
         """Rasterizes the resident mesh (the last extract_mesh or simplify_mesh) into the frames `ids` with the engine's current camera,
         at the size of the installed frames (DESIGN.md §6w).  color: "vertex" (the vertex colours), "texture" (the last bake_texture of
-        the resident mesh) or None.  Returns a dict with the requested planes [n, H, W] (depth float32, 0 = no face; face int32, -1 = no
+        the resident mesh), "relit" (the albedo of the last decompose_texture times the shading under set_relight's lighting, §6x) or
+        None.  Returns a dict with the requested planes [n, H, W] (depth float32, 0 = no face; face int32, -1 = no
         face; bary float32 [.., 2]; normal float32 [.., 3], world frame; rgb uint8 [.., 3]), stats: one dict per view (I3DRasterStats:
         covered / observed pixels, depth pairs with sum |e| and e^2 in metres, colour pairs with per-channel integer sums of |e| and e^2
         against the colour frame) and info (I3DRasterInfo).  planes=() gives the statistics only."""

@@ -248,3 +248,12 @@ def save_textured_obj(prefix: str, mesh, texture):
         with open(path, "wb") as fh:
             fh.write(data)
     return paths
+
+
+def albedo_image(albedo, scale: float = 1.0):
+    """An albedo atlas float [H, W, 3] (Engine.decompose_texture) as a uint8 image: trunc(clamp((A scale) 255 + 1/2, 0, 255)) in float32,
+    so that scale = 1 gives the relit raster's colour under the SH (1, 0, ..., 0).  The image and the texture's uv write an albedo OBJ
+    with save_textured_obj."""
+    a = np.asarray(albedo, np.float32)
+    x = (((a * np.float32(scale)).astype(np.float32) * np.float32(255)).astype(np.float32) + np.float32(0.5)).astype(np.float32)
+    return np.trunc(np.clip(x, np.float32(0), np.float32(255))).astype(np.uint8)
