@@ -297,6 +297,32 @@ int         i3d_download_surface_distance(I3DEngine* e, float* vertex_distance, 
 int         i3d_debug_set_keep_distance_samples(I3DEngine* e, int on);
 int         i3d_debug_get_distance_samples(I3DEngine* e, int direction, float* d2, int32_t* face);
 
+/* ---- registering the reference mesh to the resident mesh: point-to-plane ICP (DESIGN.md §6aa) ---- */
+uint64_t    i3d_sizeof_register_params(void);
+uint64_t    i3d_sizeof_register_info(void);
+/* samples_per_edge 1, stages {0.016, 0.008, 0.004} m with 10 iterations each, min_normal_cos 0.5, min_correspondences 100, cell_size 0. */
+void        i3d_default_register_params(I3DRegisterParams* p);
+/* Estimates the rigid T (R row-major | t, 12 doubles) with x_A = R x_B + t that maps the reference mesh B onto the resident mesh A, by
+ * point-to-plane Gauss-Newton from T_init (NULL = identity): the samples of A (i3d_surface_distance's, weighted by area / L^2) are moved
+ * by T^-1 and each is paired with the nearest face of B within the stage's max_distance; a row needs both unit face normals non-zero
+ * and dot(n_A, n_B) >= min_normal_cos.  The stages run in order with no early stop, then one more system is formed at the final pose;
+ * the 6 x 6 solve and the update are the tracker's, with its statuses.  Every result is bit-identical from run to run and does not depend
+ * on cell_size; the rounding of every operation is stated in i3d_register.cuh.  Writes T_out and *info (may be NULL) only: the reference,
+ * the resident mesh, its texture and the last distance results stay as they were.  Fails, writing nothing, when world > 1, without a
+ * resident mesh with faces, without a reference mesh, for a parameter out of its range, a T_init that is not finite or not a rotation
+ * (max |R^T R - I| > 1e-5 or det R < 0), a NULL T_out, and a search grid above the caps of i3d_surface_distance. */
+int         i3d_register_reference_mesh(I3DEngine* e, const I3DRegisterParams* params, const double* T_init, double* T_out, I3DRegisterInfo* info);
+/* Moves the reference mesh on the device: every vertex x <- float(((R0 x0 + R1 x1) + R2 x2) + t), per row of R, in double from the float
+ * x.  i3d_surface_distance and i3d_grid_from_mesh (reference source) then use the moved mesh; the last distance results are kept.  Fails,
+ * changing nothing, without a reference mesh and for a T that is not finite or not a rotation (as above). */
+int         i3d_transform_reference_mesh(I3DEngine* e, const double* T);
+/* Tests: the systems of the last i3d_register_reference_mesh, in the order they were formed (the first at T_init, the last the one
+ * without a solve at the final pose); n = their number.  systems double [n][31]: the 29 sums of the tracker's layout (21 upper-triangle
+ * entries of sum w J^T J, 6 of sum w J^T r, sum w r^2, rows), then sum w (for the first and the last system only, else 0) and 0;
+ * poses double [n][12]: T^-1 at which each was formed; faces int32 [F L^2]: per sample the nearest face of B at T_init (-1 when none or
+ * for a zero-area face).  Any pointer may be NULL.  Fails before the first successful call. */
+int         i3d_debug_get_register_systems(I3DEngine* e, int32_t* n, double* systems, double* poses, int32_t* faces);
+
 /* ---- the voxel grid from a triangle mesh: narrow-band signed distance (DESIGN.md §6v) ---- */
 uint64_t    i3d_sizeof_grid_from_mesh_params(void);
 uint64_t    i3d_sizeof_grid_from_mesh_info(void);

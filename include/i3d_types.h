@@ -338,6 +338,38 @@ typedef struct I3DGridFromMeshInfo
     double  ms_topology, ms_grid, ms_bricks, ms_query, ms_install;   /* device time per stage (CUDA events) */
 } I3DGridFromMeshInfo;
 
+/* ---- registering the reference mesh to the resident mesh: point-to-plane ICP (DESIGN.md §6aa) ---- */
+#define I3D_REGISTER_MAX_STAGES 4
+#define I3D_REGISTER_MAX_ITERATIONS 256     /* largest sum of the stages' iterations */
+
+typedef struct I3DRegisterParams
+{
+    int32_t samples_per_edge;             /* L in [1, 16]: the resident mesh's samples, as i3d_surface_distance takes them */
+    int32_t num_stages;                   /* in [1, 4], run in order */
+    float   max_distance[I3D_REGISTER_MAX_STAGES];   /* metres per stage: finite, > 0 and non-increasing */
+    int32_t iterations[I3D_REGISTER_MAX_STAGES];     /* updates per stage, >= 0, at most I3D_REGISTER_MAX_ITERATIONS in total */
+    float   min_normal_cos;               /* in [-1, 1]: a row needs dot(n_A, n_B) >= this; -1 keeps every matched sample */
+    int32_t min_correspondences;          /* >= 6: a system with fewer rows stops the call (I3D_TRACK_FEW_CORRESPONDENCES) */
+    float   cell_size;                    /* search-grid cell edge, metres; 0 = twice the reference's mean edge length.  Never changes the result */
+} I3DRegisterParams;
+
+typedef struct I3DRegisterInfo
+{
+    int32_t status;                       /* I3D_TRACK_OK, _FEW_CORRESPONDENCES, _NOT_POSITIVE_DEFINITE or _NON_FINITE */
+    int32_t iterations;                   /* updates applied */
+    int64_t initial_rows, final_rows;     /* rows of the first system (at T_init) and of the last (at the returned T) */
+    double  initial_weight, final_weight; /* sum of the rows' area weights, m^2 */
+    double  initial_residual_sq, final_residual_sq;  /* sum w r^2, m^4 */
+    double  initial_rms, final_rms;       /* sqrt(sum w r^2 / sum w), metres (0 without rows) */
+    double  update_norm;                  /* |xi| of the last update applied */
+    int64_t num_samples;                  /* samples of the resident mesh per system (F L^2) */
+    int64_t point_triangle_tests;         /* closest-point evaluations over every system */
+    float   cell_size;                    /* the reference's search grid: cell edge (metres) and cells per axis */
+    int32_t grid[3];
+    int64_t num_cells, num_cell_entries;
+    double  ms_grid, ms_rows, ms_solve;   /* device time: grid build, every rows launch, every block sum with its solve (CUDA events) */
+} I3DRegisterInfo;
+
 /* Features of the closest point on a face (i3d_debug_get_grid_from_mesh_voxels): vertex a, b, c, edge ab, ac, bc, interior */
 enum { I3D_FEATURE_VERTEX_A = 0, I3D_FEATURE_VERTEX_B, I3D_FEATURE_VERTEX_C, I3D_FEATURE_EDGE_AB, I3D_FEATURE_EDGE_AC, I3D_FEATURE_EDGE_BC,
        I3D_FEATURE_INTERIOR };

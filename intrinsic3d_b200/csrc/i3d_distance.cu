@@ -1,6 +1,8 @@
 /*
- * i3d_distance.cu — the distance between the resident mesh and a reference mesh: its kernels (i3d_distance.cuh) and the host code that
- * sizes the search grids and launches them (i3d_distance.h).  Keeping them out of i3d_engine.cu leaves the engine's device module as it is.
+ * i3d_distance.cu — the distance between the resident mesh and a reference mesh, and the registration of the reference to the resident
+ * mesh: their kernels (i3d_distance.cuh, i3d_register.cuh) and the host code that sizes the search grids and launches them
+ * (i3d_distance.h).  The registration's solve and pose update are the tracker's kernels, launched through track::pose_init / pose_step
+ * (i3d_render.cu).  Keeping them out of i3d_engine.cu leaves the engine's device module as it is.
  */
 #include <climits>
 #include <cstdarg>
@@ -9,6 +11,7 @@
 #include <cstring>
 
 #include "i3d_distance.cuh"
+#include "i3d_register.cuh"
 
 #include <cub/device/device_scan.cuh>
 
@@ -224,6 +227,123 @@ int compute(DistanceState& ds, const DistMesh& a, const I3DDistanceParams& p, I3
         *info = inf;
     }
     return 0;
+}
+
+bool check_rigid(const double* T, std::string& error)
+{
+    for (int i = 0; i < 12; ++i)
+        if (!std::isfinite(T[i])) { error = format("entry %d of the transform is not finite", i); return false; }
+    double dev = 0.0;
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j)
+        {
+            const double d = T[i] * T[j] + T[3 + i] * T[3 + j] + T[6 + i] * T[6 + j] - (i == j ? 1.0 : 0.0);
+            dev = std::max(dev, std::fabs(d));
+        }
+    const double det = T[0] * (T[4] * T[8] - T[5] * T[7]) - T[1] * (T[3] * T[8] - T[5] * T[6]) + T[2] * (T[3] * T[7] - T[4] * T[6]);
+    if (dev > 1e-5 || det < 0.0)
+    {
+        error = format("the transform's R is not a rotation (max |R^T R - I| = %g, det R = %g)", dev, det);
+        return false;
+    }
+    return true;
+}
+
+int register_reference(DistanceState& ds, const DistMesh& a, const I3DRegisterParams& p, const double* T_init, double* T_out, I3DRegisterInfo* info,
+                       std::string& error, cudaStream_t st)
+{
+    const DistMesh b{ds.ref_V, ds.ref_F, ds.ref_vpos.p, ds.ref_faces.p};
+    DistGrid g;
+    int64_t entries = 0;
+    if (!plan(ds.grid, b, p.cell_size, p.max_distance[0], g, entries, nullptr, error, st)) return 1;
+    int E = 1;                                   // every system: one per update, then the one at the final pose
+    for (int s = 0; s < p.num_stages; ++s) E += p.iterations[s];
+    const int L = p.samples_per_edge;
+    const int64_t ns = a.F * L * L;
+    const unsigned nb = blocks_for(static_cast<size_t>(ns));
+    ds.reg_state.ensure(1); ds.reg_T.ensure(12); ds.reg_partials.ensure(static_cast<size_t>(nb) * kTrackVals); ds.reg_wpartials.ensure(2 * static_cast<size_t>(nb));
+    ds.reg_sums.ensure(static_cast<size_t>(E) * kTrackVals); ds.reg_sys.ensure(kTrackVals); ds.reg_poses.ensure(12 * static_cast<size_t>(E));
+    ds.reg_face.ensure(static_cast<size_t>(ns)); ds.reg_counters.ensure(2);
+    const size_t nev = 2 + 3 * static_cast<size_t>(E);
+    while (ds.reg_ev.size() < nev) { cudaEvent_t ev; CK(cudaEventCreate(&ev)); ds.reg_ev.push_back(ev); }
+    static const double kIdentity[12] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0};
+    ds.have_reg = false;
+    CK(cudaMemcpyAsync(ds.reg_T.p, T_init ? T_init : kIdentity, 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(ds.reg_counters.p, 0, 2 * sizeof(unsigned long long), st));
+    cudaEvent_t* ev = ds.reg_ev.data();
+    CK(cudaEventRecord(ev[0], st));
+    build(ds.grid, b, g, entries, st);
+    CK(cudaEventRecord(ev[1], st));
+    track::pose_init(ds.reg_T.p, ds.reg_state.p, st);
+    int e = 0;
+    auto system = [&](float max_distance, int solve) {
+        const RegQuery q{L, max_distance, p.min_normal_cos, p.min_normal_cos > -1.0f ? 1 : 0};
+        // the pose M (TrackState::T) this system is formed at
+        CK(cudaMemcpyAsync(ds.reg_poses.p + 12 * static_cast<size_t>(e), ds.reg_state.p, 12 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        double* wp = e == 0 ? ds.reg_wpartials.p : (e == E - 1 ? ds.reg_wpartials.p + nb : nullptr);
+        CK(cudaEventRecord(ev[2 + 3 * e], st));
+        k_reg_rows<<<nb, kThreads, 0, st>>>(a, b, g, q, ds.reg_state.p, e == 0 ? ds.reg_face.p : nullptr, ds.reg_partials.p, wp, ds.reg_counters.p);
+        CK(cudaEventRecord(ev[3 + 3 * e], st));
+        track::pose_step(static_cast<int>(nb), ds.reg_partials.p, ds.reg_sums.p + static_cast<size_t>(e) * kTrackVals, ds.reg_state.p, ds.reg_sys.p,
+                         p.min_correspondences, solve, ds.reg_counters.p + 1, st);
+        CK(cudaEventRecord(ev[4 + 3 * e], st));
+        ++e;
+    };
+    for (int s = 0; s < p.num_stages; ++s)
+        for (int it = 0; it < p.iterations[s]; ++it) system(p.max_distance[s], 1);
+    system(p.max_distance[p.num_stages - 1], 0);
+    TrackState hs;
+    std::vector<double> sums(static_cast<size_t>(E) * kTrackVals), wp(2 * static_cast<size_t>(nb));
+    unsigned long long counters[2] = {0, 0};
+    CK(cudaMemcpyAsync(&hs, ds.reg_state.p, sizeof(hs), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(sums.data(), ds.reg_sums.p, sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(wp.data(), ds.reg_wpartials.p, wp.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(counters, ds.reg_counters.p, sizeof(counters), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
+    // sum w of the first and the last system: the blocks in order, as k_tile_sums adds them
+    for (int k = 0; k < 2; ++k)
+    {
+        const double* w = wp.data() + (E == 1 ? 0 : k) * static_cast<size_t>(nb);
+        double s = 0.0;
+        for (unsigned i = 0; i < nb; ++i) s += w[i];
+        ds.reg_wsum[k] = s;
+    }
+    ds.reg_n = E; ds.reg_samples = ns; ds.have_reg = true;
+    std::memcpy(T_out, hs.w2c, 12 * sizeof(double));
+    if (info)
+    {
+        I3DRegisterInfo inf;
+        std::memset(&inf, 0, sizeof(inf));
+        inf.status = hs.status; inf.iterations = hs.iterations; inf.update_norm = hs.update_norm;
+        const double* S0 = sums.data();
+        const double* S1 = sums.data() + static_cast<size_t>(E - 1) * kTrackVals;
+        inf.initial_rows = static_cast<int64_t>(S0[28]); inf.final_rows = static_cast<int64_t>(S1[28]);
+        inf.initial_weight = ds.reg_wsum[0]; inf.final_weight = ds.reg_wsum[1];
+        inf.initial_residual_sq = S0[27]; inf.final_residual_sq = S1[27];
+        inf.initial_rms = inf.initial_weight > 0.0 ? std::sqrt(S0[27] / inf.initial_weight) : 0.0;
+        inf.final_rms = inf.final_weight > 0.0 ? std::sqrt(S1[27] / inf.final_weight) : 0.0;
+        inf.num_samples = ns;
+        inf.point_triangle_tests = static_cast<int64_t>(counters[0]);
+        inf.cell_size = g.h;
+        for (int k = 0; k < 3; ++k) inf.grid[k] = g.n[k];
+        inf.num_cells = static_cast<int64_t>(g.n[0]) * g.n[1] * g.n[2];
+        inf.num_cell_entries = entries;
+        auto ms = [&](int i, int j) { float m = 0.f; CK(cudaEventElapsedTime(&m, ev[i], ev[j])); return static_cast<double>(m); };
+        inf.ms_grid = ms(0, 1);
+        for (int k = 0; k < E; ++k) { inf.ms_rows += ms(2 + 3 * k, 3 + 3 * k); inf.ms_solve += ms(3 + 3 * k, 4 + 3 * k); }
+        *info = inf;
+    }
+    return 0;
+}
+
+void transform_reference(DistanceState& ds, const double* T, cudaStream_t st)
+{
+    ds.reg_T.ensure(12);
+    CK(cudaMemcpyAsync(ds.reg_T.p, T, 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+    k_reg_transform<<<blocks_for(static_cast<size_t>(ds.ref_V)), kThreads, 0, st>>>(ds.ref_V, ds.ref_vpos.p, ds.reg_T.p);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
 }
 
 } // namespace distance

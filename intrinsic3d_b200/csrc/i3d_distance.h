@@ -9,9 +9,12 @@
 #include <stdint.h>
 
 #include <string>
+#include <vector>
 
+#include "../../include/i3d_c_api.h"
 #include "../../include/i3d_types.h"
 #include "i3d_host.h"
+#include "i3d_track.h"
 
 namespace i3d
 {
@@ -53,6 +56,13 @@ struct DistanceState
     bool have_keep = false;
     cudaEvent_t ev[14] = {};
     bool ev_ready = false;
+    // the reference-mesh registration (i3d_register.cuh), which builds its grid in `grid`: the pose state, the block partials, every
+    // system of the last call with the pose M it was formed at, the first system's per-sample faces and sum w of the first and last system
+    Dev<TrackState> reg_state; Dev<double> reg_T, reg_partials, reg_wpartials, reg_sums, reg_sys, reg_poses; Dev<int32_t> reg_face;
+    Dev<unsigned long long> reg_counters;
+    int reg_n = 0; int64_t reg_samples = 0; double reg_wsum[2] = {0.0, 0.0};
+    bool have_reg = false;
+    std::vector<cudaEvent_t> reg_ev;
 };
 
 namespace distance
@@ -69,6 +79,15 @@ int upload_reference(DistanceState& ds, int64_t V, const float* xyz, int64_t F, 
 // Both directions and the vertex query between the resident mesh a (F > 0) and the reference (present), with parameters the caller
 // validated.  Returns non-zero with the message in `error`, writing nothing, when a search grid exceeds its cell or entry cap.
 int compute(DistanceState& ds, const DistMesh& a, const I3DDistanceParams& p, I3DDistanceInfo* info, std::string& error, cudaStream_t st);
+// False with the message when T [12] (R row-major | t) is not finite or R is not a rotation: max |R^T R - I| > 1e-5 or det R < 0
+bool check_rigid(const double* T, std::string& error);
+// Registers the reference (present) to the resident mesh a (F > 0) from T_init (nullptr: identity; checked by the caller, as are the
+// parameters) into T_out [12] (DESIGN.md §6aa).  Returns non-zero with the message in `error`, writing nothing, when the search grid
+// exceeds its cell or entry cap.
+int register_reference(DistanceState& ds, const DistMesh& a, const I3DRegisterParams& p, const double* T_init, double* T_out, I3DRegisterInfo* info,
+                       std::string& error, cudaStream_t st);
+// Moves the reference (present) by T (checked by the caller) on the device
+void transform_reference(DistanceState& ds, const double* T, cudaStream_t st);
 } // namespace distance
 
 } // namespace i3d

@@ -1119,6 +1119,7 @@ void i3d_engine_destroy(I3DEngine* e)
     for (auto& ev : e->timing.pool) cudaEventDestroy(ev);
     if (e->mesh.ev_ready) for (auto& ev : e->mesh.ev) cudaEventDestroy(ev);
     if (e->tex.ev_ready) for (auto& ev : e->tex.ev) cudaEventDestroy(ev);
+    for (auto& ev : e->dist.reg_ev) cudaEventDestroy(ev);
     cudaStreamDestroy(e->stream);
     delete e;
 }
@@ -1978,6 +1979,99 @@ int i3d_debug_get_distance_samples(I3DEngine* e, int direction, float* d2, int32
         const size_t n = static_cast<size_t>(e->dist.keep_n[direction]);
         if (d2 && n) CK(cudaMemcpyAsync(d2, e->dist.keep_d2[direction].p, n * sizeof(float), cudaMemcpyDeviceToHost, st));
         if (face && n) CK(cudaMemcpyAsync(face, e->dist.keep_face[direction].p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    });
+}
+
+// ---- registering the reference mesh to the resident mesh (i3d_register.cuh, DESIGN.md §6aa) ------------
+uint64_t i3d_sizeof_register_params(void) { return sizeof(I3DRegisterParams); }
+uint64_t i3d_sizeof_register_info(void) { return sizeof(I3DRegisterInfo); }
+
+void i3d_default_register_params(I3DRegisterParams* p)
+{
+    std::memset(p, 0, sizeof(*p));
+    p->samples_per_edge = 1; p->num_stages = 3;
+    p->max_distance[0] = 0.016f; p->max_distance[1] = 0.008f; p->max_distance[2] = 0.004f;
+    p->iterations[0] = 10; p->iterations[1] = 10; p->iterations[2] = 10;
+    p->min_normal_cos = 0.5f; p->min_correspondences = 100; p->cell_size = 0.0f;
+}
+
+int i3d_register_reference_mesh(I3DEngine* e, const I3DRegisterParams* params, const double* T_init, double* T_out, I3DRegisterInfo* info)
+{
+    static const char* who = "i3d_register_reference_mesh";
+    if (!e) return 1;
+    if (!params) return fail(e, "%s: params is NULL", who);
+    if (!T_out) return fail(e, "%s: T_out is NULL", who);
+    if (e->world > 1) return fail(e, "%s: the registration runs on one GPU (world = %d)", who, e->world);
+    if (!e->mesh.have_mesh) return fail(e, "%s: no mesh (call i3d_extract_mesh after the last change of the voxel set)", who);
+    if (e->mesh.mesh_F <= 0) return fail(e, "%s: the resident mesh has no faces", who);
+    if (!e->dist.have_ref) return fail(e, "%s: no reference mesh (i3d_upload_reference_mesh)", who);
+    const I3DRegisterParams& p = *params;
+    if (p.samples_per_edge < 1 || p.samples_per_edge > I3D_DISTANCE_MAX_SAMPLES_PER_EDGE)
+        return fail(e, "%s: samples_per_edge must be in [1, %d], got %d", who, I3D_DISTANCE_MAX_SAMPLES_PER_EDGE, p.samples_per_edge);
+    if (p.num_stages < 1 || p.num_stages > I3D_REGISTER_MAX_STAGES)
+        return fail(e, "%s: num_stages must be in [1, %d], got %d", who, I3D_REGISTER_MAX_STAGES, p.num_stages);
+    int total = 0;
+    for (int s = 0; s < p.num_stages; ++s)
+    {
+        const float d = p.max_distance[s];
+        if (!std::isfinite(d) || !(d > 0.0f) || (s > 0 && d > p.max_distance[s - 1]))
+            return fail(e, "%s: max_distance must be finite, > 0 and non-increasing; stage %d has %g", who, s, static_cast<double>(d));
+        if (p.iterations[s] < 0) return fail(e, "%s: iterations must be >= 0; stage %d has %d", who, s, p.iterations[s]);
+        total += p.iterations[s];
+        if (total > I3D_REGISTER_MAX_ITERATIONS) return fail(e, "%s: at most %d iterations in total", who, I3D_REGISTER_MAX_ITERATIONS);
+    }
+    if (!(p.min_normal_cos >= -1.0f && p.min_normal_cos <= 1.0f)) return fail(e, "%s: min_normal_cos must be in [-1, 1], got %g", who, static_cast<double>(p.min_normal_cos));
+    if (p.min_correspondences < 6) return fail(e, "%s: min_correspondences must be >= 6, got %d", who, p.min_correspondences);
+    if (!std::isfinite(p.cell_size) || p.cell_size < 0.0f) return fail(e, "%s: cell_size must be finite and >= 0, got %g", who, static_cast<double>(p.cell_size));
+    std::string err;
+    if (T_init && !distance::check_rigid(T_init, err)) return fail(e, "%s: T_init: %s", who, err.c_str());
+    return guarded(e, [&]() {
+        const DistMesh a{e->mesh.mesh_V, e->mesh.mesh_F, e->mesh.mesh_vpos, e->mesh.mesh_faces};
+        if (distance::register_reference(e->dist, a, p, T_init, T_out, info, err, e->stream)) return fail(e, "%s: %s", who, err.c_str());
+        return 0;
+    });
+}
+
+int i3d_transform_reference_mesh(I3DEngine* e, const double* T)
+{
+    static const char* who = "i3d_transform_reference_mesh";
+    if (!e) return 1;
+    if (!T) return fail(e, "%s: T is NULL", who);
+    if (!e->dist.have_ref) return fail(e, "%s: no reference mesh (i3d_upload_reference_mesh)", who);
+    std::string err;
+    if (!distance::check_rigid(T, err)) return fail(e, "%s: T: %s", who, err.c_str());
+    return guarded(e, [&]() {
+        distance::transform_reference(e->dist, T, e->stream);
+        return 0;
+    });
+}
+
+int i3d_debug_get_register_systems(I3DEngine* e, int32_t* n, double* systems, double* poses, int32_t* faces)
+{
+    if (!e) return 1;
+    if (!e->dist.have_reg) return fail(e, "i3d_debug_get_register_systems: no registration (call i3d_register_reference_mesh first)");
+    return guarded(e, [&]() {
+        cudaStream_t st = e->stream;
+        const DistanceState& ds = e->dist;
+        const size_t m = static_cast<size_t>(ds.reg_n);
+        if (n) *n = ds.reg_n;
+        if (systems)
+        {
+            std::vector<double> s(m * kTrackVals);
+            CK(cudaMemcpyAsync(s.data(), ds.reg_sums.p, s.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            for (size_t k = 0; k < m; ++k)
+            {
+                double* o = systems + k * (kTrackVals + 2);
+                std::memcpy(o, s.data() + k * kTrackVals, kTrackVals * sizeof(double));
+                o[kTrackVals] = k == 0 ? ds.reg_wsum[0] : (k + 1 == m ? ds.reg_wsum[1] : 0.0);
+                o[kTrackVals + 1] = 0.0;
+            }
+        }
+        if (poses) CK(cudaMemcpyAsync(poses, ds.reg_poses.p, 12 * m * sizeof(double), cudaMemcpyDeviceToHost, st));
+        if (faces) CK(cudaMemcpyAsync(faces, ds.reg_face.p, static_cast<size_t>(ds.reg_samples) * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         return 0;
     });

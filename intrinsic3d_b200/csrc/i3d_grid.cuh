@@ -26,6 +26,18 @@ constexpr int kThreads = 256;
 #define FS(a, b) __fsub_rn((a), (b))
 #define FD(a, b) __fdiv_rn((a), (b))
 
+// R (row-major 3 x 3) times v, sums left to right, plus t when given: the float rigid transform of the tracker (i3d_track.cuh) and of the
+// reference-mesh registration (i3d_register.cuh)
+__device__ __forceinline__ void tr_xform(const float* R, const float* t, const float v[3], float out[3])
+{
+#pragma unroll
+    for (int d = 0; d < 3; ++d)
+    {
+        const float s = FA(FA(FM(R[3 * d], v[0]), FM(R[3 * d + 1], v[1])), FM(R[3 * d + 2], v[2]));
+        out[d] = t ? FA(s, t[d]) : s;
+    }
+}
+
 // ----------------------------------------------------------------------------------------------
 // device hash table of the grid (replaces unordered_map::find, sparse_voxel_grid.cpp:166-259)
 // ----------------------------------------------------------------------------------------------

@@ -436,6 +436,18 @@ void pose_compose(const double* A, const double* B, double* out)
 }
 } // namespace
 
+void track::pose_init(const double* pose_in, TrackState* state, cudaStream_t st)
+{
+    k_track_init<<<1, 64, 0, st>>>(1, pose_in, state);
+}
+
+void track::pose_step(int blocks, const double* partials, double* sums, TrackState* state, double* sys, int min_corr, int solve,
+                      unsigned long long* rows, cudaStream_t st)
+{
+    tile_sums<kTrackVals>(1, blocks, partials, sums, st);
+    k_track_solve<<<1, 64, 0, st>>>(1, sums, state, sys, min_corr, solve, rows);
+}
+
 void track::sensor_frames(TrackScratch& ts, RenderState& rs, Timing& tm, RenderGrid rg, const I3DFusionCamera& dc, const float* store_depth,
                           int store_F, int n, const int32_t* ids, const double* pose_in, const I3DTrackParams& P, const int* Wl, const int* Hl,
                           double* pose_out, I3DTrackInfo* info, cudaStream_t st, const TrackColor* col)

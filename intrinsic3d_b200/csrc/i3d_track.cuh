@@ -39,17 +39,6 @@ namespace i3d
 #define DA(a, b) __dadd_rn((a), (b))
 #define DS(a, b) __dsub_rn((a), (b))
 
-// R (row-major 3 x 3) times v, sums left to right, plus t when given
-__device__ __forceinline__ void tr_xform(const float* R, const float* t, const float v[3], float out[3])
-{
-#pragma unroll
-    for (int d = 0; d < 3; ++d)
-    {
-        const float s = FA(FA(FM(R[3 * d], v[0]), FM(R[3 * d + 1], v[1])), FM(R[3 * d + 2], v[2]));
-        out[d] = t ? FA(s, t[d]) : s;
-    }
-}
-
 // world -> camera of T_cw (R | t): R^T | -(R^T t), in double
 __device__ __forceinline__ void tr_inverse(const double* T, double* out)
 {

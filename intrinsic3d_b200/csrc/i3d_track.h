@@ -156,6 +156,12 @@ int fusion_frames(TrackScratch& ts, const FusionState& fs, bool skip, Timing& tm
 int odometry(TrackScratch& ts, FusionState& fs, bool skip, Timing& tm, const SensorStore& ss, int n, const int32_t* ids, const double* pose_first,
              const I3DTrackParams& P, const int* Wl, const int* Hl, double* pose_out, I3DTrackInfo* info, std::string& error, cudaStream_t st,
              const TrackColor* col = nullptr, bool reference = false);
+// The tracker's pose kernels for one device-resident state, for other modules' point-to-plane problems (the reference-mesh registration,
+// i3d_register.cuh).  init: k_track_init of pose_in (device [12]).  step: k_tile_sums<kTrackVals> of the partials [blocks][kTrackVals]
+// into sums, then k_track_solve of that system (solve = 0: recorded only), its copy into sys and its rows added to *rows.
+void pose_init(const double* pose_in, TrackState* state, cudaStream_t st);
+void pose_step(int blocks, const double* partials, double* sums, TrackState* state, double* sys, int min_corr, int solve, unsigned long long* rows,
+               cudaStream_t st);
 } // namespace track
 
 } // namespace i3d

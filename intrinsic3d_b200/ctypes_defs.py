@@ -338,6 +338,46 @@ class I3DDistanceInfo(C.Structure, _Dictable):
     ]
 
 
+REGISTER_MAX_STAGES = 4          # I3D_REGISTER_MAX_STAGES of include/i3d_types.h
+
+
+class I3DRegisterParams(C.Structure, _Dictable):
+    _fields_ = [
+        ("samples_per_edge", C.c_int32),
+        ("num_stages", C.c_int32),
+        ("max_distance", C.c_float * REGISTER_MAX_STAGES),
+        ("iterations", C.c_int32 * REGISTER_MAX_STAGES),
+        ("min_normal_cos", C.c_float),
+        ("min_correspondences", C.c_int32),
+        ("cell_size", C.c_float),
+    ]
+
+
+class I3DRegisterInfo(C.Structure, _Dictable):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("iterations", C.c_int32),
+        ("initial_rows", C.c_int64),
+        ("final_rows", C.c_int64),
+        ("initial_weight", C.c_double),
+        ("final_weight", C.c_double),
+        ("initial_residual_sq", C.c_double),
+        ("final_residual_sq", C.c_double),
+        ("initial_rms", C.c_double),
+        ("final_rms", C.c_double),
+        ("update_norm", C.c_double),
+        ("num_samples", C.c_int64),
+        ("point_triangle_tests", C.c_int64),
+        ("cell_size", C.c_float),
+        ("grid", C.c_int32 * 3),
+        ("num_cells", C.c_int64),
+        ("num_cell_entries", C.c_int64),
+        ("ms_grid", C.c_double),
+        ("ms_rows", C.c_double),
+        ("ms_solve", C.c_double),
+    ]
+
+
 # I3D_GRID_FROM_MESH_* sources of include/i3d_types.h
 GRID_FROM_MESH_SOURCES = {"reference": 0, "resident": 1}
 

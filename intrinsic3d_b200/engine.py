@@ -11,7 +11,8 @@ import os
 
 import numpy as np
 
-from .ctypes_defs import (DISTANCE_MAX_THRESHOLDS, GRID_FROM_MESH_SOURCES, RASTER_COLORS, RASTER_PLANES, RENDER_PLANES, SH_SOURCES, I3DDistanceInfo,
+from .ctypes_defs import (DISTANCE_MAX_THRESHOLDS, GRID_FROM_MESH_SOURCES, RASTER_COLORS, RASTER_PLANES, REGISTER_MAX_STAGES, RENDER_PLANES, SH_SOURCES,
+                          I3DDistanceInfo, I3DRegisterInfo, I3DRegisterParams,
                           I3DDistanceParams, I3DGridFromMeshInfo, I3DGridFromMeshParams, I3DFusionCamera, I3DFusionParams, I3DIntrinsicTextureInfo,
                           I3DIntrinsicTextureParams, I3DIterInfo, I3DShLighting,
                           I3DLightingInfo, I3DLightingParams, I3DMeshInfo, I3DMeshParams, I3DParams, I3DRasterCamera, I3DRasterInfo,
@@ -42,6 +43,8 @@ EXPORTED_SYMBOLS = [
     "i3d_default_intrinsic_texture_params", "i3d_decompose_texture", "i3d_download_intrinsic_texture", "i3d_set_relight",
     "i3d_sizeof_distance_params", "i3d_sizeof_distance_info", "i3d_default_distance_params", "i3d_upload_reference_mesh",
     "i3d_surface_distance", "i3d_download_surface_distance", "i3d_debug_set_keep_distance_samples", "i3d_debug_get_distance_samples",
+    "i3d_sizeof_register_params", "i3d_sizeof_register_info", "i3d_default_register_params", "i3d_register_reference_mesh",
+    "i3d_transform_reference_mesh", "i3d_debug_get_register_systems",
     "i3d_sizeof_grid_from_mesh_params", "i3d_sizeof_grid_from_mesh_info", "i3d_default_grid_from_mesh_params", "i3d_grid_from_mesh",
     "i3d_debug_get_grid_from_mesh_voxels",
     "i3d_sizeof_render_params", "i3d_sizeof_render_stats", "i3d_default_render_params", "i3d_render_keyframes", "i3d_download_render",
@@ -153,6 +156,20 @@ def load_library():
     L.i3d_debug_set_keep_distance_samples.argtypes = [C.c_void_p, C.c_int]
     L.i3d_debug_get_distance_samples.restype = C.c_int
     L.i3d_debug_get_distance_samples.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int32)]
+    L.i3d_sizeof_register_params.restype = C.c_uint64
+    L.i3d_sizeof_register_info.restype = C.c_uint64
+    if L.i3d_sizeof_register_params() != C.sizeof(I3DRegisterParams) or L.i3d_sizeof_register_info() != C.sizeof(I3DRegisterInfo):
+        raise RuntimeError("ABI mismatch between ctypes_defs.py and libi3d_b200.so (register structs)")
+    L.i3d_default_register_params.restype = None
+    L.i3d_default_register_params.argtypes = [C.POINTER(I3DRegisterParams)]
+    L.i3d_register_reference_mesh.restype = C.c_int
+    L.i3d_register_reference_mesh.argtypes = [C.c_void_p, C.POINTER(I3DRegisterParams), C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                              C.POINTER(I3DRegisterInfo)]
+    L.i3d_transform_reference_mesh.restype = C.c_int
+    L.i3d_transform_reference_mesh.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+    L.i3d_debug_get_register_systems.restype = C.c_int
+    L.i3d_debug_get_register_systems.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                                 C.POINTER(C.c_int32)]
     L.i3d_sizeof_grid_from_mesh_params.restype = C.c_uint64
     L.i3d_sizeof_grid_from_mesh_info.restype = C.c_uint64
     if L.i3d_sizeof_grid_from_mesh_params() != C.sizeof(I3DGridFromMeshParams) or L.i3d_sizeof_grid_from_mesh_info() != C.sizeof(I3DGridFromMeshInfo):
@@ -301,6 +318,12 @@ def default_texture_params() -> I3DTextureParams:
 def default_distance_params() -> I3DDistanceParams:
     p = I3DDistanceParams()
     load_library().i3d_default_distance_params(C.byref(p))
+    return p
+
+
+def default_register_params() -> I3DRegisterParams:
+    p = I3DRegisterParams()
+    load_library().i3d_default_register_params(C.byref(p))
     return p
 
 
@@ -609,6 +632,41 @@ class Engine:
 
     def debug_set_keep_distance_samples(self, on: bool = True):
         self._check(self.L.i3d_debug_set_keep_distance_samples(self.h, 1 if on else 0))
+
+    def register_reference_mesh(self, max_distance=(0.016, 0.008, 0.004), iterations=(10, 10, 10), samples_per_edge: int = 1,
+                                min_normal_cos: float = 0.5, min_correspondences: int = 100, cell_size=None, init=None):
+        """Estimates the rigid T that maps the reference mesh onto the resident mesh (x_resident = R x_reference + t), on the device
+        (DESIGN.md §6aa): point-to-plane ICP of the resident mesh's area samples against the reference's faces, one stage per
+        (max_distance metres, iterations) pair, coarse to fine, from init (T [12] R row-major | t; None = identity).  Returns (T float64
+        [12], info I3DRegisterInfo).  Nothing else changes; transform_reference_mesh(T) moves the reference.  cell_size None picks the
+        search grid's cell edge automatically; the result does not depend on it."""
+        md, it = [float(d) for d in max_distance], [int(i) for i in iterations]
+        if len(md) != len(it) or not 1 <= len(md) <= REGISTER_MAX_STAGES:
+            raise ValueError(f"max_distance and iterations need the same length in [1, {REGISTER_MAX_STAGES}], got {len(md)} and {len(it)}")
+        pad = REGISTER_MAX_STAGES - len(md)
+        prm = I3DRegisterParams(int(samples_per_edge), len(md), (C.c_float * REGISTER_MAX_STAGES)(*(md + [0.0] * pad)),
+                                (C.c_int32 * REGISTER_MAX_STAGES)(*(it + [0] * pad)), float(min_normal_cos), int(min_correspondences),
+                                0.0 if cell_size is None else float(cell_size))
+        T0 = None if init is None else np.ascontiguousarray(init, np.float64).reshape(12)
+        T = np.empty(12, np.float64)
+        info = I3DRegisterInfo()
+        self._check(self.L.i3d_register_reference_mesh(self.h, C.byref(prm), _p(T0, C.c_double), _p(T, C.c_double), C.byref(info)))
+        return T, info
+
+    def transform_reference_mesh(self, T):
+        """Moves the reference mesh by T [12] (R row-major | t) on the device: x <- float(R x + t), in double"""
+        T = np.ascontiguousarray(T, np.float64).reshape(12)
+        self._check(self.L.i3d_transform_reference_mesh(self.h, _p(T, C.c_double)))
+
+    def debug_register_systems(self, num_samples: int):
+        """The last register_reference_mesh's systems float64 [n, 31] (the 29 tracker sums, sum w for the first and the last system, 0),
+        the pose T^-1 each was formed at float64 [n, 12], and the per-sample nearest face at the initial pose int32 [num_samples]"""
+        n = C.c_int32()
+        self._check(self.L.i3d_debug_get_register_systems(self.h, C.byref(n), None, None, None))
+        S, M = np.empty((n.value, 31), np.float64), np.empty((n.value, 12), np.float64)
+        f = np.empty(num_samples, np.int32)
+        self._check(self.L.i3d_debug_get_register_systems(self.h, C.byref(n), _p(S, C.c_double), _p(M, C.c_double), _p(f, C.c_int32)))
+        return S, M, f
 
     def grid_from_mesh(self, source: str = "reference", voxel_size: float = 0.002, band: float = 3.0, cell_size=None):
         """Replaces the voxel set by the narrow-band signed distance field of a triangle mesh, built on the device (DESIGN.md §6v): every
